@@ -49,7 +49,7 @@ def agent_args(device_index=0, encoder_mode="cached"):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -153,9 +153,8 @@ def run_reference(args):
 def encoder_roofline(engine, peaks, run_utterance):
     """Dominant kernel of the step = the encoder-stack kernel (one launch per 320 ms chunk runs all 12 Conformer layers over the
     <= 16 not-yet-final rows): encoder_layers_cluster_kernel (4 clusters x 16 CTAs, activations in distributed shared memory,
-    weights streamed by TMA from repacked blobs) when the step has <= 16 rows, else encoder_layers_persistent_kernel (148 CTAs);
-    16.4 % of the summed kernel time in profiles/r2_launches_bench_window_cluster.md, 17.7 % of the utterance's device time measured here.
-    It streams every GEMM weight of the stack once per launch -> HBM roofline.  Measured live: the engine brackets each
+    weights streamed by TMA from repacked blobs) when the step has <= 16 rows, else encoder_layers_persistent_kernel (one CTA per
+    SM); its share of the utterance's device time is measured here.  It streams every GEMM weight of the stack once per launch -> HBM roofline.  Measured live: the engine brackets each
     launch with CUDA events on the launching stream while one more resident utterance is streamed (32 launches).
     algorithmic bytes per launch = 12 x (4*D*FFN + 7*D*D) x 4 B of weights (122.7 MB) + the K / V cache and
     relative-position rows the attention reads (12 x (3T + nA) x D x 4 B)."""
@@ -176,14 +175,10 @@ def encoder_roofline(engine, peaks, run_utterance):
     mt_ms, mt_n, mt_steps = engine.mt_time()
     cl = engine.cluster_steps() - c0
     engine.set_option("persistent_time", 0)
-    peak = peaks.get("hbm_gbs", 6650.0)
-    traffic = None
+    peak = peaks.get("hbm_gbs", 3350.0)
     cluster = n > 0 and cl * 2 > n  # which kernel took most of the timed launches
-    tp = os.path.join(ROOT, "profiles", "r2_cluster_kernel_traffic.json" if cluster else "r2_dominant_kernel_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get("dram_bytes_per_launch")
     if n == 0:
-        return {"bound": "hbm", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None, "traffic": traffic,
+        return {"bound": "hbm", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None,
                 "kernel": "encoder_layers_persistent_kernel", "note": "no persistent launches were recorded"}
     ach = nbytes / (ms * 1e-3) / 1e9
     if cluster:
@@ -192,7 +187,7 @@ def encoder_roofline(engine, peaks, run_utterance):
         note_ = ("batch-1 streaming: 16 rows per launch; per layer 9 distributed-shared-memory exchanges (st.async + mbarrier) and 2 split "
                  "grid barriers; bound by ~25 dependent latencies per layer (mbarrier waits, shuffle trees, L2 round trips), not by bandwidth")
     else:
-        kernel = "encoder_layers_persistent_kernel<2048> (fp32, all 12 Conformer layers of one streaming step, 148 CTAs cooperative)"
+        kernel = "encoder_layers_persistent_kernel<2048> (fp32, all 12 Conformer layers of one streaming step, one CTA per SM, cooperative)"
         note_ = ("batch-1 streaming: 16 rows per launch, 108 grid barriers; the kernel is bound by dependent-phase latency "
                  "(barrier + one L2/HBM round trip per phase), not by bandwidth")
     # second-largest kernel, measured the same way: the single-token MT kernel (one greedy step streams every decoder weight and the
@@ -205,17 +200,17 @@ def encoder_roofline(engine, peaks, run_utterance):
         mt = {"kernel": "mt_decode_persistent_kernel_v2 (fp32, one launch per burst of greedy steps)", "bound": "hbm", "achieved": mt_ach,
               "peak": peak, "unit": "GB/s", "frac": mt_ach / peak, "algorithmic_bytes_per_step": mt_bytes_step, "steps_timed": mt_steps,
               "launches_timed": mt_n, "us_per_step": mt_ms / max(mt_steps, 1.0) * 1e3, "share_of_utterance_time": mt_ms / utt_ms}
-    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
             "kernel": kernel, "cluster_kernel_launches": cl, "share_of_utterance_time": ms / utt_ms, "second_kernel": mt,
             "algorithmic_bytes_per_launch": nbytes / n, "launches_timed": n, "us_per_launch": ms / n * 1e3,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6.65 TB/s",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s",
             "note": note_}
 
 
 def gemm_rooflines(engine, peaks):
     """Secondary: the GEMM / conv kernels at the vocoder's heaviest conv shape (L = 5*500 rows, 256 -> 256 channels, k = 11):
-    fp32 CUDA cores and the tap-shift tcgen05 kernel with pre-packed weights.
-    FLOPs are fp32-equivalent (2*L*C*C*k); the tcgen05 kernels spend 3 bf16 MMAs per product (bf16x3 split)."""
+    fp32 CUDA cores and the tap-shift wgmma kernel with pre-packed weights.
+    FLOPs are fp32-equivalent (2*L*C*C*k); the wgmma kernels spend 3 bf16 MMAs per product (bf16x3 split)."""
     import torch
 
     L, C, k = 5 * 500, 256, 11
@@ -224,7 +219,7 @@ def gemm_rooflines(engine, peaks):
     b = torch.zeros(C, device=engine.device)
     out = {}
     for name, mode, mmas in (("gemm_kernel<128,64> fp32 CUDA cores", 0, 0),
-                             ("umma2_kernel tcgen05 bf16x3, tap-shift + cp.async.bulk weights (default path)", 12, 3)):
+                             ("umma2_kernel wgmma bf16x3, tap-shift + cp.async.bulk weights (default path)", 12, 3)):
         fn = lambda: engine.op_conv1d(x, w, b, k, 1, k // 2, 0.1, mode)
         for _ in range(3):
             fn()
@@ -237,7 +232,7 @@ def gemm_rooflines(engine, peaks):
         torch.cuda.synchronize()
         ms = s.elapsed_time(e) / 20
         ach = 2.0 * L * C * C * k / (ms * 1e-3) / 1e12
-        peak = peaks.get("bf16_tflops", 1590.0)
+        peak = peaks.get("bf16_tflops", 989.0)
         out[name] = {"bound": "tensor", "achieved_fp32_equivalent": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                      "us_per_launch": ms * 1e3, "shape": {"L": L, "C_in": C, "C_out": C, "k": k}}
         if mmas:  # every fp32-grade product is `mmas` bf16 MMAs: the tensor pipe itself runs at mmas x the fp32-equivalent rate
@@ -290,7 +285,7 @@ def asr_streams_leg(eng, n_streams=32, seconds=10.0, chunk_ms=160, rank=0):
 
 def offline_leg(agent, peaks, B=32, seconds=15.0):
     """BASELINE configs[2]: offline S2ST, batch of 32 padded 15 s utterances on one GPU: batched encoder over B x T = 12,000 rows
-    (tcgen05 GEMMs), CTC prints, greedy MT, T2U + unit decoder and the vocoder per utterance (the reference's vocoder script is
+    (wgmma GEMMs), CTC prints, greedy MT, T2U + unit decoder and the vocoder per utterance (the reference's vocoder script is
     batch 1 too: generate_waveform_from_code.py:40-78).  Also times the two kernels the config is quoted for: the FFN GEMM at
     M = 12,000 and the vocoder generator on 750 frames."""
     import torch
@@ -332,8 +327,8 @@ def offline_leg(agent, peaks, B=32, seconds=15.0):
     line = {"workload": f"offline S2ST, batch {B} x {seconds:.0f} s padded (BASELINE.json configs[2])", "unit": "audio-s/s",
             "value": B * seconds / ((ms_gen + ms_voc) * 1e-3), "ms_encoder_batched": ms_enc, "ms_generate": ms_gen, "ms_vocoder": ms_voc,
             "encoder_rows": rows, "encoder_tflops_fp32_equivalent": enc_flops / (ms_enc * 1e-3) / 1e12, "output_audio_s": out_s}
-    # the FFN GEMMs of the batched encoder on the tcgen05 kernel (bf16 x 6 split = fp32-grade), M = B x T rows
-    peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0))
+    # the FFN GEMMs of the batched encoder on the wgmma kernel (bf16 x 6 split = fp32-grade), M = B x T rows
+    peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0))
     g = {}
     x = torch.randn(rows, 256, device="cuda")
     hbuf = torch.randn(rows, 2048, device="cuda")
@@ -348,7 +343,9 @@ def offline_leg(agent, peaks, B=32, seconds=15.0):
             mm = 3 if pieces == 2 else 6
             g[f"{name}, bf16x{mm}"] = {"us": ms * 1e3, "tflops_fp32_equivalent": fl / (ms * 1e-3) / 1e12,
                                       "tensor_pipe_frac": mm * fl / (ms * 1e-3) / 1e12 / peak}
-    line["ffn_gemm_umma2"] = {"M": rows, "peak_tflops": peak, "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained", "kernels": g}
+    line["ffn_gemm_umma2"] = {"M": rows, "peak_tflops": peak,
+                              "peak_source": "MEASURED_PEAKS.json" if "bf16_tflops_sustained" in peaks or "bf16_tflops" in peaks
+                              else "H100 SXM data sheet, dense BF16", "kernels": g}
     # vocoder generator on 750 frames (15 s of output audio)
     codes750 = torch.randint(0, 1000, (750,), device="cuda")
     eng.vocoder_durations(codes750, False)
@@ -409,6 +406,21 @@ def mixed_pairs_leg(device_index=0, chunk_ms=640, seconds=10.0, lags=(0, 1, 2, 4
                         "latency sweep over lagging_k1 (BASELINE.json configs[4])", "unit": "audio-s/s", "sweep": out}
 
 
+def dump_outputs(out_dir, sink):
+    """The timed path's results of its last step, one entry per policy call: the concatenated waveform samples it emitted,
+    whether the call wrote, and how many samples it wrote."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    wavs = [w.detach().float().cpu().numpy().ravel() for _, w in sink if w is not None]
+    arrays = {"wav": np.concatenate(wavs).astype(np.float32) if wavs else np.zeros(0, np.float32),
+              "call_is_write": np.array([1.0 if w else 0.0 for w, _ in sink], dtype=np.float64),
+              "call_wav_samples": np.array([0.0 if x is None else float(x.numel()) for _, x in sink], dtype=np.float64)}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -418,6 +430,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--encoder-mode", type=str, default="cached", choices=["cached", "recompute"])
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2] / configs[3] legs (extra keys of the JSON line)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write what the last timed step returned (the waveform chunks of every policy call) as DIR/<name>.npy")
     ap.add_argument("--ncu-window", action="store_true",
                     help="after the timed runs, stream one more resident utterance between cudaProfilerStart/Stop (for `ncu --profile-from-start off`)")
     args = ap.parse_args()
@@ -480,9 +494,9 @@ def main():
     n = SAMPLE_RATE * CHUNK_MS // 1000
     utts = [synth.make_audio(UTT_SECONDS, seed=1234 + 7 * rank + i) for i in range(2)]  # rank-specific utterances
     utts_dev = [u.cuda() for u in utts]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 50 MB L2
 
-    def stream_resident(u):
+    def stream_resident(u, sink=None):
         agent.reset()
         out = 0
         for i in range(0, u.numel(), n):
@@ -490,6 +504,8 @@ def main():
             w, wav = agent.step_resident(u, end, end >= u.numel())
             if w and wav is not None:
                 out += wav.numel()
+            if sink is not None:  # --dump-outputs: what the caller received from this policy call
+                sink.append((bool(w), None if wav is None else wav.clone()))
         return out
 
     def stream_e2e(u_host):
@@ -501,7 +517,7 @@ def main():
                 out += len(seg.content)
         return out
 
-    def timed(fn, inputs, steps, warmup):
+    def timed(fn, inputs, steps, warmup, sink=None):
         for i in range(warmup):
             fn(inputs[i % len(inputs)])
         if dist is not None:
@@ -513,7 +529,7 @@ def main():
             flush.fill_(float(i))  # L2 flush between timed iterations (outside the events)
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             s.record()
-            out += fn(inputs[i % len(inputs)])
+            out += fn(inputs[i % len(inputs)], sink) if sink is not None and i == steps - 1 else fn(inputs[i % len(inputs)])
             e.record()
             torch.cuda.synchronize()
             total_ms += s.elapsed_time(e)
@@ -528,7 +544,10 @@ def main():
     if rank == 0:
         sampler.start()
     note("timed: resident")
-    ms_res, out_res, launches = timed(stream_resident, utts_dev, args.steps, args.warmup)
+    sink = [] if args.dump_outputs and rank == 0 else None
+    ms_res, out_res, launches = timed(stream_resident, utts_dev, args.steps, args.warmup, sink)
+    if sink is not None:
+        dump_outputs(args.dump_outputs, sink)
     note("timed: e2e")
     utts_host = [u.tolist() for u in utts]
     ms_e2e, out_e2e, _ = timed(stream_e2e, utts_host, args.steps, max(1, args.warmup // 2))

@@ -213,16 +213,16 @@ int ss_pool_step(ss_engine* h, void* stream, int n, const int32_t* slots_host, i
 /* ---- single ops exported for the parity tests (same kernels the entry points above launch) ------------- */
 int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N,
                  int act, float* out_dev);
-/* same GEMM on the tcgen05 tensor-core kernel (kernels_umma2.cu, bf16 operand splitting, pieces = 2: 3 MMAs, 3: 6 MMAs per product);
+/* same GEMM on the wgmma tensor-core kernel (kernels_umma2.cu, bf16 operand splitting, pieces = 2: 3 MMAs, 3: 6 MMAs per product);
  * parity-test / roofline hook */
 int ss_op_linear_umma(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N,
                       int act, int pieces, float* out_dev);
 /* out[L][N] = conv1d(pre_lrelu(x[L][C_in]), w[N][ksize*C_in] (tap-major), stride 1, dilation dil, left padding pad_left) + bias on
- * the kernel selected by mode: 0 = fp32 CUDA cores, 12 / 13 = tcgen05 tap-shift kernel with pre-packed weights (kernels_umma2.cu,
+ * the kernel selected by mode: 0 = fp32 CUDA cores, 12 / 13 = wgmma tap-shift kernel with pre-packed weights (kernels_umma2.cu,
  * 2 / 3 bf16 pieces per operand); parity-test hook */
 int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in, const float* w_dev, const float* bias_dev, int N,
                  int ksize, int dil, int pad_left, float pre_lrelu, int mode, float* out_dev);
-/* engine options: "umma_vocoder" / "umma_linear" = 0 (fp32 CUDA cores), 12 or 13 (tcgen05 kernel, 2 or 3 bf16 pieces per operand); "umma_min_rows" / "umma_min_channels": smaller GEMMs / convs stay on
+/* engine options: "umma_vocoder" / "umma_linear" = 0 (fp32 CUDA cores), 12 or 13 (wgmma kernel, 2 or 3 bf16 pieces per operand); "umma_min_rows" / "umma_min_channels": smaller GEMMs / convs stay on
  * the fp32 kernels; "umma2_cache_clear": drop the packed weight copies;
  * "persistent_encoder" = 1 (default): ss_encoder_stream_step runs the layer stack as one cooperative kernel when the
  * shape fits, 0: one kernel per op; "persistent_barrier" = 1 (default): that kernel's own counter barrier instead of
@@ -230,7 +230,7 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
  * on the caller's stream plus two engine-owned streams (joined before the call returns control of the stream);
  * "persistent_encoder_cluster" = 1 (0 on a fresh handle; the Python engine switches it on): steps with <= 16 active rows run on
  * the cluster kernel (4 thread-block clusters x 16 CTAs, activations in distributed shared memory; allocates 123 MB of repacked
- * weights the first time); larger steps and refused launches take the 148-CTA kernel; "cluster_cooperative" = 1 (default; 0 only
+ * weights the first time); larger steps and refused launches take the one-CTA-per-SM kernel; "cluster_cooperative" = 1 (default; 0 only
  * under a profiler that serialises kernels and cannot replay cooperative cluster launches);
  * "persistent_ffn_fused", "persistent_mt", "persistent_mt_v2", "persistent_mt_prefix", "fbank_tma" = 1 (default): kernel variants of
  * round 2, each tested against the path it replaces; "umma2_fused_reduce" = 0 (default: measured slower);

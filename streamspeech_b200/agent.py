@@ -1,4 +1,4 @@
-"""SimulEval agents backed by the B200 engine: same classes, flags, policy()/push()/pop() behaviour as
+"""SimulEval agents backed by the H100 engine: same classes, flags, policy()/push()/pop() behaviour as
 
   agent/speech_to_speech.streamspeech.agent.py   (StreamSpeechS2STAgent, :101-770)
   agent/speech_to_text.asr.streamspeech.agent.py (StreamSpeechASRAgent,  :100-433)
@@ -145,7 +145,7 @@ class _DeviceAudio:
 class _EngineAgentMixin:
     def _init_engine(self, args, need_vocoder: bool):
         if args.sample_rate not in (SAMPLE_RATE, ORG_SAMPLE_RATE):
-            raise NotImplementedError("the B200 front-end takes 16 kHz or 48 kHz input (the reference's two cases: agent:32-35)")
+            raise NotImplementedError("the H100 front-end takes 16 kHz or 48 kHz input (the reference's two cases: agent:32-35)")
         override = getattr(args, "checkpoint_override", None)  # (cfg, model state dict, vocoder state dict, gcmvn) already in memory
         if override is not None:                                # (bench.py: the NCCL-broadcast copy of rank 0's checkpoint)
             cfg, sd, vsd_o, gcmvn = override

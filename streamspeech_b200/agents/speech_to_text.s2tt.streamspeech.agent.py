@@ -1,4 +1,4 @@
-"""`simuleval --agent <this file>`: the B200-engine drop-in for the reference's agent/speech_to_text.s2tt.streamspeech.agent.py.
+"""`simuleval --agent <this file>`: the H100-engine drop-in for the reference's agent/speech_to_text.s2tt.streamspeech.agent.py.
 
 SimulEval imports the file as a top-level module and expects exactly ONE @entrypoint class in it
 (SimulEval/simuleval/utils/agent.py:25-56); the implementation lives in streamspeech_b200/agent.py."""

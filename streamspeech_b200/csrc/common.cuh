@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels.
+// Shared device helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -21,7 +21,7 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // as plain launches unless the engine option graph_pdl asks otherwise
 extern thread_local int g_pdl_off;
 
-// Shared-memory carve-out: the tcgen05 kernels need > 100 KB of shared memory per CTA, the SIMT kernels a few KB.  An SM
+// Shared-memory carve-out: the wgmma kernels need > 100 KB of shared memory per CTA, the SIMT kernels a few KB.  An SM
 // holds ONE carve-out at a time, so kernels that ask for different ones cannot share an SM and every change drains it
 // -- which is what the vocoder's three concurrent streams of alternating conv / reduce kernels would do.  With the option on
 // (default) every kernel of the library asks for the maximum shared-memory carve-out, once per kernel function.
@@ -69,7 +69,7 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   // only small grids launch early: CTAs of a large dependent grid would sit on shared memory / registers that the
-  // (multi-wave) predecessor still needs (measured: vocoder convs 35 ms -> 48 ms with unconditional PDL)
+  // (multi-wave) predecessor still needs
   const unsigned long long ctas = (unsigned long long)grid.x * grid.y * grid.z;
   attr[0].val.programmaticStreamSerializationAllowed = (ctas <= 296 && !g_pdl_off) ? 1 : 0;
   cfg.attrs = attr;

@@ -88,7 +88,7 @@ struct ss_engine {
   std::string err;
   bool finalized = false;
   int attn_chunk = 8, conv_chunk = 8;
-  int umma_vocoder = 0;   // 0 = fp32 CUDA-core convs, 2 / 3 = tcgen05 with that many bf16 pieces per operand
+  int umma_vocoder = 0;   // 0 = fp32 CUDA-core convs, 2 / 3 = wgmma with that many bf16 pieces per operand
   int umma_linear = 0;    // same for large-M linears (unit decoder, T2U, MT prefill, full-prefix encoder)
                           // 12 / 13: second-generation kernel (kernels_umma2.cu) with 2 / 3 pieces
   int unit_grouped = 1;         // unit decoder layer 1: self-attention over the S distinct rows instead of the 25*S copies
@@ -99,7 +99,7 @@ struct ss_engine {
   cudaStream_t aux_stream[2] = {nullptr, nullptr};
   cudaEvent_t fork_event = nullptr, join_event[2] = {nullptr, nullptr};
   // CUDA-graph replay of the vocoder generator (conv_pre .. conv_post) per (frames, arena, routing): value = (exec, nodes)
-  int vocoder_graph = 0;  // measured on B200: no gain (the generator is bound by kernel execution, not by host enqueue)
+  int vocoder_graph = 0;  // off: the generator is bound by kernel execution, not by host enqueue
   int graph_pdl = 0;
   cudaStream_t capture_stream = nullptr;
   std::map<std::tuple<int, uintptr_t, int, int, int>, std::pair<cudaGraphExec_t, int>> voc_graphs;
@@ -194,7 +194,7 @@ struct ss_engine {
   unsigned* persist_bar = nullptr;   // arrival counter of the kernel's own grid barrier (option persistent_barrier)
   unsigned persist_bar_target = 0;
   unsigned* async_err_pinned = nullptr;  // host copy of persist_bar[SS_BAR_ERR_WORD] (read back at synchronisation points)
-  int persistent_barrier = 1;        // 0: cooperative-groups grid.sync(), 1: own counter barrier (1.6 us cheaper per barrier)
+  int persistent_barrier = 1;        // 0: cooperative-groups grid.sync(), 1: own counter barrier (cheaper per barrier)
   ss::MtLayerP* mt_persist_layers = nullptr;   // [mt_layers] device pointer table for kernels_persist_mt.cu
   int persistent_mt = 1;                       // single-token MT decode steps as one cooperative kernel per burst
   int persistent_mt_v2 = 1;                    // single-token kernel with 6 grid barriers per layer (head-group partial projections)

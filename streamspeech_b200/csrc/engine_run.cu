@@ -34,7 +34,7 @@ void route_from(ss_engine* h) {
   g_umma2_cache = h->umma2_cache;
 }
 
-// conv-as-GEMM dispatch: the tcgen05 split-bf16 kernel (kernels_umma2.cu; mode 12 / 13 = 2 / 3 bf16 pieces per operand) when enabled and
+// conv-as-GEMM dispatch: the wgmma split-bf16 kernel (kernels_umma2.cu; mode 12 / 13 = 2 / 3 bf16 pieces per operand) when enabled and
 // the shape fits, the fp32 CUDA-core kernel otherwise
 void conv_gemm(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaStream_t st) {
   const int rows = a.B * a.L_rows;
@@ -467,7 +467,7 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
       cluster_done = c.enc_layers <= 16 && encoder_layers_cluster(h->persist_layers, h->cl_blobs, c.enc_layers, x, h->st_k, h->st_v, h->st_glu, nA, a0, T, h->Tpos, h->attn_chunk, cc,
                                             c.dw_kernel, h->persist_bar, &h->persist_bar_target, h->persistent_profile ? h->persist_ts : nullptr, pos_tabs, h->cluster_cooperative, st) == 0;
       if (cluster_done) ++h->cl_steps;
-      if (!cluster_done) cudaGetLastError();  // refused launch: the 148-CTA kernel below takes the step
+      if (!cluster_done) cudaGetLastError();  // refused launch: the one-CTA-per-SM kernel below takes the step
     }
     if (persistent && !cluster_done)
       persistent = encoder_layers_persistent(h->persistent_alias ? h->persist_alias : h->persist_layers, c.enc_layers, x, hid, qb, att, dw, h->st_k, h->st_v, h->st_glu, nA, a0, T, D,
@@ -1283,7 +1283,7 @@ int ss_op_linear_umma(ss_engine* h, void* stream, const float* x_dev, int M, int
   a.x = x_dev; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = K; a.ldx = K;
   Epilogue ep = ep_out(out_dev, N, act);
   ep.bias = bias_dev;
-  if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the tcgen05 kernel");
+  if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the wgmma kernel");
   umma2_conv(h->umma2_cache, a, w_dev, N, ep, pieces, S(stream));
   return check_launch(h, "ss_op_linear_umma");
 }
@@ -1298,10 +1298,10 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
   Epilogue ep = ep_out(out_dev, N);
   ep.bias = bias_dev;
   if (mode >= 12) {
-    if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the tcgen05 conv kernel");
+    if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the wgmma conv kernel");
     umma2_conv(h->umma2_cache, a, w_dev, N, ep, mode - 10, S(stream));
   } else if (mode >= 2) {
-    return h->fail(SS_ERR_INVALID, "modes 2 / 3 (first-generation tcgen05 kernel) were removed: use 12 / 13");
+    return h->fail(SS_ERR_INVALID, "modes 2 / 3 (first-generation tensor-core kernel) were removed: use 12 / 13");
   } else {
     gemm_conv(a, w_dev, N, ep, S(stream));
   }

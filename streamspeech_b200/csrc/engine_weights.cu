@@ -460,7 +460,7 @@ void finalize_impl(ss_engine* h) {
 
 extern "C" {
 
-const char* ss_version(void) { return "streamspeech_b200 0.1 (sm_100a)"; }
+const char* ss_version(void) { return "streamspeech_b200 0.1 (sm_90a)"; }
 
 int ss_create(ss_engine** out, int device, const ss_config* cfg) {
   if (!out || !cfg) return SS_ERR_INVALID;

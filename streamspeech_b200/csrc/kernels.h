@@ -1,4 +1,4 @@
-// Internal C++ launch API of the sm_100a kernels (streamspeech_b200/csrc/kernels_*.cu).
+// Internal C++ launch API of the sm_90a kernels (streamspeech_b200/csrc/kernels_*.cu).
 // Everything enqueues on the given stream and never synchronises.
 #pragma once
 #include <cuda_runtime.h>
@@ -73,7 +73,7 @@ unsigned* splitk_counters(int n_tiles);  // zeroed ticket counters of the curren
 void set_splitk_slot(int slot);
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st);
 
-// tcgen05 path (kernels_umma2.cu): stride-1 convolutions / linears over one sequence (B = 1) with
+// wgmma path (kernels_umma2.cu): stride-1 convolutions / linears over one sequence (B = 1) with
 // pre-packed bf16-split weights streamed by cp.async.bulk and activations converted once per channel chunk (taps are
 // descriptor row shifts).  The cache owns the packed weight copies (keyed by weight pointer and tiling).
 struct Umma2Cache;

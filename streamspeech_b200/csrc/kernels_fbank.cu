@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) fbank_kernel(const float* __restrict__ sa
   }
 }
 
-// Same arithmetic, B200 staging: the 400 samples of the frame (1600 contiguous bytes, 640-byte aligned offsets) arrive in shared
+// Same arithmetic, TMA staging: the 400 samples of the frame (1600 contiguous bytes, 640-byte aligned offsets) arrive in shared
 // memory by ONE bulk-async copy (cp.async.bulk = the TMA engine's 1-D path, UBLKCP in SASS) completing on an mbarrier while the
 // twiddle table is being computed; the mel bank is read TRANSPOSED ([257][80]) so that the 80 mel threads read coalesced rows
 // (the [80][257] layout made every lane walk its own 1 KB row: 80 uncoalesced streams per frame).

@@ -3,7 +3,7 @@
 //
 // Why fp32 CUDA cores here: the parity bar is bit-exact arg-max tokens against the reference's fp32
 // CPU path (BASELINE.json north_star); every GEMM on the path feeds an arg-max within a few layers.
-// This kernel is the exact-precision baseline; the tcgen05 path (kernels_umma2.cu) takes the large-M GEMMs.
+// This kernel is the exact-precision baseline; the wgmma path (kernels_umma2.cu) takes the large-M GEMMs.
 #include <algorithm>
 
 #include "common.cuh"
@@ -369,8 +369,9 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
   const long ctas = (long)grid.x * grid.y;
   const int nk = (K + BK - 1) / BK;
   int splits = 1;
-  if (ctas < 148 && nk >= 8) {
-    splits = (int)std::min<long>((148 + ctas - 1) / ctas, nk / 4);  // >= 4 k-tiles (64 columns) per slice
+  const long sms = std::max(1, current_device_sms());
+  if (ctas < sms && nk >= 8) {
+    splits = (int)std::min<long>((sms + ctas - 1) / ctas, nk / 4);  // >= 4 k-tiles (64 columns) per slice
     if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
   }
   float* ws = nullptr;
@@ -407,7 +408,7 @@ void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaSt
   const bool conv = !(a.ksize == 1 && a.stride == 1 && a.pad_left == 0 && a.chunk == 0 && a.lengths == nullptr &&
                       a.L_in == a.L_rows && a.t_offset == 0 && a.x_row0 == 0 && a.x_rows == 0);
   auto ctas = [&](int bm, int bn) { return (long)((M + bm - 1) / bm) * ((N + bn - 1) / bn); };
-  const long target = 148;  // one wave of SMs
+  const long target = std::max(1, current_device_sms());  // one wave of SMs
   if (N <= 16 && !ep.glu) {
     if (ctas(128, 16) >= target) launch<128, 16>(a, W, M, N, K, ep, conv, st);
     else launch<32, 16>(a, W, M, N, K, ep, conv, st);
@@ -419,7 +420,7 @@ void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaSt
     return;
   }
   // Prefer the largest tile that still fills the GPU once split-K (slices of >= 8 k-tiles, at most 8 slices) is counted:
-  // a long K walked by few small CTAs is latency-bound (r1_launches_v0: 42 us per 32x32-tile launch).
+  // a long K walked by few small CTAs is latency-bound.
   const int nk = (K + BK - 1) / BK;
   const long max_splits = std::max(1, std::min(8, nk / 8));
   if (ctas(128, 64) >= 2 * target) launch<128, 64>(a, W, M, N, K, ep, conv, st);

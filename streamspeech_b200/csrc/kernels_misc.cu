@@ -9,7 +9,7 @@
 namespace ss {
 unsigned long long g_launches = 0;
 thread_local int g_pdl_off = 0;
-int g_prefer_shared = 0;  // measured on B200: no effect on the three-stream vocoder (profiles/r1_stage_ab_v7.md)
+int g_prefer_shared = 0;  // option prefer_shared (see common.cuh)
 namespace {
 
 // one warp per row; two-pass (mean, then centred sum of squares) like ATen's RowwiseMoments result

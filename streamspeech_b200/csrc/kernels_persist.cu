@@ -1,7 +1,7 @@
 // Persistent cooperative kernel for one streaming step of the chunk-Conformer encoder stack.
 //
 // At batch 1 a 320 ms step touches <= 16 active rows and ~11 MB of fp32 weights per layer; run as separate kernels it is
-// bounded by kernel boundaries (137 dependent launches x ~8 us, profiles/r1_*), not by HBM or FLOPs.  This kernel keeps
+// bounded by kernel boundaries (137 dependent launches), not by HBM or FLOPs.  This kernel keeps
 // one CTA per SM resident for ALL layers and replaces the kernel boundaries by grid-wide barriers, 9 per layer:
 //   [LN + W1 + SiLU] | [W2 + 0.5 res] | [LN + QKV -> q, K-cache, V-cache] | [rel-pos attention] | [out + res] |
 //   [LN + PW1 + GLU -> conv cache, depthwise k31 + BN + SiLU] | [PW2 + res] | [LN + W1 + SiLU] | [W2 + 0.5 res]
@@ -406,7 +406,7 @@ __device__ void phase_gemm(Smem& sm, const float* A, const float* __restrict__ p
 }
 
 // ---- fused FFN (x += alpha * W2 act(W1 LN(x))) in TWO light phases instead of a W1 phase and a W2 phase that makes every CTA
-// read the whole 16 x 2048 hidden from L2 (16 MB per phase, measured 8 us):
+// read the whole 16 x 2048 hidden from L2 (16 MB per phase):
 //   phase A : CTA j < FFN/16 owns hidden units [16j, 16j+16): hid = SiLU(LN(x) W1[16 rows]^T + b1) stays in shared memory, then the
 //             rank-16 update  P[j][m][n] = sum_u hid[m][u] * W2T[16j+u][n]  (W2T = W2 transposed, one coalesced 1 KB row per unit)
 //             goes to a global scratch (16 KB per CTA);

@@ -1,7 +1,7 @@
 // Cluster version of the streaming encoder step (option persistent_encoder_cluster): the <= 16 active rows are split over 4
 // thread-block clusters of 16 CTAs (4 rows per cluster), and inside a cluster the activations NEVER leave the chip: every CTA keeps
 // the cluster's residual rows in shared memory and GEMM outputs are exchanged through distributed shared memory instead of global
-// memory + a 148-CTA grid barrier (~3 us per phase in kernels_persist.cu, profiles/r2_persist_phases_*).  Only two steps per layer
+// memory + a grid barrier over one CTA per SM (every phase of kernels_persist.cu).  Only two steps per layer
 // involve the other clusters -- the K / V rows and the conv-module GLU rows of the step are published to the per-layer caches in
 // global memory -- and keep a (split) grid barrier over the 64 CTAs.
 //
@@ -67,7 +67,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 
 // Exchange channels: a receive buffer in every CTA's shared memory plus an mbarrier that counts the bytes landing in it.  Senders
 // store with st.async (remote write + complete_tx on the receiver's mbarrier); the receiver arms the expected byte count and waits
-// for the phase -- no cluster barrier and no cluster-scope release fence (which is a MEMBAR.ALL.GPU: ~0.5 us each, measured).
+// for the phase -- no cluster barrier and no cluster-scope release fence (which is a MEMBAR.ALL.GPU).
 // A buffer is reused only after an all-to-all exchange on another channel, which a sender cannot pass before every receiver has
 // finished reading (it needs the receiver's own contribution, sent after those reads), so no flow control is needed.
 enum { CH_RED = 0, CH_XS = 1, CH_QS = 2, CH_ATTP = 3, CH_AS = 4, N_CH = 5 };
@@ -184,7 +184,7 @@ __device__ __noinline__ void stage_ln(ClSmem& sm, const float* g, const float* b
 // of each weight row (every lane a distinct 16 B: full-rate 128-bit shared-memory loads, each weight byte read once); the 16 (weight
 // row j = warp + 8 s, activation row r) partial sums of a warp are reduced over the 32 lanes with a halving tree (16 shuffles);
 // even lane 2 v ends with the sum v = s * 4 + r.  (A (k group, row) lane mapping needs 4 shuffles but 4 x the shared-memory
-// wavefronts -- lanes sharing a 16 B address still cost a quarter-warp phase each -- and measured slower.)
+// wavefronts -- lanes sharing a 16 B address still cost a quarter-warp phase each.)
 struct XRegs {
   float4 v[CR][2];
 };
@@ -620,7 +620,7 @@ __global__ void __launch_bounds__(CT_ALL, 1) encoder_layers_cluster_kernel(ClPar
       csync();
       {
         // scores: half a warp per key (lane l16 holds dims [4 l16, 4 l16 + 4) of q + u, q + v of the 4 rows and loads 16 B of the key row
-        // and of the 4 relative-position rows), 2 keys per half-warp in flight (4 measured slower); first the keys of earlier steps, then -- after the
+        // and of the 4 relative-position rows), 2 keys per half-warp in flight; first the keys of earlier steps, then -- after the
         // grid barrier -- the keys of this step
         const float* kb = kc + h * CHD;
         const float* pb = pos_proj + h * CHD;

@@ -1,8 +1,8 @@
 // Persistent cooperative kernel for the single-token steps of the MT decoder's greedy search (beam 1).
 //
 // One decode step is a chain of ~37 dependent M = 1 operations (4 pre-LN layers of self-attention, cross-attention and
-// FFN, the tied output projection over 6000 entries and the arg-max); as separate kernels it costs ~175 us per token,
-// nearly all of it kernel boundaries (profiles/r1_stage_*).  This kernel keeps one CTA per SM resident for a whole burst
+// FFN, the tied output projection over 6000 entries and the arg-max); as separate kernels its time per token is
+// nearly all kernel boundaries.  This kernel keeps one CTA per SM resident for a whole burst
 // of steps and separates the phases with the counter barrier of kernels_persist.cu (33 barriers per token):
 //   per layer: [LN + QKV -> q, K/V cache row] | [self-attention, CTA per head] | [out + res] | [LN + Q] |
 //              [cross-attention over the encoder states, CTA per head] | [out + res] | [LN + FC1 + ReLU] | [FC2 + res]
@@ -230,7 +230,7 @@ __device__ void attend_head(MtSmem& sm, const float* q, const float* kbase, cons
   }
   sum = block_reduce_sum(sm, sum);
   // thread (part, q): keys j = part (mod 16), dims [4q, 4q + 4); 8 keys (8 independent 16-byte loads) in flight per thread.
-  // (4 key phases x 1 float used to mean 40 dependent L2 round trips for 160 encoder rows: ~5 us per cross-attention phase)
+  // (4 key phases x 1 float used to mean 40 dependent L2 round trips for 160 encoder rows)
   const int q4 = (tid & 15) * 4, part = tid >> 4;
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 1

@@ -2,7 +2,7 @@
 // [eos, t1 .. t_{M-1}] of one generate_decoder call (agent/sequence_generator.py:165-582 re-runs the decoder on the whole prefix
 // at every policy() call, agent:179) in ONE launch.  It fills the self-attention K / V cache rows 0 .. M-1 and the final-LN
 // feature rows; the single-token kernel (kernels_persist_mt.cu) then continues at position M.  As separate kernels the pass was
-// 38 dependent launches (250-550 us, profiles/r1_mt_profile_v7.json); here it is 33 grid-barrier phases:
+// 38 dependent launches; here it is 33 grid-barrier phases:
 //   per layer: [LN + QKV -> q, K/V cache] | [causal self-attention] | [out + res] | [LN + Q] | [cross-attention] | [out + res] |
 //              [LN + FC1 + ReLU] | [FC2 + res]       then: final LN -> feature rows
 // GEMM phases are the M <= 16 scheme of kernels_persist.cu extended to row blocks of 16 with the weights of a task held in
@@ -58,7 +58,7 @@ __device__ __forceinline__ void stage_ln512(float* As, const float* x, int M, in
                                             float emb_scale, float* xg) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // the LayerNorm parameters of this lane's 16 columns and the rows of 2 row slots are all in flight before the first reduction
-  // (one row at a time meant two dependent L2 round trips per row: ~6 us per phase at 30 rows)
+  // (one row at a time meant two dependent L2 round trips per row)
   float gv[16], bv[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
@@ -272,7 +272,7 @@ __device__ __forceinline__ void attend_rows(QSmem& sm, float* S, const float* q,
   __syncwarp();
   float a0 = 0.f, a1 = 0.f;  // dims lane, lane + 32
   // 32 keys per round: 64 independent coalesced loads in flight per lane (the loop used to be 4 keys per L2 round trip:
-  // 40 dependent round trips for 160 cross-attention keys, measured ~8 us per prefix row and layer)
+  // 40 dependent round trips for 160 cross-attention keys per prefix row and layer)
 #pragma unroll 1
   for (int j0 = 0; j0 < nk; j0 += 32) {
     float v0[32], v1[32];

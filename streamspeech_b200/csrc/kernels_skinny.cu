@@ -209,7 +209,8 @@ void launch_skinny(const float* A, int lda, const float* W, int M, int N, int K,
   const int per_cta = SK_WARPS / KS;
   int grid = (ntasks + per_cta - 1) / per_cta;
   // with a fused LayerNorm every CTA recomputes the row statistics: keep the grid at two CTAs per SM and loop over tasks
-  const int cap = ep.ln_gamma ? 148 * 2 : 148 * 8;
+  const int sms = std::max(1, current_device_sms());
+  const int cap = ep.ln_gamma ? sms * 2 : sms * 8;
   if (grid > cap) grid = cap;
   launch_pdl_always(skinny_gemm_kernel<MR, KS, CPT, GLU>, dim3(grid), dim3(SK_WARPS * 32), 0, st, A, lda, W, M, N, K, ep);
 }

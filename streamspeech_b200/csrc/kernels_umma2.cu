@@ -1,10 +1,10 @@
-// tcgen05 implicit-GEMM convolution / linear kernel (warp-specialised, weights pre-packed).
+// wgmma implicit-GEMM convolution / linear kernel (warp-specialised, weights pre-packed).
 //
 //   out[t][n] = epilogue( sum_{tap j, channel ci}  pre(x[t + j*dil - pad_left][ci]) * W[n][j*C_in + ci] )
 //
 // for stride-1 convolutions over one channels-last sequence (B = 1; a plain linear layer is ksize = 1).  fp32 operands are
-// split into NP bf16 pieces (x = x0 + x1 [+ x2]) and the product is accumulated in TMEM as 3 (NP = 2, ~2^-16 relative) or
-// 6 (NP = 3, ~fp32) bf16 tcgen05 MMAs.  Structure:
+// split into NP bf16 pieces (x = x0 + x1 [+ x2]) and the product is accumulated in fp32 registers as 3 (NP = 2, ~2^-16
+// relative) or 6 (NP = 3, ~fp32) bf16 wgmma products.  Structure:
 //
 //   * weights are split and laid out ONCE (umma2_pack_kernel, cached per weight matrix) as ready-made shared-memory tiles
 //     [n-tile][channel chunk][tap][piece][BN x CK bf16, canonical no-swizzle K-major core matrices]; a producer thread
@@ -13,9 +13,11 @@
 //     [m0 - pad_left, m0 + 128 + (k-1)*dil - pad_left) x CK channels.  In the no-swizzle layout a plane of 8 channels is a
 //     linear array of rows at a 16-byte pitch, so tap j is the same staged data with the descriptor's start address moved
 //     by j*dil rows: a k-tap convolution costs k MMAs per staged chunk instead of k im2col conversions;
-//   * roles: warps 0-7 convert (global fp32 -> registers, one chunk ahead -> bf16 pieces in smem), warp 8 issues the MMAs,
-//     warp 9 runs the weight ring; all hand-offs are mbarriers, so conversion of chunk c+1, the weight copies and the MMAs
-//     of chunk c overlap.  Warps 0-7 read the accumulator back with tcgen05.ld and run the fused epilogue.
+//   * roles: warps 0-7 are two warpgroups that convert (global fp32 -> registers, one chunk ahead -> bf16 pieces in smem)
+//     and issue the wgmma of their 64 rows of the 128-row tile; warp 8 runs the weight ring.  The MMAs of a (chunk, tap)
+//     unit run asynchronously while the next unit is issued and the next chunk is converted; a unit's weight stage (and,
+//     after its last tap, the activation stage) is released once the following unit has been issued and it has completed.
+//     The accumulators go through a padded shared-memory tile so the fused epilogue writes whole rows.
 //   * split over (chunk, tap) units on gridDim.z when the tile grid alone cannot fill the GPU; partial sums are reduced
 //     in a fixed order by splitk_epilogue_kernel (kernels_gemm.cu).
 #include <cuda_bf16.h>
@@ -38,8 +40,8 @@ struct Umma2Cache {
 namespace {
 
 constexpr int U2_BM = 128;
-constexpr int U2_CONVERTERS = 256;  // warps 0-7
-constexpr int U2_THREADS = 320;     // + MMA warp + weight-ring warp
+constexpr int U2_CONVERTERS = 256;  // warps 0-7 (two warpgroups of 64 output rows each)
+constexpr int U2_THREADS = 288;     // + weight-ring warp
 constexpr int U2_MAX_UNITS = 6;     // float4 units per converter thread and chunk: rows * CK/4 <= 6 * 256
 constexpr int U2_MAX_SB = 4;
 constexpr int U2_MAX_HALO = 64;
@@ -55,37 +57,56 @@ __device__ __forceinline__ float u2_act(float x, int act) {
   }
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, version 1)
+// K-major, no-swizzle wgmma shared-memory matrix descriptor
 __device__ __forceinline__ uint64_t u2_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;  // next 8-column plane along K
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;  // next 8-row group along M / N
-  d |= (uint64_t)1 << 46;
   return d;
 }
 
-// kind::f16 instruction descriptor: D = F32, A = B = BF16, K-major, M = 128, N = n
-__device__ __forceinline__ uint32_t u2_idesc(int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= 1u << 7;
-  d |= 1u << 10;
-  d |= (uint32_t)(n >> 3) << 17;
-  d |= (uint32_t)(U2_BM >> 4) << 24;
-  return d;
-}
-
-__device__ __forceinline__ void u2_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x BN] += A[64 x 16] * B[BN x 16]^T, bf16 operands in shared memory, fp32 accumulators in registers.  Register 4 i + r of
+// thread t of the warpgroup holds row 16 (t / 32) + (t % 32) / 4 + 8 (r / 2), column 8 i + 2 (t % 4) + r % 2.
+template <int BN>
+__device__ __forceinline__ void u2_wgmma(float (&d)[BN / 2], uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void u2_wgmma<16>(float (&d)[8], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void u2_wgmma<32>(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void u2_wgmma<64>(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void u2_wgmma<128>(float (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
 }
 
-__device__ __forceinline__ void u2_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <int NACC>
+__device__ __forceinline__ void u2_fence_acc(float (&d)[NACC]) {
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 __device__ __forceinline__ void u2_wait(uint32_t bar, uint32_t parity) {
@@ -117,7 +138,7 @@ struct U2Params {
   int SB;                   // weight ring stages
   float* ws;                // split partial sums [gridDim.z][M][N] or null
   unsigned* tile_ctr;       // ticket per output tile: the last split CTA of a tile reduces and runs the epilogue (null: separate kernel)
-  unsigned long long* dbg;  // optional: %globaltimer stamps of CTA (0,0,0) at the hand-off points (tools/umma2_check.py)
+  unsigned long long* dbg;  // optional: %globaltimer stamps of CTA (0,0,0) at the hand-off points (option umma2_debug)
 };
 
 __device__ __forceinline__ void u2_stamp(const U2Params& p, int slot) {
@@ -191,11 +212,11 @@ __device__ __forceinline__ void u2_reduce_tile(const U2Params& p, int m0, int n0
 }
 
 template <int BN, int NP, int UPT, int SETS>
-__global__ void __launch_bounds__(U2_THREADS) umma2_kernel(const __grid_constant__ U2Params p) {
-  constexpr int TM_COLS = BN < 32 ? 32 : BN;
+__global__ void __launch_bounds__(U2_THREADS, 1) umma2_kernel(const __grid_constant__ U2Params p) {
+  constexpr int NACC = BN / 2;
+  constexpr int TP = BN + 8;  // pitch (floats) of the output tile: conflict-free 8-byte fragment stores
   extern __shared__ __align__(128) unsigned char smem[];
-  __shared__ __align__(8) uint64_t bars[5 + 2 * U2_MAX_SB];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bars[4 + 2 * U2_MAX_SB];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.y * U2_BM, nt = blockIdx.x, n0 = nt * BN;
   const int CK = p.CK, k = p.ksize, SB = p.SB;
@@ -207,7 +228,7 @@ __global__ void __launch_bounds__(U2_THREADS) umma2_kernel(const __grid_constant
   unsigned char* a_smem = smem + ((128u - (smem_u32(smem) & 127u)) & 127u);  // 128-byte aligned whatever the static layout is
   unsigned char* b_smem = a_smem + ((2 * a_stage + 127u) & ~127u);
   const uint32_t a_full = smem_u32(&bars[0]), a_empty = smem_u32(&bars[2]), b_full = smem_u32(&bars[4]);
-  const uint32_t b_empty = smem_u32(&bars[4 + U2_MAX_SB]), acc_full = smem_u32(&bars[4 + 2 * U2_MAX_SB]);
+  const uint32_t b_empty = smem_u32(&bars[4 + U2_MAX_SB]);
 
   const int u0 = blockIdx.z * p.units_per_split;
   const int u1 = min(p.units_total, u0 + p.units_per_split);
@@ -241,36 +262,35 @@ __global__ void __launch_bounds__(U2_THREADS) umma2_kernel(const __grid_constant
     for (int i = 0; i < UPT; ++i)
       dst[i] = goff[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(xc + goff[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
   };
-  if (warp < 8) {  // the first chunk loads do not depend on the barriers: they fly while TMEM / mbarriers are set up
+  if (warp < 8) {  // the first chunk loads do not depend on the barriers: they fly while the mbarriers are set up
 #pragma unroll
     for (int d = 0; d < SETS - 1; ++d)
       if (d < n_local) issue(c_first + d, pf[d]);
   }
 
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(TM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a_full + 8 * i), "r"(U2_CONVERTERS / 32) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a_empty + 8 * i), "r"(1) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a_empty + 8 * i), "r"(2) : "memory");  // one per warpgroup
     }
     for (int i = 0; i < U2_MAX_SB; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(b_full + 8 * i), "r"(1) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(b_empty + 8 * i), "r"(1) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(b_empty + 8 * i), "r"(2) : "memory");
     }
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(acc_full), "r"(1) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_s;
   if (tid == 0) u2_stamp(p, 1);
 
   if (warp < 8) {
-    // ---------------- converters: activation rows -> bf16 pieces, one channel chunk per stage
+    // ---------------- converters + MMA issue: activation rows -> bf16 pieces, one channel chunk per stage
+    const int wg = warp >> 2;  // warpgroup: output rows [64 wg, 64 wg + 64) of the tile
+    const bool wg_leader = (tid & 127) == 0;
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    uint32_t uc = 0;
+    int prev_sb = -1, prev_sa = -1;  // stages of the unit still in flight (prev_sa >= 0: it was the last tap of its chunk)
     for (int clb = 0; clb < n_local; clb += SETS) {
 #pragma unroll
       for (int d = 0; d < SETS; ++d) {
@@ -293,62 +313,119 @@ __global__ void __launch_bounds__(U2_THREADS) umma2_kernel(const __grid_constant
               u2_split_store<NP>(v, stage, a_piece, soff[i]);
             }
           }
-          // every lane publishes its own generic-proxy writes to the async proxy, then one lane per warp arrives (256
-          // arrivals on one mbarrier serialise; 8 do not)
+          // every lane publishes its own generic-proxy writes to the async proxy, then one lane per warp arrives
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
           __syncwarp();
           if (lane == 0) u2_arrive(a_full + 8 * sa);
-          if (tid == 0) u2_stamp(p, cl == 0 ? 2 : 6);
+          if (tid == 0 && cl == 0) u2_stamp(p, 2);
+          u2_wait(a_full + 8 * sa, (uint32_t)(ua & 1));  // both warpgroups' rows are staged
+          if (tid == 0 && cl == 0) u2_stamp(p, 3);
+          const int c = c_first + cl;
+          const int j_lo = (cl == 0) ? u0 - c * k : 0;
+          const int j_hi = (cl == n_local - 1) ? (u1 - 1) - c * k : k - 1;
+          const uint32_t a_base = smem_u32(a_smem + (size_t)sa * a_stage) + (uint32_t)wg * 64u * 16u;
+          const uint32_t b_plane = (uint32_t)BN * 16u;
+          for (int j = j_lo; j <= j_hi; ++j, ++uc) {
+            const uint32_t sb = uc % (uint32_t)SB, ub = uc / (uint32_t)SB;
+            u2_wait(b_full + 8 * sb, ub & 1u);
+            if (tid == 0 && uc == 0) u2_stamp(p, 4);
+            const uint32_t a_tap = a_base + (uint32_t)(j * p.dil) * 16u;
+            const uint32_t b_base = smem_u32(b_smem + (size_t)sb * b_unit);
+            u2_fence_acc<NACC>(acc);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+            for (int ks = 0; ks < (CK >> 4); ++ks) {
+              uint64_t ad[NP], bd[NP];
+#pragma unroll
+              for (int q = 0; q < NP; ++q) {
+                ad[q] = u2_desc(a_tap + q * a_piece + ks * 2 * a_plane, a_plane, 128);
+                bd[q] = u2_desc(b_base + q * b_piece + ks * 2 * b_plane, b_plane, 128);
+              }
+              u2_wgmma<BN>(acc, ad[0], bd[0]);
+              u2_wgmma<BN>(acc, ad[0], bd[1]);
+              u2_wgmma<BN>(acc, ad[1], bd[0]);
+              if (NP == 3) {
+                u2_wgmma<BN>(acc, ad[1], bd[1]);
+                u2_wgmma<BN>(acc, ad[0], bd[NP - 1]);
+                u2_wgmma<BN>(acc, ad[NP - 1], bd[0]);
+              }
+            }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");  // the previous unit has completed
+            u2_fence_acc<NACC>(acc);
+            if (wg_leader && prev_sb >= 0) {
+              u2_arrive(b_empty + 8 * prev_sb);
+              if (prev_sa >= 0) u2_arrive(a_empty + 8 * prev_sa);
+            }
+            prev_sb = (int)sb;
+            prev_sa = (j == j_hi) ? sa : -1;
+          }
+        }
+      }
+    }
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    u2_fence_acc<NACC>(acc);
+    if (tid == 0) u2_stamp(p, 5);
+
+    // ---------------- epilogue: accumulators -> padded shared-memory tile (the operand stages are free once both warpgroups'
+    // MMAs have completed) -> rows written with lanes on consecutive columns: full 128-byte segments, bias / residual reads
+    // coalesced too.  The mode (split partial sums / GLU / plain) is decided outside the loops.
+    asm volatile("bar.sync 1, %0;" ::"n"(U2_CONVERTERS) : "memory");
+    float* tile = reinterpret_cast<float*>(a_smem);
+    {
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        *reinterpret_cast<float2*>(tile + r0 * TP + 8 * i + c0) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(tile + (r0 + 8) * TP + 8 * i + c0) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(U2_CONVERTERS) : "memory");
+    if (tid == 0) u2_stamp(p, 7);
+    const Epilogue& ep = p.ep;
+    const int M = p.M, N = p.N;
+    const int rows = min(U2_BM, M - m0);
+    const int cols = min(BN, N - n0);
+    if (p.ws != nullptr) {  // split: raw partial sums
+      for (int idx = tid; idx < rows * BN; idx += U2_CONVERTERS) {
+        const int r = idx / BN, c = idx - r * BN;
+        if (c < cols) p.ws[((int64_t)blockIdx.z * M + m0 + r) * N + n0 + c] = tile[r * TP + c];
+      }
+    } else if (ep.glu) {  // columns are interleaved (a, gate) pairs
+      constexpr int HB = BN / 2;
+      for (int idx = tid; idx < rows * HB; idx += U2_CONVERTERS) {
+        const int r = idx / HB, c = idx - r * HB;
+        const int n = n0 + 2 * c;
+        if (2 * c < cols) {
+          const int m = m0 + r;
+          const int64_t o = (ep.out_L > 0 ? (int64_t)m * ep.out_row_stride + ep.out_row_offset : (int64_t)m) * ep.ldo + (n >> 1);  // B == 1
+          float v = tile[r * TP + 2 * c], gate = tile[r * TP + 2 * c + 1];
+          if (ep.bias != nullptr) {
+            v += ep.bias[n];
+            gate += ep.bias[n + 1];
+          }
+          float res = 0.f;
+          if (ep.residual) res = ep.res_scale * ep.residual[o];
+          if (ep.accumulate) res += ep.out[o];
+          ep.out[o] = ep.alpha * (v * (1.0f / (1.0f + expf(-gate)))) + res;
+        }
+      }
+    } else {
+      const int act = ep.act;
+      for (int idx = tid; idx < rows * BN; idx += U2_CONVERTERS) {
+        const int r = idx / BN, c = idx - r * BN;
+        if (c < cols) {
+          const int m = m0 + r, n = n0 + c;
+          const int64_t o = (ep.out_L > 0 ? (int64_t)m * ep.out_row_stride + ep.out_row_offset : (int64_t)m) * ep.ldo + n;  // B == 1
+          const float v = tile[r * TP + c] + (ep.bias != nullptr ? ep.bias[n] : 0.f);
+          float res = 0.f;
+          if (ep.residual) res = ep.res_scale * ep.residual[o];
+          if (ep.accumulate) res += ep.out[o];
+          ep.out[o] = ep.alpha * u2_act(v, act) + res;
         }
       }
     }
   } else if (warp == 8) {
-    // ---------------- MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = u2_idesc(BN);
-      const uint32_t b_plane = (uint32_t)BN * 16u;
-      uint32_t uc = 0, accumulate = 0;
-      for (int cl = 0; cl < n_local; ++cl) {
-        const int sa = cl & 1, ua = cl >> 1;
-        u2_wait(a_full + 8 * sa, (uint32_t)(ua & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (cl == 0) u2_stamp(p, 3);
-        const int c = c_first + cl;
-        const int j_lo = (cl == 0) ? u0 - c * k : 0;
-        const int j_hi = (cl == n_local - 1) ? (u1 - 1) - c * k : k - 1;
-        const uint32_t a_base = smem_u32(a_smem + (size_t)sa * a_stage);
-        for (int j = j_lo; j <= j_hi; ++j, ++uc) {
-          const uint32_t sb = uc % (uint32_t)SB, ub = uc / (uint32_t)SB;
-          u2_wait(b_full + 8 * sb, ub & 1u);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          if (uc == 0) u2_stamp(p, 4);
-          const uint32_t a_tap = a_base + (uint32_t)(j * p.dil) * 16u;
-          const uint32_t b_base = smem_u32(b_smem + (size_t)sb * b_unit);
-          for (int ks = 0; ks < (CK >> 4); ++ks) {
-            uint64_t ad[NP], bd[NP];
-#pragma unroll
-            for (int q = 0; q < NP; ++q) {
-              ad[q] = u2_desc(a_tap + q * a_piece + ks * 2 * a_plane, a_plane, 128);
-              bd[q] = u2_desc(b_base + q * b_piece + ks * 2 * b_plane, b_plane, 128);
-            }
-            u2_mma(tmem_d, ad[0], bd[0], idesc, accumulate);
-            accumulate = 1;
-            u2_mma(tmem_d, ad[0], bd[1], idesc, 1u);
-            u2_mma(tmem_d, ad[1], bd[0], idesc, 1u);
-            if (NP == 3) {
-              u2_mma(tmem_d, ad[1], bd[1], idesc, 1u);
-              u2_mma(tmem_d, ad[0], bd[NP - 1], idesc, 1u);
-              u2_mma(tmem_d, ad[NP - 1], bd[0], idesc, 1u);
-            }
-          }
-          u2_commit(b_empty + 8 * sb);  // weight stage free once these MMAs have read it
-        }
-        u2_commit(a_empty + 8 * sa);
-      }
-      u2_commit(acc_full);
-      u2_stamp(p, 5);
-    }
-  } else {
     // ---------------- weight ring: one bulk copy per (chunk, tap) unit, all pieces
     if (lane == 0) {
       const unsigned char* src = p.wp + ((size_t)nt * p.units_total + u0) * b_unit;
@@ -362,136 +439,12 @@ __global__ void __launch_bounds__(U2_THREADS) umma2_kernel(const __grid_constant
       }
     }
   }
-
-  // ---------------- epilogue (warps 0-7): warp w owns TMEM lanes 32*(w&3).. (= 32 output rows); with BN >= 64 the two
-  // warpgroups split the columns.  tcgen05.ld hands every lane ONE row (registers = columns); written out like that, each
-  // store instruction would touch 32 rows x 4 bytes = 32 sectors (measured: 10.7 us of a 15 us CTA).  So each 32 x CW
-  // block goes through a padded shared-memory tile (the operand stages are free once acc_full has completed) and is
-  // written row by row with lanes = consecutive columns: full 128-byte segments, bias / residual reads coalesced too.
-  if (warp < 8) {
-    u2_wait(acc_full, 0u);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (tid == 0) u2_stamp(p, 7);
-    const Epilogue& ep = p.ep;
-    const int M = p.M, N = p.N;
-    const int quad = warp & 3;
-    constexpr int GROUPS = BN >= 64 ? 2 : 1;
-    constexpr int COLS_PER_GROUP = BN / GROUPS;
-    constexpr int CW = COLS_PER_GROUP >= 32 ? 32 : 16;  // columns per tcgen05.ld
-    constexpr int RPI = 32 / CW;                         // rows written per store instruction
-    const int c_begin = (warp >> 2) * COLS_PER_GROUP;
-    const bool epi_active = warp < 4 * GROUPS;
-    float* tbuf = reinterpret_cast<float*>(a_smem) + warp * (32 * 33);
-    const int cc = lane % CW, rsub = lane / CW;
-#pragma unroll 1
-    for (int c0 = c_begin; epi_active && c0 < c_begin + COLS_PER_GROUP; c0 += CW) {
-      uint32_t r[CW];
-      const uint32_t taddr = tmem_d + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0;
-      if (CW == 32) {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-              "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16 % CW]), "=r"(r[17 % CW]),
-              "=r"(r[18 % CW]), "=r"(r[19 % CW]), "=r"(r[20 % CW]), "=r"(r[21 % CW]), "=r"(r[22 % CW]), "=r"(r[23 % CW]), "=r"(r[24 % CW]),
-              "=r"(r[25 % CW]), "=r"(r[26 % CW]), "=r"(r[27 % CW]), "=r"(r[28 % CW]), "=r"(r[29 % CW]), "=r"(r[30 % CW]), "=r"(r[31 % CW])
-            : "r"(taddr)
-            : "memory");
-      } else {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-              "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(taddr)
-            : "memory");
-      }
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (tid == 0 && c0 == c_begin) u2_stamp(p, 9);
-#pragma unroll
-      for (int j = 0; j < CW; ++j) tbuf[lane * 33 + j] = __uint_as_float(r[j]);
-      __syncwarp();
-      if (tid == 0 && c0 == c_begin) u2_stamp(p, 10);
-      const int n = n0 + c0 + cc;
-      const bool n_ok = n < N;
-      const int m_first = m0 + quad * 32 + rsub;  // row of iteration 0; iteration `it` handles row m_first + it * RPI
-      // The rows are independent: 8 shared-memory reads are issued back to back, then their 8 stores (one row per
-      // iteration was a ~160-cycle dependent chain with two warps per scheduler: 2.7 us per 32 x 32 block).  The mode
-      // (split partial sums / GLU / plain) is decided outside the loops.
-      if (p.ws != nullptr) {  // split: raw partial sums
-        float* wp = p.ws + ((int64_t)blockIdx.z * M + m_first) * N + n;
-#pragma unroll 1
-        for (int it0 = 0; it0 < CW; it0 += 8) {
-          float v[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) v[u] = tbuf[((it0 + u) * RPI + rsub) * 33 + cc];
-#pragma unroll
-          for (int u = 0; u < 8; ++u)
-            if (n_ok && m_first + (it0 + u) * RPI < M) wp[(int64_t)(it0 + u) * RPI * N] = v[u];
-        }
-      } else {
-        const float bias_n = (ep.bias != nullptr && n_ok) ? ep.bias[n] : 0.f;
-        const int64_t row_step = (ep.out_L > 0 ? (int64_t)ep.out_row_stride : (int64_t)1) * RPI * ep.ldo;  // B == 1
-        const int64_t o_first = (ep.out_L > 0 ? (int64_t)m_first * ep.out_row_stride + ep.out_row_offset : (int64_t)m_first) * ep.ldo;
-        if (ep.glu) {  // columns are interleaved (a, gate) pairs: the gate sits in the next lane
-#pragma unroll 1
-          for (int it0 = 0; it0 < CW; it0 += 8) {
-            float v[8], res[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) v[u] = tbuf[((it0 + u) * RPI + rsub) * 33 + cc] + bias_n;
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const float gate = __shfl_down_sync(0xffffffffu, v[u], 1);
-              const bool ok = n_ok && (n & 1) == 0 && m_first + (it0 + u) * RPI < M;
-              const int64_t o = o_first + (int64_t)(it0 + u) * row_step + (n >> 1);
-              res[u] = 0.f;
-              if (ok && ep.residual) res[u] = ep.res_scale * ep.residual[o];
-              if (ok && ep.accumulate) res[u] += ep.out[o];
-              v[u] = ep.alpha * (v[u] * (1.0f / (1.0f + expf(-gate))));
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const bool ok = n_ok && (n & 1) == 0 && m_first + (it0 + u) * RPI < M;
-              if (ok) ep.out[o_first + (int64_t)(it0 + u) * row_step + (n >> 1)] = v[u] + res[u];
-            }
-          }
-        } else {
-          const int act = ep.act;
-#pragma unroll 1
-          for (int it0 = 0; it0 < CW; it0 += 8) {
-            float v[8], res[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) v[u] = tbuf[((it0 + u) * RPI + rsub) * 33 + cc] + bias_n;
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const bool ok = n_ok && m_first + (it0 + u) * RPI < M;
-              const int64_t o = o_first + (int64_t)(it0 + u) * row_step + n;
-              res[u] = 0.f;
-              if (ok && ep.residual) res[u] = ep.res_scale * ep.residual[o];
-              if (ok && ep.accumulate) res[u] += ep.out[o];
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const bool ok = n_ok && m_first + (it0 + u) * RPI < M;
-              if (ok) ep.out[o_first + (int64_t)(it0 + u) * row_step + n] = ep.alpha * u2_act(v[u], act) + res[u];
-            }
-          }
-        }
-      }
-      if (tid == 0 && c0 == c_begin) u2_stamp(p, 11);
-      __syncwarp();  // the tile is rewritten by the next column block
-    }
-  }
   if (tid == 0) u2_stamp(p, 8);
-  if (p.tile_ctr != nullptr) __threadfence();  // this CTA's partial sums are visible device-wide before its ticket
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 8) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(TM_COLS) : "memory");
-  }
   if (p.tile_ctr != nullptr) {
+    __threadfence();  // this CTA's partial sums are visible device-wide before its ticket
     __shared__ unsigned s_last;
     unsigned* ctr = p.tile_ctr + (blockIdx.y * gridDim.x + blockIdx.x);
+    __syncthreads();
     if (tid == 0) s_last = (atomicAdd(ctr, 1u) == gridDim.z - 1) ? 1u : 0u;
     __syncthreads();
     if (s_last) {
@@ -538,13 +491,13 @@ __global__ void umma2_pack_kernel(const float* __restrict__ W, int N, int C_in, 
 }
 
 }  // namespace
-int g_umma2_split_below = 60;   // tile grids smaller than this are split over (chunk, tap) units (ss_set_option umma2_split_below;
-                                // measured: 60 beats 148 by 0.9 ms per utterance, the reduce launch costs more than the idle SMs)
+int g_umma2_split_below = 60;   // tile grids smaller than this are split over (chunk, tap) units (ss_set_option umma2_split_below:
+                                // below one wave, the extra reduce launch can cost more than the idle SMs)
 int g_umma2_min_units = 4;      // ... into slices of at least this many units
-int g_umma2_fused_reduce = 0;   // 1: the last-ticket CTA of a tile reduces the split partial sums inside the kernel.  Measured on B200
-                                // (round 2, run 5): bit-identical but SLOWER -- one CTA reads splits x tile bytes alone (up to 22 x 64 KB) where
-                                // the separate splitk_epilogue_kernel spreads the same reads over the whole GPU: vocoder 10.6 -> 31 ms per
-                                // utterance.  Kept as an option (a reduction distributed over the split CTAs needs them co-resident).
+int g_umma2_fused_reduce = 0;   // 1: the last-ticket CTA of a tile reduces the split partial sums inside the kernel.  Off by default:
+                                // bit-identical, but one CTA reads splits x tile bytes alone where the separate splitk_epilogue_kernel
+                                // spreads the same reads over the whole GPU.  Kept as an option (a reduction distributed over the
+                                // split CTAs needs them co-resident).
 unsigned long long* g_umma2_dbg = nullptr;  // device buffer of 16 stamps when the debug option is on
 namespace {
 
@@ -646,7 +599,8 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   const int min_units = std::max(1, g_umma2_min_units);
   int splits = 1;
   if (base < g_umma2_split_below && p.units_total >= 2 * min_units) {
-    splits = (int)std::min<long>((148 + base - 1) / base, p.units_total / min_units);
+    const long sms = std::max(1, current_device_sms());
+    splits = (int)std::min<long>((sms + base - 1) / base, p.units_total / min_units);
     while (splits > 1 && (size_t)splits * M * N * sizeof(float) > (32u << 20)) --splits;
   }
   int ups = (p.units_total + splits - 1) / splits;
@@ -666,7 +620,7 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   const size_t a_bytes = (size_t)2 * NP * (CK >> 3) * p.rs_pad * 16;
   const size_t b_unit = (size_t)NP * BN * CK * 2;
   p.SB = (((a_bytes + 127) & ~(size_t)127) + 4 * b_unit <= 110 * 1024) ? 4 : 3;
-  const size_t smem = std::max<size_t>(((a_bytes + 127) & ~(size_t)127) + p.SB * b_unit, 8 * 32 * 33 * sizeof(float)) + 256;  // >= the epilogue's transpose tiles
+  const size_t smem = std::max<size_t>(((a_bytes + 127) & ~(size_t)127) + p.SB * b_unit, (size_t)U2_BM * (BN + 8) * sizeof(float)) + 256;  // >= the epilogue's output tile
   dim3 grid(n_tiles, m_tiles, splits);
   if (NP == 3) {
     switch (BN) {

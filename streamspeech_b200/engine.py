@@ -1,7 +1,7 @@
 """ctypes binding of libstreamspeech_b200.so (include/streamspeech_b200.h): PyTorch tensors in, PyTorch tensors out.
 
 PyTorch is plumbing here (device memory, streams); every FLOP of the path runs in the library's own
-sm_100a kernels.  There is NO CPU fallback: importing this module without the built library, or
+sm_90a kernels.  There is NO CPU fallback: importing this module without the built library, or
 constructing an Engine without a CUDA device, raises.
 """
 from __future__ import annotations
@@ -156,7 +156,7 @@ class Engine:
     def __init__(self, cfg: ModelConfig, model_sd: Dict[str, torch.Tensor], vocoder_sd: Optional[Dict[str, torch.Tensor]] = None,
                  gcmvn: Optional[dict] = None, device: int = 0, max_enc_frames: int = 1024, max_mt_positions: int = 1024):
         if not torch.cuda.is_available():
-            raise EngineError("streamspeech_b200.Engine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise EngineError("streamspeech_b200.Engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = load_library()
         self.cfg = cfg
         self.device = torch.device("cuda", device)
@@ -198,7 +198,7 @@ class Engine:
         self.set_option("umma2_fused_reduce", int(os.environ.get("SS_UMMA2_FUSED_REDUCE", "0")))
         self.set_option("fbank_tma", int(os.environ.get("SS_FBANK_TMA", "1")))
         self.set_option("persistent_ffn_fused", int(os.environ.get("SS_PERSISTENT_FFN_FUSED", "1")))
-        # cluster kernel for encoder steps with <= 16 active rows (larger steps and refused launches take the 148-CTA kernel)
+        # cluster kernel for encoder steps with <= 16 active rows (larger steps and refused launches take the one-CTA-per-SM kernel)
         self.set_option("persistent_encoder_cluster", int(os.environ.get("SS_PERSISTENT_ENCODER_CLUSTER", "1")))
         self.set_option("cluster_cooperative", int(os.environ.get("SS_CLUSTER_COOPERATIVE", "1")))
         self.set_option("persistent_mt_v2", int(os.environ.get("SS_PERSISTENT_MT_V2", "1")))
@@ -467,7 +467,7 @@ class Engine:
 
     def op_conv1d(self, x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], ksize: int, dil: int = 1, pad_left: int = 0,
                   pre_lrelu: float = 1.0, mode: int = 0) -> torch.Tensor:
-        """x [L][C_in] channels-last, w [N][ksize*C_in] tap-major; mode 0 = fp32 CUDA cores, 12/13 = tcgen05 (bf16x3 / bf16x6)"""
+        """x [L][C_in] channels-last, w [N][ksize*C_in] tap-major; mode 0 = fp32 CUDA cores, 12/13 = wgmma (bf16x3 / bf16x6)"""
         L, C = x.shape
         N = w.shape[0]
         out = self._f32(L, N)

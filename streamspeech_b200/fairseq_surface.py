@@ -1,4 +1,4 @@
-"""The fairseq model surface of StreamSpeech on top of the B200 engine (SURVEY.md §8b(ii)).
+"""The fairseq model surface of StreamSpeech on top of the H100 engine (SURVEY.md §8b(ii)).
 
 The reference agents never call kernels directly: they poke attributes of a fairseq model object and call its sub-modules
 (agent/speech_to_speech.streamspeech.agent.py:395-413,433,520-538,638-689).  `StreamSpeechB200Model` offers exactly those

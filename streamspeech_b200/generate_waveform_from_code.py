@@ -1,4 +1,4 @@
-"""`generate_waveform_from_code.py` on the B200 engine (SURVEY.md §8 f4).
+"""`generate_waveform_from_code.py` on the H100 engine (SURVEY.md §8 f4).
 
 Front door of the reference's offline pipeline after `fairseq-generate`
 (fairseq/examples/speech_to_speech/generate_waveform_from_code.py:40-111, used by
@@ -69,7 +69,7 @@ class VocoderOnly:
 
 def main(args):
     if args.cpu:
-        raise SystemExit("--cpu: the B200 engine has no CPU path")
+        raise SystemExit("--cpu: the H100 engine has no CPU path")
     with open(args.vocoder_cfg) as f:
         vocoder_cfg = json.load(f)
     vocoder = VocoderOnly(args.vocoder, vocoder_cfg)

@@ -1,4 +1,4 @@
-"""Offline batched S2ST generation on the B200 engine (SURVEY.md §8 row O1).
+"""Offline batched S2ST generation on the H100 engine (SURVEY.md §8 row O1).
 
 Drop-in for the reference's `CTCMultiDecoderSequenceGenerator` as `fairseq-generate --task speech_to_speech_ctc` uses it
 (researches/ctc_unity/sequence_generator_multi_decoder_ctc.py:163-331, built by tasks/speech_to_speech_ctc.py:21-49) with
@@ -30,7 +30,7 @@ from .engine import Engine, EngineError
 class OfflineS2STGenerator:
     def __init__(self, engine: Engine, beam_size_mt: int = 1, beam_size: int = 1, max_len_a_mt: float = 0.0, max_len_b_mt: int = 200):
         if beam_size_mt != 1 or beam_size != 1:
-            raise NotImplementedError("the B200 offline generator implements beam_size_mt = beam_size = 1 (greedy) only")
+            raise NotImplementedError("the H100 offline generator implements beam_size_mt = beam_size = 1 (greedy) only")
         if max_len_a_mt != 0.0:
             raise NotImplementedError("max_len_a_mt != 0 is not supported (the reference default is 0)")
         self.engine = engine

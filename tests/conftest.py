@@ -11,8 +11,8 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
-    config.addinivalue_line("markers", "gpu_staged: GPU test of a path that has not had its first B200 run yet; skipped without a "
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu_staged: GPU test of a path that has not had its first H100 run yet; skipped without a "
                                        "device and NOT selected by `-m gpu` (run with `-m gpu_staged`, then promote it to `gpu`)")
 
 

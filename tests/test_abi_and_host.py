@@ -22,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(engine.EXPORTED_SYMBOLS), declared ^ set(engine.EXPORTED_SYMBOLS)
     for s in declared:
         assert hasattr(lib, s), s
-    assert b"sm_100a" in lib.ss_version()
+    assert b"sm_90a" in lib.ss_version()
     # pure host helpers need no GPU
     assert lib.ss_fbank_num_frames(160000) == 998 and lib.ss_fbank_num_frames(239) == 0
     assert lib.ss_encoder_out_frames(998) == 250 and lib.ss_encoder_out_frames(1498) == 375 and lib.ss_encoder_out_frames(1) == 1

@@ -313,12 +313,12 @@ def test_vocoder_graph_replay_is_identical(eng3, gold):
     assert replay_launches == eager_launches  # the replay accounts for every kernel node it runs
 
 
-# --------------------------------------------------------------------------------------------- tcgen05 kernels
+# --------------------------------------------------------------------------------------------- tensor-core kernels
 @pytest.mark.parametrize("shape", [(128, 32, 16, 1, 1, 0, 1.0), (100, 64, 128, 3, 1, 1, 0.1), (260, 256, 256, 11, 5, 25, 0.1),
                                    (1040, 128, 128, 7, 3, 9, 0.1), (16640, 16, 16, 7, 5, 15, 0.1), (300, 128, 512, 7, 1, 3, 1.0),
                                    (775, 512, 2048, 1, 1, 0, 1.0), (200, 512, 1005, 1, 1, 0, 1.0), (130, 48, 48, 5, 2, 4, 0.1)])
 def test_tcgen05_conv_vs_fp64_reference(eng3, shape):
-    """kernels_umma2.cu (tap-shift implicit GEMM, bf16x3 / bf16x6 operand splitting) against torch conv1d in fp64 and against
+    """kernels_umma2.cu (wgmma tap-shift implicit GEMM, bf16x3 / bf16x6 operand splitting) against torch conv1d in fp64 and against
     the fp32 CUDA-core kernel: 2 pieces within 2e-3 (vocoder path, waveform bar 1e-3 after 40 layers is checked by the
     vocoder tests), 3 pieces within 2e-4 (same bar as the fp32 kernels)."""
     import torch.nn.functional as F
@@ -340,7 +340,7 @@ def test_tcgen05_conv_vs_fp64_reference(eng3, shape):
     eng3.set_option("umma2_cache_clear", 1)
     d3 = maxdiff(eng3.op_conv1d(xd, wd, bd, k, dil, pad, slope, 13), ref)
     eng3.set_option("umma2_cache_clear", 1)
-    report("tcgen05_conv", shape=list(shape), fp32=d0, bf16x3=d2, bf16x6=d3)
+    report("umma2_conv", shape=list(shape), fp32=d0, bf16x3=d2, bf16x6=d3)
     assert d0 < FP_TOL and d2 < 2e-3 and d3 < FP_TOL, (d0, d2, d3)
 
 
@@ -630,8 +630,8 @@ def test_persistent_kernel_variants_agree(full, option):
 @pytest.mark.parametrize("attn_chunk,conv_chunk,step_frames", [(8, 8, 32), (16, 16, 64), (16, 8, 64), (8, 8, 17), (32, 16, 128), (4, 8, 16), (2, 8, 8)])
 def test_cluster_encoder_kernel_agrees(full, attn_chunk, conv_chunk, step_frames):
     """A / B of the cluster encoder kernel (kernels_persist_cl.cu: 4 clusters x 16 CTAs, activations in distributed shared memory,
-    weights streamed from repacked blobs) against the 148-CTA kernel on the same stream of calls, including ragged step sizes and a
-    chunk size whose steps exceed 16 active rows (those steps must fall back to the 148-CTA kernel, not fail).  Same function, different
+    weights streamed from repacked blobs) against the one-CTA-per-SM kernel on the same stream of calls, including ragged step sizes and a
+    chunk size whose steps exceed 16 active rows (those steps must fall back to the one-CTA-per-SM kernel, not fail).  Same function, different
     summation order; the streaming caches written by one kernel are read by the other in the mixed case."""
     cfg, e, o = full
     e.set_chunk(attn_chunk, conv_chunk)
@@ -663,7 +663,7 @@ def test_cluster_encoder_kernel_agrees(full, attn_chunk, conv_chunk, step_frames
 
 def test_cluster_encoder_kernel_long_utterance(full):
     """The cluster kernel on a 38 s stream (T up to ~950 rows: several batches of key slots per CTA in the attention, long L2 prefetch
-    lists) against the 148-CTA kernel; only every 8th call is compared in full."""
+    lists) against the one-CTA-per-SM kernel; only every 8th call is compared in full."""
     cfg, e, o = full
     e.set_chunk(8, 8)
     feats = e.fbank(cuda(synth.make_audio(38.0, seed=11)))

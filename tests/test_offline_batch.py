@@ -1,5 +1,5 @@
 """Offline batched generator (SURVEY.md §8 row O1): oracle vs the fixture dumped from the reference's own modules on a padded
-batch (CPU), and the engine's per-sample reproduction of the batch (GPU, staged: first B200 run pending)."""
+batch (CPU), and the engine's per-sample reproduction of the batch (GPU)."""
 import numpy as np
 import pytest
 import torch

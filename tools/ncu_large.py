@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Large-M launches inside a cudaProfilerStart/Stop window (BASELINE configs[2] / configs[3] shapes) for
   ncu --profile-from-start off [--set full -k regex:umma2_kernel | --metrics gpu__time_duration.sum] python tools/ncu_large.py
-1. FFN GEMMs of the offline batch (M = 32 x 375 = 12,000 rows) on the tcgen05 kernel, bf16x6
+1. FFN GEMMs of the offline batch (M = 32 x 375 = 12,000 rows) on the wgmma kernel, bf16x6
 2. the vocoder generator on 750 frames
 3. one batched multi-stream ASR step (32 streams x 8 rows)"""
 import os, sys

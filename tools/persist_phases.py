@@ -71,6 +71,7 @@ L1 = 3 + len(PHASES)  # index of the stamp taken after the last barrier of layer
 import statistics
 for p, name in enumerate(PHASES):
     start = all_ts[L1 + p - 1]
-    arr = [all_ts[512 + c * 16 + p] - start for c in range(148)]
-    order = sorted(range(148), key=lambda c: arr[c])
+    n_ctas = torch.cuda.get_device_properties(0).multi_processor_count  # one CTA per SM
+    arr = [all_ts[512 + c * 16 + p] - start for c in range(n_ctas)]
+    order = sorted(range(n_ctas), key=lambda c: arr[c])
     print(f"{name:12s} arrive ns: min {min(arr)} med {int(statistics.median(arr))} max {max(arr)}  slowest CTAs {order[-4:]}  fastest {order[:3]}  barrier done {all_ts[L1 + p] - start}")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Parity and timing of the second-generation tcgen05 conv / linear kernel (kernels_umma2.cu) against an fp64 torch
+"""Parity and timing of the wgmma conv / linear kernel (kernels_umma2.cu) against an fp64 torch
 reference and the fp32 CUDA-core kernel.  Parts: conv (single ops), time (single-op timing), e2e (vocoder + unit decoder
 with the tensor-core routing switched on).  Run every part under `timeout` (a wrong mbarrier protocol would spin)."""
 import json, os, sys
