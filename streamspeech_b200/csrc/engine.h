@@ -103,6 +103,10 @@ struct ss_engine {
   int graph_pdl = 0;
   cudaStream_t capture_stream = nullptr;
   std::map<std::tuple<int, uintptr_t, int, int, int>, std::pair<cudaGraphExec_t, int>> voc_graphs;
+  // whole generator as one persistent kernel (kernels_umma2.cu vocoder_fused): -1 = when the frame count is at most
+  // voc_fused_max_frames, 0 = never (multi-launch path), 1 = whenever the shapes allow it
+  int vocoder_fused = -1;
+  std::map<std::pair<int, uintptr_t>, ss::VocFusedParams> voc_fused;  // kernel parameters per (frames, arena)
   float* persist_ffn_scratch = nullptr;  // [enc_ffn / 16][16][enc_dim] partial sums of the fused FFN phases
   float* cl_blobs = nullptr;             // [enc_layers][16][624][256] weight blobs of the cluster encoder kernel (allocated when the option is set)
   int cluster_cooperative = 1;           // cooperative launch attribute of the cluster kernel (0 only under a serialising profiler)

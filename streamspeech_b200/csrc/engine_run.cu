@@ -122,11 +122,120 @@ void clear_graphs(ss_engine* h) {
   cudaDeviceSynchronize();
   for (auto& kv : h->voc_graphs) cudaGraphExecDestroy(kv.second.first);
   h->voc_graphs.clear();
+  h->voc_fused.clear();  // (their packed weight pointers may be gone too)
 }
 
 bool ws_begin(ss_engine* h, size_t bytes) {
   h->ws.reset();
   return h->ws.ensure(bytes);
+}
+
+// Frame counts up to this run the vocoder generator as one persistent kernel.  It was measured faster than the multi-launch path
+// at 52 (the streaming agent's calls: new frames plus the receptive field), 180 and 750 frames (the offline leg); longer sequences,
+// which were not measured, keep the multi-launch path.
+constexpr int kVocFusedMaxFrames = 1024;
+
+// Job / phase tables of the fused generator for N input frames with the arena's buffers (built once per (N, arena) and kept on
+// the device).  nullptr when a shape is outside what the kernel supports or memory runs out.
+VocFusedParams* vocoder_fused_table(ss_engine* h, int N, const float* frames, float* bufX, float* bufY, const std::vector<float*>& rbA,
+                                                    const std::vector<float*>& rbB, const std::vector<float*>& rbT, const std::vector<float*>& rbO,
+                                                    cudaStream_t st) {
+  const auto key = std::make_pair(N, (uintptr_t)h->ws.base);
+  auto it = h->voc_fused.find(key);
+  if (it != h->voc_fused.end()) return &it->second;
+  const ss_config& c = h->cfg;
+  const int grid = vocoder_fused_grid();
+  if (grid <= 0) return nullptr;
+  std::vector<VocJob> jobs;
+  std::vector<VocPhase> phases;
+  int a_stride = 0, b_stride = 0;
+  bool ok = true;
+  auto job = [&](const float* x0, const float* x1, const float* x2, int L_in, int M, int C_in, int k, int dil, int pad_left, float slope,
+                 const float* W, const float* bias, float* out, int Nout, int stride, int offset, const float* residual, float alpha, float res_scale) {
+    VocJob j{};
+    j.x0 = x0; j.x1 = x1; j.x2 = x2; j.L_in = L_in; j.M = M; j.C_in = C_in; j.ksize = k; j.dil = dil; j.pad_left = pad_left; j.slope = slope;
+    j.wp = reinterpret_cast<const unsigned char*>(W);  // replaced by the packed copy once the phase's tile width is known
+    j.bias = bias; j.out = out; j.N = Nout; j.out_row_stride = stride; j.out_row_offset = offset; j.residual = residual; j.alpha = alpha;
+    j.res_scale = res_scale;
+    j.CK = (C_in % 32 == 0) ? 32 : 16;
+    j.m_tiles = (M + VOC_FUSED_BM - 1) / VOC_FUSED_BM;
+    if (C_in % 16 != 0 || Nout % 16 != 0 || k < 1 || (k - 1) * dil > 50 || bias == nullptr) ok = false;
+    jobs.push_back(j);
+  };
+  // closes the phase of jobs [first, end): tile width, packed weights, longest jobs first
+  auto phase = [&](int first) {
+    const int n_jobs = (int)jobs.size() - first;
+    int items32 = 0;
+    for (int i = first; i < (int)jobs.size(); ++i) items32 += jobs[i].N % 32 == 0 ? jobs[i].m_tiles * (jobs[i].N / 32) : 0;
+    const bool bn32 = items32 >= grid;  // 16-column tiles when 32-column ones would leave SMs idle
+    VocPhase p{first, n_jobs, 0};
+    for (int i = first; i < (int)jobs.size(); ++i) {
+      VocJob& j = jobs[i];
+      j.BN = (bn32 && j.N % 32 == 0) ? 32 : 16;
+      j.n_tiles = j.N / j.BN;
+      j.wp = umma2_packed_weights(h->umma2_cache, reinterpret_cast<const float*>(j.wp), j.N, j.C_in, j.ksize, j.BN, j.CK, 2, st);
+      if (j.wp == nullptr) ok = false;
+      const int rs_pad = ((VOC_FUSED_BM + (j.ksize - 1) * j.dil + 7) & ~7) + 4;
+      a_stride = std::max(a_stride, 2 * (j.CK / 8) * rs_pad * 16);
+      b_stride = std::max(b_stride, j.ksize * 2 * j.BN * j.CK * 2);
+      p.n_items += j.m_tiles * j.n_tiles;
+    }
+    std::stable_sort(jobs.begin() + first, jobs.end(), [](const VocJob& a, const VocJob& b) { return a.ksize > b.ksize; });
+    phases.push_back(p);
+  };
+  jobs.reserve(1 + c.voc_n_ups * (8 + 2 * c.voc_n_rb * c.voc_rb_ndil));
+  job(frames, nullptr, nullptr, N, N, c.voc_in_dim, 7, 1, 3, 1.0f, h->conv_pre.lin.w, h->conv_pre.lin.b, bufX, c.voc_init_channels, 1, 0, nullptr,
+      1.0f, 1.0f);
+  phase(0);
+  const int nrb = c.voc_n_rb, nd = c.voc_rb_ndil;
+  int L = N;
+  for (int i = 0; i < c.voc_n_ups; ++i) {
+    const UpsampleW& U = h->ups[i];
+    const int Lout = L * U.u;
+    // stage input: conv_pre's output, or the previous stage's three resblock outputs summed while loading
+    const float* x0 = i == 0 ? bufX : rbO[0];
+    const float* x1 = i == 0 ? nullptr : rbO[1];
+    const float* x2 = i == 0 ? nullptr : rbO[2];
+    int first = (int)jobs.size();
+    for (int phi = 0; phi < U.u; ++phi) {
+      const int J = U.phase_J[phi], q0 = U.phase_q0[phi];
+      const int nrows = (Lout - 1 - phi + U.pad) / U.u - q0 + 1;
+      if (nrows <= 0) continue;
+      job(x0, x1, x2, L, nrows, U.cin, J, 1, (J - 1) - q0, 0.1f, U.phase_w[phi].w, U.bias, bufY, U.cout, U.u, q0 * U.u + phi - U.pad, nullptr,
+          1.0f, 1.0f);
+    }
+    phase(first);
+    L = Lout;
+    const int ch = U.cout;
+    for (int m = 0; m < nd; ++m) {
+      first = (int)jobs.size();
+      for (int j = 0; j < nrb; ++j) {
+        const ConvW& w1 = h->rb1[i][j][m];
+        const float* cur = m == 0 ? bufY : (m == 1 ? rbA[j] : rbB[j]);
+        job(cur, nullptr, nullptr, L, L, ch, w1.ksize, w1.dil, (w1.ksize * w1.dil - w1.dil) / 2, 0.1f, w1.lin.w, w1.lin.b, rbT[j], ch, 1, 0,
+            nullptr, 1.0f, 1.0f);
+      }
+      phase(first);
+      first = (int)jobs.size();
+      for (int j = 0; j < nrb; ++j) {
+        const ConvW& w2 = h->rb2[i][j][m];
+        const float* cur = m == 0 ? bufY : (m == 1 ? rbA[j] : rbB[j]);
+        float* out = m + 1 < nd ? (m == 0 ? rbA[j] : rbB[j]) : rbO[j];
+        const float s = m + 1 < nd ? 1.0f : 1.0f / nrb;  // last pair of the block: (xt + x) / num_kernels
+        job(rbT[j], nullptr, nullptr, L, L, ch, w2.ksize, 1, (w2.ksize - 1) / 2, 0.1f, w2.lin.w, w2.lin.b, out, ch, 1, 0, cur, s, s);
+      }
+      phase(first);
+    }
+  }
+  if (!ok || jobs.size() > VOC_MAX_JOBS || phases.size() > VOC_MAX_PHASES || vocoder_fused_smem(a_stride, b_stride) > 200 * 1024) return nullptr;
+  if (h->voc_fused.size() >= 64) h->voc_fused.clear();
+  VocFusedParams& p = h->voc_fused[key];
+  std::copy(jobs.begin(), jobs.end(), p.jobs);
+  std::copy(phases.begin(), phases.end(), p.phases);
+  p.n_phases = (int)phases.size();
+  p.a_stride = a_stride;
+  p.b_stride = b_stride;
+  return &p;
 }
 
 struct DecScratch {
@@ -992,6 +1101,21 @@ int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0
   }
   // V1 tail: repeat_interleave(x, dur) for the frame window (agent/tts/codehifigan.py:66)
   expand_frames(h->voc_unit_emb, h->voc_cumsum, h->voc_U, f_lo, N, c.voc_embedding_dim, frames, st);
+  // Short sequences (the streaming calls): conv_pre .. conv_post as one persistent kernel whose phases are separated by grid
+  // barriers.  A shape it does not support or a refused cooperative launch falls through to the multi-launch path below.
+  const bool fused = h->vocoder_fused != 0 && (h->vocoder_fused == 1 || N <= kVocFusedMaxFrames) && g_umma_conv == 12 && nrb == 3 &&
+                     h->persist_bar != nullptr;
+  if (fused) {
+    VocFusedParams* P = vocoder_fused_table(h, N, frames, bufX, bufY, rbA, rbB, rbT, rbO, st);
+    if (P) {
+      VocPost& post = P->post;
+      post.x0 = rbO[0]; post.x1 = rbO[1]; post.x2 = rbO[2];
+      post.w = h->conv_post_w; post.bias = h->conv_post_b; post.slope = 0.01f;  // leaky_relu(x) [slope 0.01, hifigan.py:166]
+      post.L = N * h->hop; post.C = h->conv_post_c; post.k = h->conv_post_k; post.t0 = ctx * h->hop;
+      post.out = wav_out_dev;
+      if (vocoder_fused(*P, h->persist_bar, &h->persist_bar_target, st) == 0) return check_launch(h, "ss_vocoder_generate");
+    }
+  }
   // Everything from conv_pre to conv_post depends on the call only through N (buffer addresses are arena offsets): ~190
   // launches on three streams whose host enqueue time exceeds their GPU time.  With option vocoder_graph the sequence is
   // recorded once per (N, arena, routing) by stream capture and replayed as one CUDA graph afterwards.
@@ -1162,6 +1286,7 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
   else if (n == "prefer_shared") g_prefer_shared = value;  // takes effect for kernels that have not been launched yet
   else if (n == "unit_grouped") h->unit_grouped = value;
   else if (n == "vocoder_graph") h->vocoder_graph = value;
+  else if (n == "vocoder_fused") h->vocoder_fused = value;
   else if (n == "graph_pdl") h->graph_pdl = value;
   else if (n == "fbank_tma") h->fbank_tma = value;
   else if (n == "umma2_fused_reduce") g_umma2_fused_reduce = value;

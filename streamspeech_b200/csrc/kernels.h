@@ -85,6 +85,51 @@ void umma2_cache_clear(Umma2Cache* c);
 void umma2_cache_destroy(Umma2Cache* c);
 bool umma2_supported(const ConvA& a, int N, const Epilogue& ep);
 void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, cudaStream_t st);
+// packed copy of W[N][ksize*C_in] in the kernels' tiling (made once per weight matrix and tiling; nullptr when out of memory)
+const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int N, int C_in, int ksize, int BN, int CK, int NP, cudaStream_t st);
+
+// ---- the whole vocoder generator of one call as one persistent cooperative wgmma kernel (kernels_umma2.cu, bf16x3)
+// One job = one stride-1 convolution of the generator, tiled into 128-row x BN-column work items:
+//   out[m * out_row_stride + out_row_offset][n] = alpha * (sum_{j, ci} pre(x[m + j*dil - pad_left][ci]) * W[n][j][ci] + bias[n])
+//                                                + res_scale * residual[same index]
+// with x = x0, or x2 + (x1 + x0) when x1 != nullptr (the sum of a stage's three resblock outputs), pre = leaky_relu(slope).
+struct VocJob {
+  const float *x0, *x1, *x2;
+  int L_in, M, C_in, ksize, dil, pad_left;
+  float slope;
+  const unsigned char* wp;  // umma2_packed_weights(W, N, C_in, ksize, BN, CK, 2)
+  const float* bias;
+  float* out;
+  int N, out_row_stride, out_row_offset;
+  const float* residual;
+  float alpha, res_scale;
+  int BN, CK, m_tiles, n_tiles;
+};
+struct VocPhase {  // jobs [first_job, first_job + n_jobs) are independent; items of the phase = sum of m_tiles * n_tiles
+  int first_job, n_jobs, n_items;
+};
+// last phase: out[t - t0] = tanh(bias + sum_{j, c} w[j][c] * leaky_relu(x2 + (x1 + x0))[t + j - (k-1)/2][c]) for t in [t0, L)
+struct VocPost {
+  const float *x0, *x1, *x2;
+  const float* w;  // [k][C]
+  float bias, slope;
+  int L, C, k, t0;
+  float* out;
+};
+constexpr int VOC_FUSED_BM = 128;
+constexpr int VOC_MAX_JOBS = 128, VOC_MAX_PHASES = 48;
+struct VocFusedParams {  // passed by value in the kernel's parameter space (~17 KB): no per-call upload
+  VocJob jobs[VOC_MAX_JOBS];
+  VocPhase phases[VOC_MAX_PHASES];
+  int n_phases;
+  int a_stride, b_stride;  // shared-memory bytes of one A stage (rows x channels x pieces) / one B stage (all taps of a chunk)
+  VocPost post;
+};
+// CTAs of the cooperative launch on the current device (0: the kernel cannot be made resident)
+int vocoder_fused_grid();
+size_t vocoder_fused_smem(int a_stride, int b_stride);
+// returns 0 (enqueued; the barrier target advanced by grid x n_phases) or < 0 (launch refused)
+int vocoder_fused(const VocFusedParams& p, unsigned* bar_ctr, unsigned* bar_target_host, cudaStream_t st);
 
 // Weight-streaming GEMM for M <= 64 rows (plain row-major A): one warp per output column, see kernels_skinny.cu.
 bool skinny_gemm_supported(int M, int N, int K, const Epilogue& ep);

@@ -42,26 +42,6 @@ __device__ __forceinline__ float4 ldw(const float* p) {
   return r;
 }
 
-// Grid barrier on a monotonic arrival counter (one red.release per CTA, relaxed polling, one acquire fence at the end).
-// `target` is the counter value that marks "every CTA has arrived at this barrier"; the host carries it across launches.
-__device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned& target) {
-  __syncthreads();
-  target += gridDim.x;
-  if (threadIdx.x == 0) {
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
-    unsigned v, spins = 0;
-    do {  // (bounded: a counter out of step with the host's target must not hang the device)
-      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-    } while ((int)(v - target) < 0 && ++spins < (1u << 20));
-    // A counter that never reaches the target (lost arrival, counter out of step with the host's target) must neither hang
-    // the device nor pass silently: the word ctr[SS_BAR_ERR_WORD] is raised and the host reports it at its next
-    // synchronisation point (ss_async_error / ss_mt_greedy), after which results of this launch are invalid.
-    if ((int)(v - target) < 0) atomicExch(ctr + SS_BAR_ERR_WORD, 1u);
-    asm volatile("fence.acq_rel.gpu;" ::: "memory");
-  }
-  __syncthreads();
-}
-
 // L2 prefetch of a weight matrix, spread over the whole grid (one 128-byte line per request)
 __device__ __forceinline__ void prefetch_l2(const float* p, int n_floats) {
   const int lines = n_floats >> 5;

@@ -8,6 +8,29 @@ namespace ss {
 // word of the barrier buffer (unsigned[64]: [0] = arrival counter) that a timed-out grid barrier raises
 #define SS_BAR_ERR_WORD 32
 
+#ifdef __CUDACC__
+// Grid barrier of the persistent cooperative kernels, on a monotonic arrival counter (one red.release per CTA, relaxed polling,
+// one acquire fence at the end).  `target` is the counter value that marks "every CTA has arrived at this barrier"; the host
+// carries it across launches.
+__device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned& target) {
+  __syncthreads();
+  target += gridDim.x;
+  if (threadIdx.x == 0) {
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
+    unsigned v, spins = 0;
+    do {  // (bounded: a counter out of step with the host's target must not hang the device)
+      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+    } while ((int)(v - target) < 0 && ++spins < (1u << 20));
+    // A counter that never reaches the target (lost arrival, counter out of step with the host's target) must neither hang
+    // the device nor pass silently: the word ctr[SS_BAR_ERR_WORD] is raised and the host reports it at its next
+    // synchronisation point (ss_async_error / ss_mt_greedy), after which results of this launch are invalid.
+    if ((int)(v - target) < 0) atomicExch(ctr + SS_BAR_ERR_WORD, 1u);
+    asm volatile("fence.acq_rel.gpu;" ::: "memory");
+  }
+  __syncthreads();
+}
+#endif
+
 struct PersistLayer {  // device pointers of one Conformer layer (fp32, layouts as in engine.h ConformerLayerW)
   const float *ffn1_g, *ffn1_b, *ffn1_w1, *ffn1_b1, *ffn1_w2, *ffn1_b2;
   const float *attn_g, *attn_b, *wqkv, *bqkv, *wo, *bo, *pos_u, *pos_v, *pos_proj;

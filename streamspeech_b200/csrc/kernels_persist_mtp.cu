@@ -31,21 +31,6 @@ __device__ __forceinline__ float4 ldw(const float* p) {
   return r;
 }
 
-__device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned& target) {
-  __syncthreads();
-  target += gridDim.x;
-  if (threadIdx.x == 0) {
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
-    unsigned v, spins = 0;
-    do {
-      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-    } while ((int)(v - target) < 0 && ++spins < (1u << 20));
-    if ((int)(v - target) < 0) atomicExch(ctr + SS_BAR_ERR_WORD, 1u);  // reported by the host (ss_async_error / ss_mt_greedy)
-    asm volatile("fence.acq_rel.gpu;" ::: "memory");
-  }
-  __syncthreads();
-}
-
 struct QSmem {                    // static part; As (staged activations [QMAXM][QD]) and S (scores [QW][QMAXT]) are dynamic
   float part[QW][4][QRB];
   float qs[QW][QHD];

@@ -29,6 +29,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "kernels_persist.h"
 
 namespace ss {
 
@@ -548,39 +549,48 @@ bool umma2_supported(const ConvA& a, int N, const Epilogue& ep) {
   return true;
 }
 
+const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int N, int C_in, int k, int BN, int CK, int NP, cudaStream_t st) {
+  auto key = std::make_tuple(W, N, C_in, k, BN, NP, CK);
+  auto it = cache->packed.find(key);
+  if (it != cache->packed.end()) return it->second;
+  const int n_chunks = C_in / CK;
+  const int n_tiles = (N + BN - 1) / BN;
+  unsigned char* wp = nullptr;
+  const size_t bytes = (size_t)n_tiles * n_chunks * k * NP * BN * CK * 2;
+  if (cudaMalloc((void**)&wp, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    return nullptr;
+  }
+  cache->allocs.push_back(wp);
+  cache->packed[key] = wp;
+  const int64_t total = (int64_t)n_tiles * n_chunks * k * (CK >> 3) * BN;
+  const int blocks = (int)((total + 255) / 256);
+  if (NP == 3)
+    umma2_pack_kernel<3><<<blocks, 256, 0, st>>>(W, N, C_in, k, BN, CK, n_tiles, wp);
+  else
+    umma2_pack_kernel<2><<<blocks, 256, 0, st>>>(W, N, C_in, k, BN, CK, n_tiles, wp);
+  return wp;
+}
+
 void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, cudaStream_t st) {
-  ++g_launches;
   const int M = a.L_rows;
-  if (M <= 0) return;
+  if (M <= 0) {
+    ++g_launches;
+    return;
+  }
   const int NP = pieces >= 3 ? 3 : 2;
   const int BN = u2_bn(N);
   const int CK = (a.C_in % 32 == 0) ? 32 : 16;
-  const int n_chunks = a.C_in / CK;
-  const int n_tiles = (N + BN - 1) / BN;
   const int k = a.ksize;
   // ---- packed weights (once per weight matrix and tiling)
-  auto key = std::make_tuple(W, N, a.C_in, k, BN, NP, CK);
-  unsigned char* wp = nullptr;
-  auto it = cache->packed.find(key);
-  if (it == cache->packed.end()) {
-    const size_t bytes = (size_t)n_tiles * n_chunks * k * NP * BN * CK * 2;
-    if (cudaMalloc((void**)&wp, bytes) != cudaSuccess) {
-      cudaGetLastError();
-      --g_launches;
-      gemm_conv(a, W, N, ep, st);  // out of memory for the packed copy: exact fp32 path
-      return;
-    }
-    cache->allocs.push_back(wp);
-    cache->packed[key] = wp;
-    const int64_t total = (int64_t)n_tiles * n_chunks * k * (CK >> 3) * BN;
-    const int blocks = (int)((total + 255) / 256);
-    if (NP == 3)
-      umma2_pack_kernel<3><<<blocks, 256, 0, st>>>(W, N, a.C_in, k, BN, CK, n_tiles, wp);
-    else
-      umma2_pack_kernel<2><<<blocks, 256, 0, st>>>(W, N, a.C_in, k, BN, CK, n_tiles, wp);
-  } else {
-    wp = it->second;
+  const unsigned char* wp = umma2_packed_weights(cache, W, N, a.C_in, k, BN, CK, NP, st);
+  if (wp == nullptr) {
+    gemm_conv(a, W, N, ep, st);  // out of memory for the packed copy: exact fp32 path
+    return;
   }
+  ++g_launches;
+  const int n_chunks = a.C_in / CK;
+  const int n_tiles = (N + BN - 1) / BN;
   U2Params p;
   p.a = a;
   p.ep = ep;
@@ -638,6 +648,233 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
     }
   }
   if (splits > 1 && p.tile_ctr == nullptr) splitk_epilogue(ws, splits, M, N, a.L_rows, ep, st);
+}
+
+// ------------------------------------------------------------------------------------------------ fused vocoder generator
+// One CTA per SM runs the phases of the generator (conv_pre | per stage: upsample phases, then 6 resblock depths with the three
+// resblocks' convs as independent jobs | conv_post + tanh) and meets the other CTAs in a grid barrier after each phase.  Work item
+// i of a phase goes to CTA i % gridDim.x; the host orders a phase's jobs by decreasing kernel size so the long items start first.
+// An item is a whole 128-row x BN output tile (two warpgroups of 64 rows), so a row's sum does not depend on the schedule.
+// Per channel chunk the item stages the activation rows (halo included, taps are descriptor row shifts as in umma2_kernel) and
+// all taps of the chunk's packed weights; both are double-buffered so the loads of chunk c+1 fly while the MMAs of chunk c run.
+namespace {
+
+constexpr int VF_THREADS = 256;
+constexpr int VF_UPT = 6;  // float4 units per thread and chunk: (128 + max halo 50) rows x 8 units <= 6 x 256
+
+__device__ __forceinline__ void vf_cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+
+template <int BN, bool ADD3>
+__device__ __forceinline__ void vf_item(const VocJob& J, int mt, int nt, unsigned char* a_smem, unsigned char* b_smem, float* tile,
+                                        uint32_t a_stride, uint32_t b_stride) {
+  constexpr int NACC = BN / 2;
+  constexpr int TP = BN + 8;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int m0 = mt * VOC_FUSED_BM, n0 = nt * BN;
+  const int CK = J.CK, k = J.ksize, dil = J.dil, C_in = J.C_in;
+  const int n_chunks = C_in / CK;
+  const int rs = VOC_FUSED_BM + (k - 1) * dil;
+  const uint32_t a_plane = (uint32_t)(((rs + 7) & ~7) + 4) * 16u;
+  const uint32_t a_piece = (uint32_t)(CK >> 3) * a_plane;
+  const uint32_t b_plane = (uint32_t)BN * 16u;
+  const uint32_t b_piece = (uint32_t)BN * CK * 2u;
+  const uint32_t b_unit = 2u * b_piece;
+  const uint32_t b_chunk = (uint32_t)k * b_unit;
+  const unsigned char* wsrc = J.wp + (size_t)nt * n_chunks * b_chunk;
+
+  const int upr_shift = (CK == 32) ? 3 : 2;
+  const int upr = 1 << upr_shift;
+  const int n_a = rs * upr;
+  int64_t goff[VF_UPT];
+  uint32_t soff[VF_UPT];
+#pragma unroll
+  for (int i = 0; i < VF_UPT; ++i) {
+    const int idx = tid + i * VF_THREADS;
+    const int r = idx >> upr_shift, q = idx & (upr - 1);
+    const int pos = m0 + r - J.pad_left;
+    const bool inb = idx < n_a && pos >= 0 && pos < J.L_in;
+    goff[i] = inb ? (int64_t)pos * C_in + q * 4 : (int64_t)-1;
+    soff[i] = (uint32_t)(q >> 1) * a_plane + (uint32_t)r * 16u + (uint32_t)(q & 1) * 8u;
+  }
+  // activations are written by earlier phases of this kernel: L2 loads (.cg), never the non-coherent read-only path
+  float4 pf[ADD3 ? 3 : 1][VF_UPT];
+  auto load_a = [&](int c) {
+#pragma unroll
+    for (int i = 0; i < VF_UPT; ++i) {
+      const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+      const int64_t o = goff[i] + (int64_t)c * CK;
+      pf[0][i] = goff[i] >= 0 ? __ldcg(reinterpret_cast<const float4*>(J.x0 + o)) : z;
+      if (ADD3) {
+        pf[ADD3 ? 1 : 0][i] = goff[i] >= 0 ? __ldcg(reinterpret_cast<const float4*>(J.x1 + o)) : z;
+        pf[ADD3 ? 2 : 0][i] = goff[i] >= 0 ? __ldcg(reinterpret_cast<const float4*>(J.x2 + o)) : z;
+      }
+    }
+  };
+  auto load_b = [&](int c, int s) {
+    const unsigned char* src = wsrc + (size_t)c * b_chunk;
+    const uint32_t dst = smem_u32(b_smem + (size_t)s * b_stride);
+    for (uint32_t i = tid; i < (b_chunk >> 4); i += VF_THREADS) vf_cp_async16(dst + 16u * i, src + 16u * i);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+
+  float acc[NACC];
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+  load_b(0, 0);
+  load_a(0);
+  const float slope = J.slope;
+  for (int c = 0; c < n_chunks; ++c) {
+    const int s = c & 1;
+    unsigned char* stage = a_smem + (size_t)s * a_stride;
+#pragma unroll
+    for (int i = 0; i < VF_UPT; ++i) {
+      if (tid + i * VF_THREADS < n_a) {
+        float4 v = pf[0][i];
+        if (ADD3) {  // the stage's resblock outputs in the reference's order: (b0 + b1) + b2
+          const float4 b1 = pf[ADD3 ? 1 : 0][i], b2 = pf[ADD3 ? 2 : 0][i];
+          v = make_float4(b2.x + (b1.x + v.x), b2.y + (b1.y + v.y), b2.z + (b1.z + v.z), b2.w + (b1.w + v.w));
+        }
+        if (slope != 1.0f) {
+          v.x = v.x > 0.f ? v.x : v.x * slope;
+          v.y = v.y > 0.f ? v.y : v.y * slope;
+          v.z = v.z > 0.f ? v.z : v.z * slope;
+          v.w = v.w > 0.f ? v.w : v.w * slope;
+        }
+        u2_split_store<2>(v, stage, a_piece, soff[i]);
+      }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // this thread's generic-proxy writes (staged rows, copied weights) become visible to the async proxy (wgmma)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    if (c + 1 < n_chunks) {  // the stages of chunk c-1 are free: every warp waited for its MMAs before the barrier above
+      load_b(c + 1, s ^ 1);
+      load_a(c + 1);
+    }
+    const uint32_t a_base = smem_u32(stage) + (uint32_t)wg * 64u * 16u;
+    const uint32_t b_base0 = smem_u32(b_smem + (size_t)s * b_stride);
+    u2_fence_acc<NACC>(acc);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    for (int j = 0; j < k; ++j) {
+      const uint32_t a_tap = a_base + (uint32_t)(j * dil) * 16u;
+      const uint32_t b_base = b_base0 + (uint32_t)j * b_unit;
+      for (int ks = 0; ks < (CK >> 4); ++ks) {
+        const uint64_t a0 = u2_desc(a_tap + ks * 2 * a_plane, a_plane, 128), a1 = u2_desc(a_tap + a_piece + ks * 2 * a_plane, a_plane, 128);
+        const uint64_t b0 = u2_desc(b_base + ks * 2 * b_plane, b_plane, 128), b1 = u2_desc(b_base + b_piece + ks * 2 * b_plane, b_plane, 128);
+        u2_wgmma<BN>(acc, a0, b0);
+        u2_wgmma<BN>(acc, a0, b1);
+        u2_wgmma<BN>(acc, a1, b0);
+      }
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    u2_fence_acc<NACC>(acc);
+  }
+  // epilogue through the padded tile: whole rows per warp, bias / residual reads coalesced
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      *reinterpret_cast<float2*>(tile + r0 * TP + 8 * i + c0) = make_float2(acc[4 * i], acc[4 * i + 1]);
+      *reinterpret_cast<float2*>(tile + (r0 + 8) * TP + 8 * i + c0) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+  }
+  __syncthreads();
+  const int rows = min(VOC_FUSED_BM, J.M - m0);
+  for (int idx = tid; idx < rows * BN; idx += VF_THREADS) {
+    const int r = idx / BN, cc = idx - r * BN;
+    const int n = n0 + cc;
+    const int64_t o = ((int64_t)(m0 + r) * J.out_row_stride + J.out_row_offset) * J.N + n;
+    const float v = tile[r * TP + cc] + J.bias[n];
+    const float res = J.residual != nullptr ? J.res_scale * __ldcg(J.residual + o) : 0.f;
+    J.out[o] = J.alpha * v + res;
+  }
+  __syncthreads();  // the tile and the operand stages are reused by the next item
+}
+
+__global__ void __launch_bounds__(VF_THREADS, 1)
+    vocoder_fused_kernel(const __grid_constant__ VocFusedParams p, unsigned* bar_ctr, unsigned bar_target) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const uint32_t a_stride = (uint32_t)p.a_stride, b_stride = (uint32_t)p.b_stride;
+  unsigned char* a_smem = smem + ((128u - (smem_u32(smem) & 127u)) & 127u);
+  unsigned char* b_smem = a_smem + 2 * (size_t)a_stride;
+  float* tile = reinterpret_cast<float*>(b_smem + 2 * (size_t)b_stride);
+  const VocJob* jobs = p.jobs;
+  const VocPost& post = p.post;
+  for (int ph = 0; ph < p.n_phases; ++ph) {
+    const VocPhase P = p.phases[ph];
+    for (int i = blockIdx.x; i < P.n_items; i += gridDim.x) {
+      int jb = P.first_job, rest = i;
+      while (rest >= jobs[jb].m_tiles * jobs[jb].n_tiles) {
+        rest -= jobs[jb].m_tiles * jobs[jb].n_tiles;
+        ++jb;
+      }
+      const VocJob& J = jobs[jb];
+      const int nt = rest % J.n_tiles, mt = rest / J.n_tiles;  // neighbouring CTAs share activation rows
+      const bool add3 = J.x1 != nullptr;
+      if (J.BN == 32) {
+        if (add3) vf_item<32, true>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+        else vf_item<32, false>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+      } else {
+        if (add3) vf_item<16, true>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+        else vf_item<16, false>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+      }
+    }
+    grid_barrier(bar_ctr, bar_target);
+  }
+  // conv_post + tanh on the new samples only, straight into the caller's buffer (same arithmetic order as conv_post_tanh_kernel)
+  const int half = (post.k - 1) >> 1;
+  for (int t = post.t0 + blockIdx.x * VF_THREADS + threadIdx.x; t < post.L; t += gridDim.x * VF_THREADS) {
+    float acc = post.bias;
+    for (int j = 0; j < post.k; ++j) {
+      const int p = t - half + j;
+      if (p < 0 || p >= post.L) continue;
+      const int64_t row = (int64_t)p * post.C;
+      for (int c = 0; c < post.C; ++c) {
+        float v = __ldcg(post.x2 + row + c) + (__ldcg(post.x1 + row + c) + __ldcg(post.x0 + row + c));
+        v = v > 0.f ? v : v * post.slope;
+        acc = fmaf(post.w[j * post.C + c], v, acc);
+      }
+    }
+    post.out[t - post.t0] = tanhf(acc);
+  }
+}
+
+}  // namespace
+
+size_t vocoder_fused_smem(int a_stride, int b_stride) {
+  return 2 * (size_t)a_stride + 2 * (size_t)b_stride + (size_t)VOC_FUSED_BM * (32 + 8) * sizeof(float) + 128;
+}
+
+int vocoder_fused_grid() {
+  // the largest shared-memory footprint the engine asks for (stage-0 resblock k = 11, dil 5, 32 channels per chunk, BN = 32)
+  static const size_t smem_max = 200 * 1024;
+  if (first_time_on_device((const void*)vocoder_fused_kernel))
+    cudaFuncSetAttribute(vocoder_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+  int occ = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vocoder_fused_kernel, VF_THREADS, smem_max) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return occ >= 1 ? current_device_sms() : 0;
+}
+
+int vocoder_fused(const VocFusedParams& p, unsigned* bar_ctr, unsigned* bar_target_host, cudaStream_t st) {
+  const int grid = vocoder_fused_grid();
+  const size_t smem = vocoder_fused_smem(p.a_stride, p.b_stride);
+  if (grid <= 0 || smem > 200 * 1024) return -1;
+  unsigned bar_target = *bar_target_host;
+  void* args[] = {(void*)&p, (void*)&bar_ctr, (void*)&bar_target};
+  if (cudaLaunchCooperativeKernel((void*)vocoder_fused_kernel, dim3(grid), dim3(VF_THREADS), args, smem, st) != cudaSuccess) {
+    cudaGetLastError();
+    return -2;
+  }
+  ++g_launches;
+  *bar_target_host += (unsigned)grid * (unsigned)p.n_phases;
+  return 0;
 }
 
 }  // namespace ss

@@ -206,6 +206,8 @@ class Engine:
         self.set_option("vocoder_streams", int(os.environ.get("SS_VOCODER_STREAMS", "1")))
         self.set_option("unit_grouped", int(os.environ.get("SS_UNIT_GROUPED", "1")))
         self.set_option("vocoder_graph", int(os.environ.get("SS_VOCODER_GRAPH", "0")))
+        # vocoder generator as one persistent kernel: -1 (default) for short frame windows, 0 never (multi-launch path), 1 always
+        self.set_option("vocoder_fused", int(os.environ.get("SS_VOCODER_FUSED", "-1")))
         self.set_option("graph_pdl", int(os.environ.get("SS_GRAPH_PDL", "0")))
         self.set_option("persistent_prefetch", int(os.environ.get("SS_PERSISTENT_PREFETCH", "0")))
         self.set_option("umma2_split_below", int(os.environ.get("SS_UMMA2_SPLIT_BELOW", "60")))
