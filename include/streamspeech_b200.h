@@ -195,12 +195,22 @@ int ss_vocoder_receptive_field(const ss_engine* h);
  * concurrent ASR streams, 32 per GPU).  The reference is one utterance per agent process (agent/speech_to_text.asr.streamspeech.
  * agent.py:385-433).  Each stream owns a slot: device audio, fbank frames, per-layer K / V / conv-input caches, encoder rows and CTC
  * arg-max rows.  Results of every stream equal the single-stream entry points' (same arithmetic per stream; GEMMs see n x rows). */
-int ss_pool_create(ss_engine* h, int n_slots, int max_seconds);
-int ss_pool_reset(ss_engine* h, int slot);                       /* new utterance on this slot */
-/* append n 16 kHz samples (host memory) to the slot's device audio: enqueue of one host->device copy */
+int ss_pool_create(ss_engine* h, int n_slots, int max_seconds);  /* 16 kHz sources: ss_pool_create_rate(h, n_slots, max_seconds, 16000) */
+/* Pool whose sources arrive at sample_rate = 16000 or 48000 Hz (anything else: SS_ERR_INVALID).  A 48 kHz pool keeps the pushed
+ * samples in a second per-slot row of max_seconds * 48000 + 1200 samples; every ss_pool_step first extends each listed slot's 16 kHz
+ * row on the device (one launch for all slots) with the samples that are final, as the single-stream 48 kHz agent does:
+ * [produced so far, ss_resample_out_len(n48, finished)), each bit-identical to ss_resample_48k_to_16k on the same 48 kHz prefix. */
+int ss_pool_create_rate(ss_engine* h, int n_slots, int max_seconds, int sample_rate);
+int ss_pool_reset(ss_engine* h, int slot);                       /* new utterance on this slot (clears the finished flag) */
+/* append n samples at the pool's rate (host memory) to the slot's device audio: enqueue of one host->device copy.  The capacity
+ * check counts samples at that rate.  SS_ERR_STATE after ss_pool_finish until ss_pool_reset */
 int ss_pool_push_audio(ss_engine* h, void* stream, int slot, const float* samples_host, int n);
-/* state of a slot: samples / fbank frames held, final encoder rows, device pointers of its encoder rows [Tcap][enc_dim] and fbank
- * frames [Fcap][feat_dim] (any out pointer may be NULL) */
+/* The slot's source is closed: in a 48 kHz pool the next step produces the 16 kHz tail up to ceil(n48 / 3) (ss_resample_out_len
+ * with finished = 1).  In a 16 kHz pool it only sets the flag, so callers need not branch on the rate. */
+int ss_pool_finish(ss_engine* h, int slot);
+/* state of a slot: 16 kHz samples available to fbank (in a 48 kHz pool: those produced by the steps so far), fbank frames held,
+ * final encoder rows, device pointers of its encoder rows [Tcap][enc_dim] and fbank frames [Fcap][feat_dim] (any out pointer may
+ * be NULL) */
 int ss_pool_info(ss_engine* h, int slot, int64_t* n_audio, int32_t* n_feat, int32_t* T_final, float** enc_out_dev, float** feats_dev);
 /* One streaming step of the n listed slots over all the audio pushed so far: OnlineFeatureExtractor (new frames only) ->
  * forward_encoder (rows not yet final, ss_encoder_stream_step semantics) -> CTCDecoder.generate for ctc_heads heads (0: none, 1: ASR,
@@ -235,10 +245,12 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
  * "persistent_ffn_fused", "persistent_mt", "persistent_mt_v2", "persistent_mt_prefix", "fbank_tma" = 1 (default): kernel variants of
  * round 2, each tested against the path it replaces; "umma2_fused_reduce" = 0 (default: measured slower);
  * "persistent_profile" = 1: the persistent kernels record %globaltimer stamps per phase; "persistent_time" = 1: CUDA events around
- * the encoder-stack kernel and the single-token MT kernel (read with ss_debug_copy "persist_time" / "mt_time") */
+ * the encoder-stack kernel, the single-token MT kernel and the stream pool's resample kernel (read with ss_debug_copy "persist_time" /
+ * "mt_time" / "pool_resample_time") */
 int ss_set_option(ss_engine* h, const char* name, int value);
 /* synchronous copy of a diagnostic buffer to the host: "persist_ts" = uint64 ns stamps of the last persistent step;
- * "persist_time" / "mt_time" = double[3] {summed ms, launches, summed algorithmic bytes / executed steps} since the last query;
+ * "persist_time" / "mt_time" / "pool_resample_time" = double[3] {summed ms, launches, summed algorithmic bytes / executed steps /
+ * algorithmic bytes} since the last query;
  * "cluster_steps" = long long, encoder steps taken by the cluster kernel */
 int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes);
 int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev,

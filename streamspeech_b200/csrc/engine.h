@@ -211,12 +211,17 @@ struct ss_engine {
   // ---- multi-stream pool (engine_pool.inc): per-slot streaming state at fixed strides
   struct StreamPool {
     int n_slots = 0, Tcap = 0, Fcap = 0;
-    int64_t audio_cap = 0;
+    int rate = 16000;                                  // source sample rate: 16000, or 48000 (resampled per slot inside ss_pool_step)
+    int64_t audio_cap = 0, audio48_cap = 0;
     float *audio = nullptr, *feats = nullptr, *k = nullptr, *v = nullptr, *glu = nullptr, *enc_out = nullptr, *melT = nullptr;
+    float* audio48 = nullptr;                          // 48 kHz pools: [slot][audio48_cap] pushed samples; `audio` holds their 16 kHz signal
     int64_t* ctc_am = nullptr;                         // [slot][2][Tcap]
     ss::MsStream *desc_dev = nullptr, *desc_pinned = nullptr, *desc_dev2 = nullptr, *desc_pinned2 = nullptr;
     std::vector<int> T_final, n_feat;
-    std::vector<int64_t> n_audio;
+    std::vector<int64_t> n_audio;                      // 16 kHz samples in `audio` (the fbank's input)
+    std::vector<int64_t> n48;                          // 48 kHz pools: samples in `audio48`
+    std::vector<char> finished;                        // ss_pool_finish: the slot's source is closed
+    std::vector<TimedLaunch> resample_events;          // option persistent_time: CUDA events around ms_resample_3to1 (bytes = 16 per output)
   } pool;
 
   int fail(int code, const std::string& msg) {

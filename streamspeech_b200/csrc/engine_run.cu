@@ -1377,12 +1377,15 @@ int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes) 
     h->mt_time_events.clear();
     return SS_OK;
   }
-  if (n == "persist_time") {  // double[3] = {summed ms, launches, summed algorithmic bytes} since the last query
-    if (bytes < 3 * sizeof(double)) return h->fail(SS_ERR_INVALID, "persist_time needs 3 doubles");
+  // double[3] = {summed ms, launches, summed algorithmic bytes} since the last query, of the persistent encoder kernel
+  // ("persist_time") or of the stream pool's resample kernel ("pool_resample_time")
+  if (n == "persist_time" || n == "pool_resample_time") {
+    if (bytes < 3 * sizeof(double)) return h->fail(SS_ERR_INVALID, n + " needs 3 doubles");
+    std::vector<ss_engine::TimedLaunch>& events = n == "persist_time" ? h->time_events : h->pool.resample_events;
     cudaDeviceSynchronize();
     double* out = (double*)host_dst;
     out[0] = out[1] = out[2] = 0.0;
-    for (auto& e : h->time_events) {
+    for (auto& e : events) {
       float ms = 0.f;
       if (cudaEventElapsedTime(&ms, e.e0, e.e1) == cudaSuccess) {
         out[0] += ms;
@@ -1393,7 +1396,7 @@ int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes) 
       cudaEventDestroy(e.e1);
     }
     cudaGetLastError();
-    h->time_events.clear();
+    events.clear();
     return SS_OK;
   }
   return h->fail(SS_ERR_INVALID, "unknown debug buffer " + n);

@@ -494,6 +494,10 @@ int ss_destroy(ss_engine* h) {
   if (h->async_err_pinned) cudaFreeHost(h->async_err_pinned);
   if (h->pool.desc_pinned) cudaFreeHost(h->pool.desc_pinned);
   if (h->pool.desc_pinned2) cudaFreeHost(h->pool.desc_pinned2);
+  for (auto& e : h->pool.resample_events) {
+    cudaEventDestroy(e.e0);
+    cudaEventDestroy(e.e1);
+  }
   if (h->voc_unit_emb) cudaFree(h->voc_unit_emb);
   if (h->voc_cumsum) cudaFree(h->voc_cumsum);
   if (h->lengths_dev) cudaFree(h->lengths_dev);

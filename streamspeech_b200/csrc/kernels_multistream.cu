@@ -5,9 +5,10 @@
 // rows of the streams of a GROUP (streams whose step has the same geometry: same number of new rows / frames) into dense
 // [n * nA][C] activations, so every GEMM of the step is the ordinary linear() over n * nA rows; the kernels here are the
 // per-stream (ragged) parts: windows gathered from / rows scattered to the slots, relative-position attention of each stream's
-// rows over ITS OWN key / value cache, the chunk-causal depthwise conv over ITS OWN conv-input cache, fbank of each stream's new
-// frames, and the CTC arg-max / collapse per stream.  Arithmetic is that of the single-stream kernels (kernels_attn.cu
-// attn_row_kernel, kernels_misc.cu depthwise_bn_silu_kernel / argmax_rows_kernel / ctc_collapse_kernel, kernels_fbank.cu).
+// rows over ITS OWN key / value cache, the chunk-causal depthwise conv over ITS OWN conv-input cache, the 48 -> 16 kHz decimation
+// and fbank of each stream's new samples / frames, and the CTC arg-max / collapse per stream.  Arithmetic is that of the
+// single-stream kernels (kernels_attn.cu attn_row_kernel, kernels_misc.cu depthwise_bn_silu_kernel / argmax_rows_kernel /
+// ctc_collapse_kernel / resample_3to1_kernel, kernels_fbank.cu).
 #include <algorithm>
 
 #include "common.cuh"
@@ -273,6 +274,36 @@ __global__ void __launch_bounds__(256) ms_fbank_kernel(const float* __restrict__
   }
 }
 
+// ---- 48 -> 16 kHz decimation of the new samples of every stream (resample_3to1_kernel of kernels_misc.cu with a per-stream
+// descriptor): block = (256 outputs, stream b).  Same taps, same shared-memory window, same fmaf order over k and zeros outside
+// [0, n48), so every 16 kHz sample equals, bit for bit, what ss_resample_48k_to_16k produces from the same 48 kHz prefix.
+__global__ void __launch_bounds__(256) ms_resample_3to1_kernel(const float* __restrict__ a48_base, int64_t a48_stride, float* __restrict__ a16_base,
+                                                              int64_t a16_stride, const MsStream* __restrict__ S, const float* __restrict__ h,
+                                                              int taps, int width) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float hs[64];
+  __shared__ float xs[3 * 256 + 64];
+  const int tid = threadIdx.x;
+  const MsStream s = S[blockIdx.y];
+  if ((int)blockIdx.x * 256 >= s.n16_new) return;
+  if (tid < taps) hs[tid] = h[tid];
+  const float* x = a48_base + (int64_t)s.slot * a48_stride;
+  const int64_t ib = s.n16_done + (int64_t)blockIdx.x * 256;  // first output of this block
+  const int64_t base = 3 * ib - width;                         // first input sample the block touches
+  const int span = 3 * 255 + taps;                             // inputs touched by 256 outputs
+  for (int j = tid; j < span; j += 256) {
+    const int64_t p = base + j;
+    xs[j] = (p >= 0 && p < s.n48) ? x[p] : 0.f;
+  }
+  __syncthreads();
+  const int64_t i = ib + tid;
+  if (i >= s.n16_done + s.n16_new) return;
+  float acc = 0.f;
+  for (int k = 0; k < taps; ++k) acc = fmaf(hs[k], xs[3 * tid + k], acc);
+  a16_base[(int64_t)s.slot * a16_stride + i] = acc;
+}
+
 // arg-max of log_softmax with masks (argmax_rows_kernel) for the new rows of every stream: block = (row r, stream b, head),
 // logits row = (b * nA + r), columns [head * V, head * V + V); result -> am_base[(slot * 2 + head) * am_stride + a0 + r]
 __global__ void __launch_bounds__(256) ms_ctc_argmax_kernel(const float* __restrict__ logits, int ld, int V, const int* __restrict__ masked,
@@ -421,6 +452,13 @@ void ms_fbank(const float* audio_base, int64_t audio_stride, float* feat_base, i
   if (n <= 0 || max_new_frames <= 0) return;
   launch_pdl(ms_fbank_kernel, dim3(max_new_frames, n), dim3(256), 0, st, audio_base, audio_stride, feat_base, feat_stride, S, melT, window, cmvn_mean,
              cmvn_std);
+}
+
+void ms_resample_3to1(const float* a48_base, int64_t a48_stride, float* a16_base, int64_t a16_stride, const MsStream* S, int n, int max_new,
+                      const float* h, int taps, int width, cudaStream_t st) {
+  ++g_launches;
+  if (n <= 0 || max_new <= 0) return;
+  launch_pdl(ms_resample_3to1_kernel, dim3((max_new + 255) / 256, n), dim3(256), 0, st, a48_base, a48_stride, a16_base, a16_stride, S, h, taps, width);
 }
 
 void ms_ctc_argmax(const float* logits, int ld, int V, const int* masked, int n_masked, int64_t* am_base, int64_t am_stride, const MsStream* S, int n,

@@ -14,8 +14,10 @@ struct MsStream {
   int f_lo;          // first fbank frame the subsampler window of this step reads
   int frame0;        // fbank: first new frame
   int n_new_frames;  // fbank: number of new frames
-  int pad_;
+  int n16_new;       // 48 kHz pools: 16 kHz samples the resampler produces in this step (0 in 16 kHz pools)
   int64_t out_off;   // CTC collapse: int64 offset of this stream's packed output
+  int64_t n48;       // 48 kHz pools: 48 kHz samples pushed to the slot so far
+  int64_t n16_done;  // 48 kHz pools: first 16 kHz sample of this step (samples below it were produced by earlier steps)
 };
 
 void ms_gather_rows(const float* src_base, int64_t slot_stride, const MsStream* S, int n, int which /*0: rows from f_lo (limit F), 1: rows from a0 (limit T)*/,
@@ -29,6 +31,10 @@ void ms_depthwise(const float* gc, int64_t slot_stride, const float* w, const fl
                   int nA, int C, int k, int chunk, cudaStream_t st);
 void ms_fbank(const float* audio_base, int64_t audio_stride, float* feat_base, int64_t feat_stride, const MsStream* S, int n, int max_new_frames,
               const float* melT /*[257][80]*/, const float* window, const float* cmvn_mean, const float* cmvn_std, cudaStream_t st);
+// 48 -> 16 kHz decimation of every stream's new samples: a16_base[slot * a16_stride + i] for i in [n16_done, n16_done + n16_new) from
+// a48_base[slot * a48_stride + 0 .. n48) (resample_3to1 of kernels.h per stream; max_new = largest n16_new)
+void ms_resample_3to1(const float* a48_base, int64_t a48_stride, float* a16_base, int64_t a16_stride, const MsStream* S, int n, int max_new,
+                      const float* h, int taps, int width, cudaStream_t st);
 void ms_ctc_argmax(const float* logits, int ld, int V, const int* masked, int n_masked, int64_t* am_base, int64_t am_stride, const MsStream* S, int n,
                    int nA, int heads, cudaStream_t st);
 void ms_ctc_collapse(const int64_t* am_base, int64_t am_stride, const MsStream* S, int n, int heads, int blank, int pad, int64_t* out, cudaStream_t st);

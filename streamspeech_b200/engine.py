@@ -95,7 +95,9 @@ def load_library() -> ctypes.CDLL:
     lib.ss_resample_out_len.restype = i64
     lib.ss_resample_48k_to_16k.argtypes = [vp, vp, vp, i64, i64, i64, vp]
     lib.ss_pool_create.argtypes = [vp, i32, i32]
+    lib.ss_pool_create_rate.argtypes = [vp, i32, i32, i32]
     lib.ss_pool_reset.argtypes = [vp, i32]
+    lib.ss_pool_finish.argtypes = [vp, i32]
     lib.ss_pool_push_audio.argtypes = [vp, vp, i32, vp, i32]
     lib.ss_pool_info.argtypes = [vp, i32, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     lib.ss_pool_step.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp]
@@ -108,6 +110,7 @@ EXPORTED_SYMBOLS = [
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
+    "ss_pool_create_rate", "ss_pool_finish",
 ]
 
 
@@ -498,16 +501,28 @@ class Engine:
         return int(buf.value)
 
     # ------------------------------------------------------------------ multi-stream pool (ss_pool_*)
-    def pool_create(self, n_slots: int, max_seconds: int = 60):
-        self._check(self.lib.ss_pool_create(self._h, int(n_slots), int(max_seconds)))
+    def pool_create(self, n_slots: int, max_seconds: int = 60, sample_rate: int = 16000):
+        """sample_rate 16000 or 48000: the rate of the samples pool_push_audio takes (48 kHz is resampled per slot on the device)"""
+        self._check(self.lib.ss_pool_create_rate(self._h, int(n_slots), int(max_seconds), int(sample_rate)))
         self._pool_slots = int(n_slots)
         self._pool_out = None
 
     def pool_reset(self, slot: int):
         self._check(self.lib.ss_pool_reset(self._h, int(slot)))
 
+    def pool_finish(self, slot: int):
+        """the slot's source is closed: the next step produces the rest of its 16 kHz signal; pushes fail until pool_reset"""
+        self._check(self.lib.ss_pool_finish(self._h, int(slot)))
+
+    def pool_resample_time(self):
+        """(summed ms, launches, summed algorithmic bytes) of the pool's resample kernel since the last query (CUDA events on the
+        launching stream; enable with set_option('persistent_time', 1))"""
+        buf = (ctypes.c_double * 3)()
+        self._check(self.lib.ss_debug_copy(self._h, b"pool_resample_time", buf, ctypes.sizeof(buf)))
+        return float(buf[0]), int(buf[1]), float(buf[2])
+
     def pool_push_audio(self, slot: int, samples: torch.Tensor):
-        """samples: fp32 CPU tensor (contiguous); appended to the slot's device audio"""
+        """samples: fp32 CPU tensor (contiguous) at the pool's rate; appended to the slot's device audio"""
         assert samples.dtype == torch.float32 and not samples.is_cuda and samples.is_contiguous()
         self._check(self.lib.ss_pool_push_audio(self._h, self._stream(), int(slot), samples.data_ptr(), samples.numel()))
 

@@ -18,11 +18,15 @@ from streamspeech_b200.simuleval_compat import ReadAction, SpeechToTextAgent, Wr
 
 
 class StreamPool:
-    def __init__(self, engine: Engine, n_slots: int, max_seconds: int = 60, ctc_heads: int = 1):
+    """sample_rate: the rate of the pushed samples, 16000 or 48000 (the reference agent's default input; decimated to 16 kHz per slot
+    inside the batched step, with the single-stream agents' rule and arithmetic)"""
+
+    def __init__(self, engine: Engine, n_slots: int, max_seconds: int = 60, ctc_heads: int = 1, sample_rate: int = 16000):
         self.engine = engine
         self.n_slots = n_slots
         self.ctc_heads = ctc_heads
-        engine.pool_create(n_slots, max_seconds)
+        self.sample_rate = sample_rate
+        engine.pool_create(n_slots, max_seconds, sample_rate)
         self.free: List[int] = list(range(n_slots))[::-1]
         self.pending: Dict[int, bool] = {}       # slot -> has pushed samples since its last step
         self.results: Dict[int, dict] = {}       # slot -> result of the last step that included it
@@ -46,11 +50,14 @@ class StreamPool:
         self.pending.pop(slot, None)
         self.results.pop(slot, None)
 
-    def push(self, slot: int, samples: Sequence[float]):
-        """register new source samples of one stream (host -> device copy enqueued, nothing computed yet)"""
+    def push(self, slot: int, samples: Sequence[float], finished: bool = False):
+        """register new source samples of one stream (host -> device copy enqueued, nothing computed yet); finished: the
+        stream's source ends with these samples (a 48 kHz stream's last 16 kHz samples are produced by the next step)"""
         if len(samples):
             t = samples if isinstance(samples, torch.Tensor) else torch.tensor(samples, dtype=torch.float32)
             self.engine.pool_push_audio(slot, t.contiguous())
+        if finished:
+            self.engine.pool_finish(slot)
         self.pending[slot] = True
         self.results.pop(slot, None)
 
@@ -74,7 +81,8 @@ class StreamPool:
 
 class PooledASRAgent(SpeechToTextAgent):
     """StreamSpeechASRAgent (agent/speech_to_text.asr.streamspeech.agent.py:100-433) bound to a slot of a shared StreamPool:
-    same push() / pop() / policy() contract and text output; the tensor work of all agents of a round is one batched step."""
+    same push() / pop() / policy() contract and text output; the tensor work of all agents of a round is one batched step.
+    Segments must come at the pool's sample rate (ValueError otherwise)."""
 
     def __init__(self, pool: StreamPool, dictionary, args=None):
         self.pool = pool
@@ -92,9 +100,12 @@ class PooledASRAgent(SpeechToTextAgent):
     def push(self, source_segment, states=None):  # GenericAgent.push (SimulEval agents/agent.py:71-83) + device mirror of the new samples
         if states is None:
             states = self.states
+        rate = getattr(source_segment, "sample_rate", -1)  # SpeechSegment's default -1 = not stated: taken as the pool's rate
+        if rate > 0 and rate != self.pool.sample_rate:
+            raise ValueError(f"a {rate} Hz segment was pushed to a {self.pool.sample_rate} Hz stream pool")
         before = len(states.source)
         states.update_source(source_segment)
-        self.pool.push(self.slot, states.source[before:])
+        self.pool.push(self.slot, states.source[before:], finished=states.source_finished)
 
     def policy(self):
         r = self.pool.result(self.slot)
