@@ -194,7 +194,8 @@ int ss_vocoder_receptive_field(const ss_engine* h);
 /* ---- multi-stream pool: n concurrent utterances per handle, ONE batched streaming step (SURVEY.md §8 f2; BASELINE configs[3] = 256
  * concurrent ASR streams, 32 per GPU).  The reference is one utterance per agent process (agent/speech_to_text.asr.streamspeech.
  * agent.py:385-433).  Each stream owns a slot: device audio, fbank frames, per-layer K / V / conv-input caches, encoder rows and CTC
- * arg-max rows.  Results of every stream equal the single-stream entry points' (same arithmetic per stream; GEMMs see n x rows). */
+ * arg-max rows.  Results of every stream equal the single-stream entry points' (same arithmetic per stream; GEMMs see the rows of
+ * all n streams). */
 int ss_pool_create(ss_engine* h, int n_slots, int max_seconds);  /* 16 kHz sources: ss_pool_create_rate(h, n_slots, max_seconds, 16000) */
 /* Pool whose sources arrive at sample_rate = 16000 or 48000 Hz (anything else: SS_ERR_INVALID).  A 48 kHz pool keeps the pushed
  * samples in a second per-slot row of max_seconds * 48000 + 1200 samples; every ss_pool_step first extends each listed slot's 16 kHz
@@ -202,6 +203,11 @@ int ss_pool_create(ss_engine* h, int n_slots, int max_seconds);  /* 16 kHz sourc
  * [produced so far, ss_resample_out_len(n48, finished)), each bit-identical to ss_resample_48k_to_16k on the same 48 kHz prefix. */
 int ss_pool_create_rate(ss_engine* h, int n_slots, int max_seconds, int sample_rate);
 int ss_pool_reset(ss_engine* h, int slot);                       /* new utterance on this slot (clears the finished flag) */
+/* The slot's own latency: attention chunk and conv chunk of its streaming encoder, as ss_set_chunk sets them for the handle
+ * (attn_chunk > 0, conv_chunk > 0 and even; otherwise SS_ERR_INVALID).  (0, 0) = follow the handle's ss_set_chunk at step time,
+ * the default.  Slots of different latencies share every batched step and its one pass over the encoder weights.  SS_ERR_STATE
+ * while the slot holds samples (a stream keeps its latency for the whole utterance); the setting survives ss_pool_reset. */
+int ss_pool_set_chunk(ss_engine* h, int slot, int attn_chunk, int conv_chunk);
 /* append n samples at the pool's rate (host memory) to the slot's device audio: enqueue of one host->device copy.  The capacity
  * check counts samples at that rate.  SS_ERR_STATE after ss_pool_finish until ss_pool_reset */
 int ss_pool_push_audio(ss_engine* h, void* stream, int slot, const float* samples_host, int n);

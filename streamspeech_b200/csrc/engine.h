@@ -221,6 +221,7 @@ struct ss_engine {
     std::vector<int64_t> n_audio;                      // 16 kHz samples in `audio` (the fbank's input)
     std::vector<int64_t> n48;                          // 48 kHz pools: samples in `audio48`
     std::vector<char> finished;                        // ss_pool_finish: the slot's source is closed
+    std::vector<int> attn_chunk, conv_chunk;           // ss_pool_set_chunk: the slot's own chunk sizes (0, 0 = the handle's ss_set_chunk)
     std::vector<TimedLaunch> resample_events;          // option persistent_time: CUDA events around ms_resample_3to1 (bytes = 16 per output)
   } pool;
 

@@ -2,8 +2,8 @@
 //
 // Every stream owns a slot of the handle's stream pool (engine_pool.cu): audio, fbank frames, per-layer K / V / conv-input
 // caches, encoder output rows and CTC arg-max rows, all at a fixed per-slot stride.  A batched step concatenates the active
-// rows of the streams of a GROUP (streams whose step has the same geometry: same number of new rows / frames) into dense
-// [n * nA][C] activations, so every GEMM of the step is the ordinary linear() over n * nA rows; the kernels here are the
+// rows of ALL its streams into dense [sum nA][C] activations (stream b at rows row0 .. row0 + nA - 1 of its descriptor; streams
+// may differ in nA and in their chunk sizes), so every GEMM of the step is the ordinary linear() over sum nA rows; the kernels here are the
 // per-stream (ragged) parts: windows gathered from / rows scattered to the slots, relative-position attention of each stream's
 // rows over ITS OWN key / value cache, the chunk-causal depthwise conv over ITS OWN conv-input cache, the 48 -> 16 kHz decimation
 // and fbank of each stream's new samples / frames, and the CTC arg-max / collapse per stream.  Arithmetic is that of the
@@ -66,15 +66,17 @@ __global__ void ms_gather_rows_kernel(const float* __restrict__ src_base, int64_
     *reinterpret_cast<float4*>(d + c) = ok ? *reinterpret_cast<const float4*>(src + c) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-// dst_base[slot[b] * slot_stride + (a0[b] + r) * C + :] = src[b][r][:]   (up to three sources -> three slot buffers in one launch)
+// dst_base[slot[b] * slot_stride + (a0[b] + r) * C + :] = src[row0[b] + r][:], r < nA[b]   (up to three sources -> three slot
+// buffers in one launch)
 __global__ void ms_scatter_rows_kernel(const float* __restrict__ s0, const float* __restrict__ s1, const float* __restrict__ s2, int lds,
                                        float* __restrict__ d0, float* __restrict__ d1, float* __restrict__ d2, int64_t slot_stride,
-                                       const MsStream* __restrict__ S, int nA, int C) {
+                                       const MsStream* __restrict__ S, int C) {
   pdl_trigger();
   pdl_wait();
   const int b = blockIdx.y, r = blockIdx.x;
   const MsStream s = S[b];
-  const int64_t so = ((int64_t)b * nA + r) * lds;
+  if (r >= s.nA) return;
+  const int64_t so = ((int64_t)s.row0 + r) * lds;
   const int64_t dof = (int64_t)s.slot * slot_stride + (int64_t)(s.a0 + r) * C;
   for (int c = threadIdx.x * 4; c < C; c += blockDim.x * 4) {
     *reinterpret_cast<float4*>(d0 + dof + c) = *reinterpret_cast<const float4*>(s0 + so + c);
@@ -84,12 +86,13 @@ __global__ void ms_scatter_rows_kernel(const float* __restrict__ s0, const float
 }
 
 // Relative-position attention (attn_row_kernel<RELPOS> of kernels_attn.cu): CTA = (active row r, head h, stream b); keys 0 .. lim-1
-// of stream b's cache at kc / vc + slot * slot_stride (this layer's [Tcap][D] block), lim = end of the query's attention chunk.
+// of stream b's cache at kc / vc + slot * slot_stride (this layer's [Tcap][D] block), lim = end of the query's attention chunk
+// (the stream's own chunk size).  Query / output row row0[b] + r; CTAs with r >= nA[b] exit before any barrier.
 __global__ void __launch_bounds__(MS_NT) ms_relpos_attn_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ kc,
                                                                const float* __restrict__ vc, int64_t slot_stride, int D,
                                                                const float* __restrict__ pos, int Tpos, const float* __restrict__ bias_u,
                                                                const float* __restrict__ bias_v, float* __restrict__ out, int ldo,
-                                                               const MsStream* __restrict__ S, int nA, int chunk) {
+                                                               const MsStream* __restrict__ S) {
   pdl_trigger();
   pdl_wait();
   extern __shared__ __align__(16) float smem[];
@@ -99,10 +102,13 @@ __global__ void __launch_bounds__(MS_NT) ms_relpos_attn_kernel(const float* __re
   __shared__ float red[4];
   const int r = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const MsStream s = S[b];
+  if (r >= s.nA) return;
+  const int chunk = s.attn_chunk;
   const int i = s.a0 + r;
   const int lim = chunk > 0 ? min((i / chunk + 1) * chunk, s.T) : s.T;
   const int n = max(1, lim);
-  const float* qp = q + ((int64_t)b * nA + r) * ldq + h * HD;
+  const int64_t row = (int64_t)s.row0 + r;
+  const float* qp = q + row * ldq + h * HD;
   const float* kb = kc + (int64_t)s.slot * slot_stride + h * HD;
   const float* vb = vc + (int64_t)s.slot * slot_stride + h * HD;
   if (threadIdx.x < HD) {
@@ -141,18 +147,20 @@ __global__ void __launch_bounds__(MS_NT) ms_relpos_attn_kernel(const float* __re
   __syncthreads();
   if (threadIdx.x < HD) {
     const float t = (part[0][threadIdx.x] + part[1][threadIdx.x]) + (part[2][threadIdx.x] + part[3][threadIdx.x]);
-    out[((int64_t)b * nA + r) * ldo + h * HD + threadIdx.x] = t / sum;
+    out[row * ldo + h * HD + threadIdx.x] = t / sum;
   }
 }
 
-// depthwise chunk-causal conv + BN + SiLU over stream b's conv-input cache (depthwise_bn_silu_kernel of kernels_misc.cu)
+// depthwise chunk-causal conv + BN + SiLU over stream b's conv-input cache (depthwise_bn_silu_kernel of kernels_misc.cu), with the
+// stream's own conv chunk; output row row0[b] + r
 __global__ void ms_depthwise_kernel(const float* __restrict__ gc, int64_t slot_stride, const float* __restrict__ w, const float* __restrict__ scale,
-                                    const float* __restrict__ shift, float* __restrict__ y, int ldy, const MsStream* __restrict__ S, int nA, int C,
-                                    int k, int chunk) {
+                                    const float* __restrict__ shift, float* __restrict__ y, int ldy, const MsStream* __restrict__ S, int C, int k) {
   pdl_trigger();
   pdl_wait();
   const int b = blockIdx.y, r = blockIdx.x;
   const MsStream s = S[b];
+  if (r >= s.nA) return;
+  const int chunk = s.conv_chunk;
   const int t = s.a0 + r;
   const int half = (k - 1) >> 1;
   const int lim = chunk > 0 ? min(s.T, (t / chunk + 1) * chunk) : s.T;
@@ -172,7 +180,7 @@ __global__ void ms_depthwise_kernel(const float* __restrict__ gc, int64_t slot_s
       for (int jj = 0; jj < 8; ++jj) acc = fmaf(wv[jj], xv[jj], acc);
     }
     const float v = acc * scale[c] + shift[c];
-    y[((int64_t)b * nA + r) * ldy + c] = v / (1.0f + expf(-v));
+    y[((int64_t)s.row0 + r) * ldy + c] = v / (1.0f + expf(-v));
   }
 }
 
@@ -305,10 +313,10 @@ __global__ void __launch_bounds__(256) ms_resample_3to1_kernel(const float* __re
 }
 
 // arg-max of log_softmax with masks (argmax_rows_kernel) for the new rows of every stream: block = (row r, stream b, head),
-// logits row = (b * nA + r), columns [head * V, head * V + V); result -> am_base[(slot * 2 + head) * am_stride + a0 + r]
+// logits row = (row0 + r), r < nA, columns [head * V, head * V + V); result -> am_base[(slot * 2 + head) * am_stride + a0 + r]
 __global__ void __launch_bounds__(256) ms_ctc_argmax_kernel(const float* __restrict__ logits, int ld, int V, const int* __restrict__ masked,
                                                             int n_masked, int64_t* __restrict__ am_base, int64_t am_stride,
-                                                            const MsStream* __restrict__ S, int nA) {
+                                                            const MsStream* __restrict__ S) {
   pdl_trigger();
   pdl_wait();
   __shared__ float red[32];
@@ -317,7 +325,8 @@ __global__ void __launch_bounds__(256) ms_ctc_argmax_kernel(const float* __restr
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int r = blockIdx.x, b = blockIdx.y, head = blockIdx.z;
   const MsStream s = S[b];
-  const float* x = logits + ((int64_t)b * nA + r) * ld + head * V;
+  if (r >= s.nA) return;
+  const float* x = logits + ((int64_t)s.row0 + r) * ld + head * V;
   float mx = -INFINITY;
   for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
   mx = warp_max(mx);
@@ -421,29 +430,28 @@ void ms_gather_rows(const float* src_base, int64_t slot_stride, const MsStream* 
 }
 
 void ms_scatter_rows(const float* s0, const float* s1, const float* s2, int lds, float* d0, float* d1, float* d2, int64_t slot_stride, const MsStream* S,
-                     int n, int nA, int C, cudaStream_t st) {
+                     int n, int max_nA, int C, cudaStream_t st) {
   ++g_launches;
-  if (n * nA <= 0) return;
-  launch_pdl(ms_scatter_rows_kernel, dim3(nA, n), dim3(64), 0, st, s0, s1, s2, lds, d0, d1, d2, slot_stride, S, nA, C);
+  if (n * max_nA <= 0) return;
+  launch_pdl(ms_scatter_rows_kernel, dim3(max_nA, n), dim3(64), 0, st, s0, s1, s2, lds, d0, d1, d2, slot_stride, S, C);
 }
 
 void ms_relpos_attention(const float* q, int ldq, const float* kc, const float* vc, int64_t slot_stride, int D, const float* pos, int Tpos,
-                         const float* bias_u, const float* bias_v, float* out, int ldo, const MsStream* S, int n, int nA, int H, int chunk,
-                         int Tmax, cudaStream_t st) {
+                         const float* bias_u, const float* bias_v, float* out, int ldo, const MsStream* S, int n, int max_nA, int H, int Tmax,
+                         cudaStream_t st) {
   ++g_launches;
-  if (n * nA <= 0) return;
+  if (n * max_nA <= 0) return;
   const size_t smem = (size_t)((Tmax + 3) & ~3) * sizeof(float);
   if (smem > 40 * 1024 && first_time_on_device((const void*)ms_relpos_attn_kernel))
     cudaFuncSetAttribute(ms_relpos_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-  launch_pdl(ms_relpos_attn_kernel, dim3(nA, H, n), dim3(MS_NT), smem, st, q, ldq, kc, vc, slot_stride, D, pos, Tpos, bias_u, bias_v, out, ldo, S, nA,
-             chunk);
+  launch_pdl(ms_relpos_attn_kernel, dim3(max_nA, H, n), dim3(MS_NT), smem, st, q, ldq, kc, vc, slot_stride, D, pos, Tpos, bias_u, bias_v, out, ldo, S);
 }
 
 void ms_depthwise(const float* gc, int64_t slot_stride, const float* w, const float* scale, const float* shift, float* y, int ldy, const MsStream* S, int n,
-                  int nA, int C, int k, int chunk, cudaStream_t st) {
+                  int max_nA, int C, int k, cudaStream_t st) {
   ++g_launches;
-  if (n * nA <= 0) return;
-  launch_pdl(ms_depthwise_kernel, dim3(nA, n), dim3(256), 0, st, gc, slot_stride, w, scale, shift, y, ldy, S, nA, C, k, chunk);
+  if (n * max_nA <= 0) return;
+  launch_pdl(ms_depthwise_kernel, dim3(max_nA, n), dim3(256), 0, st, gc, slot_stride, w, scale, shift, y, ldy, S, C, k);
 }
 
 void ms_fbank(const float* audio_base, int64_t audio_stride, float* feat_base, int64_t feat_stride, const MsStream* S, int n, int max_new_frames,
@@ -462,10 +470,10 @@ void ms_resample_3to1(const float* a48_base, int64_t a48_stride, float* a16_base
 }
 
 void ms_ctc_argmax(const float* logits, int ld, int V, const int* masked, int n_masked, int64_t* am_base, int64_t am_stride, const MsStream* S, int n,
-                   int nA, int heads, cudaStream_t st) {
+                   int max_nA, int heads, cudaStream_t st) {
   ++g_launches;
-  if (n * nA <= 0) return;
-  launch_pdl(ms_ctc_argmax_kernel, dim3(nA, n, heads), dim3(256), 0, st, logits, ld, V, masked, n_masked, am_base, am_stride, S, nA);
+  if (n * max_nA <= 0) return;
+  launch_pdl(ms_ctc_argmax_kernel, dim3(max_nA, n, heads), dim3(256), 0, st, logits, ld, V, masked, n_masked, am_base, am_stride, S);
 }
 
 void ms_ctc_collapse(const int64_t* am_base, int64_t am_stride, const MsStream* S, int n, int heads, int blank, int pad, int64_t* out, cudaStream_t st) {

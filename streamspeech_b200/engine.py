@@ -98,6 +98,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_pool_create_rate.argtypes = [vp, i32, i32, i32]
     lib.ss_pool_reset.argtypes = [vp, i32]
     lib.ss_pool_finish.argtypes = [vp, i32]
+    lib.ss_pool_set_chunk.argtypes = [vp, i32, i32, i32]
     lib.ss_pool_push_audio.argtypes = [vp, vp, i32, vp, i32]
     lib.ss_pool_info.argtypes = [vp, i32, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     lib.ss_pool_step.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp]
@@ -110,7 +111,7 @@ EXPORTED_SYMBOLS = [
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
-    "ss_pool_create_rate", "ss_pool_finish",
+    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk",
 ]
 
 
@@ -509,6 +510,11 @@ class Engine:
 
     def pool_reset(self, slot: int):
         self._check(self.lib.ss_pool_reset(self._h, int(slot)))
+
+    def pool_set_chunk(self, slot: int, attn_chunk: int, conv_chunk: int):
+        """the slot's own latency (attention chunk, even conv chunk, as set_chunk); (0, 0) = follow the handle's set_chunk.  Only
+        while the slot holds no samples (after pool_reset); the setting survives pool_reset"""
+        self._check(self.lib.ss_pool_set_chunk(self._h, int(slot), int(attn_chunk), int(conv_chunk)))
 
     def pool_finish(self, slot: int):
         """the slot's source is closed: the next step produces the rest of its 16 kHz signal; pushes fail until pool_reset"""

@@ -41,9 +41,18 @@ class StreamPool:
         return slot
 
     def release(self, slot: int):
+        """give the slot back; it follows the handle's chunk setting again, so whoever acquires it next starts at the default
+        latency"""
+        self.engine.pool_reset(slot)
+        self.engine.pool_set_chunk(slot, 0, 0)
         self.pending.pop(slot, None)
         self.results.pop(slot, None)
         self.free.append(slot)
+
+    def set_chunk(self, slot: int, attn_chunk: int, conv_chunk: int):
+        """the slot's own latency (encoder attention chunk, even conv chunk; (0, 0) = follow the engine's set_chunk).  Streams of
+        different latencies share every batched step.  Only between utterances (the slot holds no samples); it survives reset()."""
+        self.engine.pool_set_chunk(slot, attn_chunk, conv_chunk)
 
     def reset(self, slot: int):
         self.engine.pool_reset(slot)
@@ -82,12 +91,17 @@ class StreamPool:
 class PooledASRAgent(SpeechToTextAgent):
     """StreamSpeechASRAgent (agent/speech_to_text.asr.streamspeech.agent.py:100-433) bound to a slot of a shared StreamPool:
     same push() / pop() / policy() contract and text output; the tensor work of all agents of a round is one batched step.
-    Segments must come at the pool's sample rate (ValueError otherwise)."""
+    Segments must come at the pool's sample rate (ValueError otherwise).  With args, the slot runs at args.source_segment_size
+    like the single agent (chunk c = seg // 40, conv chunk min(c, 16), agent:361-375), whatever latency the other slots of the pool
+    use; without args it follows the engine's set_chunk."""
 
     def __init__(self, pool: StreamPool, dictionary, args=None):
         self.pool = pool
         self.dictionary = dictionary
         self.slot = pool.acquire()
+        if args is not None and getattr(args, "source_segment_size", None):
+            chunk_size = args.source_segment_size // 40
+            pool.set_chunk(self.slot, chunk_size, min(chunk_size, 16))  # once: it survives the reset between utterances
         super().__init__(args)
         self.trace = {}
 
