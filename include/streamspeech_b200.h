@@ -138,6 +138,17 @@ int ss_ctc_greedy_pair(ss_engine* h, void* stream, const float* enc_dev, int row
 int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* prefix_host, int n_prefix,
                  int max_new_tokens, int max_len_b, int64_t* tokens_out_host, int max_out, int* n_out,
                  float* feats_out_dev);
+/* Greedy MT search (beam 1, no prefix, max_len = min(max_len_b, max_mt_positions - 1)) for B independent samples.
+ * enc_dev: [B][T_stride][enc_dim] (e.g. ss_encoder_forward's padded output); T_host[b]: sample b's unpadded rows, 1 <= T_b <= T_stride.
+ * tokens_out_host: [B][max_out], hypothesis without eos; n_out_host[b]: its length.  Each row equals ss_mt_greedy on enc_b[:T_b].
+ * Up to 32 samples are decoded together in one persistent kernel (larger B: consecutive groups of 32), reading the MT weights
+ * once per step for all of them, with its own caches: the single-stream MT state of the handle is not touched.  Where that
+ * kernel cannot run (option persistent_mt = 0, an unsupported shape, a refused cooperative launch) and for groups of fewer
+ * than 2 samples (option mt_batch_min_rows), samples are decoded one by one through ss_mt_greedy; that path leaves the
+ * single-stream cross K / V cache invalid, so the next streaming call projects all its rows again.
+ * Errors: SS_ERR_INVALID for B <= 0, a T_b outside [1, T_stride] or a null pointer; SS_ERR_CAPACITY when max_len > max_out. */
+int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int max_len_b,
+                       int64_t* tokens_out_host, int max_out, int32_t* n_out_host);
 /* Streaming hint for the NEXT ss_mt_greedy / ss_mt_features call: rows [0, rows) of the encoder output passed to it are
  * final, i.e. bit-identical in every later call with the same buffer until ss_encoder_stream_reset (ss_encoder_stream_step
  * reports that count as T_final).  Their cross-attention keys / values are then projected once instead of on every call.

@@ -204,6 +204,13 @@ struct ss_engine {
   int persistent_mt_v2 = 1;                    // single-token kernel with 6 grid barriers per layer (head-group partial projections)
   float* mt_part = nullptr;                    // [9][mt_dim] scratch of that kernel (per-head partials + FFN delta)
   int persistent_mt_prefix = 1;                // ... and the forced-prefix pass (M <= 64 rows) as one cooperative kernel
+  // batched greedy search (ss_mt_greedy_batch): caches of its own, so that a streaming agent's MT state on the handle survives it
+  float* mtb_self_kv = nullptr;                // K then V: 2 x [mt_layers][MT_BATCH_MAX_ROWS][mtb_tok_ld][mt_dim]
+  int mtb_tok_ld = 0;
+  float* mtb_cross_kv = nullptr;               // [mt_layers][MT_BATCH_MAX_ROWS][mtb_cross_cap][2 * mt_dim]
+  int mtb_cross_cap = 0;
+  int64_t* mtb_tok_pinned = nullptr;           // [MT_BATCH_MAX_ROWS][16] tokens of one burst
+  int mt_batch_min_rows = 2;                   // groups with fewer rows decode per sample on the single-token kernel (faster at B = 1)
   ss::PersistLayer* persist_layers = nullptr;  // [enc_layers] device copy of the per-layer pointer table
   int* lengths_dev = nullptr;     // [Bcap]
   int lengths_cap = 0;

@@ -337,6 +337,112 @@ DecScratch dec_scratch(ss_engine* h, int n, int dim, int ffn) {
   return s;
 }
 
+// device buffers of the batched greedy search, grown on demand: self K / V for tok_ld positions, cross K / V for Tmax rows per sample
+int ensure_mt_batch(ss_engine* h, int tok_ld, int Tmax) {
+  const ss_config& c = h->cfg;
+  const size_t R = MT_BATCH_MAX_ROWS;
+  if (tok_ld > h->mtb_tok_ld || Tmax > h->mtb_cross_cap) cudaDeviceSynchronize();  // earlier launches may still read the old buffers
+  if (tok_ld > h->mtb_tok_ld) {
+    if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);
+    h->mtb_self_kv = nullptr;
+    h->mtb_tok_ld = 0;
+    if (cudaMalloc((void**)&h->mtb_self_kv, (size_t)2 * c.mt_layers * R * tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
+      h->mtb_self_kv = nullptr;
+      return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt self kv) failed");
+    }
+    h->mtb_tok_ld = tok_ld;
+  }
+  if (Tmax > h->mtb_cross_cap) {
+    const int cap = std::max(Tmax + Tmax / 2, 512);
+    if (h->mtb_cross_kv) cudaFree(h->mtb_cross_kv);
+    h->mtb_cross_kv = nullptr;
+    h->mtb_cross_cap = 0;
+    if (cudaMalloc((void**)&h->mtb_cross_kv, (size_t)c.mt_layers * R * cap * 2 * c.mt_dim * sizeof(float)) != cudaSuccess) {
+      h->mtb_cross_kv = nullptr;
+      return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt cross kv) failed");
+    }
+    h->mtb_cross_cap = cap;
+  }
+  if (!h->mtb_tok_pinned && cudaHostAlloc((void**)&h->mtb_tok_pinned, R * 16 * sizeof(int64_t), cudaHostAllocDefault) != cudaSuccess) {
+    h->mtb_tok_pinned = nullptr;
+    return h->fail(SS_ERR_CUDA, "cudaHostAlloc(batched mt tokens) failed");
+  }
+  return SS_OK;
+}
+
+// Greedy search of samples g0 .. g0 + Bg - 1 (Bg <= MT_BATCH_MAX_ROWS) on mt_decode_batch_kernel.  Returns SS_OK, an error code
+// (reported), or -1 when the first cooperative launch was refused (nothing written to the outputs yet: the caller falls back).
+int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, int Bg, int T_stride, const int32_t* T_host, int max_len,
+                   int64_t* tokens_out_host, int max_out, int32_t* n_out_host) {
+  const ss_config& c = h->cfg;
+  const int dim = c.mt_dim;
+  const size_t R = MT_BATCH_MAX_ROWS;
+  int Tmax = 0;
+  for (int b = 0; b < Bg; ++b) Tmax = std::max(Tmax, (int)T_host[g0 + b]);
+  int rc = ensure_mt_batch(h, max_len + 2, Tmax);
+  if (rc) return rc;
+  const int ld = h->mtb_tok_ld;
+  // cross K / V: the same projection call as mt_begin with the sample's own row count (the GEMM routing depends on M)
+  for (int b = 0; b < Bg; ++b)
+    for (int l = 0; l < c.mt_layers; ++l)
+      linear(enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, c.enc_dim, T_host[g0 + b], h->mt[l].ckv,
+             ep_out(h->mtb_cross_kv + ((size_t)l * R + b) * h->mtb_cross_cap * 2 * dim, 2 * dim), st);
+  const size_t floats = (size_t)Bg * (dim * 11 + c.mt_ffn + c.tgt_vocab);
+  if (!ws_begin(h, floats * sizeof(float) + (size_t)Bg * ld * sizeof(int64_t) + (size_t)Bg * 2 * sizeof(int) + 16 * 256))
+    return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  MtBatchParams P;
+  P.n_layers = c.mt_layers; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
+  P.rows = Bg; P.tok_ld = ld; P.cross_cap = h->mtb_cross_cap;
+  P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
+  P.self_k = h->mtb_self_kv; P.self_v = h->mtb_self_kv + (size_t)c.mt_layers * R * ld * dim; P.cross_kv = h->mtb_cross_kv;
+  P.q = h->ws.f32((size_t)Bg * dim); P.part = h->ws.f32((size_t)Bg * 8 * dim); P.delta = h->ws.f32((size_t)Bg * dim);
+  P.hid = h->ws.f32((size_t)Bg * c.mt_ffn); P.logits = h->ws.f32((size_t)Bg * c.tgt_vocab);
+  P.tok = (int64_t*)h->ws.raw((size_t)Bg * ld * sizeof(int64_t));
+  int* ints = (int*)h->ws.raw((size_t)Bg * 2 * sizeof(int));  // [fin | cross_len]
+  if (!P.q || !P.part || !P.delta || !P.hid || !P.logits || !P.tok || !ints) return h->fail(SS_ERR_CUDA, "workspace too small");
+  P.fin = ints;
+  P.cross_len = ints + Bg;
+  std::vector<int64_t> tok0((size_t)Bg * ld, c.eos);  // column 0 = eos (the decoder's bos); the kernel writes the rest
+  std::vector<int> ints0(2 * Bg, 0);
+  for (int b = 0; b < Bg; ++b) ints0[Bg + b] = T_host[g0 + b];
+  cudaMemcpyAsync(P.tok, tok0.data(), tok0.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(ints, ints0.data(), ints0.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+  cudaStreamSynchronize(st);  // (host vectors)
+  for (int b = 0; b < Bg; ++b) n_out_host[g0 + b] = 0;
+  std::vector<char> done(Bg, 0);
+  int active = Bg;
+  constexpr int kBurst = 16;  // steps per launch, as ss_mt_greedy; the host reads the tokens back once per burst
+  for (int step = 0; step < max_len && active > 0; step += kBurst) {  // step max_len is the forced eos: no work
+    const int cnt = std::min(kBurst, max_len - step);
+    if (mt_decode_batch(P, h->mt_persist_layers, step, cnt, h->persist_bar, &h->persist_bar_target, st) != 0) {
+      cudaGetLastError();
+      if (step == 0) return -1;
+      return h->fail(SS_ERR_CUDA, "cooperative launch of the batched MT kernel was refused");
+    }
+    cudaMemcpy2DAsync(h->mtb_tok_pinned, cnt * sizeof(int64_t), P.tok + step + 1, ld * sizeof(int64_t), cnt * sizeof(int64_t), Bg,
+                      cudaMemcpyDeviceToHost, st);
+    if (h->async_err_pinned) cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_mt_greedy_batch: ") + cudaGetErrorString(cudaGetLastError()));
+    if (h->async_err_pinned && *h->async_err_pinned) {
+      const unsigned f = *h->async_err_pinned;
+      *h->async_err_pinned = 0;
+      return report_async_error(h, f, "ss_mt_greedy_batch");
+    }
+    for (int b = 0; b < Bg; ++b) {
+      for (int i = 0; i < cnt && !done[b]; ++i) {
+        const int64_t next = h->mtb_tok_pinned[(size_t)b * cnt + i];
+        if (next == c.eos) {
+          done[b] = 1;
+          --active;
+        } else {
+          tokens_out_host[(size_t)(g0 + b) * max_out + n_out_host[g0 + b]++] = next;
+        }
+      }
+    }
+  }
+  return SS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -722,10 +828,12 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
   if (rc) return rc;
   const int dim = c.mt_dim;
   const int nmax = std::max(start + 1, 1);
-  if (!ws_begin(h, ((size_t)nmax * (dim * 7 + c.mt_ffn) + c.tgt_vocab + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  const size_t feat_floats = feats_out_dev ? 0 : (size_t)(max_len + 2) * dim;  // no caller buffer: features go to scratch
+  if (!ws_begin(h, ((size_t)nmax * (dim * 7 + c.mt_ffn) + c.tgt_vocab + feat_floats + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
   DecScratch s = dec_scratch(h, nmax, dim, c.mt_ffn);
   float* x = h->ws.f32((size_t)nmax * dim);
   float* logits = h->ws.f32(c.tgt_vocab);
+  if (!feats_out_dev) feats_out_dev = h->ws.f32(feat_floats);
   Linear outp;
   outp.w = h->mt_emb; outp.b = nullptr; outp.N = c.tgt_vocab; outp.K = dim;
   // tokens buffer = [eos, prefix...]
@@ -839,6 +947,53 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
   }
   *n_out = n_tok;
   return check_launch(h, "ss_mt_greedy");
+}
+
+int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int max_len_b,
+                       int64_t* tokens_out_host, int max_out, int32_t* n_out_host) {
+  if (h) route_from(h);
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || T_stride <= 0 || !enc_dev || !T_host || !tokens_out_host || !n_out_host)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_mt_greedy_batch");
+  int Tmax = 0;
+  for (int b = 0; b < B; ++b) {
+    if (T_host[b] < 1 || T_host[b] > T_stride) return h->fail(SS_ERR_INVALID, "ss_mt_greedy_batch: sample length outside [1, T_stride]");
+    Tmax = std::max(Tmax, (int)T_host[b]);
+  }
+  const int max_len = std::min(max_len_b, c.max_mt_positions - 1);
+  if (max_len < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
+  if (max_len + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
+  cudaStream_t st = S(stream);
+  // the batched kernel reproduces the rows of the 6-barrier single-token kernel: it runs where ss_mt_greedy would run that one
+  const bool batched = h->persistent_mt && h->persistent_mt_v2 && h->mt_part && h->persist_bar && c.mt_heads == 8 &&
+                       mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, Tmax);
+  for (int g0 = 0; g0 < B; g0 += MT_BATCH_MAX_ROWS) {
+    const int Bg = std::min(MT_BATCH_MAX_ROWS, B - g0);
+    if (batched && Bg >= h->mt_batch_min_rows) {
+      const int rc = mt_batch_group(h, st, enc_dev, g0, Bg, T_stride, T_host, max_len, tokens_out_host, max_out, n_out_host);
+      if (rc != -1) {
+        if (rc) return rc;
+        continue;
+      }
+    }
+    // sample by sample on ss_mt_greedy's path.  It uses the single-stream MT buffers, so their cross K / V cache is marked
+    // invalid afterwards (a streaming call on this handle then projects every row again) and a pending stable-rows hint is kept.
+    const int hint = h->mt_stable_hint;
+    h->mt_stable_hint = 0;
+    int rc = SS_OK;
+    for (int b = g0; b < g0 + Bg && rc == SS_OK; ++b) {
+      int n = 0;
+      rc = ss_mt_greedy(h, stream, enc_dev + (size_t)b * T_stride * c.enc_dim, T_host[b], nullptr, 0, -1, max_len_b,
+                        tokens_out_host + (size_t)b * max_out, max_out, &n, nullptr);
+      n_out_host[b] = n;
+    }
+    h->mt_cross_enc = nullptr;
+    h->mt_cross_final = 0;
+    h->mt_stable_hint = hint;
+    if (rc) return rc;
+  }
+  return check_launch(h, "ss_mt_greedy_batch");
 }
 
 int ss_mt_incremental_reset(ss_engine* h) {
@@ -1309,6 +1464,7 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
   else if (n == "persistent_mt") h->persistent_mt = value;
   else if (n == "persistent_mt_prefix") h->persistent_mt_prefix = value;
   else if (n == "persistent_mt_v2") h->persistent_mt_v2 = value;
+  else if (n == "mt_batch_min_rows") h->mt_batch_min_rows = value;
   else if (n == "persistent_prefetch") h->persistent_prefetch = value;
   else if (n == "persistent_time") h->persistent_time = value;
   else if (n == "persistent_barrier") {

@@ -490,6 +490,9 @@ int ss_destroy(ss_engine* h) {
   ss::umma2_cache_destroy(h->umma2_cache);
   if (h->ws.base) cudaFree(h->ws.base);
   if (h->mt_cross_kv) cudaFree(h->mt_cross_kv);
+  if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);
+  if (h->mtb_cross_kv) cudaFree(h->mtb_cross_kv);
+  if (h->mtb_tok_pinned) cudaFreeHost(h->mtb_tok_pinned);
   if (h->mt_next_pinned) cudaFreeHost(h->mt_next_pinned);
   if (h->async_err_pinned) cudaFreeHost(h->async_err_pinned);
   if (h->pool.desc_pinned) cudaFreeHost(h->pool.desc_pinned);

@@ -29,6 +29,24 @@ __device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned& target) {
   }
   __syncthreads();
 }
+// split form of the grid barrier: arrive publishes this CTA's writes; everything issued between arrive and wait (the next phase's
+// weight, bias and LayerNorm-parameter loads: they do not depend on the phase that just ended) flies while the other CTAs arrive
+__device__ __forceinline__ void grid_arrive(unsigned* ctr, unsigned& target) {
+  __syncthreads();
+  target += gridDim.x;
+  if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
+}
+__device__ __forceinline__ void grid_wait(unsigned* ctr, unsigned target) {
+  if (threadIdx.x == 0) {
+    unsigned v, spins = 0;
+    do {
+      asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+    } while ((int)(v - target) < 0 && ++spins < (1u << 20));
+    if ((int)(v - target) < 0) atomicExch(ctr + SS_BAR_ERR_WORD, 1u);
+    asm volatile("fence.acq_rel.gpu;" ::: "memory");
+  }
+  __syncthreads();
+}
 #endif
 
 struct PersistLayer {  // device pointers of one Conformer layer (fp32, layouts as in engine.h ConformerLayerW)
@@ -82,6 +100,26 @@ bool mt_decode_persistent_supported(int dim, int ffn, int heads, int vocab, int 
 // enqueue `nsteps` greedy steps starting with the token at position step0; returns 0, or < 0 if the launch was refused
 int mt_decode_persistent(const MtDecodeParams& P, const MtLayerP* layers_dev, int step0, int nsteps, int max_len, int T,
                          unsigned* barrier_counter_dev, unsigned* barrier_target_host, cudaStream_t st);
+
+// ---- MT decoder, greedy search of up to MT_BATCH_MAX_ROWS independent samples per launch (kernels_persist_mtb.cu)
+#define MT_BATCH_MAX_ROWS 32
+struct MtBatchParams {
+  int n_layers, vocab, pad, eos;
+  int rows;                                 // rows of this launch (<= MT_BATCH_MAX_ROWS)
+  int tok_ld;                               // row stride of tok and of the self-attention cache (> the last step fed)
+  int cross_cap;                            // rows per sample in cross_kv
+  const float *emb, *pos, *out_g, *out_b;   // as MtDecodeParams
+  float *self_k, *self_v;                   // [layers][MT_BATCH_MAX_ROWS][tok_ld][dim]
+  const float* cross_kv;                    // [layers][MT_BATCH_MAX_ROWS][cross_cap][2 * dim] (K | V per encoder row)
+  const int* cross_len;                     // [rows] encoder rows of each sample
+  int64_t* tok;                             // [rows][tok_ld]: tok[b][s] is fed at step s, the arg-max goes to tok[b][s + 1]
+  int* fin;                                 // [rows]: set once the row produced eos; finished rows are skipped
+  float *q, *part, *delta, *hid, *logits;   // scratch per row: dim, 8 x dim, dim, ffn, vocab floats
+};
+// enqueue steps step0 .. step0 + nsteps - 1 (all < max_len: the forced-eos step needs no work) for every unfinished row;
+// returns 0, or < 0 if the launch was refused
+int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step0, int nsteps, unsigned* barrier_counter_dev,
+                    unsigned* barrier_target_host, cudaStream_t st);
 
 // ---- MT decoder, prefix pass over M <= 64 rows (kernels_persist_mtp.cu): fills self-attention cache rows 0 .. M-1 and feature
 // rows 0 .. M-1 from P.tok[0 .. M-1]; P.x / P.q / P.attn hold M x dim floats, P.hid M x ffn

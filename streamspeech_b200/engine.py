@@ -72,6 +72,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_ctc_greedy_rows.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp]
     lib.ss_ctc_greedy_pair.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
     lib.ss_mt_greedy.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp, i32, ctypes.POINTER(i32), vp]
+    lib.ss_mt_greedy_batch.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, i32, vp]
     lib.ss_mt_stable_rows.argtypes = [vp, i32]
     lib.ss_mt_incremental_reset.argtypes = [vp]
     lib.ss_mt_greedy_incremental.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp, i32, ctypes.POINTER(i32)]
@@ -111,7 +112,7 @@ EXPORTED_SYMBOLS = [
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
-    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk",
+    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch",
 ]
 
 
@@ -390,6 +391,20 @@ class Engine:
                                           int(max_len_b), out, cap, ctypes.byref(n_out), feats.data_ptr()))
         n = n_out.value
         return [int(out[i]) for i in range(n)], feats[: n + 1]
+
+    def mt_greedy_batch(self, enc: torch.Tensor, enc_lengths: Sequence[int], max_len_b: int) -> List[List[int]]:
+        """Greedy MT search of every sample of a padded encoder batch enc [B, T, C] (ss_mt_greedy_batch): sample b uses its
+        first enc_lengths[b] rows.  Returns the hypotheses without eos; each equals mt_greedy(enc[b, :T_b], None, -1, max_len_b)."""
+        assert enc.is_cuda and enc.is_contiguous() and enc.dim() == 3
+        B, T = int(enc.shape[0]), int(enc.shape[1])
+        if len(enc_lengths) != B:
+            raise EngineError(f"{len(enc_lengths)} lengths for a batch of {B}")
+        lens = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in enc_lengths])
+        cap = self.max_mt_positions
+        out = (ctypes.c_int64 * (max(B, 1) * cap))()
+        n_out = (ctypes.c_int32 * max(B, 1))()
+        self._check(self.lib.ss_mt_greedy_batch(self._h, self._stream(), enc.data_ptr(), B, T, lens, int(max_len_b), out, cap, n_out))
+        return [[int(out[b * cap + i]) for i in range(n_out[b])] for b in range(B)]
 
     def mt_incremental_reset(self):
         self._check(self.lib.ss_mt_incremental_reset(self._h))

@@ -6,7 +6,7 @@ Drop-in for the reference's `CTCMultiDecoderSequenceGenerator` as `fairseq-gener
 
     batched padded encoder (offline model: chunk_size None)                       ss_encoder_forward(B, lengths)
     ASR / ST CTC prints over all T rows of every sample (:206-246)                ss_ctc_greedy
-    MT greedy search per sample, max_len = max_len_b_mt (:251-260)                ss_mt_greedy
+    MT greedy search of the batch, max_len = max_len_b_mt (:251-260)              ss_mt_greedy_batch
     prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum (:262-271) host
     mt_decoder(features_only) -> T2U encoder -> CTC unit decoder (:287-330)       ss_mt_features, ss_t2u_unit_decode
 
@@ -53,18 +53,19 @@ class OfflineS2STGenerator:
         T = enc.shape[1]
         out_len = [eng.encoder_out_frames(n) for n in lengths]
         results: List[Dict[str, object]] = []
-        hyps: List[List[int]] = []
         for b in range(B):
             eb = enc[b].contiguous()
             am = torch.zeros(T, dtype=torch.int64, device=eb.device)
             asr, _ = eng.ctc_greedy_rows(0, eb, 0, am)       # padded frames are NOT trimmed (ctc_decoder.py:60-63)
             st, _ = eng.ctc_greedy_rows(1, eb, 0, am)
-            if forced_mt is not None:
-                toks = list(forced_mt[b])
-            else:
-                toks, _ = eng.mt_greedy(eb[: out_len[b]].contiguous(), None, -1, max_len_b=self.max_len_b_mt)
-            hyps.append(toks)
-            results.append({"asr_tokens": asr, "st_tokens": st, "mt_tokens": toks})
+            results.append({"asr_tokens": asr, "st_tokens": st})
+        hyps: List[List[int]]
+        if forced_mt is not None:
+            hyps = [list(h) for h in forced_mt]
+        else:
+            hyps = eng.mt_greedy_batch(enc, out_len, self.max_len_b_mt)  # all samples in one search
+        for b in range(B):
+            results[b]["mt_tokens"] = hyps[b]
         max_tgt_len = max(len(h) for h in hyps) + 1  # hypothesis + eos (:262)
         try:
             for b in range(B):
