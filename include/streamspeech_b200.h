@@ -252,15 +252,14 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
 /* engine options: "umma_vocoder" / "umma_linear" = 0 (fp32 CUDA cores), 12 or 13 (wgmma kernel, 2 or 3 bf16 pieces per operand); "umma_min_rows" / "umma_min_channels": smaller GEMMs / convs stay on
  * the fp32 kernels; "umma2_cache_clear": drop the packed weight copies;
  * "persistent_encoder" = 1 (default): ss_encoder_stream_step runs the layer stack as one cooperative kernel when the
- * shape fits, 0: one kernel per op; "persistent_barrier" = 1 (default): that kernel's own counter barrier instead of
- * cooperative-groups grid.sync(); "vocoder_streams" = 1 (default): the three parallel resblocks of a vocoder stage run
+ * shape fits, 0: one kernel per op; "vocoder_streams" = 1 (default): the three parallel resblocks of a vocoder stage run
  * on the caller's stream plus two engine-owned streams (joined before the call returns control of the stream);
  * "persistent_encoder_cluster" = 1 (0 on a fresh handle; the Python engine switches it on): steps with <= 16 active rows run on
  * the cluster kernel (4 thread-block clusters x 16 CTAs, activations in distributed shared memory; allocates 123 MB of repacked
  * weights the first time); larger steps and refused launches take the one-CTA-per-SM kernel; "cluster_cooperative" = 1 (default; 0 only
  * under a profiler that serialises kernels and cannot replay cooperative cluster launches);
- * "persistent_ffn_fused", "persistent_mt", "persistent_mt_v2", "persistent_mt_prefix", "fbank_tma" = 1 (default): kernel variants of
- * round 2, each tested against the path it replaces; "umma2_fused_reduce" = 0 (default: measured slower);
+ * "persistent_ffn_fused", "persistent_mt", "persistent_mt_prefix", "fbank_tma" = 1 (default): kernel variants of
+ * round 2, each tested against the path it replaces;
  * "persistent_profile" = 1: the persistent kernels record %globaltimer stamps per phase; "persistent_time" = 1: CUDA events around
  * the encoder-stack kernel, the single-token MT kernel and the stream pool's resample kernel (read with ss_debug_copy "persist_time" /
  * "mt_time" / "pool_resample_time") */

@@ -17,10 +17,6 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 // ... and the matching wait: everything the previous kernels of the stream wrote is visible after it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// set while a stream capture is recording the launches (CUDA-graph replay of a stage): programmatic launches are recorded
-// as plain launches unless the engine option graph_pdl asks otherwise
-extern thread_local int g_pdl_off;
-
 // Shared-memory carve-out: the wgmma kernels need > 100 KB of shared memory per CTA, the SIMT kernels a few KB.  An SM
 // holds ONE carve-out at a time, so kernels that ask for different ones cannot share an SM and every change drains it
 // -- which is what the vocoder's three concurrent streams of alternating conv / reduce kernels would do.  With the option on
@@ -71,7 +67,7 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   // only small grids launch early: CTAs of a large dependent grid would sit on shared memory / registers that the
   // (multi-wave) predecessor still needs
   const unsigned long long ctas = (unsigned long long)grid.x * grid.y * grid.z;
-  attr[0].val.programmaticStreamSerializationAllowed = (ctas <= 296 && !g_pdl_off) ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = ctas <= 296 ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
@@ -88,7 +84,7 @@ inline void launch_pdl_always(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = g_pdl_off ? 0 : 1;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);

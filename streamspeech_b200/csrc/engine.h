@@ -4,7 +4,6 @@
 #include <cuda_runtime.h>
 
 #include <map>
-#include <tuple>
 #include <utility>
 #include <string>
 #include <vector>
@@ -98,11 +97,6 @@ struct ss_engine {
   int vocoder_streams = 1;     // 1: the parallel resblocks of a vocoder stage run on three streams, 0: one stream
   cudaStream_t aux_stream[2] = {nullptr, nullptr};
   cudaEvent_t fork_event = nullptr, join_event[2] = {nullptr, nullptr};
-  // CUDA-graph replay of the vocoder generator (conv_pre .. conv_post) per (frames, arena, routing): value = (exec, nodes)
-  int vocoder_graph = 0;  // off: the generator is bound by kernel execution, not by host enqueue
-  int graph_pdl = 0;
-  cudaStream_t capture_stream = nullptr;
-  std::map<std::tuple<int, uintptr_t, int, int, int>, std::pair<cudaGraphExec_t, int>> voc_graphs;
   // whole generator as one persistent kernel (kernels_umma2.cu vocoder_fused): -1 = when the frame count is at most
   // voc_fused_max_frames, 0 = never (multi-launch path), 1 = whenever the shapes allow it
   int vocoder_fused = -1;
@@ -188,20 +182,15 @@ struct ss_engine {
   float* st_glu = nullptr;  // conv-module GLU outputs (depthwise-conv inputs)
   unsigned long long* persist_ts = nullptr;    // [4096] phase timestamps when option persistent_profile is set
   int persistent_profile = 0;
-  int persistent_prefetch = 0;       // persistent encoder kernel prefetches the next layer's weights into L2
   int persistent_time = 0;           // record CUDA events around the persistent encoder kernel (bench roofline)
   struct TimedLaunch { cudaEvent_t e0, e1; double bytes; };
   std::vector<TimedLaunch> time_events;
   std::vector<TimedLaunch> mt_time_events;  // the single-token MT kernel's launches (bytes field = steps executed)
-  ss::PersistLayer* persist_alias = nullptr;   // debug: every layer entry = layer 0 (timing experiments only)
-  int persistent_alias = 0;
-  unsigned* persist_bar = nullptr;   // arrival counter of the kernel's own grid barrier (option persistent_barrier)
+  unsigned* persist_bar = nullptr;   // arrival counter of the persistent kernels' grid barrier (allocated by ss_finalize)
   unsigned persist_bar_target = 0;
   unsigned* async_err_pinned = nullptr;  // host copy of persist_bar[SS_BAR_ERR_WORD] (read back at synchronisation points)
-  int persistent_barrier = 1;        // 0: cooperative-groups grid.sync(), 1: own counter barrier (cheaper per barrier)
   ss::MtLayerP* mt_persist_layers = nullptr;   // [mt_layers] device pointer table for kernels_persist_mt.cu
   int persistent_mt = 1;                       // single-token MT decode steps as one cooperative kernel per burst
-  int persistent_mt_v2 = 1;                    // single-token kernel with 6 grid barriers per layer (head-group partial projections)
   float* mt_part = nullptr;                    // [9][mt_dim] scratch of that kernel (per-head partials + FFN delta)
   int persistent_mt_prefix = 1;                // ... and the forced-prefix pass (M <= 64 rows) as one cooperative kernel
   // batched greedy search (ss_mt_greedy_batch): caches of its own, so that a streaming agent's MT state on the handle survives it

@@ -118,10 +118,8 @@ int report_async_error(ss_engine* h, unsigned flag, const char* where) {
                                                    "last check are invalid (barrier re-armed)");
 }
 
-void clear_graphs(ss_engine* h) {
+void clear_voc_fused(ss_engine* h) {
   cudaDeviceSynchronize();
-  for (auto& kv : h->voc_graphs) cudaGraphExecDestroy(kv.second.first);
-  h->voc_graphs.clear();
   h->voc_fused.clear();  // (their packed weight pointers may be gone too)
 }
 
@@ -335,6 +333,20 @@ DecScratch dec_scratch(ss_engine* h, int n, int dim, int ffn) {
   s.qkv = h->ws.f32((size_t)n * 3 * dim);
   s.kv = nullptr;
   return s;
+}
+
+// parameters of the persistent MT kernels over the handle's single-stream buffers (mt_begin's caches, mt_tok_dev)
+MtDecodeParams mt_decode_params(ss_engine* h, const DecScratch& s, float* x, float* logits, float* feats, int kv_off) {
+  const ss_config& c = h->cfg;
+  MtDecodeParams P;
+  P.n_layers = c.mt_layers; P.heads = c.mt_heads; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
+  P.max_pos = c.max_mt_positions; P.cross_cap = h->mt_cross_cap; P.kv_off = kv_off;
+  P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
+  P.self_k = h->mt_self_k; P.self_v = h->mt_self_v; P.cross_kv = h->mt_cross_kv;
+  P.tok = h->mt_tok_dev; P.feats = feats; P.x = x; P.q = s.q; P.attn = s.attn; P.hid = s.hid; P.logits = logits;
+  P.part = h->mt_part; P.delta = h->mt_part + (size_t)8 * c.mt_dim;
+  if (h->persistent_profile) P.ts = h->persist_ts;
+  return P;
 }
 
 // device buffers of the batched greedy search, grown on demand: self K / V for tok_ld positions, cross K / V for Tmax rows per sample
@@ -675,7 +687,7 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
       }
     }
     bool cluster_done = false;
-    if (persistent && h->persistent_encoder_cluster && h->cl_blobs && h->persist_bar &&
+    if (persistent && h->persistent_encoder_cluster && h->cl_blobs &&
         encoder_layers_cluster_supported(nA, D, c.enc_ffn, c.enc_heads, T, c.dw_kernel)) {
       const float* pos_tabs[16];
       for (int i = 0; i < 16; ++i) pos_tabs[i] = i < c.enc_layers ? h->enc[i].pos_proj : nullptr;
@@ -685,11 +697,10 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
       if (!cluster_done) cudaGetLastError();  // refused launch: the one-CTA-per-SM kernel below takes the step
     }
     if (persistent && !cluster_done)
-      persistent = encoder_layers_persistent(h->persistent_alias ? h->persist_alias : h->persist_layers, c.enc_layers, x, hid, qb, att, dw, h->st_k, h->st_v, h->st_glu, nA, a0, T, D,
+      persistent = encoder_layers_persistent(h->persist_layers, c.enc_layers, x, hid, qb, att, dw, h->st_k, h->st_v, h->st_glu, nA, a0, T, D,
                                              c.enc_ffn, c.enc_heads, h->Tpos, h->attn_chunk, cc, c.dw_kernel,
-                                             h->persistent_profile ? h->persist_ts : nullptr,
-                                             h->persistent_barrier ? h->persist_bar : nullptr, &h->persist_bar_target,
-                                             h->persistent_prefetch, h->persistent_ffn_fused ? h->persist_ffn_scratch : nullptr, st) == 0;
+                                             h->persistent_profile ? h->persist_ts : nullptr, h->persist_bar, &h->persist_bar_target,
+                                             h->persistent_ffn_fused ? h->persist_ffn_scratch : nullptr, st) == 0;
     if (ev0 && ev1) {
       cudaEventRecord(ev1, st);
       // algorithmic bytes of this launch: every GEMM weight once + the K / V caches and relative-position rows the attention reads
@@ -853,16 +864,9 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
   const bool persistent_mt = h->persistent_mt && mt_decode_persistent_supported(dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, T);
   int step = start;
   bool done = false;
-  if (persistent_mt && h->persistent_mt_prefix && h->persist_bar && start >= 1 && mt_prefix_persistent_supported(dim, c.mt_ffn, c.mt_heads, start, T)) {
+  if (persistent_mt && h->persistent_mt_prefix && start >= 1 && mt_prefix_persistent_supported(dim, c.mt_ffn, c.mt_heads, start, T)) {
     // rows 0 .. start-1 ([eos, p1 .. p_{start-1}]) in one cooperative launch; the single-token kernel continues at position `start`
-    MtDecodeParams P;
-    P.n_layers = c.mt_layers; P.heads = c.mt_heads; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
-    P.max_pos = c.max_mt_positions; P.cross_cap = h->mt_cross_cap;
-    P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
-    P.self_k = h->mt_self_k; P.self_v = h->mt_self_v; P.cross_kv = h->mt_cross_kv;
-    P.tok = h->mt_tok_dev; P.feats = feats_out_dev; P.x = x; P.q = s.q; P.attn = s.attn; P.hid = s.hid; P.logits = logits;
-        if (h->persistent_mt_v2 && h->mt_part) { P.part = h->mt_part; P.delta = h->mt_part + (size_t)8 * c.mt_dim; }
-        if (h->persistent_profile) P.ts = h->persist_ts;
+    const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats_out_dev, 0);
     if (mt_prefix_persistent(P, h->mt_persist_layers, start, T, h->persist_bar, &h->persist_bar_target, st) == 0)
       fed = start;
     else
@@ -874,17 +878,10 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
     for (; step <= max_len && enq < burst; ++step, ++enq) {
       // feed tokens[fed .. step]  (first iteration: the whole prefix; afterwards one token)
       int n = step + 1 - fed;
-      if (n == 1 && persistent_mt && h->persist_bar) {
+      if (n == 1 && persistent_mt) {
         // the rest of the burst as ONE cooperative launch (it stops by itself at eos / max_len)
         const int cnt = std::min(max_len - step + 1, burst - enq);
-        MtDecodeParams P;
-        P.n_layers = c.mt_layers; P.heads = c.mt_heads; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
-        P.max_pos = c.max_mt_positions; P.cross_cap = h->mt_cross_cap;
-        P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
-        P.self_k = h->mt_self_k; P.self_v = h->mt_self_v; P.cross_kv = h->mt_cross_kv;
-        P.tok = h->mt_tok_dev; P.feats = feats_out_dev; P.x = x; P.q = s.q; P.attn = s.attn; P.hid = s.hid; P.logits = logits;
-        if (h->persistent_mt_v2 && h->mt_part) { P.part = h->mt_part; P.delta = h->mt_part + (size_t)8 * c.mt_dim; }
-        if (h->persistent_profile) P.ts = h->persist_ts;
+        const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats_out_dev, 0);
         cudaEvent_t ev0 = nullptr, ev1 = nullptr;
         if (h->persistent_time && h->mt_time_events.size() < 4096 && cudaEventCreate(&ev0) == cudaSuccess && cudaEventCreate(&ev1) == cudaSuccess)
           cudaEventRecord(ev0, st);
@@ -922,7 +919,7 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
     int produced = step - burst_first - (done ? 1 : 0);
     if (produced > 0) {
       cudaMemcpyAsync(h->mt_next_pinned, h->mt_tok_dev + burst_first + 1, produced * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
-      if (h->persist_bar && h->async_err_pinned)
+      if (h->async_err_pinned)
         cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
       if (cudaStreamSynchronize(st) != cudaSuccess)
         return h->fail(SS_ERR_CUDA, std::string("ss_mt_greedy: ") + cudaGetErrorString(cudaGetLastError()));
@@ -965,9 +962,8 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
   if (max_len < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
   if (max_len + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
   cudaStream_t st = S(stream);
-  // the batched kernel reproduces the rows of the 6-barrier single-token kernel: it runs where ss_mt_greedy would run that one
-  const bool batched = h->persistent_mt && h->persistent_mt_v2 && h->mt_part && h->persist_bar && c.mt_heads == 8 &&
-                       mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, Tmax);
+  // the batched kernel reproduces the rows of the single-token kernel: it runs where ss_mt_greedy would run that one
+  const bool batched = h->persistent_mt && mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, Tmax);
   for (int g0 = 0; g0 < B; g0 += MT_BATCH_MAX_ROWS) {
     const int Bg = std::min(MT_BATCH_MAX_ROWS, B - g0);
     if (batched && Bg >= h->mt_batch_min_rows) {
@@ -1019,7 +1015,7 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
   const int kv_off = h->mt_inc_self_len - start;
   if (kv_off < 0) return h->fail(SS_ERR_STATE, "incremental MT state is shorter than the prefix (reset missing, or a prefix that this state did not produce)");
   if (max_len + kv_off + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
-  if (!h->persistent_mt || !h->persist_bar || !mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, std::max(T, h->mt_inc_cross_rows)))
+  if (!h->persistent_mt || !mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, std::max(T, h->mt_inc_cross_rows)))
     return h->fail(SS_ERR_STATE, "incremental MT decoding runs on the persistent MT kernel, which is off or does not support this shape");
   int rc = ensure_mt_cross(h, std::max(T, h->mt_inc_cross_rows), h->mt_inc_cross_rows);
   if (rc) return rc;
@@ -1057,14 +1053,7 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
   bool done = false;
   while (!done) {
     const int cnt = std::min(max_len - step + 1, burst);
-    MtDecodeParams P;
-    P.n_layers = c.mt_layers; P.heads = c.mt_heads; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
-    P.max_pos = c.max_mt_positions; P.cross_cap = h->mt_cross_cap; P.kv_off = kv_off;
-    P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
-    P.self_k = h->mt_self_k; P.self_v = h->mt_self_v; P.cross_kv = h->mt_cross_kv;
-    P.tok = h->mt_tok_dev; P.feats = feats; P.x = x; P.q = s.q; P.attn = s.attn; P.hid = s.hid; P.logits = logits;
-        if (h->persistent_mt_v2 && h->mt_part) { P.part = h->mt_part; P.delta = h->mt_part + (size_t)8 * c.mt_dim; }
-        if (h->persistent_profile) P.ts = h->persist_ts;
+    const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats, kv_off);
     if (mt_decode_persistent(P, h->mt_persist_layers, step, cnt, max_len, Tk, h->persist_bar, &h->persist_bar_target, st) != 0) {
       cudaGetLastError();
       return h->fail(SS_ERR_CUDA, "cooperative launch of the persistent MT kernel was refused");
@@ -1258,8 +1247,7 @@ int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0
   expand_frames(h->voc_unit_emb, h->voc_cumsum, h->voc_U, f_lo, N, c.voc_embedding_dim, frames, st);
   // Short sequences (the streaming calls): conv_pre .. conv_post as one persistent kernel whose phases are separated by grid
   // barriers.  A shape it does not support or a refused cooperative launch falls through to the multi-launch path below.
-  const bool fused = h->vocoder_fused != 0 && (h->vocoder_fused == 1 || N <= kVocFusedMaxFrames) && g_umma_conv == 12 && nrb == 3 &&
-                     h->persist_bar != nullptr;
+  const bool fused = h->vocoder_fused != 0 && (h->vocoder_fused == 1 || N <= kVocFusedMaxFrames) && g_umma_conv == 12 && nrb == 3;
   if (fused) {
     VocFusedParams* P = vocoder_fused_table(h, N, frames, bufX, bufY, rbA, rbB, rbT, rbO, st);
     if (P) {
@@ -1271,10 +1259,6 @@ int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0
       if (vocoder_fused(*P, h->persist_bar, &h->persist_bar_target, st) == 0) return check_launch(h, "ss_vocoder_generate");
     }
   }
-  // Everything from conv_pre to conv_post depends on the call only through N (buffer addresses are arena offsets): ~190
-  // launches on three streams whose host enqueue time exceeds their GPU time.  With option vocoder_graph the sequence is
-  // recorded once per (N, arena, routing) by stream capture and replayed as one CUDA graph afterwards.
-  auto generator_body = [&](cudaStream_t st) {
   // conv_pre
   {
     ConvA a;
@@ -1368,48 +1352,6 @@ int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0
   }
   // x = leaky_relu(x) [slope 0.01, hifigan.py:166]; conv_post; tanh
   conv_post_tanh(bufX, L, ch, h->conv_post_w, h->conv_post_b, h->conv_post_k, 0.01f, wav, st);
-  };
-  bool replayed = false;
-  if (h->vocoder_graph) {
-    const auto key = std::make_tuple(N, (uintptr_t)h->ws.base, g_umma_conv, g_umma_min_rows * 4096 + g_umma_min_channels, h->vocoder_streams);
-    auto it = h->voc_graphs.find(key);
-    if (it != h->voc_graphs.end()) {
-      if (cudaGraphLaunch(it->second.first, st) == cudaSuccess) {
-        g_launches += it->second.second;
-        replayed = true;
-      } else {
-        cudaGetLastError();
-      }
-    } else {
-      // first sight of this key: run eagerly now (that also performs every lazy initialisation: packed weights, split
-      // scratch, function attributes), then record the same sequence for the next call.  The capture runs on an
-      // engine-owned stream because the caller's stream may be the legacy default stream, which cannot be captured.
-      generator_body(st);
-      replayed = true;
-      if (!h->capture_stream) cudaStreamCreateWithFlags(&h->capture_stream, cudaStreamNonBlocking);
-      const unsigned long long before = g_launches;
-      if (h->capture_stream && cudaStreamBeginCapture(h->capture_stream, cudaStreamCaptureModeRelaxed) == cudaSuccess) {
-        g_pdl_off = h->graph_pdl ? 0 : 1;
-        generator_body(h->capture_stream);
-        g_pdl_off = 0;
-        cudaGraph_t graph = nullptr;
-        cudaGraphExec_t exec = nullptr;
-        if (cudaStreamEndCapture(h->capture_stream, &graph) == cudaSuccess && graph != nullptr &&
-            cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
-          h->voc_graphs[key] = std::make_pair(exec, (int)(g_launches - before));
-        } else {
-          cudaGetLastError();
-          h->vocoder_graph = 0;  // capture is not possible here: stay on the eager path
-        }
-        if (graph) cudaGraphDestroy(graph);
-      } else {
-        cudaGetLastError();
-        h->vocoder_graph = 0;
-      }
-      g_launches = before;
-    }
-  }
-  if (!replayed) generator_body(st);
   copy_f32(wav + (size_t)ctx * h->hop, wav_out_dev, (int64_t)n_frames * h->hop, st);
   return check_launch(h, "ss_vocoder_generate");
 }
@@ -1423,10 +1365,10 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
   else if (n == "umma_min_channels") h->umma_min_channels = value;
   else if (n == "umma2_cache_clear") {  // debug tools that reuse a weight address
     umma2_cache_clear(h->umma2_cache);
-    clear_graphs(h);
+    clear_voc_fused(h);
   }
-  else if (n == "umma2_split_below") { g_umma2_split_below = value; clear_graphs(h); }
-  else if (n == "umma2_min_units") { g_umma2_min_units = value; clear_graphs(h); }
+  else if (n == "umma2_split_below") { g_umma2_split_below = value; clear_voc_fused(h); }
+  else if (n == "umma2_min_units") { g_umma2_min_units = value; clear_voc_fused(h); }
   else if (n == "umma2_debug") {
     if (value && !g_umma2_dbg) {
       if (cudaMalloc(&g_umma2_dbg, 16 * sizeof(unsigned long long)) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");
@@ -1440,11 +1382,8 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
   }
   else if (n == "prefer_shared") g_prefer_shared = value;  // takes effect for kernels that have not been launched yet
   else if (n == "unit_grouped") h->unit_grouped = value;
-  else if (n == "vocoder_graph") h->vocoder_graph = value;
   else if (n == "vocoder_fused") h->vocoder_fused = value;
-  else if (n == "graph_pdl") h->graph_pdl = value;
   else if (n == "fbank_tma") h->fbank_tma = value;
-  else if (n == "umma2_fused_reduce") g_umma2_fused_reduce = value;
   else if (n == "persistent_encoder") h->persistent_encoder = value;
   else if (n == "persistent_ffn_fused") h->persistent_ffn_fused = value;
   else if (n == "cluster_cooperative") h->cluster_cooperative = value;  // 0: plain cluster launch (ncu cannot replay cooperative cluster launches)
@@ -1463,28 +1402,8 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
   else if (n == "vocoder_streams") h->vocoder_streams = value;
   else if (n == "persistent_mt") h->persistent_mt = value;
   else if (n == "persistent_mt_prefix") h->persistent_mt_prefix = value;
-  else if (n == "persistent_mt_v2") h->persistent_mt_v2 = value;
   else if (n == "mt_batch_min_rows") h->mt_batch_min_rows = value;
-  else if (n == "persistent_prefetch") h->persistent_prefetch = value;
   else if (n == "persistent_time") h->persistent_time = value;
-  else if (n == "persistent_barrier") {
-    if (value && !h->persist_bar) {
-      if (cudaMalloc(&h->persist_bar, 256) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");
-      h->dev_allocs.push_back(h->persist_bar);
-      cudaMemset(h->persist_bar, 0, 256);
-      h->persist_bar_target = 0;
-    }
-    h->persistent_barrier = value;
-  }
-  else if (n == "persistent_alias") {  // timing experiment: all layers read layer 0's weights (results are wrong)
-    if (value && !h->persist_alias) {
-      const int L = h->cfg.enc_layers;
-      if (cudaMalloc(&h->persist_alias, L * sizeof(PersistLayer)) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");
-      h->dev_allocs.push_back(h->persist_alias);
-      for (int i = 0; i < L; ++i) cudaMemcpy(h->persist_alias + i, h->persist_layers, sizeof(PersistLayer), cudaMemcpyDeviceToDevice);
-    }
-    h->persistent_alias = value;
-  }
   else if (n == "persistent_profile") {
     if (value && !h->persist_ts) {
       if (cudaMalloc(&h->persist_ts, 4096 * sizeof(unsigned long long)) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");

@@ -484,9 +484,6 @@ int ss_destroy(ss_engine* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
   for (void* p : h->dev_allocs) cudaFree(p);
-  for (auto& kv : h->voc_graphs) cudaGraphExecDestroy(kv.second.first);
-  h->voc_graphs.clear();
-  if (h->capture_stream) cudaStreamDestroy(h->capture_stream);
   ss::umma2_cache_destroy(h->umma2_cache);
   if (h->ws.base) cudaFree(h->ws.base);
   if (h->mt_cross_kv) cudaFree(h->mt_cross_kv);

@@ -8,7 +8,6 @@ namespace ss {
 
 extern unsigned long long g_launches;  // kernels launched by this library (process-wide)
 extern int g_prefer_shared;            // 1: every kernel asks for the maximum shared-memory carve-out (see common.cuh)
-extern thread_local int g_pdl_off;     // 1 while a stream capture records launches (see common.cuh)
 
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3 };
 
@@ -68,7 +67,6 @@ void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaSt
 
 // split-K scratch (one per process; launches of a handle are stream-ordered) and its fixed-order reduce + epilogue
 float* splitk_workspace(size_t bytes);
-unsigned* splitk_counters(int n_tiles);  // zeroed ticket counters of the current split-K slot (nullptr if n_tiles is too large)
 // split-K scratch region (0..2) used by the GEMM launches of the calling thread from now on; 0 is the default
 void set_splitk_slot(int slot);
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st);
@@ -78,7 +76,6 @@ void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, cons
 // descriptor row shifts).  The cache owns the packed weight copies (keyed by weight pointer and tiling).
 struct Umma2Cache;
 extern int g_umma2_split_below, g_umma2_min_units;  // split heuristics (tuning knobs)
-extern int g_umma2_fused_reduce;                    // 1: the last CTA of a tile reduces the split partial sums in the kernel (no extra launch)
 extern unsigned long long* g_umma2_dbg;             // optional %globaltimer stamps of CTA (0,0,0)
 Umma2Cache* umma2_cache_create();
 void umma2_cache_clear(Umma2Cache* c);

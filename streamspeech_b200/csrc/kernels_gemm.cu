@@ -59,9 +59,11 @@ __device__ __forceinline__ float apply_act(float x, int act) {
 
 // gridDim.z > 1: split-K.  Slice z accumulates k-tiles [z*tiles_per_split, (z+1)*tiles_per_split) and stores the raw
 // partial sums to ws[z][M][N]; splitk_epilogue_kernel then reduces the slices in a fixed order and applies the epilogue.
+// The plain 128 x 16 tile is picked for M >= 128 x #SMs rows: it is held to 64 registers (4 CTAs per SM), which ptxas does not
+// choose for it unasked.
 template <int BM, int BN, bool CONV>
-__global__ void __launch_bounds__(NT) gemm_kernel(ConvA a, const float* __restrict__ W, int M, int N, int K, Epilogue ep,
-                                                  int tiles_per_split, float* __restrict__ ws, unsigned* tile_ctr) {
+__global__ void __launch_bounds__(NT, (BM == 128 && BN == 16 && !CONV) ? 4 : 0) gemm_kernel(ConvA a, const float* __restrict__ W, int M, int N, int K, Epilogue ep,
+                                                  int tiles_per_split, float* __restrict__ ws) {
   pdl_trigger();
   pdl_wait();
   constexpr int TM = BM / 16;
@@ -175,58 +177,6 @@ __global__ void __launch_bounds__(NT) gemm_kernel(ConvA a, const float* __restri
         if (n < N) wz[(int64_t)m * N + n] = acc[i][j];
       }
     }
-    if (tile_ctr == nullptr) return;  // a separate splitk_epilogue_kernel launch reduces
-    // in-kernel reduction: the CTA that takes the last ticket of this output tile sums the slices in order (same order and
-    // arithmetic as splitk_epilogue_kernel, hence bit-identical) and applies the epilogue
-    __shared__ unsigned s_last;
-    __threadfence();
-    __syncthreads();
-    unsigned* ctr = tile_ctr + (blockIdx.y * gridDim.x + blockIdx.x);
-    if (tid == 0) s_last = (atomicAdd(ctr, 1u) == gridDim.z - 1) ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    if (tid == 0) *ctr = 0u;
-    const int splits = gridDim.z;
-    const int rows = min(BM, M - m0), cols = min(BN, N - n0);
-    const int ctile = ep.glu ? cols / 2 : cols;
-    for (int idx = tid; idx < rows * ctile; idx += NT) {
-      const int r = idx / ctile, c = idx - r * ctile;
-      const int m = m0 + r;
-      int64_t orow = m;
-      if (ep.out_L > 0) {
-        int b = m / a.L_rows;
-        int t = m - b * a.L_rows;
-        orow = (int64_t)b * ep.out_L + (int64_t)t * ep.out_row_stride + ep.out_row_offset;
-      }
-      float y;
-      int oc;
-      if (ep.glu) {
-        const int n = n0 + 2 * c;
-        oc = n >> 1;
-        float av_ = 0.f, gv = 0.f;
-        for (int z = 0; z < splits; ++z) {
-          const float* q = ws + ((int64_t)z * M + m) * N + n;
-          av_ += __ldcg(q);
-          gv += __ldcg(q + 1);
-        }
-        if (ep.bias) {
-          av_ += ep.bias[n];
-          gv += ep.bias[n + 1];
-        }
-        y = ep.alpha * (av_ * (1.0f / (1.0f + expf(-gv))));
-      } else {
-        oc = n0 + c;
-        float sum = 0.f;
-        for (int z = 0; z < splits; ++z) sum += __ldcg(ws + ((int64_t)z * M + m) * N + oc);
-        if (ep.bias) sum += ep.bias[oc];
-        y = ep.alpha * apply_act(sum, ep.act);
-      }
-      float* op = ep.out + orow * ep.ldo + oc;
-      if (ep.residual) y += ep.res_scale * ep.residual[orow * ep.ldo + oc];
-      if (ep.accumulate) y += *op;
-      *op = y;
-    }
     return;
   }
   // ---- epilogue
@@ -332,22 +282,6 @@ float* splitk_region() {
 
 }  // namespace
 
-// per-slot ticket counters of the in-kernel split reduction (kernels_umma2.cu): zero at rest (the last CTA of a tile resets its counter)
-unsigned* splitk_counters(int n) {
-  constexpr int CAP = 1 << 16;
-  static unsigned* base = nullptr;
-  if (n > CAP) return nullptr;
-  if (!base) {
-    if (cudaMalloc((void**)&base, (size_t)CAP * SPLITK_SLOTS * sizeof(unsigned)) != cudaSuccess) {
-      base = nullptr;
-      cudaGetLastError();
-      return nullptr;
-    }
-    cudaMemset(base, 0, (size_t)CAP * SPLITK_SLOTS * sizeof(unsigned));
-  }
-  return base + (size_t)g_splitk_slot * CAP;
-}
-
 float* splitk_workspace(size_t bytes) {
   if (bytes > SPLITK_WS_BYTES) return nullptr;
   return splitk_region();
@@ -386,12 +320,11 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
     grid.z = splits;
   }
   prefer_shared_once(conv ? (const void*)gemm_kernel<BM, BN, true> : (const void*)gemm_kernel<BM, BN, false>);
-  unsigned* ctr = (splits > 1 && g_umma2_fused_reduce) ? splitk_counters((int)ctas) : nullptr;
   if (conv)
-    gemm_kernel<BM, BN, true><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws, ctr);  // tile GEMMs never launch early (see launch_pdl)
+    gemm_kernel<BM, BN, true><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws);  // tile GEMMs never launch early (see launch_pdl)
   else
-    gemm_kernel<BM, BN, false><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws, ctr);
-  if (splits > 1 && ctr == nullptr) {
+    gemm_kernel<BM, BN, false><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws);
+  if (splits > 1) {
     ++g_launches;
     int total = M * (ep.glu ? N / 2 : N);
     launch_pdl(splitk_epilogue_kernel, dim3((total + 255) / 256), dim3(256), 0, st, ws, splits, M, N, a.L_rows, ep);

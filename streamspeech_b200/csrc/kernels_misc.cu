@@ -8,7 +8,6 @@
 
 namespace ss {
 unsigned long long g_launches = 0;
-thread_local int g_pdl_off = 0;
 int g_prefer_shared = 0;  // option prefer_shared (see common.cuh)
 namespace {
 

@@ -13,13 +13,9 @@
 // HBM latency overlaps the LayerNorm), reduces the 16 row sums with a halving shuffle tree and a fixed-order K-slice sum.
 // Same arithmetic as the per-kernel path of ss_encoder_stream_step, which remains the fallback for shapes this kernel
 // does not cover (nA > 16, D != 256, ...).
-#include <cooperative_groups.h>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "kernels_persist.h"
-
-namespace cg = cooperative_groups;
 
 namespace ss {
 namespace {
@@ -40,26 +36,6 @@ __device__ __forceinline__ float4 ldw(const float* p) {
   float4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
   return r;
-}
-
-// L2 prefetch of a weight matrix, spread over the whole grid (one 128-byte line per request)
-__device__ __forceinline__ void prefetch_l2(const float* p, int n_floats) {
-  const int lines = n_floats >> 5;
-  for (int i = blockIdx.x * PT + threadIdx.x; i < lines; i += gridDim.x * PT)
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p + (size_t)i * 32));
-}
-
-// All GEMM weights of one layer (~10 MB): issued one layer ahead, so the phases of the next layer stream their weights from
-// L2 instead of paying an HBM round trip right after every grid barrier.
-__device__ __forceinline__ void prefetch_layer(const PersistLayer& L, int D, int FFN) {
-  prefetch_l2(L.ffn1_w1, D * FFN);
-  prefetch_l2(L.ffn1_w2, D * FFN);
-  prefetch_l2(L.wqkv, 3 * D * D);
-  prefetch_l2(L.wo, D * D);
-  prefetch_l2(L.pw1, 2 * D * D);
-  prefetch_l2(L.pw2, D * D);
-  prefetch_l2(L.ffn2_w1, D * FFN);
-  prefetch_l2(L.ffn2_w2, D * FFN);
 }
 
 struct GemmEpi {
@@ -642,10 +618,8 @@ __global__ void __launch_bounds__(PT, 1) encoder_layers_persistent_kernel(const 
                                                                           float* hid, float* qb, float* att, float* dw, float* kc_all,
                                                                           float* vc_all, float* gc_all, int nA, int a0, int T, int H, int Tpos,
                                                                           int chunk, int conv_chunk, int dw_k, unsigned long long* ts,
-                                                                          unsigned* bar_ctr, unsigned bar_target, int prefetch,
-                                                                          float* ffn_scratch) {
+                                                                          unsigned* bar_ctr, unsigned bar_target, float* ffn_scratch) {
   constexpr int D = PD;
-  cg::grid_group grid = cg::this_grid();
   __shared__ __align__(16) Smem sm;
   int nts = 0;
   const bool stamp = ts != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
@@ -653,29 +627,22 @@ __global__ void __launch_bounds__(PT, 1) encoder_layers_persistent_kernel(const 
     sm.fine = nullptr;
     sm.nfine = 0;
   }
-#define GRID_SYNC()                                       \
-  if (bar_ctr != nullptr) grid_barrier(bar_ctr, bar_target); \
-  else grid.sync();
   if (ts != nullptr) {  // profile mode: two back-to-back barriers first (pure barrier cost)
     if (stamp) ts[nts++] = globaltimer_ns();
-    GRID_SYNC();
+    grid_barrier(bar_ctr, bar_target);
     if (stamp) ts[nts++] = globaltimer_ns();
-    GRID_SYNC();
+    grid_barrier(bar_ctr, bar_target);
     if (stamp) ts[nts++] = globaltimer_ns();
   }
   // profile mode: every CTA also records when it ARRIVES at each barrier of layer 1 (ts[512 + cta * 16 + phase])
 #define PHASE_END(tag)                                                                                          \
   fine_stamp(sm, tag);                                                                                          \
   if (ts != nullptr && li == 1 && threadIdx.x == 0) ts[512 + blockIdx.x * 16 + (tag) / 10 - 1] = globaltimer_ns(); \
-  GRID_SYNC();                                                                                                  \
+  grid_barrier(bar_ctr, bar_target);                                                                            \
   if (stamp) ts[nts++] = globaltimer_ns();
   for (int li = 0; li < n_layers; ++li) {
     if (threadIdx.x == 0) sm.fine = (ts != nullptr && blockIdx.x == 0 && li == 1) ? ts + 256 : nullptr;
     const PersistLayer L = layers[li];
-    if (prefetch) {
-      if (li == 0 && prefetch > 1) prefetch_layer(L, D, FFN);
-      if (li + 1 < n_layers) prefetch_layer(layers[li + 1], D, FFN);
-    }
     // the previous layer's final LayerNorm is still pending on x (applied on the fly in the first two phases)
     const float* pre_g = li > 0 ? layers[li - 1].fin_g : nullptr;
     const float* pre_b = li > 0 ? layers[li - 1].fin_b : nullptr;
@@ -730,7 +697,6 @@ __global__ void __launch_bounds__(PT, 1) encoder_layers_persistent_kernel(const 
     }
   }
 #undef PHASE_END
-#undef GRID_SYNC
   phase_layer_norm(x, layers[n_layers - 1].fin_g, layers[n_layers - 1].fin_b, nA, D);
 }
 
@@ -742,7 +708,7 @@ bool encoder_layers_persistent_supported(int nA, int D, int FFN, int H, int T, i
 
 int encoder_layers_persistent(const PersistLayer* layers_dev, int n_layers, float* x, float* hid, float* qb, float* att, float* dw, float* kc,
                               float* vc, float* gc, int nA, int a0, int T, int D, int FFN, int H, int Tpos, int chunk, int conv_chunk, int dw_k,
-                              unsigned long long* ts, unsigned* bar_ctr, unsigned* bar_target_host, int prefetch, float* ffn_scratch,
+                              unsigned long long* ts, unsigned* bar_ctr, unsigned* bar_target_host, float* ffn_scratch,
                               cudaStream_t st) {
   ++g_launches;
   (void)D;
@@ -755,14 +721,14 @@ int encoder_layers_persistent(const PersistLayer* layers_dev, int n_layers, floa
   }
   const int grid = current_device_sms();
   if (grid <= 0) return -1;
-  unsigned bar_target = bar_target_host ? *bar_target_host : 0u;
+  unsigned bar_target = *bar_target_host;
   if (grid < 2048 / FFN_UNITS) ffn_scratch = nullptr;  // the fused FFN phases give every hidden-unit group its own CTA
   void* args[] = {(void*)&layers_dev, (void*)&n_layers, (void*)&x, (void*)&hid, (void*)&qb, (void*)&att, (void*)&dw, (void*)&kc, (void*)&vc,
                   (void*)&gc, (void*)&nA, (void*)&a0, (void*)&T, (void*)&H, (void*)&Tpos, (void*)&chunk, (void*)&conv_chunk, (void*)&dw_k,
-                  (void*)&ts, (void*)&bar_ctr, (void*)&bar_target, (void*)&prefetch, (void*)&ffn_scratch};
+                  (void*)&ts, (void*)&bar_ctr, (void*)&bar_target, (void*)&ffn_scratch};
   cudaError_t e = cudaLaunchCooperativeKernel((void*)kernel, dim3(grid), dim3(PT), args, 0, st);
   if (e != cudaSuccess) return -2;
-  if (bar_ctr != nullptr && bar_target_host != nullptr) *bar_target_host += (unsigned)grid * (unsigned)(9 * n_layers + (ts != nullptr ? 2 : 0));
+  *bar_target_host += (unsigned)grid * (unsigned)(9 * n_layers + (ts != nullptr ? 2 : 0));
   return 0;
 }
 

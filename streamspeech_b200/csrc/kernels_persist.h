@@ -62,8 +62,7 @@ bool encoder_layers_persistent_supported(int nA, int D, int FFN, int H, int T, i
 // returns 0 on success (kernel enqueued on `st`), < 0 if the cooperative launch was refused
 int encoder_layers_persistent(const PersistLayer* layers_dev, int n_layers, float* x, float* hid, float* qb, float* att, float* dw, float* kc,
                               float* vc, float* gc, int nA, int a0, int T, int D, int FFN, int H, int Tpos, int chunk, int conv_chunk, int dw_k,
-                              unsigned long long* timestamps_or_null, unsigned* barrier_counter_dev_or_null,
-                              unsigned* barrier_target_host, int prefetch /*0 off, 1 next layer, 2 also layer 0*/,
+                              unsigned long long* timestamps_or_null, unsigned* barrier_counter_dev, unsigned* barrier_target_host,
                               float* ffn_scratch_or_null /* [FFN/16][16][D]: fused FFN phases; nullptr = W1 / W2 phases */, cudaStream_t st);
 
 // ---- cluster version of the encoder step (kernels_persist_cl.cu): 4 clusters x 16 CTAs, activations in distributed shared memory,
@@ -93,8 +92,7 @@ struct MtDecodeParams {
   float* feats;                             // [.][dim] final-LN features, row s
   float *x, *q, *attn, *hid, *logits;       // scratch: dim, dim, dim, ffn, vocab floats
   unsigned long long* ts = nullptr;         // profiling (option persistent_profile): ns stamps of CTA 0 for the 2nd step's layer 1
-  float *part = nullptr, *delta = nullptr;  // version-2 step (6 barriers per layer): per-head out-projection partials [8][dim], FFN delta [dim];
-                                            // nullptr selects the 8-barrier kernel
+  float *part, *delta;                      // per-head out-projection partials [8][dim], FFN delta [dim]
 };
 bool mt_decode_persistent_supported(int dim, int ffn, int heads, int vocab, int max_pos, int T);
 // enqueue `nsteps` greedy steps starting with the token at position step0; returns 0, or < 0 if the launch was refused

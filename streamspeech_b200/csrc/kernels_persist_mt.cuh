@@ -54,19 +54,6 @@ __device__ __forceinline__ float block_reduce_max(MtSmem& sm, float v) {
   return t;
 }
 
-// sm.v[0..dim) = LayerNorm(sm.x[0..dim)) (two-pass, as layer_norm_kernel); dim == 512: two values per thread
-__device__ __forceinline__ void ln_to_v(MtSmem& sm, const float* __restrict__ g, const float* __restrict__ b, int dim) {
-  const int t = threadIdx.x;
-  float a0 = sm.x[t], a1 = sm.x[t + MTT];
-  float mean = block_reduce_sum(sm, a0 + a1) / (float)dim;
-  float d0 = a0 - mean, d1 = a1 - mean;
-  float var = block_reduce_sum(sm, fmaf(d0, d0, d1 * d1)) / (float)dim;
-  float rstd = 1.0f / sqrtf(var + 1e-5f);
-  sm.v[t] = d0 * rstd * g[t] + b[t];
-  sm.v[t + MTT] = d1 * rstd * g[t + MTT] + b[t + MTT];
-  __syncthreads();
-}
-
 // LayerNorm parameters of this thread's two columns, loaded ahead of use (the loads fly while the phase's input arrives)
 struct LnP {
   float g0, g1, b0, b1;
@@ -75,6 +62,7 @@ __device__ __forceinline__ LnP ln_load(const float* __restrict__ g, const float*
   const int t = threadIdx.x;
   return LnP{__ldg(g + t), __ldg(g + t + MTT), __ldg(b + t), __ldg(b + t + MTT)};
 }
+// sm.v[0..dim) = LayerNorm(sm.x[0..dim)) (two-pass, as layer_norm_kernel); dim == 512: two values per thread
 __device__ __forceinline__ void ln_to_v(MtSmem& sm, const LnP& p, int dim) {
   const int t = threadIdx.x;
   float a0 = sm.x[t], a1 = sm.x[t + MTT];
@@ -223,13 +211,15 @@ __device__ __forceinline__ int masked_argmax(MtSmem& sm, const float* x, int voc
 // w0 / w1 = the column's weights at the same inputs; every lane gets the sum
 __device__ __forceinline__ float head_col_partial(float a0, float a1, float w0, float w1) { return warp_sum(fmaf(a0, w0, a1 * w1)); }
 
-// out-projection of a head (v2's per-head partials): columns are split over the CTAs of a head group
+// out-projection of a head (per-head partials): columns are split over the CTAs of a head group
 constexpr int GRP = 16;                 // CTAs per head group (8 heads x 16 = 128 CTAs)
 constexpr int PCOLS = 512 / GRP;        // out-projection columns per CTA of a group
 constexpr int PCOLS_PER_WARP = PCOLS / MW;
 
-// attend_head with every independent load issued up front: the key row of this thread, the first 8 value rows of its part and the
-// query are all in flight together (one L2 round trip instead of three dependent ones); n <= 256 keys take a single pass
+// softmax(q . K^T * scale) V for one head by one CTA: q[64], K/V rows at kbase/vbase + j * ld, n keys; out[64].
+// Every independent load is issued up front: the key row of this thread, the first 8 value rows of its part and the
+// query are all in flight together (one L2 round trip instead of three dependent ones); n <= 256 keys take a single pass.
+// Thread (part, q) sums keys j = part (mod 16) over dims [4q, 4q + 4), 8 keys (8 independent 16-byte loads) in flight per thread.
 __device__ void attend_head_early(MtSmem& sm, const float* q, const float* kbase, const float* vbase, int ld, int n, float* out) {
   const int tid = threadIdx.x;
   const int q4 = (tid & 15) * 4, part = tid >> 4;

@@ -138,7 +138,6 @@ struct U2Params {
   int units_per_split;
   int SB;                   // weight ring stages
   float* ws;                // split partial sums [gridDim.z][M][N] or null
-  unsigned* tile_ctr;       // ticket per output tile: the last split CTA of a tile reduces and runs the epilogue (null: separate kernel)
   unsigned long long* dbg;  // optional: %globaltimer stamps of CTA (0,0,0) at the hand-off points (option umma2_debug)
 };
 
@@ -166,49 +165,6 @@ __device__ __forceinline__ void u2_split_store(float4 v, unsigned char* stage, u
       v.z -= __low2float(h23);
       v.w -= __high2float(h23);
     }
-  }
-}
-
-// Split reduction inside the kernel: the CTA that takes the last ticket of an output tile sums the gridDim.z partial tiles in slice
-// order (deterministic, same order and arithmetic as splitk_epilogue_kernel) and applies the epilogue.
-__device__ __forceinline__ void u2_reduce_tile(const U2Params& p, int m0, int n0, int bn) {
-  const Epilogue& ep = p.ep;
-  const int M = p.M, N = p.N, splits = gridDim.z;
-  const int rows = min(U2_BM, M - m0);
-  const int cols = min(bn, N - n0);
-  const int ctile = ep.glu ? cols / 2 : cols;
-  for (int idx = threadIdx.x; idx < rows * ctile; idx += U2_THREADS) {
-    const int r = idx / ctile, c = idx - r * ctile;
-    const int m = m0 + r;
-    int64_t orow = m;
-    if (ep.out_L > 0) orow = (int64_t)m * ep.out_row_stride + ep.out_row_offset;  // B == 1
-    float y;
-    int oc;
-    if (ep.glu) {
-      const int n = n0 + 2 * c;
-      oc = n >> 1;
-      float av_ = 0.f, gv = 0.f;
-      for (int z = 0; z < splits; ++z) {
-        const float* q = p.ws + ((int64_t)z * M + m) * N + n;
-        av_ += __ldcg(q);
-        gv += __ldcg(q + 1);
-      }
-      if (ep.bias) {
-        av_ += ep.bias[n];
-        gv += ep.bias[n + 1];
-      }
-      y = ep.alpha * (av_ * (1.0f / (1.0f + expf(-gv))));
-    } else {
-      oc = n0 + c;
-      float acc = 0.f;
-      for (int z = 0; z < splits; ++z) acc += __ldcg(p.ws + ((int64_t)z * M + m) * N + oc);
-      if (ep.bias) acc += ep.bias[oc];
-      y = ep.alpha * u2_act(acc, ep.act);
-    }
-    float* op = ep.out + orow * ep.ldo + oc;
-    if (ep.residual) y += ep.res_scale * ep.residual[orow * ep.ldo + oc];
-    if (ep.accumulate) y += *op;
-    *op = y;
   }
 }
 
@@ -441,19 +397,6 @@ __global__ void __launch_bounds__(U2_THREADS, 1) umma2_kernel(const __grid_const
     }
   }
   if (tid == 0) u2_stamp(p, 8);
-  if (p.tile_ctr != nullptr) {
-    __threadfence();  // this CTA's partial sums are visible device-wide before its ticket
-    __shared__ unsigned s_last;
-    unsigned* ctr = p.tile_ctr + (blockIdx.y * gridDim.x + blockIdx.x);
-    __syncthreads();
-    if (tid == 0) s_last = (atomicAdd(ctr, 1u) == gridDim.z - 1) ? 1u : 0u;
-    __syncthreads();
-    if (s_last) {
-      __threadfence();
-      if (tid == 0) *ctr = 0u;  // at rest for the next launch that uses this slot
-      u2_reduce_tile(p, m0, n0, BN);
-    }
-  }
 }
 
 // W[N][ksize*C_in] fp32 (tap-major columns) -> [n-tile][chunk][tap][piece][plane (8 channels)][row (BN)][8 bf16]
@@ -495,10 +438,6 @@ __global__ void umma2_pack_kernel(const float* __restrict__ W, int N, int C_in, 
 int g_umma2_split_below = 60;   // tile grids smaller than this are split over (chunk, tap) units (ss_set_option umma2_split_below:
                                 // below one wave, the extra reduce launch can cost more than the idle SMs)
 int g_umma2_min_units = 4;      // ... into slices of at least this many units
-int g_umma2_fused_reduce = 0;   // 1: the last-ticket CTA of a tile reduces the split partial sums inside the kernel.  Off by default:
-                                // bit-identical, but one CTA reads splits x tile bytes alone where the separate splitk_epilogue_kernel
-                                // spreads the same reads over the whole GPU.  Kept as an option (a reduction distributed over the
-                                // split CTAs needs them co-resident).
 unsigned long long* g_umma2_dbg = nullptr;  // device buffer of 16 stamps when the debug option is on
 namespace {
 
@@ -625,7 +564,6 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   }
   p.units_per_split = ups;
   p.ws = ws;
-  p.tile_ctr = (splits > 1 && g_umma2_fused_reduce) ? splitk_counters(n_tiles * m_tiles) : nullptr;
   p.dbg = g_umma2_dbg;
   const size_t a_bytes = (size_t)2 * NP * (CK >> 3) * p.rs_pad * 16;
   const size_t b_unit = (size_t)NP * BN * CK * 2;
@@ -647,7 +585,7 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
       default: u2_launch<16, 2>(p, grid, smem, st); break;
     }
   }
-  if (splits > 1 && p.tile_ctr == nullptr) splitk_epilogue(ws, splits, M, N, a.L_rows, ep, st);
+  if (splits > 1) splitk_epilogue(ws, splits, M, N, a.L_rows, ep, st);
 }
 
 // ------------------------------------------------------------------------------------------------ fused vocoder generator

@@ -200,24 +200,18 @@ class Engine:
         self.set_option("umma_min_channels", int(os.environ.get("SS_UMMA_MIN_CHANNELS", "16")))
         self.set_option("persistent_encoder", int(os.environ.get("SS_PERSISTENT_ENCODER", "1")))
         self.set_option("persistent_mt", int(os.environ.get("SS_PERSISTENT_MT", "1")))
-        self.set_option("umma2_fused_reduce", int(os.environ.get("SS_UMMA2_FUSED_REDUCE", "0")))
         self.set_option("fbank_tma", int(os.environ.get("SS_FBANK_TMA", "1")))
         self.set_option("persistent_ffn_fused", int(os.environ.get("SS_PERSISTENT_FFN_FUSED", "1")))
         # cluster kernel for encoder steps with <= 16 active rows (larger steps and refused launches take the one-CTA-per-SM kernel)
         self.set_option("persistent_encoder_cluster", int(os.environ.get("SS_PERSISTENT_ENCODER_CLUSTER", "1")))
         self.set_option("cluster_cooperative", int(os.environ.get("SS_CLUSTER_COOPERATIVE", "1")))
-        self.set_option("persistent_mt_v2", int(os.environ.get("SS_PERSISTENT_MT_V2", "1")))
         self.set_option("persistent_mt_prefix", int(os.environ.get("SS_PERSISTENT_MT_PREFIX", "1")))
         self.set_option("vocoder_streams", int(os.environ.get("SS_VOCODER_STREAMS", "1")))
         self.set_option("unit_grouped", int(os.environ.get("SS_UNIT_GROUPED", "1")))
-        self.set_option("vocoder_graph", int(os.environ.get("SS_VOCODER_GRAPH", "0")))
         # vocoder generator as one persistent kernel: -1 (default) for short frame windows, 0 never (multi-launch path), 1 always
         self.set_option("vocoder_fused", int(os.environ.get("SS_VOCODER_FUSED", "-1")))
-        self.set_option("graph_pdl", int(os.environ.get("SS_GRAPH_PDL", "0")))
-        self.set_option("persistent_prefetch", int(os.environ.get("SS_PERSISTENT_PREFETCH", "0")))
         self.set_option("umma2_split_below", int(os.environ.get("SS_UMMA2_SPLIT_BELOW", "60")))
         self.set_option("umma2_min_units", int(os.environ.get("SS_UMMA2_MIN_UNITS", "4")))
-        self.set_option("persistent_barrier", int(os.environ.get("SS_PERSISTENT_BARRIER", "1")))
         self.hop = self.lib.ss_vocoder_hop(self._h)
         self.vocoder_receptive_field = self.lib.ss_vocoder_receptive_field(self._h)
 

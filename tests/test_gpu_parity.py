@@ -289,30 +289,6 @@ def test_vocoder_golden(eng3, gold):
     assert dur1.tolist() == [1] * codes.numel() and int(cum1[-1].item()) == codes.numel()
 
 
-def test_vocoder_graph_replay_is_identical(eng3, gold):
-    """The generator runs eagerly the first time a frame count is seen and as a CUDA-graph replay afterwards: same kernels,
-    same split decisions, so the samples must be bit-identical; and identical to the eager path with the option off."""
-    g = gold["vocoder"]
-    codes = cuda(g["code"][0].astype(np.int64))
-    dur, cum = eng3.vocoder_durations(codes, True)
-    total = int(cum[-1].item())
-    eng3.set_option("vocoder_graph", 1)
-    first = eng3.vocoder_generate(total, total - 21, 21, -1).clone()   # eager + capture
-    l0 = eng3.launch_count()
-    second = eng3.vocoder_generate(total, total - 21, 21, -1).clone()  # replay
-    replay_launches = eng3.launch_count() - l0
-    third = eng3.vocoder_generate(total, total - 21, 21, -1).clone()
-    eng3.set_option("vocoder_graph", 0)
-    l0 = eng3.launch_count()
-    eager = eng3.vocoder_generate(total, total - 21, 21, -1).clone()
-    eager_launches = eng3.launch_count() - l0
-    eng3.set_option("vocoder_graph", 1)
-    report("vocoder_graph", replay_vs_first=maxdiff(second, first), eager_vs_replay=maxdiff(eager, second), replay_launches=replay_launches,
-           eager_launches=eager_launches)
-    assert torch.equal(first, second) and torch.equal(second, third) and torch.equal(eager, second)
-    assert replay_launches == eager_launches  # the replay accounts for every kernel node it runs
-
-
 # --------------------------------------------------------------------------------------------- tensor-core kernels
 @pytest.mark.parametrize("shape", [(128, 32, 16, 1, 1, 0, 1.0), (100, 64, 128, 3, 1, 1, 0.1), (260, 256, 256, 11, 5, 25, 0.1),
                                    (1040, 128, 128, 7, 3, 9, 0.1), (16640, 16, 16, 7, 5, 15, 0.1), (300, 128, 512, 7, 1, 3, 1.0),
@@ -601,12 +577,12 @@ def test_ctc_pair_equals_single_heads(eng3, gold):
             assert toks == g[f"ctc_{name}_tokens"].tolist() and idx == g[f"ctc_{name}_index"].tolist(), (row0, name)
 
 
-@pytest.mark.parametrize("option", ["persistent_ffn_fused", "persistent_mt_prefix", "persistent_mt_v2"])
+@pytest.mark.parametrize("option", ["persistent_ffn_fused", "persistent_mt_prefix", "persistent_mt"])
 def test_persistent_kernel_variants_agree(full, option):
     """A / B of the round-2 persistent-kernel restructurings against the paths they replace: fused FFN phases (hidden-split
     rank-16 updates + deterministic reduce) vs separate W1 / W2 phases in the encoder step; cooperative MT prefix pass vs the
-    per-kernel prefix pass; single-token MT kernel with 6 barriers per layer (head-group partial projections) vs 8.  Same function,
-    different summation order."""
+    per-kernel prefix pass; cooperative MT search (prefix pass and single-token kernel) vs the per-kernel path, which stays the
+    fallback for unsupported shapes and refused launches.  Same function, different summation order."""
     cfg, e, o = full
     e.set_chunk(8, 8)
     feats = e.fbank(cuda(synth.make_audio(3.0, seed=5)))
@@ -807,31 +783,10 @@ def test_generate_waveform_from_code_front_door(tmp_path, gold):
     assert float(np.abs(pcm - np.clip(g["wav"], -1, 32767 / 32768)).max()) < 1e-3 + 1.0 / 32768
 
 
-def test_umma2_in_kernel_split_reduction_is_bit_identical(eng3, gold):
-    """The last-ticket CTA of an output tile reduces the split partial sums inside umma2_kernel (no splitk_epilogue launch): same
-    slice order and arithmetic as the separate reduce kernel, so the vocoder waveform and the unit-decoder logits must be
-    bit-identical with the option on and off."""
-    g = gold["vocoder"]
-    code = torch.from_numpy(g["code"][0]).cuda()
-    feats = cuda(gold["decoders"]["mt_feats"])
-    res = {}
-    for v in (0, 1):
-        eng3.set_option("umma2_fused_reduce", v)
-        l0 = eng3.launch_count()
-        dur, cum = eng3.vocoder_durations(code, True)
-        total = int(cum[-1].item())
-        wav = eng3.vocoder_generate(total, 0, total, 0).clone()
-        r = eng3.t2u_unit_decode(feats.repeat(5, 1).contiguous(), debug=True)
-        res[v] = (wav, r["logits"].clone(), eng3.launch_count() - l0)
-    eng3.set_option("umma2_fused_reduce", 0)  # the engine default (the in-kernel reduction measured slower, kernels_umma2.cu)
-    assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1])
-    report("umma2_fused_reduce", launches_separate=res[0][2], launches_fused=res[1][2])
-    assert res[1][2] < res[0][2]
-
-
 def test_capacity_and_misuse_fail_loudly(eng3):
     """Error behaviour of the C-ABI (SURVEY.md §5: status codes, never a silent wrong answer): sequences beyond the configured
-    maximum, a chunk-less model on the streaming entry point, a prefix the incremental MT state did not produce."""
+    maximum, a chunk-less model on the streaming entry point, a prefix the incremental MT state did not produce, engine options
+    that were retired (an unknown name, not a silent no-op)."""
     from streamspeech_b200.engine import Engine, EngineError
 
     cfg = golden_cfg()
@@ -854,5 +809,9 @@ def test_capacity_and_misuse_fail_loudly(eng3):
             e.mt_greedy_incremental(enc, [17, 18, 19], 2, 100)
         with pytest.raises(EngineError, match="no vocoder"):
             e.vocoder_durations(torch.zeros(4, dtype=torch.int64, device="cuda"))
+        for name in ("vocoder_graph", "graph_pdl", "persistent_alias", "persistent_barrier", "persistent_prefetch", "persistent_mt_v2",
+                     "umma2_fused_reduce"):
+            with pytest.raises(EngineError, match="unknown option"):
+                e.set_option(name, 1)
     finally:
         e.close()

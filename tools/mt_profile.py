@@ -15,9 +15,7 @@ enc = torch.randn(1024, 256, device="cuda") * 0.5
 res = {}
 toks, _ = eng.mt_greedy(enc[:160], None, 40)
 toks = (toks + [17] * 40)[:40]
-for prefix_kernel in (1, 0):   # here: A / B of the single-token kernel version (1 = 6 barriers per layer, 0 = 8)
-  eng.set_option("persistent_mt_v2", prefix_kernel)
-  for T in (160,):
+for T in (160,):
     for npre in (10, 30, 40):
         for new in (0, 3, 12):
             for stable in (T - 16,):
@@ -38,7 +36,7 @@ for prefix_kernel in (1, 0):   # here: A / B of the single-token kernel version 
                     e.record(); torch.cuda.synchronize()
                     ts.append(s.elapsed_time(e))
                 ts.sort()
-                res[f"prefixkernel{prefix_kernel}_T{T}_prefix{npre}_new{new}_stable{stable}"] = {"ms": ts[2], "launches": eng.launch_count() - l0}
-                print("prefix_kernel", prefix_kernel, T, npre, new, stable, round(ts[2] * 1e3, 1), "us", eng.launch_count() - l0, "launches", flush=True)
+                res[f"T{T}_prefix{npre}_new{new}_stable{stable}"] = {"ms": ts[2], "launches": eng.launch_count() - l0}
+                print(T, npre, new, stable, round(ts[2] * 1e3, 1), "us", eng.launch_count() - l0, "launches", flush=True)
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "gpurun_out", "mt_profile.json"), "w"), indent=1)
