@@ -129,6 +129,19 @@ int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_de
 int ss_ctc_greedy_pair(ss_engine* h, void* stream, const float* enc_dev, int rows, int row0, int64_t* argmax0_dev, int64_t* argmax1_dev,
                        int64_t* packed_out_dev);
 
+/* Samples per launch group of ss_ctc_greedy_batch: at most max(1, SS_CTC_BATCH_ROWS / T) samples (their logits, 2 x vocab floats per
+ * row, live in the workspace together). */
+#define SS_CTC_BATCH_ROWS 8192
+/* Both CTC heads over every row of B padded utterances (the offline generator's prints, ctc_decoder.py:40-111 on the padded
+ * encoder output: padded rows are NOT trimmed).  enc_dev [B][T][enc_dim].  Per launch group: one [rows][2V] projection over the
+ * concatenated head weights (one projection per head when the two vocabularies differ), one arg-max launch over every row of both
+ * heads and one collapse launch with one CTA per (sample, head).  packed_out_dev holds, for sample b at int64 offset
+ * b * 2 * (2T + 2), ss_ctc_greedy_pair's packing of its two heads: head h at + h * (2T + 2) = [count (int32) | tokens[T] int64 |
+ * index[T] int32], so one device->host copy reads the whole batch.  Sample b's output equals ss_ctc_greedy_rows(head, enc_b, T, 0)
+ * (the projection may take another GEMM kernel at a different row count).  Keeps no state.
+ * Errors: SS_ERR_INVALID for B <= 0, T <= 0 or a null pointer.  enqueue only */
+int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T, int64_t* packed_out_dev);
+
 /* ---- M1/M2: SequenceGenerator.generate_decoder, beam 1 (agent/sequence_generator.py:165-582) + the extra
  * mt_decoder(prev_output_tokens, features_only=True) forward (agent:638-642).
  * prefix_host[n_prefix] = tgt_subwords_indices; max_new_tokens as in the agent (-1 = source finished:
@@ -158,6 +171,22 @@ int ss_mt_stable_rows(ss_engine* h, int rows);
  * (ctc_unity/modules/transformer_decoder.py:257-403).  feats_out_dev [n][mt_dim]; logits_last_dev (optional) [tgt_vocab]. enqueue only */
 int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* tokens_host, int n,
                    float* feats_out_dev, float* logits_last_dev);
+/* Samples per launch group of ss_mt_features_batch and ss_t2u_unit_decode_batch: at most max(1, SS_UNIT_BATCH_ROWS / (S * rate))
+ * samples, i.e. the unit decoder's upsampled rows of a group stay within this budget (about 28 KB of workspace per row with the
+ * StreamSpeech sizes); larger batches run as consecutive groups. */
+#define SS_UNIT_BATCH_ROWS 32768
+/* ss_mt_features for B samples of one padded batch (the offline generator's mt_decoder(prev_output_tokens_mt, features_only),
+ * sequence_generator_multi_decoder_ctc.py:287-291).  enc_dev [B][T_stride][enc_dim]; sample b's cross-attention keys are its
+ * first T_host[b] rows, 1 <= T_b <= T_stride.  tokens_host [B][S] = [eos, hyp_b..., pad...] (pads only as a tail; positions
+ * restart for every sample and pads get the padding position); self-attention is causal over sample b's S_b non-pad tokens.
+ * feats_out_dev [B][S][mt_dim].  The cross K / V are projected into the call's workspace, one layer at a time: the handle's
+ * single-stream MT state (cross K / V cache, stable-rows hint, incremental caches, token buffer) is neither read nor written.
+ * Sample b's rows equal ss_mt_features(enc_b[:T_b], tokens_b) within float tolerance (the GEMMs may take another kernel at
+ * B * S rows; the attention arithmetic of a sample is the same).  Synchronises `stream` once (upload of the tokens and lengths).
+ * Errors: SS_ERR_INVALID for B <= 0, S <= 0 or S > max_mt_positions, T_stride <= 0, a T_b outside [1, T_stride], a token outside
+ * the vocabulary, a pad before a non-pad token, or a null pointer. */
+int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, const int64_t* tokens_host,
+                         int S, float* feats_out_dev);
 
 /* ---- M1 with the reference's incremental states (use_incremental_states=True: speech_to_text.s2tt.streamspeech.agent.py:136,178;
  * SURVEY.md N12).  The decoder state lives in the handle ACROSS calls until ss_mt_incremental_reset (the agent's reset()):
@@ -180,12 +209,25 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
  * t2u_out_dev / logits_dev optional (NULL) debug outputs [S][unit_dim], [S*rate][unit_vocab].  enqueue only */
 int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, int S, int n_pad_tail, int mask_eos,
                        int64_t* argmax_dev, int64_t* units_dev, int32_t* count_dev, float* t2u_out_dev, float* logits_dev);
+/* ss_t2u_unit_decode for B samples of one padded batch (sequence_generator_multi_decoder_ctc.py:293-330): T2U encoder with each
+ * sample's padding mask -> LayerNorm -> x rate upsample plus sample b's positional row pos_rows_dev[b] (N1: the row the reference
+ * gives batch element b, i.e. sinusoidal row pad + 1 + b of the WHOLE batch, even when the batch runs in several groups) -> the
+ * unit decoder layers -> LayerNorm -> out-projection -> arg-max (pad, unk masked, + eos when mask_eos: N3) -> CTC collapse of each
+ * sample.  mt_feats_dev [B][S][mt_dim]; n_pad_tail_host[b] in [0, S): trailing pad positions of sample b, whose rows are decoded
+ * too (N2); pos_rows_dev [B][unit_dim].  argmax_dev [B][S * rate]; packed_units_dev [B][S * rate + 1], row b = [count (int32 in the
+ * first int64) | units], so that one device->host copy reads every sample.  Sample b equals ss_t2u_unit_decode(mt_feats_b,
+ * n_pad_tail_b) with the positional row set to pos_rows_dev[b] (within float tolerance for the activations; the GEMMs may take
+ * another kernel at more rows).  Neither reads nor writes the handle's positional row (ss_unit_position_row) and does not
+ * synchronise the device (unless the workspace has to grow); synchronises `stream` once (upload of the key lengths).
+ * Errors: SS_ERR_INVALID for B <= 0, S <= 0 or S > max_mt_positions, an n_pad_tail outside [0, S), or a null pointer. */
+int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
+                             int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);
 
 /* Positional-embedding row (unit_dim floats, host memory) the CTC unit decoder adds to every upsampled T2U state.  The
  * reference computes positions from x[:, :, 0] viewed as [bsz, seq] (ctc_transformer_unit_decoder.py:176-181, SURVEY.md N1), so
  * every time step of batch element b gets the sinusoidal row pad + 1 + b.  The engine is created with the row of b = 0 (the
- * streaming agents); the offline batched generator (streamspeech_b200/offline.py) sets the row of each sample before decoding
- * it.  Synchronises the device. */
+ * streaming agents); a per-sample reproduction of a batch sets the row of each sample before decoding it (the offline generator
+ * passes every sample's row to ss_t2u_unit_decode_batch instead).  Synchronises the device. */
 int ss_unit_position_row(ss_engine* h, const float* row_host);
 /* ---- V1: CodeGenerator.forward front half (agent/tts/codehifigan.py:56-66): embedding + duration predictor.
  * codes_dev[U] int64 unit ids (0..num_embeddings-1); dur_out_dev[U] int64; cumsum_out_dev[U+1] int32 (frame offsets).

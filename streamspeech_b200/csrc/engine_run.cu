@@ -25,6 +25,14 @@ thread_local int g_umma_conv = 0;
 thread_local int g_umma_min_rows = 128;
 thread_local int g_umma_min_channels = 16;
 thread_local Umma2Cache* g_umma2_cache = nullptr;
+// Batched calls that stack g_route_samples samples of equal row counts into one GEMM decide the tensor-core routing from one
+// sample's rows (M / g_route_samples), so that a sample's GEMMs take the same class of kernel (fp32 or wgmma) as in the
+// single-sample call: the batch then reproduces the single-sample rounding instead of adding the split-bf16 error.
+thread_local int g_route_samples = 1;
+struct RouteSamples {  // scope of one such group
+  explicit RouteSamples(int n) { g_route_samples = n; }
+  ~RouteSamples() { g_route_samples = 1; }
+};
 
 void route_from(ss_engine* h) {
   g_umma_linear = h->umma_linear;
@@ -51,7 +59,7 @@ void linear(const float* x, int ldx, int M, const Linear& l, Epilogue ep, cudaSt
   ep.bias = l.b;
   if (skinny_gemm_supported(M, l.N, l.K, ep) && (ldx & 3) == 0)
     skinny_gemm(x, ldx, l.w, M, l.N, l.K, ep, st);
-  else if (g_umma_linear >= 12 && g_umma2_cache && M >= g_umma_min_rows && umma2_supported(a, l.N, ep))
+  else if (g_umma_linear >= 12 && g_umma2_cache && M / g_route_samples >= g_umma_min_rows && umma2_supported(a, l.N, ep))
     umma2_conv(g_umma2_cache, a, l.w, l.N, ep, g_umma_linear - 10, st);
   else
     gemm_conv(a, l.w, l.N, ep, st);
@@ -243,29 +251,33 @@ struct DecScratch {
 // pre-LN transformer layer over x[n][dim] (TransformerDecoderLayerBase.forward / TransformerEncoderLayerBase.forward,
 // ctc_unity/modules/transformer_layer.py:165-230,388-551).  Self-attention keys/values come either from the
 // layer's own fused qkv (full sequence, cache == nullptr) or from an external KV cache that already holds `past` rows.
+// nb > 1 (no cache): x holds nb samples of n / nb rows each; sample b attends to its own rows, cross_kv rows b*Tk .., and the
+// key-length arrays are indexed by sample.
 void dec_layer(const DecLayerW& L, float* x, int n, int dim, int ffn, int heads, bool causal, int self_kv_len_limit,
                const int* self_kv_len_dev, float* cache_k, float* cache_v, int past, const float* cross_kv, int Tk,
-               const int* cross_len_dev, DecScratch& s, cudaStream_t st, int group_R = 0, const int* group_len_dev = nullptr) {
+               const int* cross_len_dev, DecScratch& s, cudaStream_t st, int group_R = 0, const int* group_len_dev = nullptr, int nb = 1) {
   const float scale = 0.125f;  // head_dim ** -0.5, head_dim = 64
-  if (group_R > 1 && !cache_k && causal && n % group_R == 0) {
+  const int rows = n / nb;       // per sample
+  if (group_R > 1 && !cache_k && causal && rows % group_R == 0) {
     // rows come in groups of group_R identical consecutive rows (unit decoder layer 1): project the n / group_R distinct
     // rows only and collapse the causal softmax over the copies analytically (grouped_causal_attn_kernel)
     const int S = n / group_R;
     ln_linear(x, dim * group_R, S, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st);
-    grouped_causal_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, S, group_R, heads, scale, group_len_dev, st);
+    grouped_causal_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, S / nb, group_R, heads, scale,
+                             group_len_dev, nb, st);
   } else if (cache_k) {
     ln_qkv_routed(x, dim, n, L.self_ln, L.qkv, dim, s.q, dim, cache_k + (size_t)past * dim, dim, cache_v + (size_t)past * dim, dim, s.y, st);
     mha_attention(s.q, dim, cache_k, dim, cache_v, dim, s.attn, dim, 1, n, past + n, heads, scale, 1, past, self_kv_len_dev, st);
   } else {
     ln_linear(x, dim, n, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st);
-    mha_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, 1, n, n, heads, scale,
+    mha_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, nb, rows, rows, heads, scale,
                   causal ? 1 : 0, 0, self_kv_len_dev, st);
   }
   (void)self_kv_len_limit;
   linear(s.attn, dim, n, L.out, ep_residual(x, dim), st);
   if (L.has_cross) {
     ln_linear(x, dim, n, L.cross_ln, L.cq, ep_out(s.q, dim), s.y, st);
-    mha_attention(s.q, dim, cross_kv, 2 * dim, cross_kv + dim, 2 * dim, s.attn, dim, 1, n, Tk, heads, scale, 0, 0, cross_len_dev, st);
+    mha_attention(s.q, dim, cross_kv, 2 * dim, cross_kv + dim, 2 * dim, s.attn, dim, nb, rows, Tk, heads, scale, 0, 0, cross_len_dev, st);
     linear(s.attn, dim, n, L.cout, ep_residual(x, dim), st);
   }
   ln_linear(x, dim, n, L.final_ln, L.fc1, ep_out(s.hid, ffn, ACT_RELU), s.y, st);
@@ -1115,7 +1127,7 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
   float* ckv = h->ws.f32((size_t)Slen * 2 * dim);
   float* logits = logits_dev ? logits_dev : h->ws.f32((size_t)L * c.unit_vocab);
   if (!xu || !ckv || !logits) return h->fail(SS_ERR_CUDA, "workspace too small");
-  repeat_rows_add(t2u, Slen, R, dim, h->unit_pos_row, xu, st);
+  repeat_rows_add(t2u, Slen, R, dim, h->unit_pos_row, xu, 1, st);
   for (int l = 0; l < c.unit_layers; ++l) {
     linear(t2u, dim, Slen, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
     // layer 0 sees R identical copies of every T2U state (same positional row for every step, N1): grouped self-attention
@@ -1138,6 +1150,175 @@ int ss_unit_position_row(ss_engine* h, const float* row_host) {
   if (cudaMemcpy(h->unit_pos_row, row_host, (size_t)h->cfg.unit_dim * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess)
     return h->fail(SS_ERR_CUDA, "cudaMemcpy(unit positional row) failed");
   return SS_OK;
+}
+
+int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T, int64_t* packed_out_dev) {
+  if (h) route_from(h);
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (B <= 0 || T <= 0 || !enc_dev || !packed_out_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_ctc_greedy_batch");
+  const ss_config& c = h->cfg;
+  cudaStream_t st = S(stream);
+  const bool pair = h->ctc_pair.N == 2 * c.src_vocab && c.tgt_vocab == c.src_vocab;
+  const int Vmax = std::max(c.src_vocab, c.tgt_vocab);
+  const int64_t W = 2 * (int64_t)T + 2;  // one head's packed output
+  const int G = std::max(1, SS_CTC_BATCH_ROWS / T);
+  for (int g0 = 0; g0 < B; g0 += G) {
+    const int Bg = std::min(G, B - g0);
+    RouteSamples route(Bg);
+    const int rows = Bg * T;
+    if (!ws_begin(h, (size_t)rows * 2 * Vmax * sizeof(float) + (size_t)rows * 2 * sizeof(int64_t) + 4 * 256))
+      return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+    float* logits = h->ws.f32((size_t)rows * 2 * Vmax);
+    int64_t* am = (int64_t*)h->ws.raw((size_t)rows * 2 * sizeof(int64_t));
+    if (!logits || !am) return h->fail(SS_ERR_CUDA, "workspace too small");
+    const float* x = enc_dev + (size_t)g0 * T * c.enc_dim;
+    int64_t* out = packed_out_dev + (size_t)g0 * 2 * W;
+    if (pair) {
+      // [rows][2V] logits = 2 * rows arg-max rows of V (head-minor); sequence s = 2 b + head is sample b's head, at out + s * W
+      linear(x, c.enc_dim, rows, h->ctc_pair, ep_out(logits, 2 * c.src_vocab), st);
+      argmax_rows(logits, c.src_vocab, 2 * rows, c.src_vocab, h->mask_pad_unk, 2, am, nullptr, st);  // never select pad, unk
+      ctc_collapse_segments(am, T, 2, 2 * Bg, 0 /* <s> = CTC blank */, c.pad, out + 1, reinterpret_cast<int*>(out + 1 + T),
+                            reinterpret_cast<int*>(out), W, st);
+    } else {
+      for (int hd = 0; hd < 2; ++hd) {
+        const Linear& l = h->ctc_head[hd];
+        linear(x, c.enc_dim, rows, l, ep_out(logits, l.N), st);
+        argmax_rows(logits, l.N, rows, l.N, h->mask_pad_unk, 2, am, nullptr, st);
+        int64_t* o = out + hd * W;
+        ctc_collapse_segments(am, T, 1, Bg, 0, c.pad, o + 1, reinterpret_cast<int*>(o + 1 + T), reinterpret_cast<int*>(o), 2 * W, st);
+      }
+    }
+  }
+  return check_launch(h, "ss_ctc_greedy_batch");
+}
+
+int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, const int64_t* tokens_host,
+                         int Slen, float* feats_out_dev) {
+  if (h) route_from(h);
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || T_stride <= 0 || Slen <= 0 || Slen > c.max_mt_positions || !enc_dev || !T_host || !tokens_host || !feats_out_dev)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_mt_features_batch");
+  // host side: [tokens int64 B*S | positions B*S | self key lengths B | cross key lengths B], one upload
+  std::vector<int64_t> toks(tokens_host, tokens_host + (size_t)B * Slen);
+  std::vector<int> ints((size_t)B * Slen + 2 * B);
+  int* pos = ints.data();
+  int* self_len = pos + (size_t)B * Slen;
+  int* cross_len = self_len + B;
+  for (int b = 0; b < B; ++b) {
+    if (T_host[b] < 1 || T_host[b] > T_stride) return h->fail(SS_ERR_INVALID, "ss_mt_features_batch: sample length outside [1, T_stride]");
+    const int64_t* t = tokens_host + (size_t)b * Slen;
+    int n_valid = Slen;  // trailing pads are masked as keys (ss_mt_features)
+    while (n_valid > 0 && t[n_valid - 1] == c.pad) --n_valid;
+    for (int i = 0; i < Slen; ++i) {
+      if (t[i] < 0 || t[i] >= c.tgt_vocab) return h->fail(SS_ERR_INVALID, "ss_mt_features_batch: token outside the vocabulary");
+      if (i < n_valid && t[i] == c.pad) return h->fail(SS_ERR_INVALID, "pads are only supported as a tail");
+      pos[(size_t)b * Slen + i] = t[i] == c.pad ? c.pad : c.pad + 1 + i;  // make_positions, restarting for every sample
+    }
+    self_len[b] = n_valid;
+    cross_len[b] = T_host[b];
+  }
+  cudaStream_t st = S(stream);
+  const int dim = c.mt_dim;
+  const int G = std::max(1, SS_UNIT_BATCH_ROWS / (Slen * c.ctc_upsample_rate));
+  const int Bg_max = std::min(G, B);
+  const size_t n_max = (size_t)Bg_max * Slen;
+  const size_t int_bytes = toks.size() * sizeof(int64_t) + ints.size() * sizeof(int);
+  if (!ws_begin(h, (n_max * (dim * 8 + c.mt_ffn) + (size_t)Bg_max * T_stride * 2 * dim) * sizeof(float) + int_bytes + 16 * 256))
+    return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  int64_t* tok_dev = (int64_t*)h->ws.raw(toks.size() * sizeof(int64_t));
+  int* ints_dev = (int*)h->ws.raw(ints.size() * sizeof(int));
+  DecScratch s = dec_scratch(h, (int)n_max, dim, c.mt_ffn);
+  float* x = h->ws.f32(n_max * dim);
+  float* ckv = h->ws.f32((size_t)Bg_max * T_stride * 2 * dim);
+  if (!tok_dev || !ints_dev || !s.hid || !s.qkv || !x || !ckv) return h->fail(SS_ERR_CUDA, "workspace too small");
+  cudaMemcpyAsync(tok_dev, toks.data(), toks.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(ints_dev, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess)  // (host vectors)
+    return h->fail(SS_ERR_CUDA, std::string("ss_mt_features_batch: ") + cudaGetErrorString(cudaGetLastError()));
+  const int* pos_dev = ints_dev;
+  const int* self_len_dev = pos_dev + (size_t)B * Slen;
+  const int* cross_len_dev = self_len_dev + B;
+  for (int g0 = 0; g0 < B; g0 += G) {
+    const int Bg = std::min(G, B - g0);
+    RouteSamples route(Bg);
+    const int n = Bg * Slen;
+    embed_tokens_pos(tok_dev + (size_t)g0 * Slen, pos_dev + (size_t)g0 * Slen, 0, h->mt_emb, h->mt_pos, sqrtf((float)dim), x, n, dim, c.pad, st);
+    for (int l = 0; l < c.mt_layers; ++l) {
+      // this layer's cross K / V of every row of the group's samples (rows past T_b are masked by cross_len)
+      linear(enc_dev + (size_t)g0 * T_stride * c.enc_dim, c.enc_dim, Bg * T_stride, h->mt[l].ckv, ep_out(ckv, 2 * dim), st);
+      dec_layer(h->mt[l], x, n, dim, c.mt_ffn, c.mt_heads, true, 0, self_len_dev + g0, nullptr, nullptr, 0, ckv, T_stride, cross_len_dev + g0, s, st,
+                0, nullptr, Bg);
+    }
+    layer_norm(x, dim, feats_out_dev + (size_t)g0 * Slen * dim, dim, h->mt_ln.g, h->mt_ln.b, n, dim, st);
+  }
+  return check_launch(h, "ss_mt_features_batch");
+}
+
+int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
+                             int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
+  if (h) route_from(h);
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || Slen <= 0 || Slen > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev || !packed_units_dev)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_batch");
+  const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
+  std::vector<int> lens(2 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B]
+  for (int b = 0; b < B; ++b) {
+    const int np = n_pad_tail_host[b];
+    if (np < 0 || np >= Slen) return h->fail(SS_ERR_INVALID, "ss_t2u_unit_decode_batch: n_pad_tail outside [0, S)");
+    lens[b] = Slen - np;
+    lens[B + b] = (Slen - np) * R;
+  }
+  cudaStream_t st = S(stream);
+  const int G = std::max(1, SS_UNIT_BATCH_ROWS / L);
+  const int Bg_max = std::min(G, B);
+  const size_t n_max = (size_t)Bg_max * Slen, rows_max = (size_t)Bg_max * L;
+  const size_t need = (rows_max * (dim * 8 + c.unit_ffn + c.unit_vocab) + n_max * (dim * 11 + c.unit_ffn)) * sizeof(float) + lens.size() * sizeof(int) +
+                      16 * 256;
+  if (!ws_begin(h, need)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  int* lens_dev = (int*)h->ws.raw(lens.size() * sizeof(int));
+  DecScratch s1 = dec_scratch(h, (int)n_max, dim, c.unit_ffn);
+  float* x = h->ws.f32(n_max * dim);
+  float* t2u = h->ws.f32(n_max * dim);
+  float* ckv = h->ws.f32(n_max * 2 * dim);
+  DecScratch s2 = dec_scratch(h, (int)rows_max, dim, c.unit_ffn);
+  float* xu = h->ws.f32(rows_max * dim);
+  float* logits = h->ws.f32(rows_max * c.unit_vocab);
+  if (!lens_dev || !s1.qkv || !x || !t2u || !ckv || !s2.qkv || !xu || !logits) return h->fail(SS_ERR_CUDA, "workspace too small");
+  cudaMemcpyAsync(lens_dev, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess)  // (host vector)
+    return h->fail(SS_ERR_CUDA, std::string("ss_t2u_unit_decode_batch: ") + cudaGetErrorString(cudaGetLastError()));
+  Linear outp;
+  outp.w = h->unit_emb; outp.b = nullptr; outp.N = c.unit_vocab; outp.K = dim;
+  for (int g0 = 0; g0 < B; g0 += G) {
+    const int Bg = std::min(G, B - g0);
+    RouteSamples route(Bg);
+    const int n = Bg * Slen, rows = Bg * L;
+    const int* s_len = lens_dev + g0;       // T2U key lengths, unit cross-attention key lengths, valid groups of layer 1
+    const int* up_len = lens_dev + B + g0;  // unit self-attention key lengths
+    // ---- T1 on the group's samples (the encoder_padding_mask of each sample's pad tail)
+    copy_f32(mt_feats_dev + (size_t)g0 * Slen * dim, x, (int64_t)n * dim, st);
+    for (int l = 0; l < c.t2u_layers; ++l)
+      dec_layer(h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, 0, s_len, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st, 0,
+                nullptr, Bg);
+    layer_norm(x, dim, t2u, dim, h->t2u_ln.g, h->t2u_ln.b, n, dim, st);
+    // ---- U1: x R upsample + the positional row of each sample's index in the whole batch (N1), 2 layers, out-proj
+    repeat_rows_add(t2u, Slen, R, dim, pos_rows_dev + (size_t)g0 * dim, xu, Bg, st);
+    for (int l = 0; l < c.unit_layers; ++l) {
+      linear(t2u, dim, n, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
+      const int gR = (l == 0 && h->unit_grouped) ? R : 0;
+      dec_layer(h->unit[l], xu, rows, dim, c.unit_ffn, c.unit_heads, true, 0, up_len, nullptr, nullptr, 0, ckv, Slen, s_len, s2, st, gR, s_len, Bg);
+    }
+    layer_norm(xu, dim, xu, dim, h->unit_ln.g, h->unit_ln.b, rows, dim, st);
+    linear(xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st);
+    // ---- U2: never select pad, unk [+ eos], then each sample's collapse into its [count | units] row of packed_units_dev
+    int64_t* am = argmax_dev + (size_t)g0 * L;
+    int64_t* out = packed_units_dev + (size_t)g0 * (L + 1);
+    argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, nullptr, st);
+    ctc_collapse_segments(am, L, 1, Bg, c.unit_vocab - 1, c.pad, out + 1, nullptr, reinterpret_cast<int*>(out), L + 1, st);
+  }
+  return check_launch(h, "ss_t2u_unit_decode_batch");
 }
 
 int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, int U, int dur_prediction, int64_t* dur_out_dev,

@@ -154,16 +154,18 @@ void relpos_attention(const float* q, int ldq, const float* k, int ldk, const fl
                       const float* bias_u, const float* bias_v, float* out, int B, int nQ, int q_offset, int T, int H, int D,
                       int chunk /*0 = full*/, const int* lengths_dev, cudaStream_t st);
 
-// Standard multi-head attention, head_dim 64.  q rows = b*Tq + t.  kv_len[b] (device, optional) masks keys >= len.
-// causal: key j visible to query i iff j <= i + causal_offset.
+// Standard multi-head attention, head_dim 64.  q rows = b*Tq + t, k / v rows = b*Tk + j.  kv_len[b] (device, optional) masks
+// keys >= len.  causal: key j visible to query i iff j <= i + causal_offset.  Each sample gets the same kernel and arithmetic
+// as a call with B = 1.
 void mha_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int B,
                    int Tq, int Tk, int H, float scale, int causal, int causal_offset, const int* kv_len_dev,
                    cudaStream_t st);
 
-// Causal self-attention over S groups of R identical consecutive rows (unit decoder layer 1, see kernels_attn.cu): q / k / v
-// hold the S distinct rows, out gets S*R rows.  kv_len[0] (device, optional) = number of valid (non-pad) groups.
+// Causal self-attention over S groups of R identical consecutive rows (unit decoder layer 1, see kernels_attn.cu), for B samples:
+// q / k / v hold each sample's S distinct rows (rows b*S + g), out gets S*R rows per sample (rows (b*S + g)*R + r).
+// kv_len[b] (device, optional) = number of valid (non-pad) groups of sample b.
 void grouped_causal_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int S, int R,
-                              int H, float scale, const int* kv_len_dev, cudaStream_t st);
+                              int H, float scale, const int* kv_len_dev, int B, cudaStream_t st);
 
 // depthwise chunk-causal conv (k taps, left context (k-1)/2) + folded BatchNorm + SiLU, channels-last.
 // x: [B*T][C] (absolute positions 0..T-1); computes positions t0..t0+n-1 into y rows 0..n-1 per batch element.
@@ -174,12 +176,18 @@ void depthwise_bn_silu(const float* x, int ldx, const float* w /*[k][C]*/, const
 void scale_rows(float* x, int64_t n, float s, cudaStream_t st);
 void embed_tokens_pos(const int64_t* tokens, const int* positions_or_null, int pos_offset, const float* emb,
                       const float* pos_table, float scale, float* out, int rows, int C, int pad_idx, cudaStream_t st);
-void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, cudaStream_t st);
+// x [B*S][C] -> out [B*S*R][C]: every row repeated R times, plus row b of addvec [B][C] for sample b (N1 quirk, see the kernel)
+void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, int B, cudaStream_t st);
 void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx,
                  float* out_lprob_or_null, cudaStream_t st);
 // CTC collapse on one sequence: dedup consecutive, drop blank/pad.  Single CTA.
 void ctc_collapse(const int64_t* argmax, int n, int blank, int pad, int64_t* out_tokens, int* out_index, int* out_count,
                   cudaStream_t st);
+// The same for n_seg sequences of n entries, one CTA each.  Sequence s reads argmax[((s / inner) * n + i) * inner + s % inner]
+// (inner = 2: the arg-max rows of two heads interleaved) and writes out_tokens + s * seg_stride, and out_index (optional) /
+// out_count + 2 * s * seg_stride (seg_stride in int64 words, so that one packed buffer holds every sequence's output).
+void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,
+                           int* out_count, int64_t seg_stride, cudaStream_t st);
 // both CTC heads: arg-max of the new rows [row0, row0 + n_new) from logits [n_new][ld] (head h at columns h*V..), then collapse
 // of all n_rows rows of both arg-max arrays into out[head] = [count | tokens[n_rows] | index[n_rows] (int32)]
 void ctc_argmax_collapse_pair(const float* logits, int ld, int V, int n_new, int row0, int n_rows, const int* masked, int n_masked, int blank,

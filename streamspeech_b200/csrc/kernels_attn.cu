@@ -284,7 +284,8 @@ __global__ void __launch_bounds__(ATT_NT) attn_row_kernel(const float* __restric
 // multiplicities R (earlier groups) and r + 1 (own group):
 //     out[g, r] = (R * A_g + c * e_g * v_g) / (R * a_g + c * e_g),   A_g = sum_{j < g'} e_j v_j,  a_g = sum_{j < g'} e_j,
 // e_j = exp(s_j - max), g' = min(g, n_valid), c = r + 1 if g < n_valid else 0 (keys of padded groups are masked).
-// One CTA per (group, head); q / k / v are the S group rows.  out: [S*R][ldo].
+// One CTA per (group, head, sample); q / k / v of sample b are its S group rows b*S .. b*S + S-1, out gets its rows b*S*R ..
+// (S*R rows per sample) and kv_len[b] is its valid group count.  A sample's arithmetic does not depend on the batch.
 __global__ void __launch_bounds__(ATT_NT) grouped_causal_attn_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
                                                                       const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo,
                                                                       int S, int R, float scale, const int* __restrict__ kv_len) {
@@ -294,8 +295,12 @@ __global__ void __launch_bounds__(ATT_NT) grouped_causal_attn_kernel(const float
   __shared__ __align__(16) float qs[HD];
   __shared__ float red[4];
   __shared__ float part[2][HD];
-  const int g = blockIdx.x, h = blockIdx.y;
-  const int n_valid = kv_len ? min(kv_len[0], S) : S;
+  const int g = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  q += (int64_t)b * S * ldq;
+  k += (int64_t)b * S * ldk;
+  v += (int64_t)b * S * ldv;
+  out += (int64_t)b * S * R * ldo;
+  const int n_valid = kv_len ? min(kv_len[b], S) : S;
   const int n_prev = min(g, n_valid);           // earlier groups, every one of their R copies is visible
   const bool own = g < n_valid;
   const int n = n_prev + (own ? 1 : 0);         // distinct visible keys (own group last)
@@ -339,8 +344,10 @@ __global__ void __launch_bounds__(ATT_NT) grouped_causal_attn_kernel(const float
 template <bool RELPOS>
 void launch_attn(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* pos, int Tpos, int ldp,
                  const float* bias_u, const float* bias_v, float* out, int ldo, int B, int nQ, int q_offset, int T, int H, float scale,
-                 int chunk, int causal, int causal_offset, const int* lengths, cudaStream_t st) {
-  const long tiles = (long)((nQ + QT - 1) / QT) * H * B;
+                 int chunk, int causal, int causal_offset, const int* lengths, int B_choice, cudaStream_t st) {
+  // row or tile kernel, chosen from B_choice samples of this shape (1: from one sample, so that batching never switches a
+  // sample's arithmetic to the other kernel)
+  const long tiles = (long)((nQ + QT - 1) / QT) * H * B_choice;
   if (tiles < 96 && (size_t)T * sizeof(float) <= 160 * 1024) {
     size_t smem_row = (size_t)((T + 3) & ~3) * sizeof(float);
     if (smem_row > 40 * 1024 && first_time_on_device((const void*)attn_row_kernel<RELPOS>))
@@ -363,15 +370,15 @@ void relpos_attention(const float* q, int ldq, const float* k, int ldk, const fl
                       int chunk, const int* lengths_dev, cudaStream_t st) {
   ++g_launches;
   if (B <= 0 || T <= 0 || nQ <= 0) return;
-  launch_attn<true>(q, ldq, k, ldk, v, ldv, pos, Tpos, D, bias_u, bias_v, out, D, B, nQ, q_offset, T, H, 0.125f, chunk, 0, 0, lengths_dev, st);
+  launch_attn<true>(q, ldq, k, ldk, v, ldv, pos, Tpos, D, bias_u, bias_v, out, D, B, nQ, q_offset, T, H, 0.125f, chunk, 0, 0, lengths_dev, B, st);
 }
 
 void grouped_causal_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int S, int R,
-                              int H, float scale, const int* kv_len_dev, cudaStream_t st) {
+                              int H, float scale, const int* kv_len_dev, int B, cudaStream_t st) {
   ++g_launches;
-  if (S <= 0 || R <= 0) return;
-  launch_pdl(grouped_causal_attn_kernel, dim3(S, H), dim3(ATT_NT), (size_t)((S + 3) & ~3) * sizeof(float), st, q, ldq, k, ldk, v, ldv, out, ldo, S, R,
-             scale, kv_len_dev);
+  if (S <= 0 || R <= 0 || B <= 0) return;
+  launch_pdl(grouped_causal_attn_kernel, dim3(S, H, B), dim3(ATT_NT), (size_t)((S + 3) & ~3) * sizeof(float), st, q, ldq, k, ldk, v, ldv, out, ldo, S,
+             R, scale, kv_len_dev);
 }
 
 void mha_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int B,
@@ -380,7 +387,7 @@ void mha_attention(const float* q, int ldq, const float* k, int ldk, const float
   ++g_launches;
   if (B <= 0 || Tq <= 0 || Tk <= 0) return;
   launch_attn<false>(q, ldq, k, ldk, v, ldv, nullptr, 0, 0, nullptr, nullptr, out, ldo, B, Tq, 0, Tk, H, scale, 0, causal, causal_offset,
-                     kv_len_dev, st);
+                     kv_len_dev, 1, st);
 }
 
 }  // namespace ss

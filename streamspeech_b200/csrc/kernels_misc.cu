@@ -123,10 +123,11 @@ __global__ void repeat_rows_add_kernel(const float* __restrict__ x, int S, int R
                                        float* __restrict__ out) {
   pdl_trigger();
   pdl_wait();
-  int r = blockIdx.x;  // output row s*R + rr
+  int r = blockIdx.x;  // output row (b*S + s)*R + rr
   int s = r / R;
   const float* xr = x + (int64_t)s * C;
-  // N1 quirk: position index comes from the VALUE x[t, b, 0]: != 1.0 -> pad+1 (addvec), == 1.0 -> pad (zero row)
+  if (addvec) addvec += (int64_t)(r / (S * R)) * C;  // sample b's row
+  // N1 quirk: position index comes from the VALUE x[t, b, 0]: != 1.0 -> pad+1+b (addvec), == 1.0 -> pad (zero row)
   bool add = addvec != nullptr && xr[0] != 1.0f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = xr[c] + (add ? addvec[c] : 0.f);
 }
@@ -192,19 +193,26 @@ __global__ void argmax_rows_kernel(const float* __restrict__ logits, int ld, int
   }
 }
 
-__global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, int blank, int pad, int64_t* __restrict__ toks,
-                                    int* __restrict__ index, int* __restrict__ count) {
+// sequence s = blockIdx.x: entries am[((s / inner) * n + i) * inner + s % inner], outputs at s * seg_stride int64 words
+__global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, int inner, int blank, int pad, int64_t* __restrict__ toks,
+                                    int* __restrict__ index, int* __restrict__ count, int64_t seg_stride) {
   pdl_trigger();
   pdl_wait();
-  // one CTA of 1024 threads; thread t owns the contiguous slice [t*per, (t+1)*per); block-wide exclusive scan of the keep counts
+  // one CTA of 1024 threads per sequence; thread t owns the contiguous slice [t*per, (t+1)*per); block-wide exclusive scan of the
+  // keep counts
   __shared__ int wsum[32];
+  const int s = blockIdx.x;
+  am += (int64_t)(s / inner) * n * inner + s % inner;
+  toks += s * seg_stride;
+  if (index) index += 2 * s * seg_stride;
+  count += 2 * s * seg_stride;
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
   const int per = (n + 1023) / 1024;
   const int lo = min(n, t * per), hi = min(n, lo + per);
   int c = 0;
   for (int i = lo; i < hi; ++i) {
-    int64_t v = am[i];
-    c += ((i == 0 || v != am[i - 1]) && v != blank && v != pad) ? 1 : 0;
+    int64_t v = am[(int64_t)i * inner];
+    c += ((i == 0 || v != am[(int64_t)(i - 1) * inner]) && v != blank && v != pad) ? 1 : 0;
   }
   int inc = c;  // inclusive scan inside the warp
 #pragma unroll
@@ -226,8 +234,8 @@ __global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, int b
   __syncthreads();
   int base = (w > 0 ? wsum[w - 1] : 0) + inc - c;
   for (int i = lo; i < hi; ++i) {
-    int64_t v = am[i];
-    if ((i == 0 || v != am[i - 1]) && v != blank && v != pad) {
+    int64_t v = am[(int64_t)i * inner];
+    if ((i == 0 || v != am[(int64_t)(i - 1) * inner]) && v != blank && v != pad) {
       toks[base] = v;
       if (index) index[base] = i;
       ++base;
@@ -462,10 +470,10 @@ void embed_tokens_pos(const int64_t* tokens, const int* positions_or_null, int p
   launch_pdl(embed_tokens_pos_kernel, dim3(rows), dim3(128), 0, st, tokens, positions_or_null, pos_offset, emb, pos_table, scale, out, rows, C, pad_idx);
 }
 
-void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, cudaStream_t st) {
+void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, int B, cudaStream_t st) {
   ++g_launches;
-  if (S * R <= 0) return;
-  launch_pdl(repeat_rows_add_kernel, dim3(S * R), dim3(128), 0, st, x, S, R, C, addvec_or_null, out);
+  if (S * R <= 0 || B <= 0) return;
+  launch_pdl(repeat_rows_add_kernel, dim3(B * S * R), dim3(128), 0, st, x, S, R, C, addvec_or_null, out);
 }
 
 void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx,
@@ -478,7 +486,14 @@ void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked
 void ctc_collapse(const int64_t* argmax, int n, int blank, int pad, int64_t* out_tokens, int* out_index, int* out_count,
                   cudaStream_t st) {
   ++g_launches;
-  launch_pdl(ctc_collapse_kernel, dim3(1), dim3(1024), 0, st, argmax, n, blank, pad, out_tokens, out_index, out_count);
+  launch_pdl(ctc_collapse_kernel, dim3(1), dim3(1024), 0, st, argmax, n, 1, blank, pad, out_tokens, out_index, out_count, (int64_t)0);
+}
+
+void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,
+                           int* out_count, int64_t seg_stride, cudaStream_t st) {
+  ++g_launches;
+  if (n_seg <= 0) return;
+  launch_pdl(ctc_collapse_kernel, dim3(n_seg), dim3(1024), 0, st, argmax, n, inner, blank, pad, out_tokens, out_index, out_count, seg_stride);
 }
 
 void ctc_argmax_collapse_pair(const float* logits, int ld, int V, int n_new, int row0, int n_rows, const int* masked, int n_masked, int blank,

@@ -78,6 +78,9 @@ def load_library() -> ctypes.CDLL:
     lib.ss_mt_greedy_incremental.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp, i32, ctypes.POINTER(i32)]
     lib.ss_mt_features.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp]
     lib.ss_t2u_unit_decode.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp]
+    lib.ss_ctc_greedy_batch.argtypes = [vp, vp, vp, i32, i32, vp]
+    lib.ss_mt_features_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, vp]
+    lib.ss_t2u_unit_decode_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, vp, vp]
     lib.ss_unit_position_row.argtypes = [vp, vp]
     lib.ss_vocoder_durations.argtypes = [vp, vp, vp, i32, i32, vp, vp]
     lib.ss_vocoder_generate.argtypes = [vp, vp, i32, i32, i32, i32, vp]
@@ -112,7 +115,8 @@ EXPORTED_SYMBOLS = [
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
-    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch",
+    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
+    "ss_t2u_unit_decode_batch",
 ]
 
 
@@ -446,11 +450,71 @@ class Engine:
         n = int(host[:1].view(torch.int32)[0])
         return host[1:1 + n].tolist()
 
+    def unit_position_row(self, b: int) -> torch.Tensor:
+        """positional row of batch element b in the reference's unit decoder: pad + 1 + b at every time step (SURVEY.md N1)"""
+        return constants.sinusoidal_table(self.cfg.pad + 4 + int(b), self.cfg.unit_dim, self.cfg.pad)[self.cfg.pad + 1 + int(b)].contiguous().float()
+
     def set_unit_batch_index(self, b: int):
         """Batch element b of the reference's unit decoder gets positional row pad + 1 + b at every time step (SURVEY.md N1).
         b = 0 is what the streaming agents use (and what the engine is created with)."""
-        row = constants.sinusoidal_table(self.cfg.pad + 4 + int(b), self.cfg.unit_dim, self.cfg.pad)[self.cfg.pad + 1 + int(b)].contiguous().float()
+        row = self.unit_position_row(b)
         self._check(self.lib.ss_unit_position_row(self._h, row.data_ptr()))
+
+    # ------------------------------------------------------------------ offline batch (one call per stage for all samples)
+    def ctc_greedy_batch(self, enc: torch.Tensor):
+        """Both CTC heads over every row of a padded batch enc [B, T, C] (ss_ctc_greedy_batch, padded rows included).  Returns
+        ([((tokens0, index0), (tokens1, index1)) per sample], packed device tensor) after ONE device->host copy."""
+        assert enc.is_cuda and enc.is_contiguous() and enc.dim() == 3
+        B, T = int(enc.shape[0]), int(enc.shape[1])
+        W = 2 * T + 2
+        packed = torch.empty(B * 2 * W, dtype=torch.int64, device=self.device)
+        self._check(self.lib.ss_ctc_greedy_batch(self._h, self._stream(), enc.data_ptr(), B, T, packed.data_ptr()))
+        host = packed.cpu()
+        res = []
+        for b in range(B):
+            heads = []
+            for hd in (0, 1):
+                row = host[(2 * b + hd) * W:(2 * b + hd + 1) * W]
+                n = int(row[:1].view(torch.int32)[0])
+                heads.append((row[1:1 + n].tolist(), row[1 + T:].view(torch.int32)[:n].tolist()))
+            res.append((heads[0], heads[1]))
+        return res, packed
+
+    def mt_features_batch(self, enc: torch.Tensor, enc_lengths: Sequence[int], tokens: Sequence[Sequence[int]]) -> torch.Tensor:
+        """mt_features for every sample of a padded batch (ss_mt_features_batch): enc [B, T, C], sample b attends to its first
+        enc_lengths[b] rows; tokens [B][S] = [eos, hyp..., pad...].  Returns the features [B, S, mt_dim] (device)."""
+        assert enc.is_cuda and enc.is_contiguous() and enc.dim() == 3
+        B, T = int(enc.shape[0]), int(enc.shape[1])
+        if len(enc_lengths) != B or len(tokens) != B:
+            raise EngineError(f"{len(enc_lengths)} lengths and {len(tokens)} token rows for a batch of {B}")
+        S = len(tokens[0]) if B else 0
+        if any(len(t) != S for t in tokens):
+            raise EngineError("every token row of the batch must have the same length")
+        lens = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in enc_lengths])
+        toks = (ctypes.c_int64 * max(B * S, 1))(*[int(t) for row in tokens for t in row])
+        feats = self._f32(B, S, self.cfg.mt_dim)
+        self._check(self.lib.ss_mt_features_batch(self._h, self._stream(), enc.data_ptr(), B, T, lens, toks, S, feats.data_ptr()))
+        return feats
+
+    def t2u_unit_decode_batch(self, mt_feats: torch.Tensor, n_pad_tail: Sequence[int], mask_eos: bool = False):
+        """t2u_unit_decode for every sample of a padded batch mt_feats [B, S, mt_dim] (ss_t2u_unit_decode_batch), sample b with
+        positional row unit_position_row(b) (N1).  Returns (units per sample, arg-max per sample, {"argmax": [B, S*rate],
+        "packed": [B, S*rate + 1]} device tensors); the python lists come from ONE device->host copy."""
+        assert mt_feats.is_cuda and mt_feats.is_contiguous() and mt_feats.dim() == 3
+        B, S = int(mt_feats.shape[0]), int(mt_feats.shape[1])
+        if len(n_pad_tail) != B:
+            raise EngineError(f"{len(n_pad_tail)} pad-tail lengths for a batch of {B}")
+        L = S * self.cfg.ctc_upsample_rate
+        rows = torch.stack([self.unit_position_row(b) for b in range(B)]).to(self.device) if B else self._f32(0, self.cfg.unit_dim)
+        buf = torch.empty(B * (2 * L + 1), dtype=torch.int64, device=self.device)  # [argmax B*L | packed B*(L+1)]
+        am, packed = buf[:B * L].view(B, L), buf[B * L:].view(B, L + 1)
+        pads = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in n_pad_tail])
+        self._check(self.lib.ss_t2u_unit_decode_batch(self._h, self._stream(), mt_feats.data_ptr(), B, S, pads, rows.data_ptr(), int(mask_eos),
+                                                      am.data_ptr(), packed.data_ptr()))
+        host = buf.cpu()
+        h_am, h_packed = host[:B * L].view(B, L), host[B * L:].view(B, L + 1)
+        units = [h_packed[b, 1:1 + int(h_packed[b, :1].view(torch.int32)[0])].tolist() for b in range(B)]
+        return units, [h_am[b].tolist() for b in range(B)], {"argmax": am, "packed": packed}
 
     def vocoder_durations(self, codes: torch.Tensor, dur_prediction: bool = True):
         assert codes.is_cuda and codes.dtype == torch.int64 and codes.is_contiguous()

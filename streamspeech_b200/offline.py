@@ -5,15 +5,17 @@ Drop-in for the reference's `CTCMultiDecoderSequenceGenerator` as `fairseq-gener
 `--beam-mt 1 --beam 1`, plus the batch-1 vocoder pass of `generate_waveform_from_code.py:40-78`:
 
     batched padded encoder (offline model: chunk_size None)                       ss_encoder_forward(B, lengths)
-    ASR / ST CTC prints over all T rows of every sample (:206-246)                ss_ctc_greedy
+    ASR / ST CTC prints over all T rows of every sample (:206-246)                ss_ctc_greedy_batch
     MT greedy search of the batch, max_len = max_len_b_mt (:251-260)              ss_mt_greedy_batch
     prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum (:262-271) host
-    mt_decoder(features_only) -> T2U encoder -> CTC unit decoder (:287-330)       ss_mt_features, ss_t2u_unit_decode
+    mt_decoder(features_only) on the padded batch (:287-291)                      ss_mt_features_batch
+    T2U encoder -> CTC unit decoder -> CTC generate (:293-330)                    ss_t2u_unit_decode_batch
 
-The reference runs the last three on the padded batch; utterances only interact through three quirks, which the per-sample
-calls reproduce exactly (oracle/offline_oracle.py is pinned against the reference modules on a padded batch):
+Each stage is one call for the whole batch (the entry points split batches larger than their workspace budget into groups
+themselves), so the host synchronisations of generate() do not grow with B.  Samples only interact through three quirks of the
+reference, which the batched calls reproduce (oracle/offline_oracle.py is pinned against the reference modules on a padded batch):
   N1  the unit decoder's positional embedding is indexed by the BATCH axis: sample b gets position b + 2 at every step
-      -> Engine.set_unit_batch_index(b)
+      -> Engine.t2u_unit_decode_batch passes every sample's row (Engine.unit_position_row(b))
   N2  hypotheses keep the tokens emitted at padded T2U positions -> the pad tail is decoded too (n_pad_tail)
   N3  pad, unk and eos are masked before the arg-max (researches/ctc_unity/ctc_generator.py:56-58) -> mask_eos
 Beam search over the MT decoder (beam_size_mt > 1) is not implemented: the constructor refuses it.
@@ -50,35 +52,21 @@ class OfflineS2STGenerator:
         B = src_tokens.shape[0]
         lengths = [int(x) for x in src_lengths]
         enc = eng.encoder(src_tokens.contiguous(), lengths)  # [B, T, C], padded rows included
-        T = enc.shape[1]
         out_len = [eng.encoder_out_frames(n) for n in lengths]
-        results: List[Dict[str, object]] = []
-        for b in range(B):
-            eb = enc[b].contiguous()
-            am = torch.zeros(T, dtype=torch.int64, device=eb.device)
-            asr, _ = eng.ctc_greedy_rows(0, eb, 0, am)       # padded frames are NOT trimmed (ctc_decoder.py:60-63)
-            st, _ = eng.ctc_greedy_rows(1, eb, 0, am)
-            results.append({"asr_tokens": asr, "st_tokens": st})
+        prints, _ = eng.ctc_greedy_batch(enc)  # padded frames are NOT trimmed (ctc_decoder.py:60-63)
+        results: List[Dict[str, object]] = [{"asr_tokens": asr[0], "st_tokens": st[0]} for asr, st in prints]
         hyps: List[List[int]]
         if forced_mt is not None:
             hyps = [list(h) for h in forced_mt]
         else:
             hyps = eng.mt_greedy_batch(enc, out_len, self.max_len_b_mt)  # all samples in one search
-        for b in range(B):
-            results[b]["mt_tokens"] = hyps[b]
         max_tgt_len = max(len(h) for h in hyps) + 1  # hypothesis + eos (:262)
-        try:
-            for b in range(B):
-                n_pad = max_tgt_len - (len(hyps[b]) + 1)
-                prev = [c.eos] + hyps[b] + [c.pad] * n_pad
-                feats = eng.mt_features(enc[b, : out_len[b]].contiguous(), prev)
-                eng.set_unit_batch_index(b)  # N1
-                r = eng.t2u_unit_decode(feats.contiguous(), n_pad_tail=n_pad, mask_eos=True)  # N2, N3
-                results[b]["units"] = eng.units_to_host(r)
-                results[b]["unit_argmax"] = r["argmax"].tolist()
-                results[b]["mt_feats"] = feats
-        finally:
-            eng.set_unit_batch_index(0)
+        n_pad = [max_tgt_len - (len(h) + 1) for h in hyps]
+        prev = [[c.eos] + h + [c.pad] * n for h, n in zip(hyps, n_pad)]
+        feats = eng.mt_features_batch(enc, out_len, prev)  # [B, max_tgt_len, mt_dim]
+        units, argmax, _ = eng.t2u_unit_decode_batch(feats, n_pad, mask_eos=True)  # N1, N2, N3
+        for b in range(B):
+            results[b].update(mt_tokens=hyps[b], units=units[b], unit_argmax=argmax[b], mt_feats=feats[b])
         return results
 
     def units_to_codes(self, units: Sequence[int]) -> List[int]:
