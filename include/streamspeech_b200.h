@@ -218,7 +218,8 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
  * first int64) | units], so that one device->host copy reads every sample.  Sample b equals ss_t2u_unit_decode(mt_feats_b,
  * n_pad_tail_b) with the positional row set to pos_rows_dev[b] (within float tolerance for the activations; the GEMMs may take
  * another kernel at more rows).  Neither reads nor writes the handle's positional row (ss_unit_position_row) and does not
- * synchronise the device (unless the workspace has to grow); synchronises `stream` once (upload of the key lengths).
+ * synchronise the device (unless the workspace has to grow); synchronises `stream` once (upload of the key lengths) when some
+ * sample has a pad tail, not at all otherwise.  ss_t2u_unit_decode is the same code with B = 1.
  * Errors: SS_ERR_INVALID for B <= 0, S <= 0 or S > max_mt_positions, an n_pad_tail outside [0, S), or a null pointer. */
 int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
                              int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);

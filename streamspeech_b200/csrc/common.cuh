@@ -118,4 +118,109 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return red[0];
 }
 
+// arg-max of log_softmax(x[0 .. V)) with the columns masked[0 .. n_masked) excluded, first index wins on ties, for a block of 256
+// threads (CTCDecoder.generate, agent/ctc_decoder.py:53-62; F.log_softmax = (x - max) - log(sum(exp(x - max)))).  Every row of
+// every caller goes through this one reduction order, so all arg-maxes agree bit for bit.  The index is valid in thread 0.
+__device__ __forceinline__ int block_masked_argmax256(const float* __restrict__ x, int V, const int* __restrict__ masked, int n_masked) {
+  __shared__ float red[32];
+  __shared__ float sval[8];
+  __shared__ int sidx[8];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  float mx = -INFINITY;
+  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
+  mx = warp_max(mx);
+  if (lane == 0) red[w] = mx;
+  __syncthreads();
+  mx = red[0];
+  for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
+  __syncthreads();
+  float s = 0.f;
+  for (int c = tid; c < V; c += 256) s += expf(x[c] - mx);
+  s = block_sum(s, red);
+  const float lse = logf(s);
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
+  for (int c = tid; c < V; c += 256) {
+    bool m = false;
+    for (int q = 0; q < n_masked; ++q) m |= (masked[q] == c);
+    const float lp = m ? -INFINITY : (x[c] - mx) - lse;
+    if (lp > best || (lp == best && c < bi)) {
+      best = lp;
+      bi = c;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) {
+      best = ob;
+      bi = oi;
+    }
+  }
+  __syncthreads();
+  if (lane == 0) {
+    sval[w] = best;
+    sidx[w] = bi;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int i = 1; i < 8; ++i)  // per-warp winners in warp order
+      if (sval[i] > best || (sval[i] == best && sidx[i] < bi)) {
+        best = sval[i];
+        bi = sidx[i];
+      }
+  }
+  return bi;
+}
+
+// CTC collapse (CTCDecoder.generate, agent/ctc_decoder.py:64-111) of one arg-max sequence am[i * stride], i < n: repeats, then
+// blank and pad, are dropped; the kept tokens go to toks[0 .. count), their positions to index (optional), the count to *count.
+// Any block size that is a multiple of 32 up to 1024: thread t owns the contiguous slice [t * per, (t + 1) * per) and a block-wide
+// exclusive scan of the keep counts places its outputs.  The loads bypass L1 (__ldcg), so the arg-max may have been written by
+// other CTAs of the same grid.  `wsum` is 32 ints of shared memory; a caller that collapses twice synchronises in between.
+__device__ __forceinline__ void block_ctc_collapse(const int64_t* am, int64_t stride, int n, int blank, int pad, int64_t* __restrict__ toks,
+                                                   int* __restrict__ index, int* __restrict__ count, int* wsum) {
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5, nw = blockDim.x >> 5;
+  const int per = (n + (int)blockDim.x - 1) / (int)blockDim.x;
+  const int lo = min(n, t * per), hi = min(n, lo + per);
+  int c = 0;
+  int64_t prev = lo > 0 ? __ldcg(am + (int64_t)(lo - 1) * stride) : -1;
+  for (int i = lo; i < hi; ++i) {
+    const int64_t v = __ldcg(am + (int64_t)i * stride);
+    if ((i == 0 || v != prev) && v != blank && v != pad) ++c;
+    prev = v;
+  }
+  int inc = c;  // inclusive scan inside the warp, then over the warp totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  if (lane == 31) wsum[w] = inc;
+  __syncthreads();
+  if (w == 0) {
+    int s = lane < nw ? wsum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += y;
+    }
+    wsum[lane] = s;  // wsum[31] = the total
+  }
+  __syncthreads();
+  int base = (w > 0 ? wsum[w - 1] : 0) + inc - c;
+  prev = lo > 0 ? __ldcg(am + (int64_t)(lo - 1) * stride) : -1;
+  for (int i = lo; i < hi; ++i) {
+    const int64_t v = __ldcg(am + (int64_t)i * stride);
+    if ((i == 0 || v != prev) && v != blank && v != pad) {
+      toks[base] = v;
+      if (index) index[base] = i;
+      ++base;
+    }
+    prev = v;
+  }
+  if (t == 0) *count = wsum[31];
+}
+
 }  // namespace ss

@@ -126,6 +126,21 @@ int report_async_error(ss_engine* h, unsigned flag, const char* where) {
                                                    "last check are invalid (barrier re-armed)");
 }
 
+// Read-back of a burst of MT steps: `rows` rows of `width` tokens at a device pitch of `pitch` tokens (width 0: nothing to read)
+// into dst_pinned [rows][width], and the barrier error word; then one synchronisation.  A timed-out grid barrier is reported.
+int sync_burst(ss_engine* h, cudaStream_t st, int64_t* dst_pinned, const int64_t* src_dev, int width, int pitch, int rows, const char* where) {
+  if (width > 0)
+    cudaMemcpy2DAsync(dst_pinned, width * sizeof(int64_t), src_dev, pitch * sizeof(int64_t), width * sizeof(int64_t), rows, cudaMemcpyDeviceToHost, st);
+  if (h->async_err_pinned) cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string(where) + ": " + cudaGetErrorString(cudaGetLastError()));
+  if (h->async_err_pinned && *h->async_err_pinned) {
+    const unsigned f = *h->async_err_pinned;
+    *h->async_err_pinned = 0;
+    return report_async_error(h, f, where);
+  }
+  return SS_OK;
+}
+
 void clear_voc_fused(ss_engine* h) {
   cudaDeviceSynchronize();
   h->voc_fused.clear();  // (their packed weight pointers may be gone too)
@@ -443,15 +458,8 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
       if (step == 0) return -1;
       return h->fail(SS_ERR_CUDA, "cooperative launch of the batched MT kernel was refused");
     }
-    cudaMemcpy2DAsync(h->mtb_tok_pinned, cnt * sizeof(int64_t), P.tok + step + 1, ld * sizeof(int64_t), cnt * sizeof(int64_t), Bg,
-                      cudaMemcpyDeviceToHost, st);
-    if (h->async_err_pinned) cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_mt_greedy_batch: ") + cudaGetErrorString(cudaGetLastError()));
-    if (h->async_err_pinned && *h->async_err_pinned) {
-      const unsigned f = *h->async_err_pinned;
-      *h->async_err_pinned = 0;
-      return report_async_error(h, f, "ss_mt_greedy_batch");
-    }
+    rc = sync_burst(h, st, h->mtb_tok_pinned, P.tok + step + 1, cnt, ld, Bg, "ss_mt_greedy_batch");
+    if (rc) return rc;
     for (int b = 0; b < Bg; ++b) {
       for (int i = 0; i < cnt && !done[b]; ++i) {
         const int64_t next = h->mtb_tok_pinned[(size_t)b * cnt + i];
@@ -465,6 +473,78 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
     }
   }
   return SS_OK;
+}
+
+// T2U encoder -> unit decoder -> unit CTC of B samples of Slen positions (mt_feats [B][Slen][dim]); sample b adds positional row
+// pos_rows[b] (N1) and has n_pad_tail_host[b] trailing pad positions.  Its arg-max goes to argmax_dev + b * Slen * R, its units
+// to units_dev + b * seg_stride and its count to count_dev + 2 * b * seg_stride (int64 words, as ctc_collapse_segments).  Key
+// lengths are uploaded (one synchronisation) only when some sample has a pad tail; otherwise every attention runs at full length.
+// t2u_out_dev / logits_dev (optional, B = 1): the T2U encoder output and the unit logits are written there.
+int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
+                    int mask_eos, int64_t* argmax_dev, int64_t* units_dev, int32_t* count_dev, int64_t seg_stride, float* t2u_out_dev,
+                    float* logits_dev, const char* where) {
+  const ss_config& c = h->cfg;
+  const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
+  std::vector<int> lens(2 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B]
+  bool padded = false;
+  for (int b = 0; b < B; ++b) {
+    const int np = n_pad_tail_host[b];
+    if (np < 0 || np >= Slen) return h->fail(SS_ERR_INVALID, std::string(where) + ": n_pad_tail outside [0, S)");
+    lens[b] = Slen - np;
+    lens[B + b] = (Slen - np) * R;
+    padded |= np > 0;
+  }
+  const int G = std::max(1, SS_UNIT_BATCH_ROWS / L);
+  const int Bg_max = std::min(G, B);
+  const size_t n_max = (size_t)Bg_max * Slen, rows_max = (size_t)Bg_max * L;
+  const size_t need = (rows_max * (dim * 8 + c.unit_ffn + c.unit_vocab) + n_max * (dim * 11 + c.unit_ffn)) * sizeof(float) + lens.size() * sizeof(int) +
+                      16 * 256;
+  if (!ws_begin(h, need)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  int* lens_dev = padded ? (int*)h->ws.raw(lens.size() * sizeof(int)) : nullptr;
+  DecScratch s1 = dec_scratch(h, (int)n_max, dim, c.unit_ffn);
+  float* x = h->ws.f32(n_max * dim);
+  float* t2u = t2u_out_dev ? t2u_out_dev : h->ws.f32(n_max * dim);
+  float* ckv = h->ws.f32(n_max * 2 * dim);
+  DecScratch s2 = dec_scratch(h, (int)rows_max, dim, c.unit_ffn);
+  float* xu = h->ws.f32(rows_max * dim);
+  float* logits = logits_dev ? logits_dev : h->ws.f32(rows_max * c.unit_vocab);
+  if ((padded && !lens_dev) || !s1.qkv || !x || !t2u || !ckv || !s2.qkv || !xu || !logits) return h->fail(SS_ERR_CUDA, "workspace too small");
+  if (padded) {  // the encoder_padding_mask of each sample's pad tail
+    cudaMemcpyAsync(lens_dev, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess)  // (host vector)
+      return h->fail(SS_ERR_CUDA, std::string(where) + ": " + cudaGetErrorString(cudaGetLastError()));
+  }
+  Linear outp;
+  outp.w = h->unit_emb; outp.b = nullptr; outp.N = c.unit_vocab; outp.K = dim;
+  for (int g0 = 0; g0 < B; g0 += G) {
+    const int Bg = std::min(G, B - g0);
+    RouteSamples route(Bg);
+    const int n = Bg * Slen, rows = Bg * L;
+    const int* s_len = padded ? lens_dev + g0 : nullptr;       // T2U key lengths, unit cross-attention key lengths, valid groups of layer 1
+    const int* up_len = padded ? lens_dev + B + g0 : nullptr;  // unit self-attention key lengths
+    // ---- T1: UniTransformerEncoderNoEmb.forward on the group's samples
+    copy_f32(mt_feats_dev + (size_t)g0 * Slen * dim, x, (int64_t)n * dim, st);
+    for (int l = 0; l < c.t2u_layers; ++l)
+      dec_layer(h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, 0, s_len, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st, 0,
+                nullptr, Bg);
+    layer_norm(x, dim, t2u, dim, h->t2u_ln.g, h->t2u_ln.b, n, dim, st);
+    // ---- U1: CTCTransformerUnitDecoder: x R upsample + (quirky) positional row of each sample (N1), 2 layers, out-proj
+    repeat_rows_add(t2u, Slen, R, dim, pos_rows_dev + (size_t)g0 * dim, xu, Bg, st);
+    for (int l = 0; l < c.unit_layers; ++l) {
+      linear(t2u, dim, n, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
+      // layer 0 sees R identical copies of every T2U state (same positional row for every step, N1): grouped self-attention
+      const int gR = (l == 0 && h->unit_grouped) ? R : 0;
+      dec_layer(h->unit[l], xu, rows, dim, c.unit_ffn, c.unit_heads, true, 0, up_len, nullptr, nullptr, 0, ckv, Slen, s_len, s2, st, gR, s_len, Bg);
+    }
+    layer_norm(xu, dim, xu, dim, h->unit_ln.g, h->unit_ln.b, rows, dim, st);
+    linear(xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st);
+    // ---- U2: never select pad, unk (agent version) [+ eos: offline version], then each sample's collapse
+    int64_t* am = argmax_dev + (size_t)g0 * L;
+    argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, st);
+    ctc_collapse_segments(am, L, 1, Bg, c.unit_vocab - 1, c.pad, units_dev + g0 * seg_stride, nullptr, count_dev + 2 * g0 * seg_stride, seg_stride,
+                          st);
+  }
+  return check_launch(h, where);
 }
 
 }  // namespace
@@ -761,9 +841,10 @@ int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_de
     if (!ws_begin(h, (size_t)nr * l.N * sizeof(float) + 4096)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
     float* logits = h->ws.f32((size_t)nr * l.N);
     linear(enc_dev + (size_t)row0 * h->cfg.enc_dim, h->cfg.enc_dim, nr, l, ep_out(logits, l.N), st);
-    argmax_rows(logits, l.N, nr, l.N, h->mask_pad_unk, 2, argmax_dev + row0, nullptr, st);  // never select pad, unk
+    argmax_rows(logits, l.N, nr, l.N, h->mask_pad_unk, 2, argmax_dev + row0, st);  // never select pad, unk
   }
-  ctc_collapse(argmax_dev, rows, 0 /* <s> is the CTC blank (agent/ctc_decoder.py:72-76) */, h->cfg.pad, tokens_dev, index_dev, count_dev, st);
+  // <s> is the CTC blank (agent/ctc_decoder.py:72-76)
+  ctc_collapse_segments(argmax_dev, rows, 1, 1, 0, h->cfg.pad, tokens_dev, index_dev, count_dev, 0, st);
   return check_launch(h, "ss_ctc_greedy");
 }
 
@@ -923,23 +1004,15 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
       linear(feats_out_dev + (size_t)step * dim, dim, 1, outp, ep_out(logits, c.tgt_vocab), st);
       // lprobs[pad] = -inf; eos banned while step < min_len (=1)
       if (step < 1)
-        argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_eos, 2, h->mt_tok_dev + step + 1, nullptr, st);
+        argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_eos, 2, h->mt_tok_dev + step + 1, st);
       else
-        argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_unk, 1, h->mt_tok_dev + step + 1, nullptr, st);
+        argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_unk, 1, h->mt_tok_dev + step + 1, st);
     }
     // tokens produced by this burst live at mt_tok_dev[burst_first+1 .. ]; the forced-eos step produced none
     int produced = step - burst_first - (done ? 1 : 0);
     if (produced > 0) {
-      cudaMemcpyAsync(h->mt_next_pinned, h->mt_tok_dev + burst_first + 1, produced * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
-      if (h->async_err_pinned)
-        cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
-      if (cudaStreamSynchronize(st) != cudaSuccess)
-        return h->fail(SS_ERR_CUDA, std::string("ss_mt_greedy: ") + cudaGetErrorString(cudaGetLastError()));
-      if (h->async_err_pinned && *h->async_err_pinned) {
-        const unsigned f = *h->async_err_pinned;
-        *h->async_err_pinned = 0;
-        return report_async_error(h, f, "ss_mt_greedy");
-      }
+      rc = sync_burst(h, st, h->mt_next_pinned, h->mt_tok_dev + burst_first + 1, produced, produced, 1, "ss_mt_greedy");
+      if (rc) return rc;
       int steps_run = produced;
       for (int i = 0; i < produced; ++i) {
         int64_t next = h->mt_next_pinned[i];
@@ -1071,14 +1144,8 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
       return h->fail(SS_ERR_CUDA, "cooperative launch of the persistent MT kernel was refused");
     }
     const int readable = std::min(cnt, max_len - step);  // the forced-eos step writes no token
-    if (readable > 0) cudaMemcpyAsync(h->mt_next_pinned, h->mt_tok_dev + step + 1, readable * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
-    if (h->async_err_pinned) cudaMemcpyAsync(h->async_err_pinned, h->persist_bar + SS_BAR_ERR_WORD, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_mt_greedy_incremental: ") + cudaGetErrorString(cudaGetLastError()));
-    if (h->async_err_pinned && *h->async_err_pinned) {
-      const unsigned f = *h->async_err_pinned;
-      *h->async_err_pinned = 0;
-      return report_async_error(h, f, "ss_mt_greedy_incremental");
-    }
+    rc = sync_burst(h, st, h->mt_next_pinned, h->mt_tok_dev + step + 1, readable, readable, 1, "ss_mt_greedy_incremental");
+    if (rc) return rc;
     for (int i = 0; i < cnt && !done; ++i) {
       const int sidx = step + i;            // this step fed the token at position sidx (one more cache entry)
       h->mt_inc_self_len = sidx + kv_off + 1;
@@ -1098,50 +1165,10 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
                        int64_t* units_dev, int32_t* count_dev, float* t2u_out_dev, float* logits_dev) {
   if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
-  const ss_config& c = h->cfg;
-  cudaStream_t st = S(stream);
   if (Slen <= 0 || n_pad_tail < 0 || n_pad_tail >= Slen) return h->fail(SS_ERR_INVALID, "bad T2U sequence length");
-  const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
-  size_t need = ((size_t)L * (dim * 8 + c.unit_ffn + c.unit_vocab) + (size_t)Slen * dim * 12 + (size_t)Slen * c.unit_ffn + 8192) * sizeof(float);
-  if (!ws_begin(h, need)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
-  // ---- T1: UniTransformerEncoderNoEmb.forward
-  DecScratch s1 = dec_scratch(h, Slen, dim, c.unit_ffn);
-  float* x = h->ws.f32((size_t)Slen * dim);
-  float* t2u = t2u_out_dev ? t2u_out_dev : h->ws.f32((size_t)Slen * dim);
-  int* kvlen = nullptr;
-  int* kvlen_up = nullptr;
-  if (n_pad_tail > 0) {  // encoder_padding_mask on the trailing pad positions
-    int v[2] = {Slen - n_pad_tail, (Slen - n_pad_tail) * R};
-    kvlen = (int*)h->ws.raw(2 * sizeof(int));
-    kvlen_up = kvlen + 1;
-    cudaMemcpyAsync(kvlen, v, sizeof(v), cudaMemcpyHostToDevice, st);
-    cudaStreamSynchronize(st);
-  }
-  copy_f32(mt_feats_dev, x, (int64_t)Slen * dim, st);
-  for (int l = 0; l < c.t2u_layers; ++l)
-    dec_layer(h->t2u[l], x, Slen, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, 0, kvlen, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st);
-  layer_norm(x, dim, t2u, dim, h->t2u_ln.g, h->t2u_ln.b, Slen, dim, st);
-  // ---- U1: CTCTransformerUnitDecoder: x25 upsample + (quirky) positional embedding, 2 layers, out-proj
-  DecScratch s2 = dec_scratch(h, L, dim, c.unit_ffn);
-  float* xu = h->ws.f32((size_t)L * dim);
-  float* ckv = h->ws.f32((size_t)Slen * 2 * dim);
-  float* logits = logits_dev ? logits_dev : h->ws.f32((size_t)L * c.unit_vocab);
-  if (!xu || !ckv || !logits) return h->fail(SS_ERR_CUDA, "workspace too small");
-  repeat_rows_add(t2u, Slen, R, dim, h->unit_pos_row, xu, 1, st);
-  for (int l = 0; l < c.unit_layers; ++l) {
-    linear(t2u, dim, Slen, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
-    // layer 0 sees R identical copies of every T2U state (same positional row for every step, N1): grouped self-attention
-    const int gR = (l == 0 && h->unit_grouped) ? R : 0;
-    dec_layer(h->unit[l], xu, L, dim, c.unit_ffn, c.unit_heads, true, 0, kvlen_up, nullptr, nullptr, 0, ckv, Slen, kvlen, s2, st, gR, kvlen);
-  }
-  layer_norm(xu, dim, xu, dim, h->unit_ln.g, h->unit_ln.b, L, dim, st);
-  Linear outp;
-  outp.w = h->unit_emb; outp.b = nullptr; outp.N = c.unit_vocab; outp.K = dim;
-  linear(xu, dim, L, outp, ep_out(logits, c.unit_vocab), st);
-  // ---- U2: never select pad, unk (agent version) [+ eos: offline version]
-  argmax_rows(logits, c.unit_vocab, L, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, argmax_dev, nullptr, st);
-  ctc_collapse(argmax_dev, L, c.unit_vocab - 1, c.pad, units_dev, nullptr, count_dev, st);
-  return check_launch(h, "ss_t2u_unit_decode");
+  const int32_t np = n_pad_tail;
+  return t2u_unit_decode(h, S(stream), mt_feats_dev, 1, Slen, &np, h->unit_pos_row, mask_eos, argmax_dev, units_dev, count_dev, 0, t2u_out_dev,
+                         logits_dev, "ss_t2u_unit_decode");
 }
 
 int ss_unit_position_row(ss_engine* h, const float* row_host) {
@@ -1176,14 +1203,14 @@ int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B,
     if (pair) {
       // [rows][2V] logits = 2 * rows arg-max rows of V (head-minor); sequence s = 2 b + head is sample b's head, at out + s * W
       linear(x, c.enc_dim, rows, h->ctc_pair, ep_out(logits, 2 * c.src_vocab), st);
-      argmax_rows(logits, c.src_vocab, 2 * rows, c.src_vocab, h->mask_pad_unk, 2, am, nullptr, st);  // never select pad, unk
+      argmax_rows(logits, c.src_vocab, 2 * rows, c.src_vocab, h->mask_pad_unk, 2, am, st);  // never select pad, unk
       ctc_collapse_segments(am, T, 2, 2 * Bg, 0 /* <s> = CTC blank */, c.pad, out + 1, reinterpret_cast<int*>(out + 1 + T),
                             reinterpret_cast<int*>(out), W, st);
     } else {
       for (int hd = 0; hd < 2; ++hd) {
         const Linear& l = h->ctc_head[hd];
         linear(x, c.enc_dim, rows, l, ep_out(logits, l.N), st);
-        argmax_rows(logits, l.N, rows, l.N, h->mask_pad_unk, 2, am, nullptr, st);
+        argmax_rows(logits, l.N, rows, l.N, h->mask_pad_unk, 2, am, st);
         int64_t* o = out + hd * W;
         ctc_collapse_segments(am, T, 1, Bg, 0, c.pad, o + 1, reinterpret_cast<int*>(o + 1 + T), reinterpret_cast<int*>(o), 2 * W, st);
       }
@@ -1262,63 +1289,10 @@ int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_d
   const ss_config& c = h->cfg;
   if (B <= 0 || Slen <= 0 || Slen > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev || !packed_units_dev)
     return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_batch");
-  const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
-  std::vector<int> lens(2 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B]
-  for (int b = 0; b < B; ++b) {
-    const int np = n_pad_tail_host[b];
-    if (np < 0 || np >= Slen) return h->fail(SS_ERR_INVALID, "ss_t2u_unit_decode_batch: n_pad_tail outside [0, S)");
-    lens[b] = Slen - np;
-    lens[B + b] = (Slen - np) * R;
-  }
-  cudaStream_t st = S(stream);
-  const int G = std::max(1, SS_UNIT_BATCH_ROWS / L);
-  const int Bg_max = std::min(G, B);
-  const size_t n_max = (size_t)Bg_max * Slen, rows_max = (size_t)Bg_max * L;
-  const size_t need = (rows_max * (dim * 8 + c.unit_ffn + c.unit_vocab) + n_max * (dim * 11 + c.unit_ffn)) * sizeof(float) + lens.size() * sizeof(int) +
-                      16 * 256;
-  if (!ws_begin(h, need)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
-  int* lens_dev = (int*)h->ws.raw(lens.size() * sizeof(int));
-  DecScratch s1 = dec_scratch(h, (int)n_max, dim, c.unit_ffn);
-  float* x = h->ws.f32(n_max * dim);
-  float* t2u = h->ws.f32(n_max * dim);
-  float* ckv = h->ws.f32(n_max * 2 * dim);
-  DecScratch s2 = dec_scratch(h, (int)rows_max, dim, c.unit_ffn);
-  float* xu = h->ws.f32(rows_max * dim);
-  float* logits = h->ws.f32(rows_max * c.unit_vocab);
-  if (!lens_dev || !s1.qkv || !x || !t2u || !ckv || !s2.qkv || !xu || !logits) return h->fail(SS_ERR_CUDA, "workspace too small");
-  cudaMemcpyAsync(lens_dev, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess)  // (host vector)
-    return h->fail(SS_ERR_CUDA, std::string("ss_t2u_unit_decode_batch: ") + cudaGetErrorString(cudaGetLastError()));
-  Linear outp;
-  outp.w = h->unit_emb; outp.b = nullptr; outp.N = c.unit_vocab; outp.K = dim;
-  for (int g0 = 0; g0 < B; g0 += G) {
-    const int Bg = std::min(G, B - g0);
-    RouteSamples route(Bg);
-    const int n = Bg * Slen, rows = Bg * L;
-    const int* s_len = lens_dev + g0;       // T2U key lengths, unit cross-attention key lengths, valid groups of layer 1
-    const int* up_len = lens_dev + B + g0;  // unit self-attention key lengths
-    // ---- T1 on the group's samples (the encoder_padding_mask of each sample's pad tail)
-    copy_f32(mt_feats_dev + (size_t)g0 * Slen * dim, x, (int64_t)n * dim, st);
-    for (int l = 0; l < c.t2u_layers; ++l)
-      dec_layer(h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, 0, s_len, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st, 0,
-                nullptr, Bg);
-    layer_norm(x, dim, t2u, dim, h->t2u_ln.g, h->t2u_ln.b, n, dim, st);
-    // ---- U1: x R upsample + the positional row of each sample's index in the whole batch (N1), 2 layers, out-proj
-    repeat_rows_add(t2u, Slen, R, dim, pos_rows_dev + (size_t)g0 * dim, xu, Bg, st);
-    for (int l = 0; l < c.unit_layers; ++l) {
-      linear(t2u, dim, n, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
-      const int gR = (l == 0 && h->unit_grouped) ? R : 0;
-      dec_layer(h->unit[l], xu, rows, dim, c.unit_ffn, c.unit_heads, true, 0, up_len, nullptr, nullptr, 0, ckv, Slen, s_len, s2, st, gR, s_len, Bg);
-    }
-    layer_norm(xu, dim, xu, dim, h->unit_ln.g, h->unit_ln.b, rows, dim, st);
-    linear(xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st);
-    // ---- U2: never select pad, unk [+ eos], then each sample's collapse into its [count | units] row of packed_units_dev
-    int64_t* am = argmax_dev + (size_t)g0 * L;
-    int64_t* out = packed_units_dev + (size_t)g0 * (L + 1);
-    argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, nullptr, st);
-    ctc_collapse_segments(am, L, 1, Bg, c.unit_vocab - 1, c.pad, out + 1, nullptr, reinterpret_cast<int*>(out), L + 1, st);
-  }
-  return check_launch(h, "ss_t2u_unit_decode_batch");
+  // sample b's [count | units] row of packed_units_dev: L + 1 int64 words
+  const int64_t W = (int64_t)Slen * c.ctc_upsample_rate + 1;
+  return t2u_unit_decode(h, S(stream), mt_feats_dev, B, Slen, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev + 1,
+                         reinterpret_cast<int32_t*>(packed_units_dev), W, nullptr, nullptr, "ss_t2u_unit_decode_batch");
 }
 
 int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, int U, int dur_prediction, int64_t* dur_out_dev,

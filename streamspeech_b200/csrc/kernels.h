@@ -178,14 +178,12 @@ void embed_tokens_pos(const int64_t* tokens, const int* positions_or_null, int p
                       const float* pos_table, float scale, float* out, int rows, int C, int pad_idx, cudaStream_t st);
 // x [B*S][C] -> out [B*S*R][C]: every row repeated R times, plus row b of addvec [B][C] for sample b (N1 quirk, see the kernel)
 void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, int B, cudaStream_t st);
-void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx,
-                 float* out_lprob_or_null, cudaStream_t st);
-// CTC collapse on one sequence: dedup consecutive, drop blank/pad.  Single CTA.
-void ctc_collapse(const int64_t* argmax, int n, int blank, int pad, int64_t* out_tokens, int* out_index, int* out_count,
-                  cudaStream_t st);
-// The same for n_seg sequences of n entries, one CTA each.  Sequence s reads argmax[((s / inner) * n + i) * inner + s % inner]
-// (inner = 2: the arg-max rows of two heads interleaved) and writes out_tokens + s * seg_stride, and out_index (optional) /
-// out_count + 2 * s * seg_stride (seg_stride in int64 words, so that one packed buffer holds every sequence's output).
+// arg-max of log_softmax over V columns of every row, masked columns excluded, first index wins on ties
+void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx, cudaStream_t st);
+// CTC collapse (dedup consecutive, drop blank/pad) of n_seg sequences of n entries, one CTA each.  Sequence s reads
+// argmax[((s / inner) * n + i) * inner + s % inner] (inner = 2: the arg-max rows of two heads interleaved) and writes
+// out_tokens + s * seg_stride, and out_index (optional) / out_count + 2 * s * seg_stride (seg_stride in int64 words, so that one
+// packed buffer holds every sequence's output; a single sequence passes n_seg = 1, inner = 1).
 void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,
                            int* out_count, int64_t seg_stride, cudaStream_t st);
 // both CTC heads: arg-max of the new rows [row0, row0 + n_new) from logits [n_new][ld] (head h at columns h*V..), then collapse

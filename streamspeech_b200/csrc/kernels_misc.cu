@@ -132,121 +132,29 @@ __global__ void repeat_rows_add_kernel(const float* __restrict__ x, int S, int R
   for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = xr[c] + (add ? addvec[c] : 0.f);
 }
 
-// arg-max of log_softmax(logits) with masked columns, first index wins on ties
-// (CTCDecoder.generate, agent/ctc_decoder.py:53-62; F.log_softmax = (x - max) - log(sum(exp(x - max))))
+// arg-max rows (block_masked_argmax256), one CTA of 256 threads per row
 __global__ void argmax_rows_kernel(const float* __restrict__ logits, int ld, int V, const int* __restrict__ masked, int n_masked,
-                                   int64_t* __restrict__ out_idx, float* __restrict__ out_lprob) {
+                                   int64_t* __restrict__ out_idx) {
   pdl_trigger();
   pdl_wait();
-  __shared__ float red[32];
-  __shared__ float sval[32];
-  __shared__ int sidx[32];
-  int row = blockIdx.x;
-  const float* x = logits + (int64_t)row * ld;
-  float mx = -INFINITY;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) mx = fmaxf(mx, x[c]);
-  mx = warp_max(mx);
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (lane == 0) red[w] = mx;
-  __syncthreads();
-  mx = red[0];
-  for (int i = 1; i < nw; ++i) mx = fmaxf(mx, red[i]);
-  __syncthreads();
-  float s = 0.f;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) s += expf(x[c] - mx);
-  s = block_sum(s, red);
-  float lse = logf(s);
-  float best = -INFINITY;
-  int bi = 0x7fffffff;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) {
-    bool m = false;
-    for (int q = 0; q < n_masked; ++q) m |= (masked[q] == c);
-    float lp = m ? -INFINITY : (x[c] - mx) - lse;
-    if (lp > best || (lp == best && c < bi)) {
-      best = lp;
-      bi = c;
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ob > best || (ob == best && oi < bi)) {
-      best = ob;
-      bi = oi;
-    }
-  }
-  __syncthreads();
-  if (lane == 0) {
-    sval[w] = best;
-    sidx[w] = bi;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < nw; ++i)
-      if (sval[i] > best || (sval[i] == best && sidx[i] < bi)) {
-        best = sval[i];
-        bi = sidx[i];
-      }
-    out_idx[row] = bi;
-    if (out_lprob) out_lprob[row] = best;
-  }
+  const int bi = block_masked_argmax256(logits + (int64_t)blockIdx.x * ld, V, masked, n_masked);
+  if (threadIdx.x == 0) out_idx[blockIdx.x] = bi;
 }
 
-// sequence s = blockIdx.x: entries am[((s / inner) * n + i) * inner + s % inner], outputs at s * seg_stride int64 words
+// CTC collapse (block_ctc_collapse), one CTA of 1024 threads per sequence s = blockIdx.x: entries am[((s / inner) * n + i) * inner +
+// s % inner], outputs at s * seg_stride int64 words
 __global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, int inner, int blank, int pad, int64_t* __restrict__ toks,
                                     int* __restrict__ index, int* __restrict__ count, int64_t seg_stride) {
   pdl_trigger();
   pdl_wait();
-  // one CTA of 1024 threads per sequence; thread t owns the contiguous slice [t*per, (t+1)*per); block-wide exclusive scan of the
-  // keep counts
   __shared__ int wsum[32];
   const int s = blockIdx.x;
-  am += (int64_t)(s / inner) * n * inner + s % inner;
-  toks += s * seg_stride;
-  if (index) index += 2 * s * seg_stride;
-  count += 2 * s * seg_stride;
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  const int per = (n + 1023) / 1024;
-  const int lo = min(n, t * per), hi = min(n, lo + per);
-  int c = 0;
-  for (int i = lo; i < hi; ++i) {
-    int64_t v = am[(int64_t)i * inner];
-    c += ((i == 0 || v != am[(int64_t)(i - 1) * inner]) && v != blank && v != pad) ? 1 : 0;
-  }
-  int inc = c;  // inclusive scan inside the warp
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int y = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += y;
-  }
-  if (lane == 31) wsum[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    int s = wsum[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    wsum[lane] = s;
-  }
-  __syncthreads();
-  int base = (w > 0 ? wsum[w - 1] : 0) + inc - c;
-  for (int i = lo; i < hi; ++i) {
-    int64_t v = am[(int64_t)i * inner];
-    if ((i == 0 || v != am[(int64_t)(i - 1) * inner]) && v != blank && v != pad) {
-      toks[base] = v;
-      if (index) index[base] = i;
-      ++base;
-    }
-  }
-  if (t == 1023) *count = wsum[31];
+  block_ctc_collapse(am + (int64_t)(s / inner) * n * inner + s % inner, inner, n, blank, pad, toks + s * seg_stride,
+                     index ? index + 2 * s * seg_stride : nullptr, count + 2 * s * seg_stride, wsum);
 }
 
-// Both CTC heads of one policy() call after the fused [rows][2V] projection: block b = (head, new row) computes the arg-max of
-// log_softmax with masks exactly like argmax_rows_kernel; the LAST block to finish (ticket) then collapses both arg-max
-// sequences (CTCDecoder.generate, agent/ctc_decoder.py:64-111) into the packed outputs
+// Both CTC heads of one policy() call after the fused [rows][2V] projection: block b = (head, new row) computes the arg-max; the
+// LAST block to finish (ticket) then collapses both arg-max sequences into the packed outputs
 //   out[head] = [count (int32 in the first int64) | tokens[n_rows] int64 | index[n_rows] int32], stride out_stride int64 words.
 __global__ void __launch_bounds__(256) ctc_argmax_collapse_pair_kernel(const float* __restrict__ logits, int ld, int V, int n_new, int row0,
                                                                       int n_rows, const int* __restrict__ masked, int n_masked, int blank,
@@ -254,61 +162,13 @@ __global__ void __launch_bounds__(256) ctc_argmax_collapse_pair_kernel(const flo
                                                                       unsigned* ticket) {
   pdl_trigger();
   pdl_wait();
-  __shared__ float red[32];
-  __shared__ float sval[8];
-  __shared__ int sidx[8];
-  __shared__ int scount[256];
+  __shared__ int wsum[32];
   __shared__ unsigned s_last;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int tid = threadIdx.x;
   if ((int)blockIdx.x < 2 * n_new) {
     const int head = blockIdx.x / n_new, r = blockIdx.x - head * n_new;
-    const float* x = logits + (int64_t)r * ld + head * V;
-    float mx = -INFINITY;
-    for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
-    mx = warp_max(mx);
-    if (lane == 0) red[w] = mx;
-    __syncthreads();
-    mx = red[0];
-    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
-    __syncthreads();
-    float s = 0.f;
-    for (int c = tid; c < V; c += 256) s += expf(x[c] - mx);
-    s = block_sum(s, red);
-    const float lse = logf(s);
-    float best = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int c = tid; c < V; c += 256) {
-      bool m = false;
-      for (int q = 0; q < n_masked; ++q) m |= (masked[q] == c);
-      float lp = m ? -INFINITY : (x[c] - mx) - lse;
-      if (lp > best || (lp == best && c < bi)) {
-        best = lp;
-        bi = c;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ob > best || (ob == best && oi < bi)) {
-        best = ob;
-        bi = oi;
-      }
-    }
-    __syncthreads();
-    if (lane == 0) {
-      sval[w] = best;
-      sidx[w] = bi;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      for (int i = 1; i < 8; ++i)
-        if (sval[i] > best || (sval[i] == best && sidx[i] < bi)) {
-          best = sval[i];
-          bi = sidx[i];
-        }
-      (head ? am1 : am0)[row0 + r] = bi;
-    }
+    const int bi = block_masked_argmax256(logits + (int64_t)r * ld + head * V, V, masked, n_masked);
+    if (tid == 0) (head ? am1 : am0)[row0 + r] = bi;
   }
   // ---- ticket: the last block collapses both sequences
   __syncthreads();
@@ -320,41 +180,9 @@ __global__ void __launch_bounds__(256) ctc_argmax_collapse_pair_kernel(const flo
   if (!s_last) return;
   if (tid == 0) *ticket = 0u;
   __threadfence();
-  const int per = (n_rows + 255) / 256;
   for (int head = 0; head < 2; ++head) {
-    const int64_t* am = head ? am1 : am0;
     int64_t* o = out + (int64_t)head * out_stride;
-    int64_t* toks = o + 1;
-    int* index = reinterpret_cast<int*>(o + 1 + n_rows);
-    const int lo = min(tid * per, n_rows), hi = min(lo + per, n_rows);
-    int c = 0;
-    int64_t prev = lo > 0 ? __ldcg(am + lo - 1) : -1;
-    for (int i = lo; i < hi; ++i) {
-      int64_t v = __ldcg(am + i);
-      if ((i == 0 || v != prev) && v != blank && v != pad) ++c;
-      prev = v;
-    }
-    scount[tid] = c;
-    __syncthreads();
-    // inclusive scan over 256 counts (Hillis-Steele)
-    for (int off = 1; off < 256; off <<= 1) {
-      int add = tid >= off ? scount[tid - off] : 0;
-      __syncthreads();
-      scount[tid] += add;
-      __syncthreads();
-    }
-    int base = scount[tid] - c;
-    prev = lo > 0 ? __ldcg(am + lo - 1) : -1;
-    for (int i = lo; i < hi; ++i) {
-      int64_t v = __ldcg(am + i);
-      if ((i == 0 || v != prev) && v != blank && v != pad) {
-        toks[base] = v;
-        index[base] = i;
-        ++base;
-      }
-      prev = v;
-    }
-    if (tid == 255) *reinterpret_cast<int*>(o) = scount[255];
+    block_ctc_collapse(head ? am1 : am0, 1, n_rows, blank, pad, o + 1, reinterpret_cast<int*>(o + 1 + n_rows), reinterpret_cast<int*>(o), wsum);
     __syncthreads();
   }
 }
@@ -476,17 +304,10 @@ void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or
   launch_pdl(repeat_rows_add_kernel, dim3(B * S * R), dim3(128), 0, st, x, S, R, C, addvec_or_null, out);
 }
 
-void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx,
-                 float* out_lprob_or_null, cudaStream_t st) {
+void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx, cudaStream_t st) {
   ++g_launches;
   if (rows <= 0) return;
-  launch_pdl(argmax_rows_kernel, dim3(rows), dim3(256), 0, st, logits, ld, V, masked_cols, n_masked, out_idx, out_lprob_or_null);
-}
-
-void ctc_collapse(const int64_t* argmax, int n, int blank, int pad, int64_t* out_tokens, int* out_index, int* out_count,
-                  cudaStream_t st) {
-  ++g_launches;
-  launch_pdl(ctc_collapse_kernel, dim3(1), dim3(1024), 0, st, argmax, n, 1, blank, pad, out_tokens, out_index, out_count, (int64_t)0);
+  launch_pdl(argmax_rows_kernel, dim3(rows), dim3(256), 0, st, logits, ld, V, masked_cols, n_masked, out_idx);
 }
 
 void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,

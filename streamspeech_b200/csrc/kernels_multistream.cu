@@ -7,8 +7,8 @@
 // per-stream (ragged) parts: windows gathered from / rows scattered to the slots, relative-position attention of each stream's
 // rows over ITS OWN key / value cache, the chunk-causal depthwise conv over ITS OWN conv-input cache, the 48 -> 16 kHz decimation
 // and fbank of each stream's new samples / frames, and the CTC arg-max / collapse per stream.  Arithmetic is that of the
-// single-stream kernels (kernels_attn.cu attn_row_kernel, kernels_misc.cu depthwise_bn_silu_kernel / argmax_rows_kernel /
-// ctc_collapse_kernel / resample_3to1_kernel, kernels_fbank.cu).
+// single-stream kernels (kernels_attn.cu attn_row_kernel, kernels_misc.cu depthwise_bn_silu_kernel / resample_3to1_kernel,
+// kernels_fbank.cu); the CTC kernels call the same block_masked_argmax256 / block_ctc_collapse (common.cuh).
 #include <algorithm>
 
 #include "common.cuh"
@@ -312,113 +312,33 @@ __global__ void __launch_bounds__(256) ms_resample_3to1_kernel(const float* __re
   a16_base[(int64_t)s.slot * a16_stride + i] = acc;
 }
 
-// arg-max of log_softmax with masks (argmax_rows_kernel) for the new rows of every stream: block = (row r, stream b, head),
-// logits row = (row0 + r), r < nA, columns [head * V, head * V + V); result -> am_base[(slot * 2 + head) * am_stride + a0 + r]
+// arg-max (block_masked_argmax256) of the new rows of every stream: block = (row r, stream b, head), logits row = (row0 + r),
+// r < nA, columns [head * V, head * V + V); result -> am_base[(slot * 2 + head) * am_stride + a0 + r]
 __global__ void __launch_bounds__(256) ms_ctc_argmax_kernel(const float* __restrict__ logits, int ld, int V, const int* __restrict__ masked,
                                                             int n_masked, int64_t* __restrict__ am_base, int64_t am_stride,
                                                             const MsStream* __restrict__ S) {
   pdl_trigger();
   pdl_wait();
-  __shared__ float red[32];
-  __shared__ float sval[8];
-  __shared__ int sidx[8];
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int r = blockIdx.x, b = blockIdx.y, head = blockIdx.z;
   const MsStream s = S[b];
   if (r >= s.nA) return;
-  const float* x = logits + ((int64_t)s.row0 + r) * ld + head * V;
-  float mx = -INFINITY;
-  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
-  mx = warp_max(mx);
-  if (lane == 0) red[w] = mx;
-  __syncthreads();
-  mx = red[0];
-  for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
-  __syncthreads();
-  float su = 0.f;
-  for (int c = tid; c < V; c += 256) su += expf(x[c] - mx);
-  su = block_sum(su, red);
-  const float lse = logf(su);
-  float best = -INFINITY;
-  int bi = 0x7fffffff;
-  for (int c = tid; c < V; c += 256) {
-    bool m = false;
-    for (int q = 0; q < n_masked; ++q) m |= (masked[q] == c);
-    const float lp = m ? -INFINITY : (x[c] - mx) - lse;
-    if (lp > best || (lp == best && c < bi)) {
-      best = lp;
-      bi = c;
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ob > best || (ob == best && oi < bi)) {
-      best = ob;
-      bi = oi;
-    }
-  }
-  __syncthreads();
-  if (lane == 0) {
-    sval[w] = best;
-    sidx[w] = bi;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    for (int i = 1; i < 8; ++i)
-      if (sval[i] > best || (sval[i] == best && sidx[i] < bi)) {
-        best = sval[i];
-        bi = sidx[i];
-      }
-    am_base[((int64_t)s.slot * 2 + head) * am_stride + s.a0 + r] = bi;
-  }
+  const int bi = block_masked_argmax256(logits + ((int64_t)s.row0 + r) * ld + head * V, V, masked, n_masked);
+  if (threadIdx.x == 0) am_base[((int64_t)s.slot * 2 + head) * am_stride + s.a0 + r] = bi;
 }
 
-// CTC collapse of stream b / head over rows 0 .. T-1 of its arg-max rows -> out + S[b].out_off + head * (2 T + 2):
+// CTC collapse (block_ctc_collapse) of stream b / head over rows 0 .. T-1 of its arg-max rows -> out + S[b].out_off + head * (2 T + 2):
 // [count (int32) | tokens[T] int64 | index[T] int32]
 __global__ void __launch_bounds__(256) ms_ctc_collapse_kernel(const int64_t* __restrict__ am_base, int64_t am_stride, const MsStream* __restrict__ S,
                                                               int blank, int pad, int64_t* __restrict__ out) {
   pdl_trigger();
   pdl_wait();
-  __shared__ int scount[256];
-  const int tid = threadIdx.x;
-  const int b = blockIdx.x, head = blockIdx.y;
-  const MsStream s = S[b];
+  __shared__ int wsum[32];
+  const int head = blockIdx.y;
+  const MsStream s = S[blockIdx.x];
   const int n = s.T;
-  const int64_t* am = am_base + ((int64_t)s.slot * 2 + head) * am_stride;
   int64_t* o = out + s.out_off + (int64_t)head * (2 * n + 2);
-  int64_t* toks = o + 1;
-  int* index = reinterpret_cast<int*>(o + 1 + n);
-  const int per = (n + 255) / 256;
-  const int lo = min(tid * per, n), hi = min(lo + per, n);
-  int c = 0;
-  int64_t prev = lo > 0 ? am[lo - 1] : -1;
-  for (int i = lo; i < hi; ++i) {
-    const int64_t v = am[i];
-    if ((i == 0 || v != prev) && v != blank && v != pad) ++c;
-    prev = v;
-  }
-  scount[tid] = c;
-  __syncthreads();
-  for (int off = 1; off < 256; off <<= 1) {
-    const int add = tid >= off ? scount[tid - off] : 0;
-    __syncthreads();
-    scount[tid] += add;
-    __syncthreads();
-  }
-  int base = scount[tid] - c;
-  prev = lo > 0 ? am[lo - 1] : -1;
-  for (int i = lo; i < hi; ++i) {
-    const int64_t v = am[i];
-    if ((i == 0 || v != prev) && v != blank && v != pad) {
-      toks[base] = v;
-      index[base] = i;
-      ++base;
-    }
-    prev = v;
-  }
-  if (tid == 255) *reinterpret_cast<int*>(o) = scount[255];
+  block_ctc_collapse(am_base + ((int64_t)s.slot * 2 + head) * am_stride, 1, n, blank, pad, o + 1, reinterpret_cast<int*>(o + 1 + n),
+                     reinterpret_cast<int*>(o), wsum);
 }
 
 }  // namespace

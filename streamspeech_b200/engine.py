@@ -159,6 +159,13 @@ def remove_weight_norm(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     return out
 
 
+def ctc_record(host: torch.Tensor, off: int, T: int) -> Tuple[List[int], List[int]]:
+    """(tokens, index) of the packed CTC record [count (int32 in the first int64) | tokens[T] | index[T] (int32)] at host[off:]"""
+    row = host[off:off + 2 * T + 2]
+    n = int(row[:1].view(torch.int32)[0])
+    return row[1:1 + n].tolist(), row[1 + T:].view(torch.int32)[:n].tolist()
+
+
 class Engine:
     """One model replica on one GPU.  Not thread-safe (one host thread per handle)."""
 
@@ -344,9 +351,7 @@ class Engine:
         cnt.zero_()
         self._check(self.lib.ss_ctc_greedy_rows(self._h, self._stream(), head, enc.data_ptr(), T, int(row0), argmax.data_ptr(), toks.data_ptr(),
                                                 idx.data_ptr(), cnt.data_ptr()))
-        host = out.cpu()
-        n = int(host[:1].view(torch.int32)[0])
-        return host[1:1 + n].tolist(), host[1 + T:].view(torch.int32)[:n].tolist()
+        return ctc_record(out.cpu(), 0, T)
 
     def ctc_greedy_rows_pair(self, enc: torch.Tensor, row0s: Sequence[int], argmaxes: Sequence[torch.Tensor]):
         """Both CTC heads (0 = ASR, 1 = ST) of one policy() call: the two launches are enqueued back to back and read with
@@ -365,12 +370,7 @@ class Engine:
                 self._check(self.lib.ss_ctc_greedy_rows(self._h, self._stream(), hd, enc.data_ptr(), T, int(row0s[hd]), argmaxes[hd].data_ptr(),
                                                         o[1:1 + T].data_ptr(), o[1 + T:].view(torch.int32)[:T].data_ptr(), o[:1].view(torch.int32).data_ptr()))
         host = out.cpu()
-        res = []
-        for hd in (0, 1):
-            hrow = host[hd * W:(hd + 1) * W]
-            n = int(hrow[:1].view(torch.int32)[0])
-            res.append((hrow[1:1 + n].tolist(), hrow[1 + T:].view(torch.int32)[:n].tolist()))
-        return res[0], res[1]
+        return ctc_record(host, 0, T), ctc_record(host, W, T)
 
     def mt_greedy(self, enc: torch.Tensor, prefix: Optional[Sequence[int]], max_new_tokens: int, max_len_b: int = 100,
                   stable_rows: int = 0) -> Tuple[List[int], torch.Tensor]:
@@ -470,15 +470,7 @@ class Engine:
         packed = torch.empty(B * 2 * W, dtype=torch.int64, device=self.device)
         self._check(self.lib.ss_ctc_greedy_batch(self._h, self._stream(), enc.data_ptr(), B, T, packed.data_ptr()))
         host = packed.cpu()
-        res = []
-        for b in range(B):
-            heads = []
-            for hd in (0, 1):
-                row = host[(2 * b + hd) * W:(2 * b + hd + 1) * W]
-                n = int(row[:1].view(torch.int32)[0])
-                heads.append((row[1:1 + n].tolist(), row[1 + T:].view(torch.int32)[:n].tolist()))
-            res.append((heads[0], heads[1]))
-        return res, packed
+        return [(ctc_record(host, 2 * b * W, T), ctc_record(host, (2 * b + 1) * W, T)) for b in range(B)], packed
 
     def mt_features_batch(self, enc: torch.Tensor, enc_lengths: Sequence[int], tokens: Sequence[Sequence[int]]) -> torch.Tensor:
         """mt_features for every sample of a padded batch (ss_mt_features_batch): enc [B, T, C], sample b attends to its first
@@ -627,11 +619,7 @@ class Engine:
             host = self._pool_out[:used].cpu()
             for i in range(n):
                 Ti = int(T[i])
-                for hd in range(ctc_heads):
-                    o = int(off[i]) + hd * (2 * Ti + 2)
-                    row = host[o:o + 2 * Ti + 2]
-                    cnt = int(row[:1].view(torch.int32)[0])
-                    res[i]["ctc"].append((row[1:1 + cnt].tolist(), row[1 + Ti:].view(torch.int32)[:cnt].tolist()))
+                res[i]["ctc"] = [ctc_record(host, int(off[i]) + hd * (2 * Ti + 2), Ti) for hd in range(ctc_heads)]
         return res
 
     def set_option(self, name: str, value: int):

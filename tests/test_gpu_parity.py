@@ -575,6 +575,30 @@ def test_ctc_pair_equals_single_heads(eng3, gold):
         for hd, name, (toks, idx) in ((0, "source_unigram", a), (1, "ctc_target_unigram", b)):
             assert am[hd].tolist() == g[f"ctc_{name}_argmax"].tolist(), (row0, name)
             assert toks == g[f"ctc_{name}_tokens"].tolist() and idx == g[f"ctc_{name}_index"].tolist(), (row0, name)
+    # The collapse alone (row0 = rows: no new arg-max row) of hand-made arg-max sequences, through the 1024-thread collapse kernel
+    # (ctc_greedy_rows) and the 256-thread ticket tail of the pair kernel, against a Python collapse.  Runs of up to 13 entries
+    # cross the per-thread slices of both block sizes; the sequences start and end with blanks and pads.
+    blank, pad = 0, eng3.cfg.pad
+
+    def collapse(seq):
+        keep = [i for i, v in enumerate(seq) if (i == 0 or v != seq[i - 1]) and v != blank and v != pad]
+        return [seq[i] for i in keep], keep
+
+    rng = np.random.default_rng(3)
+    for n in (1, 255, 256, 257, 1023, 1024, 1025, 3000):
+        runs = []
+        while sum(len(r) for r in runs) < n:
+            runs.append([int(rng.choice([blank, pad, 5, 6, 7, 1000]))] * int(rng.integers(1, 14)))
+        body = [v for r in runs for v in r]
+        mixed = ([blank, blank, pad] + body[: max(0, n - 6)] + [pad, blank, blank])[:n] if n >= 6 else body[:n]
+        enc = torch.zeros(n, eng3.cfg.enc_dim, device="cuda")
+        for seqs in (([blank] * n, mixed), (mixed, [6] * n), (mixed[::-1], body[:n])):
+            am = [torch.tensor(s, dtype=torch.int64, device="cuda") for s in seqs]
+            single = [eng3.ctc_greedy_rows(hd, enc, n, am[hd]) for hd in (0, 1)]
+            pair = eng3.ctc_greedy_rows_pair(enc, [n, n], am)
+            for hd in (0, 1):
+                want = collapse(seqs[hd])
+                assert single[hd] == want and pair[hd] == want, (n, hd)
 
 
 @pytest.mark.parametrize("option", ["persistent_ffn_fused", "persistent_mt_prefix", "persistent_mt"])

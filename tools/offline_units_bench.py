@@ -83,7 +83,8 @@ def batched_arm(eng, enc, out_len, hyps, stage):
         prev = [[c.eos] + h + [c.pad] * (max_tgt_len - 1 - len(h)) for h in hyps]
         return eng.mt_features_batch(enc, out_len, prev), 1  # token / length upload
     units, argmax, _ = eng.t2u_unit_decode_batch(hyps, n_pad_of, mask_eos=True)
-    return (units, argmax), 3  # positional rows upload, key-length upload, one device->host copy
+    # positional rows upload, one device->host copy, and the key-length upload when some sample has a pad tail
+    return (units, argmax), 2 + (1 if any(n_pad_of) else 0)
 
 
 def timed(eng, fn):
