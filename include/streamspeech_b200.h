@@ -223,6 +223,17 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
  * Errors: SS_ERR_INVALID for B <= 0, S <= 0 or S > max_mt_positions, an n_pad_tail outside [0, S), or a null pointer. */
 int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
                              int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);
+/* ss_t2u_unit_decode_batch over ragged lengths (the stream pool's S2ST agents: every writing stream has its own number of MT
+ * positions).  mt_feats_dev [B][S_stride][mt_dim]; sample b has S_host[b] positions, 1 <= S_b <= S_stride (S_host NULL: all S_stride),
+ * of which the last n_pad_tail_host[b] (in [0, S_b)) are N2 pad positions that are decoded; positions >= S_b are neither keys nor
+ * decoded into units.  argmax_dev [B][S_stride * rate] (rows >= S_b * rate unspecified) and packed_units_dev [B][S_stride * rate + 1]
+ * as ss_t2u_unit_decode_batch, whose call this is with every S_b = S_stride.  Sample b equals ss_t2u_unit_decode(mt_feats_b[:S_b],
+ * n_pad_tail_b) with positional row pos_rows_dev[b] (within float tolerance; the GEMMs may take another kernel at more rows).
+ * Synchronises `stream` once (upload of the key lengths) when some sample has a pad tail or S_b < S_stride, not at all otherwise.
+ * Errors: SS_ERR_INVALID for B <= 0, S_stride <= 0 or S_stride > max_mt_positions, an S_b outside [1, S_stride], an n_pad_tail
+ * outside [0, S_b), or a null pointer. */
+int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
+                              const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);
 
 /* Positional-embedding row (unit_dim floats, host memory) the CTC unit decoder adds to every upsampled T2U state.  The
  * reference computes positions from x[:, :, 0] viewed as [bsz, seq] (ctc_transformer_unit_decoder.py:176-181, SURVEY.md N1), so
@@ -279,6 +290,24 @@ int ss_pool_info(ss_engine* h, int slot, int64_t* n_audio, int32_t* n_feat, int3
  * return).  Synchronises `stream` once at entry (descriptor staging); everything else is enqueue only. */
 int ss_pool_step(ss_engine* h, void* stream, int n, const int32_t* slots_host, int ctc_heads, int64_t* packed_out_dev, int64_t packed_capacity,
                  int32_t* T_out_host, int32_t* T_final_out_host, int64_t* out_off_host);
+/* Greedy MT search (M1) of n pool streams at once, each continuing its own forced prefix: stream i (slot slots_host[i]) gets what
+ * ss_mt_greedy(enc, prefix_i, n_prefix_host[i], max_new_tokens_host[i], max_len_b) gives on the slot's encoder rows [0, T_i) of its
+ * last ss_pool_step: max_len = n_prefix + max_new_tokens, or min(max_len_b, max_mt_positions - 1) for -1 (source finished); eos banned
+ * at position 0 and forced at max_len.  prefix_host holds the n prefixes concatenated.  tokens_out_host [n][max_out]: the hypothesis
+ * without eos (prefix included), n_out_host[i] its length; feats_out_dev [n][feats_ld][mt_dim]: the decoder features of [eos, tokens...]
+ * (rows 0 .. n_out_host[i]).  Up to 32 streams are decoded together on the batched MT kernel after one teacher-forced pass over all
+ * their prefixes; larger n run as consecutive groups.  The cross-attention K / V of every slot are cached in the pool ([slot][mt_layers]
+ * [Tcap][2 * mt_dim], allocated by the first call): rows below the slot's T_final are projected once, as ss_mt_stable_rows does for one
+ * stream, until ss_pool_reset.  Groups of fewer than mt_batch_min_rows streams and refused cooperative launches decode stream by stream
+ * through ss_mt_greedy (which leaves the single-stream cross K / V cache invalid, as ss_mt_greedy_batch's fallback does); otherwise the
+ * handle's single-stream MT state (cross K / V cache, stable-rows hint, incremental state, token buffer) is neither read nor written.
+ * Tokens equal ss_mt_greedy's; features within float tolerance (the prefix rows are computed by the per-operation kernels).
+ * Synchronises `stream` once per group for the uploads and once per burst of 16 steps.
+ * Errors: SS_ERR_INVALID for a bad or repeated slot, a slot without encoder rows, a prefix longer than max_len, a prefix token outside
+ * the vocabulary or a null pointer; SS_ERR_CAPACITY when max_len + 2 > max_mt_positions, max_len > max_out or max_len >= feats_ld. */
+int ss_pool_mt_greedy(ss_engine* h, void* stream, int n, const int32_t* slots_host, const int64_t* prefix_host, const int32_t* n_prefix_host,
+                      const int32_t* max_new_tokens_host, int max_len_b, int64_t* tokens_out_host, int max_out, int32_t* n_out_host,
+                      float* feats_out_dev, int feats_ld);
 
 /* ---- single ops exported for the parity tests (same kernels the entry points above launch) ------------- */
 int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N,

@@ -43,6 +43,7 @@ SAMPLE_RATE = 16000
 FEATURE_DIM = 80
 BOW_PREFIX = "▁"
 DEFAULT_EOS = 2
+READ = ("read", None, False, False)  # the policy's READ action as (kind, wav, SpeechSegment.finished, WriteAction.finished)
 
 
 def load_streamspeech_checkpoint(args):
@@ -327,10 +328,11 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
 
     @torch.inference_mode()
     def _policy_impl(self):
-        """The body of the reference policy(); returns (kind, wav on the device, SpeechSegment.finished, WriteAction.finished)."""
-        eng, c = self.engine, self.cfg
+        """The body of the reference policy(); returns (kind, wav on the device, SpeechSegment.finished, WriteAction.finished).
+        The host stages between the engine calls are methods of their own (_gate, _after_mt, _after_t2u), which the pooled agent
+        (scheduler.PooledS2STAgent) calls between its batched engine calls."""
+        eng = self.engine
         tr = self.trace = {}
-        READ = ("read", None, False, False)
         feature = self._features()
         if feature.size(0) == 0 and not self.states.source_finished:
             return READ
@@ -338,14 +340,38 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
         self.encoder_out = enc
         (src_ctc_indices, _), (tgt_ctc_indices, _) = self._ctc_pair(enc)  # agent:437, 461
         tr["asr_tokens"], tr["st_tokens"] = src_ctc_indices, tgt_ctc_indices
+        new_subword_tokens = self._gate(src_ctc_indices, tgt_ctc_indices)
+        if new_subword_tokens is None:
+            return READ
 
+        # 1. MT decoder (agent:520-538); the hypothesis comes back without its trailing eos
+        # encoder rows below T_final are final in cached mode: their cross-attention K / V are projected once (ss_mt_stable_rows)
+        stable = self._enc_final if self.encoder_mode == "cached" else 0
+        tokens, feats = eng.mt_greedy(enc, self.tgt_subwords_indices, new_subword_tokens, max_len_b=100, stable_rows=stable)
+        action, t2u_input = self._after_mt(tokens)
+        if action is not None:
+            return action
+        prev_output_tokens_mt, n_pad_tail = t2u_input
+        # mt_decoder(prev_output_tokens_mt, features_only=True) (agent:638-642): already produced by the greedy pass
+        # unless whole-word trimming changed the sequence
+        if n_pad_tail:
+            feats = eng.mt_features(enc, prev_output_tokens_mt, stable_rows=stable)
+        else:  # causal decoder: the features of [eos, t1..tj] are the first j + 1 rows of the greedy pass
+            feats = feats[: len(prev_output_tokens_mt)]
+        # 2./3. T2U encoder + CTC unit decoder (agent:662-689)
+        r = eng.t2u_unit_decode(feats.contiguous(), n_pad_tail=n_pad_tail)
+        return self._after_t2u(eng.units_to_host(r), new_subword_tokens)
+
+    def _gate(self, src_ctc_indices, tgt_ctc_indices) -> Optional[int]:
+        """READ / WRITE gate on the CTC prefixes (agent:480-509): None = READ, else the MT call's new_subword_tokens (-1 once the
+        source is finished)."""
         if not self.states.source_finished:  # agent:480-509
             src_ctc_prefix_length = len(src_ctc_indices)
             tgt_ctc_prefix_length = len(tgt_ctc_indices)
             self.src_ctc_indices = src_ctc_indices
             if (src_ctc_prefix_length < self.src_ctc_prefix_length + self.stride_n
                     or tgt_ctc_prefix_length < self.tgt_ctc_prefix_length + self.stride_n):
-                return READ
+                return None
             self.src_ctc_prefix_length = max(src_ctc_prefix_length, self.src_ctc_prefix_length)
             self.tgt_ctc_prefix_length = max(tgt_ctc_prefix_length, self.tgt_ctc_prefix_length)
             subword_tokens = ((tgt_ctc_prefix_length - self.lagging_k1) // self.stride_n) * self.stride_n
@@ -353,17 +379,18 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
                 subword_tokens += 1
             new_subword_tokens = (subword_tokens - len(self.tgt_subwords_indices)) if self.tgt_subwords_indices is not None else subword_tokens
             if new_subword_tokens < 1:
-                return READ
+                return None
         else:
             self.src_ctc_indices = src_ctc_indices
             new_subword_tokens = -1
         new_subword_tokens = int(new_subword_tokens)
-        tr["new_subword_tokens"] = new_subword_tokens
+        self.trace["new_subword_tokens"] = new_subword_tokens
+        return new_subword_tokens
 
-        # 1. MT decoder (agent:520-538); the hypothesis comes back without its trailing eos
-        # encoder rows below T_final are final in cached mode: their cross-attention K / V are projected once (ss_mt_stable_rows)
-        stable = self._enc_final if self.encoder_mode == "cached" else 0
-        tokens, feats = eng.mt_greedy(enc, self.tgt_subwords_indices, new_subword_tokens, max_len_b=100, stable_rows=stable)
+    def _after_mt(self, tokens: List[int]):
+        """Whole-word trimming and the "same hypothesis" / "not longer" checks on the MT hypothesis (agent:540-636).  Returns
+        (action, None) when the call ends here, else (None, (prev_output_tokens_mt, n_pad_tail)): the T2U input."""
+        c = self.cfg
         tgt_subwords_indices = list(tokens)
         n_pad_tail = 0
         if self.whole_word:  # agent:540-574
@@ -375,32 +402,29 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
                 tgt_subwords_indices = tgt_subwords_indices[:j]
                 tokens = tokens[:j]
                 if j == 0:
-                    return READ
+                    return READ, None
             else:
                 # source finished: the hypothesis keeps its eos, max_tgt_len = len + 1 -> ONE trailing <pad> (agent:576-591).
                 # While reading, the hypothesis was cut to [:j] (no eos) and max_tgt_len = j + 1: no pad position.
                 n_pad_tail = 1
         prev_output_tokens_mt = [c.eos] + list(tokens) + [c.pad] * n_pad_tail  # agent:576-591
-        tr["mt_tokens"] = list(tokens)
+        self.trace["mt_tokens"] = list(tokens)
 
         if self.tgt_subwords_indices is not None and self.tgt_subwords_indices == tgt_subwords_indices:  # agent:609-626
             if not self.states.source_finished:
-                return READ
-            return self._finished_write_tuple()
+                return READ, None
+            return self._finished_write_tuple(), None
         self.tgt_subwords_indices = tgt_subwords_indices
         if not self.states.source_finished and self.prev_output_tokens_mt is not None:  # agent:629-636
             if self.prev_output_tokens_mt == prev_output_tokens_mt or len(prev_output_tokens_mt) <= len(self.prev_output_tokens_mt):
-                return READ
+                return READ, None
         self.prev_output_tokens_mt = prev_output_tokens_mt
-        # mt_decoder(prev_output_tokens_mt, features_only=True) (agent:638-642): already produced by the greedy pass
-        # unless whole-word trimming changed the sequence
-        if n_pad_tail:
-            feats = eng.mt_features(enc, prev_output_tokens_mt, stable_rows=stable)
-        else:  # causal decoder: the features of [eos, t1..tj] are the first j + 1 rows of the greedy pass
-            feats = feats[: len(prev_output_tokens_mt)]
-        # 2./3. T2U encoder + CTC unit decoder (agent:662-689)
-        r = eng.t2u_unit_decode(feats.contiguous(), n_pad_tail=n_pad_tail)
-        tmp = eng.units_to_host(r)
+        return None, (prev_output_tokens_mt, n_pad_tail)
+
+    def _after_t2u(self, tmp: List[int], new_subword_tokens: int):
+        """From the collapsed unit indices of the T2U + unit-decoder call to the action (agent:690-770): unit dictionary mapping,
+        the new units (cur_unit), the vocoder on them (one engine call per stream), the wav tail and the reset quirk."""
+        eng = self.engine
         if len(tmp) == 0:
             if not self.states.source_finished:
                 return READ
@@ -412,7 +436,7 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
             u = self.dict["tgt"][t].replace("<s>", "").replace("</s>", "")
             if u != "":
                 unit.append(int(u))
-        tr["units"] = list(unit)
+        self.trace["units"] = list(unit)
         cur_unit = unit if self.unit is None else unit[len(self.unit):]
         if len(unit) < 1 or len(cur_unit) < 1:
             if not self.states.source_finished:
@@ -425,7 +449,7 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
         cum_h = cum.tolist()
         total = cum_h[-1]
         new_frames = total - cum_h[len(unit) - len(cur_unit)]
-        tr["dur"] = [cum_h[i + 1] - cum_h[i] for i in range(len(unit))]
+        self.trace["dur"] = [cum_h[i + 1] - cum_h[i] for i in range(len(unit))]
         if self.vocoder_context == "full":
             wav_all = eng.vocoder_generate(total, 0, total, 0)
             new_wav = wav_all[-new_frames * eng.hop:]

@@ -219,6 +219,11 @@ struct ss_engine {
     std::vector<char> finished;                        // ss_pool_finish: the slot's source is closed
     std::vector<int> attn_chunk, conv_chunk;           // ss_pool_set_chunk: the slot's own chunk sizes (0, 0 = the handle's ss_set_chunk)
     std::vector<TimedLaunch> resample_events;          // option persistent_time: CUDA events around ms_resample_3to1 (bytes = 16 per output)
+    std::vector<int> T_rows;                           // encoder rows of the slot after its last step (0: none yet)
+    // ss_pool_mt_greedy: cross-attention K / V of every slot [slot][mt_layers][Tcap][2 * mt_dim] (allocated by its first call); rows
+    // [0, mt_cross_rows[slot]) were projected from final encoder rows and are not projected again until ss_pool_reset
+    float* mt_cross = nullptr;
+    std::vector<int> mt_cross_rows;
   } pool;
 
   int fail(int code, const std::string& msg) {

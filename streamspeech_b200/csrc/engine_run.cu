@@ -476,23 +476,28 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
 }
 
 // T2U encoder -> unit decoder -> unit CTC of B samples of Slen positions (mt_feats [B][Slen][dim]); sample b adds positional row
-// pos_rows[b] (N1) and has n_pad_tail_host[b] trailing pad positions.  Its arg-max goes to argmax_dev + b * Slen * R, its units
+// pos_rows[b] (N1), has S_host[b] positions (nullptr: every sample has Slen; positions >= S_b are neither keys nor decoded into
+// units) and n_pad_tail_host[b] trailing pad positions among them.  Its arg-max goes to argmax_dev + b * Slen * R, its units
 // to units_dev + b * seg_stride and its count to count_dev + 2 * b * seg_stride (int64 words, as ctc_collapse_segments).  Key
-// lengths are uploaded (one synchronisation) only when some sample has a pad tail; otherwise every attention runs at full length.
+// lengths are uploaded (one synchronisation) only when some sample has a pad tail or fewer than Slen positions; otherwise every
+// attention runs at full length.
 // t2u_out_dev / logits_dev (optional, B = 1): the T2U encoder output and the unit logits are written there.
-int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
-                    int mask_eos, int64_t* argmax_dev, int64_t* units_dev, int32_t* count_dev, int64_t seg_stride, float* t2u_out_dev,
-                    float* logits_dev, const char* where) {
+int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, int B, int Slen, const int32_t* S_host, const int32_t* n_pad_tail_host,
+                    const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* units_dev, int32_t* count_dev, int64_t seg_stride,
+                    float* t2u_out_dev, float* logits_dev, const char* where) {
   const ss_config& c = h->cfg;
   const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
-  std::vector<int> lens(2 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B]
-  bool padded = false;
+  std::vector<int> lens(3 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B | decoded upsampled rows B]
+  bool padded = false, ragged = false;
   for (int b = 0; b < B; ++b) {
-    const int np = n_pad_tail_host[b];
-    if (np < 0 || np >= Slen) return h->fail(SS_ERR_INVALID, std::string(where) + ": n_pad_tail outside [0, S)");
-    lens[b] = Slen - np;
-    lens[B + b] = (Slen - np) * R;
-    padded |= np > 0;
+    const int Sb = S_host ? S_host[b] : Slen, np = n_pad_tail_host[b];
+    if (Sb < 1 || Sb > Slen) return h->fail(SS_ERR_INVALID, std::string(where) + ": sample length outside [1, S_stride]");
+    if (np < 0 || np >= Sb) return h->fail(SS_ERR_INVALID, std::string(where) + ": n_pad_tail outside [0, S)");
+    lens[b] = Sb - np;
+    lens[B + b] = (Sb - np) * R;
+    lens[2 * B + b] = Sb * R;
+    padded |= np > 0 || Sb < Slen;
+    ragged |= Sb < Slen;
   }
   const int G = std::max(1, SS_UNIT_BATCH_ROWS / L);
   const int Bg_max = std::min(G, B);
@@ -522,6 +527,7 @@ int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, in
     const int n = Bg * Slen, rows = Bg * L;
     const int* s_len = padded ? lens_dev + g0 : nullptr;       // T2U key lengths, unit cross-attention key lengths, valid groups of layer 1
     const int* up_len = padded ? lens_dev + B + g0 : nullptr;  // unit self-attention key lengths
+    const int* dec_len = ragged ? lens_dev + 2 * B + g0 : nullptr;  // upsampled rows collapsed into units
     // ---- T1: UniTransformerEncoderNoEmb.forward on the group's samples
     copy_f32(mt_feats_dev + (size_t)g0 * Slen * dim, x, (int64_t)n * dim, st);
     for (int l = 0; l < c.t2u_layers; ++l)
@@ -542,7 +548,7 @@ int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, in
     int64_t* am = argmax_dev + (size_t)g0 * L;
     argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, st);
     ctc_collapse_segments(am, L, 1, Bg, c.unit_vocab - 1, c.pad, units_dev + g0 * seg_stride, nullptr, count_dev + 2 * g0 * seg_stride, seg_stride,
-                          st);
+                          st, dec_len);
   }
   return check_launch(h, where);
 }
@@ -1167,7 +1173,7 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (Slen <= 0 || n_pad_tail < 0 || n_pad_tail >= Slen) return h->fail(SS_ERR_INVALID, "bad T2U sequence length");
   const int32_t np = n_pad_tail;
-  return t2u_unit_decode(h, S(stream), mt_feats_dev, 1, Slen, &np, h->unit_pos_row, mask_eos, argmax_dev, units_dev, count_dev, 0, t2u_out_dev,
+  return t2u_unit_decode(h, S(stream), mt_feats_dev, 1, Slen, nullptr, &np, h->unit_pos_row, mask_eos, argmax_dev, units_dev, count_dev, 0, t2u_out_dev,
                          logits_dev, "ss_t2u_unit_decode");
 }
 
@@ -1282,17 +1288,23 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
   return check_launch(h, "ss_mt_features_batch");
 }
 
-int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
-                             int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
+int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
+                              const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
   if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
-  if (B <= 0 || Slen <= 0 || Slen > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev || !packed_units_dev)
-    return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_batch");
+  if (B <= 0 || S_stride <= 0 || S_stride > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev ||
+      !packed_units_dev)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_ragged");
   // sample b's [count | units] row of packed_units_dev: L + 1 int64 words
-  const int64_t W = (int64_t)Slen * c.ctc_upsample_rate + 1;
-  return t2u_unit_decode(h, S(stream), mt_feats_dev, B, Slen, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev + 1,
-                         reinterpret_cast<int32_t*>(packed_units_dev), W, nullptr, nullptr, "ss_t2u_unit_decode_batch");
+  const int64_t W = (int64_t)S_stride * c.ctc_upsample_rate + 1;
+  return t2u_unit_decode(h, S(stream), mt_feats_dev, B, S_stride, S_host, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev + 1,
+                         reinterpret_cast<int32_t*>(packed_units_dev), W, nullptr, nullptr, "ss_t2u_unit_decode_ragged");
+}
+
+int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
+                             int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
+  return ss_t2u_unit_decode_ragged(h, stream, mt_feats_dev, B, Slen, nullptr, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev);
 }
 
 int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, int U, int dur_prediction, int64_t* dur_out_dev,

@@ -183,9 +183,10 @@ void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked
 // CTC collapse (dedup consecutive, drop blank/pad) of n_seg sequences of n entries, one CTA each.  Sequence s reads
 // argmax[((s / inner) * n + i) * inner + s % inner] (inner = 2: the arg-max rows of two heads interleaved) and writes
 // out_tokens + s * seg_stride, and out_index (optional) / out_count + 2 * s * seg_stride (seg_stride in int64 words, so that one
-// packed buffer holds every sequence's output; a single sequence passes n_seg = 1, inner = 1).
+// packed buffer holds every sequence's output; a single sequence passes n_seg = 1, inner = 1).  n_seq_dev (device, optional): sample
+// s / inner has only its first n_seq_dev[s / inner] entries (ragged lengths at a common stride n).
 void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,
-                           int* out_count, int64_t seg_stride, cudaStream_t st);
+                           int* out_count, int64_t seg_stride, cudaStream_t st, const int* n_seq_dev = nullptr);
 // both CTC heads: arg-max of the new rows [row0, row0 + n_new) from logits [n_new][ld] (head h at columns h*V..), then collapse
 // of all n_rows rows of both arg-max arrays into out[head] = [count | tokens[n_rows] | index[n_rows] (int32)]
 void ctc_argmax_collapse_pair(const float* logits, int ld, int V, int n_new, int row0, int n_rows, const int* masked, int n_masked, int blank,

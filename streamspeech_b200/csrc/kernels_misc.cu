@@ -142,14 +142,14 @@ __global__ void argmax_rows_kernel(const float* __restrict__ logits, int ld, int
 }
 
 // CTC collapse (block_ctc_collapse), one CTA of 1024 threads per sequence s = blockIdx.x: entries am[((s / inner) * n + i) * inner +
-// s % inner], outputs at s * seg_stride int64 words
-__global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, int inner, int blank, int pad, int64_t* __restrict__ toks,
-                                    int* __restrict__ index, int* __restrict__ count, int64_t seg_stride) {
+// s % inner] for i < n (or < n_seq[s / inner]), outputs at s * seg_stride int64 words
+__global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, const int* __restrict__ n_seq, int inner, int blank, int pad,
+                                    int64_t* __restrict__ toks, int* __restrict__ index, int* __restrict__ count, int64_t seg_stride) {
   pdl_trigger();
   pdl_wait();
   __shared__ int wsum[32];
   const int s = blockIdx.x;
-  block_ctc_collapse(am + (int64_t)(s / inner) * n * inner + s % inner, inner, n, blank, pad, toks + s * seg_stride,
+  block_ctc_collapse(am + (int64_t)(s / inner) * n * inner + s % inner, inner, n_seq ? n_seq[s / inner] : n, blank, pad, toks + s * seg_stride,
                      index ? index + 2 * s * seg_stride : nullptr, count + 2 * s * seg_stride, wsum);
 }
 
@@ -311,10 +311,11 @@ void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked
 }
 
 void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,
-                           int* out_count, int64_t seg_stride, cudaStream_t st) {
+                           int* out_count, int64_t seg_stride, cudaStream_t st, const int* n_seq_dev) {
   ++g_launches;
   if (n_seg <= 0) return;
-  launch_pdl(ctc_collapse_kernel, dim3(n_seg), dim3(1024), 0, st, argmax, n, inner, blank, pad, out_tokens, out_index, out_count, seg_stride);
+  launch_pdl(ctc_collapse_kernel, dim3(n_seg), dim3(1024), 0, st, argmax, n, n_seq_dev, inner, blank, pad, out_tokens, out_index, out_count,
+             seg_stride);
 }
 
 void ctc_argmax_collapse_pair(const float* logits, int ld, int V, int n_new, int row0, int n_rows, const int* masked, int n_masked, int blank,

@@ -113,9 +113,18 @@ struct MtBatchParams {
   int64_t* tok;                             // [rows][tok_ld]: tok[b][s] is fed at step s, the arg-max goes to tok[b][s + 1]
   int* fin;                                 // [rows]: set once the row produced eos; finished rows are skipped
   float *q, *part, *delta, *hid, *logits;   // scratch per row: dim, 8 x dim, dim, ffn, vocab floats
+  // Optional per-row fields of a search that continues a forced prefix (ss_pool_mt_greedy), set all four together (a separate
+  // instantiation of the kernel reads them).  Left null, every row starts at position 0, the host stops all rows at one max_len,
+  // row r reads cross block r and no features are written.
+  const int* start = nullptr;       // [rows] position row r feeds at step 0; tok[r][k] then holds the token of position start[r] + k
+                                    // and the self-attention cache row of position p is p (the prefix rows are filled by the caller)
+  const int* max_len = nullptr;     // [rows] eos is forced at this position; that step still runs (it produces the last feature)
+  const int* cross_row = nullptr;   // [rows] cross_kv is [.][layers][cross_cap][2 * dim] and row r reads block cross_row[r]
+  float* feats = nullptr;           // [rows][feats_ld][dim]: the final-LN row of every position a row feeds
+  int feats_ld = 0;
 };
-// enqueue steps step0 .. step0 + nsteps - 1 (all < max_len: the forced-eos step needs no work) for every unfinished row;
-// returns 0, or < 0 if the launch was refused
+// enqueue steps step0 .. step0 + nsteps - 1 for every unfinished row (without P.max_len, all < the host's max_len: the forced-eos
+// step needs no work); returns 0, or < 0 if the launch was refused
 int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step0, int nsteps, unsigned* barrier_counter_dev,
                     unsigned* barrier_target_host, cudaStream_t st);
 

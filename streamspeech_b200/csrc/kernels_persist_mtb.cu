@@ -4,6 +4,9 @@
 //   per layer: [LN + QKV] | [self-attn + Wo partials] | [x += sum, LN + Wcq] | [cross-attn + Wco partials] |
 //              [x += sum, LN + FC1 + ReLU] | [FC2 -> delta]
 //   then:      [x += delta, final LN, logits = E @ feat] | [arg-max of log_softmax, row i on CTA i]
+// The stream pool's search (ss_pool_mt_greedy) continues each row after a forced prefix: with MtBatchParams' per-row fields a row
+// feeds position start + step (position embedding, cache row, self-attention length and the position-0 eos ban follow), stops at
+// its own max_len with eos forced, reads its slot's cross K / V and writes its final-LN rows as features.
 // Every CTA keeps the residual rows of all samples in shared memory (32 x 2 KB); the LayerNorm outputs share a second
 // 64 KB buffer with the FFN hidden rows, which do not fit at once (8 KB each) and are staged 8 rows at a time.
 //
@@ -144,6 +147,10 @@ __device__ __forceinline__ void attend_rows(MtSmem& sm, MtbSmem& sb, const float
   }
 }
 
+// position row r feeds at step s (kRows: a search that continues a forced prefix, MtBatchParams' per-row fields set)
+template <bool kRows>
+__device__ __forceinline__ int row_pos(const MtBatchParams& P, int r, int s) { return kRows ? P.start[r] + s : s; }
+
 __device__ __forceinline__ void load_active(MtbSmem& sb, const int* fin, int rows) {
   if (threadIdx.x == 0) {
     int n = 0;
@@ -154,6 +161,8 @@ __device__ __forceinline__ void load_active(MtbSmem& sb, const int* fin, int row
   __syncthreads();
 }
 
+// kRows = false: the per-row fields are null and compiled out (the offline generator's search as before they existed)
+template <bool kRows>
 __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P, const MtLayerP* __restrict__ layers, int step0, int nsteps,
                                                                  unsigned* bar_ctr, unsigned bar_target) {
   __shared__ __align__(16) MtSmem sm;
@@ -180,7 +189,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     for (int e = tid; e < sb.nact * DIM; e += MTT) {
       const int r = sb.act[e / DIM], c = e % DIM;
       const int64_t tok = P.tok[(size_t)r * P.tok_ld + s];
-      const int p = (tok == P.pad) ? P.pad : P.pad + 1 + s;
+      const int p = (tok == P.pad) ? P.pad : P.pad + 1 + row_pos<kRows>(P, r, s);
       xs[r * DIM + c] = emb_scale * P.emb[tok * DIM + c] + P.pos[(int64_t)p * DIM + c];
     }
     __syncthreads();
@@ -198,14 +207,14 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       }
       float* kl = P.self_k + (size_t)l * MAXR * P.tok_ld * DIM;
       float* vl = P.self_v + (size_t)l * MAXR * P.tok_ld * DIM;
-      const float* cl = P.cross_kv + (size_t)l * MAXR * P.cross_cap * 2 * DIM;
       // (1) x += FFN delta of the previous layer; q | k | v = LN(x) Wqkv^T
       if (l > 0) add_delta_rows(sb, xs, P.delta);
       ln_rows(sb, xs, vb, L.self_g, L.self_b);
       for (int i = 0; i < sb.nact; ++i) {
         const int r = sb.act[i];
-        float* kc = kl + ((size_t)r * P.tok_ld + s) * DIM;
-        float* vc = vl + ((size_t)r * P.tok_ld + s) * DIM;
+        const int pos = row_pos<kRows>(P, r, s);
+        float* kc = kl + ((size_t)r * P.tok_ld + pos) * DIM;
+        float* vc = vl + ((size_t)r * P.tok_ld + pos) * DIM;
         gemv_finish_b(w_qkv, vb + r * DIM, 3 * DIM, [&](int col, float y) {
           if (col < DIM) P.q[(size_t)r * DIM + col] = y;
           else if (col < 2 * DIM) kc[col - DIM] = y;
@@ -220,7 +229,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
           kb = kl + (size_t)r * P.tok_ld * DIM;
           vbs = vl + (size_t)r * P.tok_ld * DIM;
           ld = DIM;
-          n = s + 1;
+          n = row_pos<kRows>(P, r, s) + 1;
         }, L.wo, grp_h, grp_j, P.part);
       ARRIVE();
       GemvW<DIM, 1> w_cq;
@@ -238,7 +247,8 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       // (4) cross-attention over the first cross_len[r] encoder rows of each sample + partial out-projections
       if (in_group)
         attend_rows(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
-          kb = cl + (size_t)r * P.cross_cap * 2 * DIM;
+          const size_t blk = kRows ? (size_t)P.cross_row[r] * P.n_layers + l : (size_t)l * MAXR + r;
+          kb = P.cross_kv + blk * P.cross_cap * 2 * DIM;
           vbs = kb + DIM;
           ld = 2 * DIM;
           n = P.cross_len[r];
@@ -282,15 +292,21 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     gemv_issue(w_out, P.emb, P.vocab);
     add_delta_rows(sb, xs, P.delta);
     ln_rows(sb, xs, vb, P.out_g, P.out_b);
+    if (kRows && blockIdx.x == 0)
+      for (int e = tid; e < sb.nact * DIM; e += MTT) {
+        const int r = sb.act[e / DIM], c = e % DIM;
+        P.feats[((size_t)r * P.feats_ld + row_pos<kRows>(P, r, s)) * DIM + c] = vb[r * DIM + c];
+      }
     for (int i = 0; i < sb.nact; ++i) {
       const int r = sb.act[i];
       gemv_finish(w_out, vb + r * DIM, P.vocab, [&](int col, float acc) { P.logits[(size_t)r * P.vocab + col] = acc; });
     }
     BAR();
-    // ---- arg-max: unfinished row i on CTA i
+    // ---- arg-max: unfinished row i on CTA i (eos forced at the row's max_len)
     for (int i = blockIdx.x; i < sb.nact; i += gridDim.x) {
       const int r = sb.act[i];
-      const int tk = masked_argmax(sm, P.logits + (size_t)r * P.vocab, P.vocab, P.pad, P.eos, s);
+      const int pos = row_pos<kRows>(P, r, s);
+      const int tk = (kRows && pos >= P.max_len[r]) ? P.eos : masked_argmax(sm, P.logits + (size_t)r * P.vocab, P.vocab, P.pad, P.eos, pos);
       if (tid == 0) {
         P.tok[(size_t)r * P.tok_ld + s + 1] = tk;
         if (tk == P.eos) P.fin[r] = 1;
@@ -313,10 +329,13 @@ int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step
                     cudaStream_t st) {
   ++g_launches;
   if (P.rows < 1 || P.rows > MAXR) return -1;
-  if (first_time_on_device((const void*)mt_decode_batch_kernel)) {  // cooperative launch needs one resident CTA per SM
-    cudaFuncSetAttribute(mt_decode_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDynSmem);
+  const bool rows = P.start != nullptr;
+  if (rows && (!P.max_len || !P.cross_row || !P.feats)) return -1;  // the per-row fields come together
+  const void* kernel = rows ? (const void*)mt_decode_batch_kernel<true> : (const void*)mt_decode_batch_kernel<false>;
+  if (first_time_on_device(kernel)) {  // cooperative launch needs one resident CTA per SM
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDynSmem);
     int occ = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mt_decode_batch_kernel, MTT, kDynSmem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, MTT, kDynSmem);
     if (occ < 1) return -1;
   }
   const int grid = current_device_sms();
@@ -324,7 +343,7 @@ int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step
   MtBatchParams p = P;
   unsigned bar_target = *bar_target_host;
   void* args[] = {(void*)&p, (void*)&layers_dev, (void*)&step0, (void*)&nsteps, (void*)&bar_ctr, (void*)&bar_target};
-  if (cudaLaunchCooperativeKernel((void*)mt_decode_batch_kernel, dim3(grid), dim3(MTT), args, kDynSmem, st) != cudaSuccess) return -2;
+  if (cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(MTT), args, kDynSmem, st) != cudaSuccess) return -2;
   *bar_target_host += (unsigned)grid * (unsigned)(nsteps * (P.n_layers * 6 + 2));
   return 0;
 }

@@ -106,6 +106,8 @@ def load_library() -> ctypes.CDLL:
     lib.ss_pool_push_audio.argtypes = [vp, vp, i32, vp, i32]
     lib.ss_pool_info.argtypes = [vp, i32, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     lib.ss_pool_step.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp]
+    lib.ss_pool_mt_greedy.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32]
+    lib.ss_t2u_unit_decode_ragged.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i32, vp, vp]
     _lib = lib
     return lib
 
@@ -116,7 +118,7 @@ EXPORTED_SYMBOLS = [
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
-    "ss_t2u_unit_decode_batch",
+    "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_t2u_unit_decode_ragged",
 ]
 
 
@@ -508,6 +510,33 @@ class Engine:
         units = [h_packed[b, 1:1 + int(h_packed[b, :1].view(torch.int32)[0])].tolist() for b in range(B)]
         return units, [h_am[b].tolist() for b in range(B)], {"argmax": am, "packed": packed}
 
+    def t2u_unit_decode_ragged(self, mt_feats: torch.Tensor, lengths: Sequence[int], n_pad_tail: Sequence[int], pos_rows: Optional[torch.Tensor] = None,
+                               mask_eos: bool = False):
+        """t2u_unit_decode for every sample of mt_feats [B, S_stride, mt_dim] where sample b has only its first lengths[b] positions
+        (ss_t2u_unit_decode_ragged), n_pad_tail[b] of them N2 pad positions.  pos_rows [B, unit_dim] (device): each sample's positional
+        row, default unit_position_row(0) for every sample (what each streaming agent uses).  Returns (units per sample, arg-max per
+        sample (its lengths[b] * rate rows), {"argmax": [B, S_stride*rate], "packed": [B, S_stride*rate + 1]} device tensors); the python
+        lists come from ONE device->host copy."""
+        assert mt_feats.is_cuda and mt_feats.is_contiguous() and mt_feats.dim() == 3
+        B, S = int(mt_feats.shape[0]), int(mt_feats.shape[1])
+        if len(lengths) != B or len(n_pad_tail) != B:
+            raise EngineError(f"{len(lengths)} lengths and {len(n_pad_tail)} pad-tail lengths for a batch of {B}")
+        R = self.cfg.ctc_upsample_rate
+        L = S * R
+        if pos_rows is None:
+            pos_rows = self.unit_position_row(0).to(self.device).expand(max(B, 1), -1).contiguous()
+        assert pos_rows.is_cuda and pos_rows.is_contiguous() and pos_rows.shape[0] >= B
+        buf = torch.empty(B * (2 * L + 1), dtype=torch.int64, device=self.device)  # [argmax B*L | packed B*(L+1)]
+        am, packed = buf[:B * L].view(B, L), buf[B * L:].view(B, L + 1)
+        lens = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in lengths])
+        pads = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in n_pad_tail])
+        self._check(self.lib.ss_t2u_unit_decode_ragged(self._h, self._stream(), mt_feats.data_ptr(), B, S, lens, pads, pos_rows.data_ptr(),
+                                                       int(mask_eos), am.data_ptr(), packed.data_ptr()))
+        host = buf.cpu()
+        h_am, h_packed = host[:B * L].view(B, L), host[B * L:].view(B, L + 1)
+        units = [h_packed[b, 1:1 + int(h_packed[b, :1].view(torch.int32)[0])].tolist() for b in range(B)]
+        return units, [h_am[b, :int(lengths[b]) * R].tolist() for b in range(B)], {"argmax": am, "packed": packed}
+
     def vocoder_durations(self, codes: torch.Tensor, dur_prediction: bool = True):
         assert codes.is_cuda and codes.dtype == torch.int64 and codes.is_contiguous()
         U = codes.numel()
@@ -621,6 +650,40 @@ class Engine:
                 Ti = int(T[i])
                 res[i]["ctc"] = [ctc_record(host, int(off[i]) + hd * (2 * Ti + 2), Ti) for hd in range(ctc_heads)]
         return res
+
+    def pool_mt_greedy(self, slots: Sequence[int], prefixes: Sequence[Optional[Sequence[int]]], max_new_tokens: Sequence[int],
+                       max_len_b: int = 100) -> Tuple[List[List[int]], torch.Tensor]:
+        """Greedy MT search of several pool streams at once (ss_pool_mt_greedy) on each slot's encoder rows of its last pool_step:
+        stream i continues prefixes[i] (None = empty) with max_new_tokens[i] (-1 = source finished).  Returns (hypotheses without eos,
+        prefix included; decoder features [n, feats_ld, mt_dim] on the device, stream i's features of [eos] + hyp_i in its first
+        len(hyp_i) + 1 rows).  Each stream equals mt_greedy(enc_slot, prefixes[i], max_new_tokens[i], max_len_b)."""
+        n = len(slots)
+        if len(prefixes) != n or len(max_new_tokens) != n:
+            raise EngineError(f"{len(prefixes)} prefixes and {len(max_new_tokens)} token limits for {n} streams")
+        pfx = [list(p) if p is not None else [] for p in prefixes]
+        cap = self.max_mt_positions
+        mlen = [min(int(max_len_b), cap - 1) if int(m) == -1 else len(p) + int(m) for p, m in zip(pfx, max_new_tokens)]
+        feats_ld = max(max(mlen, default=0), 0) + 1
+        flat = [int(t) for p in pfx for t in p]
+        sl = (ctypes.c_int32 * max(n, 1))(*[int(x) for x in slots])
+        cat = (ctypes.c_int64 * max(len(flat), 1))(*flat)
+        npf = (ctypes.c_int32 * max(n, 1))(*[len(p) for p in pfx])
+        mnt = (ctypes.c_int32 * max(n, 1))(*[int(m) for m in max_new_tokens])
+        out = (ctypes.c_int64 * (max(n, 1) * cap))()
+        n_out = (ctypes.c_int32 * max(n, 1))()
+        feats = self._f32(max(n, 1), feats_ld, self.cfg.mt_dim)
+        self._check(self.lib.ss_pool_mt_greedy(self._h, self._stream(), n, sl, cat, npf, mnt, int(max_len_b), out, cap, n_out, feats.data_ptr(),
+                                               feats_ld))
+        return [[int(out[i * cap + k]) for k in range(n_out[i])] for i in range(n)], feats[:n]
+
+    def pool_encoder_rows(self, slot: int, T: int) -> torch.Tensor:
+        """the slot's first T encoder rows [T, enc_dim] as a tensor over the pool's device memory (a view: valid until the next pool_step)"""
+        ptr = self.pool_info(slot)["enc_out_ptr"]
+        numel = int(T) * self.cfg.enc_dim
+
+        class _Rows:
+            __cuda_array_interface__ = {"shape": (numel,), "typestr": "<f4", "data": (ptr, False), "version": 3}
+        return torch.as_tensor(_Rows(), device=self.device).view(int(T), self.cfg.enc_dim)
 
     def set_option(self, name: str, value: int):
         self._check(self.lib.ss_set_option(self._h, name.encode(), int(value)))

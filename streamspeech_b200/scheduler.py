@@ -6,6 +6,11 @@ to a slot, `push()` only registers the new samples, and the first `pop()` after 
 streams that have pending input (fbank -> chunk-Conformer encoder -> CTC heads over the concatenated rows), after which every agent
 of the round finds its result ready.  A harness that feeds the agents round-robin (push all, pop all) -- or calls
 `pushpop_many()` -- therefore gets cross-utterance batching without any change to the agent API.
+
+`PooledS2STAgent` extends this to simultaneous speech-to-speech translation: the flush that serves its streams also runs ONE batched
+MT search (ss_pool_mt_greedy) for every stream whose policy gate says WRITE and ONE T2U + unit-decoder call
+(ss_t2u_unit_decode_ragged) for every stream that still has something to say; the vocoder stays one call per stream.  The host
+stages around those calls are the single agent's own methods (StreamSpeechS2STAgent._gate / _after_mt / _after_t2u).
 """
 from __future__ import annotations
 
@@ -13,8 +18,9 @@ from typing import Dict, List, Optional, Sequence
 
 import torch
 
+from streamspeech_b200.agent import READ, SAMPLE_RATE, StreamSpeechS2STAgent
 from streamspeech_b200.engine import Engine
-from streamspeech_b200.simuleval_compat import ReadAction, SpeechToTextAgent, WriteAction
+from streamspeech_b200.simuleval_compat import ReadAction, SpeechToSpeechAgent, SpeechToTextAgent, WriteAction
 
 
 class StreamPool:
@@ -32,6 +38,8 @@ class StreamPool:
         self.results: Dict[int, dict] = {}       # slot -> result of the last step that included it
         self.steps = 0                           # batched steps run (for tests / bench)
         self.rows_per_step: List[int] = []
+        self.s2st: Dict[int, "PooledS2STAgent"] = {}  # slot -> its S2ST agent: a flush also runs the decoders of these slots
+        self.stage_ms: Optional[Dict[str, float]] = None  # a dict: device time per stage of every flush is added to it (CUDA events)
 
     def acquire(self) -> int:
         if not self.free:
@@ -47,6 +55,7 @@ class StreamPool:
         self.engine.pool_set_chunk(slot, 0, 0)
         self.pending.pop(slot, None)
         self.results.pop(slot, None)
+        self.s2st.pop(slot, None)
         self.free.append(slot)
 
     def set_chunk(self, slot: int, attn_chunk: int, conv_chunk: int):
@@ -71,16 +80,22 @@ class StreamPool:
         self.results.pop(slot, None)
 
     def flush(self):
-        """one batched step for every stream with pending input"""
+        """one batched step for every stream with pending input (and the decoders of its S2ST streams)"""
         slots = sorted(self.pending)
         if not slots:
             return
+        clock = _StageClock(self.stage_ms)
+        clock.mark("pool_step")
         res = self.engine.pool_step(slots, self.ctc_heads)
         for s, r in zip(slots, res):
             self.results[s] = r
         self.pending.clear()
         self.steps += 1
         self.rows_per_step.append(len(slots))
+        agents = [self.s2st[s] for s in slots if s in self.s2st]
+        if agents:
+            PooledS2STAgent.decode_round(self, agents, clock)
+        clock.close()
 
     def result(self, slot: int) -> dict:
         if slot not in self.results:
@@ -88,7 +103,44 @@ class StreamPool:
         return self.results[slot]
 
 
-class PooledASRAgent(SpeechToTextAgent):
+class _StageClock:
+    """CUDA events on the current stream at stage boundaries; close() adds each stage's time to `into` (nothing without a dict)"""
+
+    def __init__(self, into: Optional[Dict[str, float]]):
+        self.into = into
+        self.events = []
+
+    def mark(self, name: str):
+        if self.into is not None:
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            self.events.append((name, ev))
+
+    def close(self):
+        if self.into is None or not self.events:
+            return
+        self.mark("")
+        self.events[-1][1].synchronize()
+        for (name, e0), (_, e1) in zip(self.events, self.events[1:]):
+            self.into[name] = self.into.get(name, 0.0) + e0.elapsed_time(e1)
+        self.events = []
+
+
+class _PooledSource:
+    """push() of a pooled agent: the segment's samples go to the agent's slot (they must come at the pool's sample rate)"""
+
+    def push(self, source_segment, states=None):  # GenericAgent.push (SimulEval agents/agent.py:71-83) + device mirror of the new samples
+        if states is None:
+            states = self.states
+        rate = getattr(source_segment, "sample_rate", -1)  # SpeechSegment's default -1 = not stated: taken as the pool's rate
+        if rate > 0 and rate != self.pool.sample_rate:
+            raise ValueError(f"a {rate} Hz segment was pushed to a {self.pool.sample_rate} Hz stream pool")
+        before = len(states.source)
+        states.update_source(source_segment)
+        self.pool.push(self.slot, states.source[before:], finished=states.source_finished)
+
+
+class PooledASRAgent(_PooledSource, SpeechToTextAgent):
     """StreamSpeechASRAgent (agent/speech_to_text.asr.streamspeech.agent.py:100-433) bound to a slot of a shared StreamPool:
     same push() / pop() / policy() contract and text output; the tensor work of all agents of a round is one batched step.
     Segments must come at the pool's sample rate (ValueError otherwise).  With args, the slot runs at args.source_segment_size
@@ -111,16 +163,6 @@ class PooledASRAgent(SpeechToTextAgent):
         if hasattr(self, "slot"):
             self.pool.reset(self.slot)
 
-    def push(self, source_segment, states=None):  # GenericAgent.push (SimulEval agents/agent.py:71-83) + device mirror of the new samples
-        if states is None:
-            states = self.states
-        rate = getattr(source_segment, "sample_rate", -1)  # SpeechSegment's default -1 = not stated: taken as the pool's rate
-        if rate > 0 and rate != self.pool.sample_rate:
-            raise ValueError(f"a {rate} Hz segment was pushed to a {self.pool.sample_rate} Hz stream pool")
-        before = len(states.source)
-        states.update_source(source_segment)
-        self.pool.push(self.slot, states.source[before:], finished=states.source_finished)
-
     def policy(self):
         r = self.pool.result(self.slot)
         if r["T"] == 0 and not self.states.source_finished:
@@ -136,7 +178,116 @@ class PooledASRAgent(SpeechToTextAgent):
         return WriteAction(new_text, finished=self.states.target_finished)
 
 
-def pushpop_many(agents: Sequence[PooledASRAgent], segments: Sequence) -> list:
+class PooledS2STAgent(_PooledSource, StreamSpeechS2STAgent):
+    """StreamSpeechS2STAgent (agent/speech_to_speech.streamspeech.agent.py:101-770) bound to a slot of a shared StreamPool: same
+    push() / pop() / policy() contract and WriteAction(SpeechSegment) output, the same policy code (the single agent's host stages),
+    but the tensor work of all agents of a round runs as one pool step, one batched MT search and one T2U + unit-decoder call.
+    The pool needs both CTC heads (StreamPool(..., ctc_heads=2)).  The slot takes the S2ST agent's latency rule: chunk c =
+    source_segment_size // 40, conv chunk 16 if c >= 16 else 8 (agent:406-413); whole-word output at >= 640 ms (agent:207-210).
+    args: the single agent's flags (lagging_k1, stride_n, dur_prediction, vocoder_context, ...); the model comes from the pool's
+    engine and `dicts` (the single agent's `dict`: "target_unigram" and "tgt" are read)."""
+
+    def __init__(self, pool: StreamPool, dicts, args):
+        if pool.ctc_heads != 2:
+            raise ValueError("a pooled S2ST agent needs a stream pool with both CTC heads (ctc_heads=2)")
+        self.pool = pool
+        self.engine = pool.engine
+        self.cfg = pool.engine.cfg
+        self.torch_device = pool.engine.device
+        self.dict = dicts
+        self.eos = self.cfg.eos
+        self.max_len = args.max_len
+        self.force_finish = args.force_finish
+        self.dur_prediction = args.dur_prediction
+        self.lagging_k1 = args.lagging_k1
+        self.lagging_k2 = args.lagging_k2
+        self.segment_size = args.segment_size
+        self.stride_n = args.stride_n
+        self.unit_per_subword = args.unit_per_subword
+        self.stride_n2 = args.stride_n2
+        self.whole_word = args.source_segment_size >= 640  # agent:207-210
+        self.vocoder_context = getattr(args, "vocoder_context", "receptive-field")
+        self.trace = {}
+        self._action = None
+        self.slot = pool.acquire()
+        chunk_size = args.source_segment_size // 40  # agent:395-413
+        pool.set_chunk(self.slot, chunk_size, 16 if chunk_size >= 16 else 8)  # once: it survives the reset between utterances
+        pool.s2st[self.slot] = self
+        SpeechToSpeechAgent.__init__(self, args)  # states + reset()
+
+    def _reset_caches(self):
+        """new utterance: the slot starts over (audio, encoder state, cross K / V cache)"""
+        if hasattr(self, "slot"):
+            self.pool.reset(self.slot)
+        self._action = None
+
+    def _policy_impl(self):
+        if self._action is None:
+            self.pool.flush()  # this agent's segment is pending: the round computes the action of every pending agent
+        action, self._action = self._action, None
+        if action is None:
+            raise RuntimeError("policy() of a pooled agent needs a pushed segment first")
+        return action
+
+    @staticmethod
+    @torch.inference_mode()
+    def decode_round(pool: StreamPool, agents: Sequence["PooledS2STAgent"], clock: _StageClock):
+        """Stages 2-7 of a flush for the agents whose slots the pool step just ran: the gate per stream, one batched MT search for
+        the writing streams, the post-MT checks per stream, teacher-forced features for finishing whole-word streams (once per
+        utterance, N2 pad tail), one T2U + unit-decoder call for every stream that goes on, then the vocoder stream by stream."""
+        eng = pool.engine
+        writing = []
+        for a in agents:
+            a.trace = {}
+            r = pool.results[a.slot]
+            if r["T"] == 0:  # no encoder row yet (fewer samples than one fbank frame)
+                a._action = READ
+                continue
+            (src, _), (tgt, _) = r["ctc"]  # agent:437, 461
+            a.trace["asr_tokens"], a.trace["st_tokens"] = src, tgt
+            new = a._gate(src, tgt)
+            if new is None:
+                a._action = READ
+            else:
+                writing.append((a, new, r["T"]))
+        if not writing:
+            return
+        clock.mark("mt")
+        hyps, feats = eng.pool_mt_greedy([a.slot for a, _, _ in writing], [a.tgt_subwords_indices for a, _, _ in writing],
+                                         [new for _, new, _ in writing], max_len_b=100)
+        going = []  # (agent, new_subword_tokens, T, row of feats, prev_output_tokens_mt, n_pad_tail)
+        for k, (a, new, T) in enumerate(writing):
+            action, t2u_input = a._after_mt(hyps[k])
+            if action is not None:
+                a._action = action
+            else:
+                going.append((a, new, T, k) + t2u_input)
+        if not going:
+            return
+        lengths = [len(g[4]) for g in going]
+        S = max(lengths)
+        rows = feats[torch.tensor([g[3] for g in going], device=feats.device), :S]  # [B, S, mt_dim] (rows >= S_b unused)
+        x = torch.nn.functional.pad(rows, (0, 0, 0, S - rows.shape[1])).contiguous()  # (a pad position can lie past the search's rows)
+        padded = [j for j, g in enumerate(going) if g[5]]
+        if padded:  # whole-word streams at their end: mt_decoder(prev_output_tokens_mt) with the pad position (agent:576-642)
+            clock.mark("features")
+            Tp = max(going[j][2] for j in padded)
+            enc = torch.zeros(len(padded), Tp, eng.cfg.enc_dim, dtype=torch.float32, device=eng.device)
+            for m, j in enumerate(padded):
+                enc[m, :going[j][2]] = eng.pool_encoder_rows(going[j][0].slot, going[j][2])
+            Sp = max(lengths[j] for j in padded)
+            toks = [going[j][4] + [eng.cfg.pad] * (Sp - lengths[j]) for j in padded]
+            pf = eng.mt_features_batch(enc, [going[j][2] for j in padded], toks)
+            for m, j in enumerate(padded):
+                x[j, :lengths[j]] = pf[m, :lengths[j]]
+        clock.mark("t2u")
+        units, _, _ = eng.t2u_unit_decode_ragged(x, lengths, [g[5] for g in going])
+        clock.mark("vocoder")
+        for (a, new, _, _, _, _), u in zip(going, units):
+            a._action = a._after_t2u(u, new)
+
+
+def pushpop_many(agents: Sequence, segments: Sequence) -> list:
     """the batched front door: push one segment to every agent, then pop all (one batched engine step)"""
     for a, s in zip(agents, segments):
         a.push(s)
