@@ -343,6 +343,39 @@ int ss_set_option(ss_engine* h, const char* name, int value);
 int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes);
 int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev,
                      float* out_dev);
+/* Attention and depthwise-conv hooks: each launches the launch function the engine uses (kernels.h) on `stream`; the hooks that take host arrays
+ * copy them to the device and synchronise `stream`.  head_dim is 64 and D = H * 64; row strides are in floats, >= D and multiples
+ * of 4.  kernel: 0 = the row / tile kernel the engine would choose for this shape, 1 = row kernel, 2 = tile kernel.
+ * Errors: SS_ERR_INVALID for a null pointer or any shape outside what the kernels take; the handle stays usable. */
+/* rel-pos self-attention: q rows b * nQ + r (absolute positions q_offset + r), k / v rows b * T + j, pos [2 * Tpos - 1][D] (row
+ * (i - j) + Tpos - 1), out [B * nQ][D].  Needs T <= Tpos, q_offset + nQ <= T, chunk >= 0 (0 = full), lengths_host (optional) in
+ * [1, T], and for kernel = 1, T * 4 bytes <= 160 KB. */
+int ss_op_relpos_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv,
+                           const float* pos_dev, int Tpos, const float* bias_u_dev, const float* bias_v_dev, float* out_dev, int B, int nQ,
+                           int q_offset, int T, int H, int D, int chunk, const int32_t* lengths_host, int kernel);
+/* multi-head attention: q rows b * Tq + t, k / v rows b * Tk + j; causal: key j visible to query t iff j <= t + causal_offset;
+ * kv_len_host (optional) in [1, Tk]; for kernel = 1, Tk * 4 bytes <= 160 KB */
+int ss_op_mha_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv, float* out_dev,
+                        int ldo, int B, int Tq, int Tk, int H, float scale, int causal, int causal_offset, const int32_t* kv_len_host, int kernel);
+/* causal self-attention over S groups of R identical rows (the unit decoder's first layer): q / k / v rows b * S + g, out rows
+ * (b * S + g) * R + r; kv_len_host (optional) = valid groups per sample, in [1, S]; S <= 12288 */
+int ss_op_grouped_causal_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv,
+                                   float* out_dev, int ldo, int S, int R, int H, float scale, int B, const int32_t* kv_len_host);
+/* chunk-causal depthwise conv (w [k][C], odd k) + folded BatchNorm (scale, shift [C]) + SiLU over x [B * T][ldx] at positions t0 .. t0 + n - 1
+ * (t0 + n <= T) -> y rows b * n + r; chunk >= 0 (0 = no chunk) */
+int ss_op_depthwise_bn_silu(ss_engine* h, void* stream, const float* x_dev, int ldx, const float* w_dev, const float* scale_dev, const float* shift_dev,
+                            float* y_dev, int ldy, int B, int T, int t0, int n, int C, int k, int chunk);
+/* the stream pool's ragged kernels over n streams: stream b uses slot slot_host[b] in [0, n_slots) of the slot buffers (slot_stride floats
+ * apart; keys / conv inputs are rows of D / C floats), computes its rows a0 .. a0 + nA - 1 (0 <= nA <= T - a0) with its own chunk, and
+ * reads / writes rows row0 .. row0 + nA - 1 of q / out / y (row0 + nA <= rows).  Relative-position attention needs T <= Tpos and
+ * T * 4 bytes <= 160 KB. */
+int ss_op_ms_relpos_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* kc_dev, const float* vc_dev, int64_t slot_stride,
+                              int n_slots, const float* pos_dev, int Tpos, const float* bias_u_dev, const float* bias_v_dev, float* out_dev, int ldo,
+                              int rows, int H, int n, const int32_t* slot_host, const int32_t* a0_host, const int32_t* nA_host, const int32_t* T_host,
+                              const int32_t* attn_chunk_host, const int32_t* row0_host);
+int ss_op_ms_depthwise(ss_engine* h, void* stream, const float* x_dev, int64_t slot_stride, int n_slots, const float* w_dev, const float* scale_dev,
+                       const float* shift_dev, float* y_dev, int ldy, int rows, int C, int k, int n, const int32_t* slot_host, const int32_t* a0_host,
+                       const int32_t* nA_host, const int32_t* T_host, const int32_t* conv_chunk_host, const int32_t* row0_host);
 
 /* number of kernels this library has launched in this process (bench.py reports the difference over the timed region as
  * gpu_launches; the counter is process-wide, not per handle) */

@@ -183,12 +183,18 @@ def mha(sd, prefix, query, key, num_heads, attn_mask=None, key_padding_mask=None
     (researches/ctc_unity/modules/multihead_attention.py:439-784; fast path is commented
     out there, N11).  query [Tq,B,C], key [Tk,B,Ck]; attn_mask: bool [Tq,Tk] True=masked;
     key_padding_mask bool [B,Tk]."""
-    Tq, B, C = query.shape
-    Tk = key.shape[0]
-    hd = C // num_heads
+    hd = query.shape[2] // num_heads
     q = _lin(query, sd, prefix + ".q_proj") * (hd ** -0.5)
     k = _lin(key, sd, prefix + ".k_proj")
     v = _lin(key, sd, prefix + ".v_proj")
+    return _lin(mha_core(q, k, v, num_heads, attn_mask, key_padding_mask), sd, prefix + ".out_proj")
+
+
+def mha_core(q, k, v, num_heads, attn_mask=None, key_padding_mask=None):
+    """The attention of `mha` between its projections: q [Tq,B,C] (already scaled), k / v [Tk,B,C] -> [Tq,B,C], in q's dtype."""
+    Tq, B, C = q.shape
+    Tk = k.shape[0]
+    hd = C // num_heads
     q = q.contiguous().view(Tq, B * num_heads, hd).transpose(0, 1)
     k = k.contiguous().view(Tk, B * num_heads, hd).transpose(0, 1)
     v = v.contiguous().view(Tk, B * num_heads, hd).transpose(0, 1)
@@ -197,9 +203,36 @@ def mha(sd, prefix, query, key, num_heads, attn_mask=None, key_padding_mask=None
         w = w.view(B, num_heads, Tq, Tk).masked_fill(key_padding_mask[:, None, None, :], NEG_INF).view(B * num_heads, Tq, Tk)
     if attn_mask is not None:
         w = w.masked_fill(attn_mask.unsqueeze(0), NEG_INF)
-    p = F.softmax(w, dim=-1, dtype=torch.float32)
-    a = torch.bmm(p, v).transpose(0, 1).contiguous().view(Tq, B, C)
-    return _lin(a, sd, prefix + ".out_proj")
+    p = F.softmax(w, dim=-1, dtype=q.dtype)  # fp32 in the reference, whose activations are fp32
+    return torch.bmm(p, v).transpose(0, 1).contiguous().view(Tq, B, C)
+
+
+def rel_attention_core(q, k, v, pp, bias_u, bias_v, mask=None, key_padding_mask=None):
+    """The attention of RelPositionMultiHeadedAttention.forward between its projections (espnet_multihead_attention.py:186-209):
+    q [B,T,H,dk], k / v [B,H,T,dk], pp [1,H,2T-1,dk] projected position rows (row k: relative position T-1-k), bias_u / bias_v [H,dk],
+    mask [T,T] / key_padding_mask [B,T] True = masked -> [B,T,H*dk], in q's dtype."""
+    B, T, H, dk = q.shape
+    qu = (q + bias_u).transpose(1, 2)
+    qv = (q + bias_v).transpose(1, 2)
+    ac = torch.matmul(qu, k.transpose(-2, -1))
+    bd = rel_shift(torch.matmul(qv, pp.transpose(-2, -1)))
+    scores = (ac + bd) / math.sqrt(dk)
+    if mask is not None:
+        scores = scores.masked_fill(mask[None, None], NEG_INF)
+    if key_padding_mask is not None:
+        scores = scores.masked_fill(key_padding_mask[:, None, None, :], NEG_INF)
+    attn = torch.softmax(scores, dim=-1)
+    return torch.matmul(attn, v).transpose(1, 2).contiguous().view(B, -1, H * dk)
+
+
+def depthwise_bn_silu_core(y, w, bn_mean, bn_var, bn_weight, bn_bias, conv_chunk_size):
+    """Depthwise conv + BatchNorm (eval) + SiLU of ConvolutionModule.forward (conformer_layer.py:106-111): y [B,C,T], w [C,1,k]
+    -> [B,C,T], in y's dtype; conv_chunk_size None = the plain padded conv, else ChunkCausalConv1d."""
+    if conv_chunk_size is None:
+        y = F.conv1d(y, w, None, padding=(w.shape[-1] - 1) // 2, groups=w.shape[0])
+    else:
+        y = chunk_causal_conv1d(y, w, None, 1, w.shape[0], conv_chunk_size)
+    return F.silu(F.batch_norm(y, bn_mean, bn_var, bn_weight, bn_bias, False, 0.0, 1e-5))
 
 
 # --------------------------------------------------------------------------------------
@@ -207,12 +240,16 @@ def mha(sd, prefix, query, key, num_heads, attn_mask=None, key_padding_mask=None
 # --------------------------------------------------------------------------------------
 class StreamSpeechOracle:
     def __init__(self, cfg, model_sd: Dict[str, torch.Tensor], vocoder_sd: Optional[Dict[str, torch.Tensor]] = None,
-                 gcmvn=None, chunk_size: Optional[int] = 8, conv_chunk_size: Optional[int] = None):
+                 gcmvn=None, chunk_size: Optional[int] = 8, conv_chunk_size: Optional[int] = None, dtype: torch.dtype = torch.float32):
+        """dtype: the arithmetic of every block (float64 makes a high-precision reference of the fp32 model).  Weights are taken as
+        fp32 and then converted, and the position tables are computed in fp32 and then converted, so a float64 oracle sees exactly
+        the numbers the fp32 model (and the engine) see; inputs are converted on entry."""
         self.cfg = cfg
-        self.sd = {k: (v.float() if v.is_floating_point() else v) for k, v in model_sd.items()}
+        self.dtype = dtype
+        self.sd = {k: (v.float().to(dtype) if v.is_floating_point() else v) for k, v in model_sd.items()}
         self.vsd = None
         if vocoder_sd is not None:
-            self.vsd = _remove_weight_norm({k: v.float() for k, v in vocoder_sd.items()})
+            self.vsd = {k: v.to(dtype) for k, v in _remove_weight_norm({k: v.float() for k, v in vocoder_sd.items()}).items()}
         self.gcmvn = gcmvn
         self.set_chunk(chunk_size, conv_chunk_size)
 
@@ -225,7 +262,7 @@ class StreamSpeechOracle:
 
     # ---- E1 Conv1dSubsampler (chunk_unity/modules/convolution.py:75-89)
     def subsample(self, feats: torch.Tensor, lengths: torch.Tensor):
-        x = feats.transpose(1, 2).contiguous()  # B x C x T
+        x = feats.to(self.dtype).transpose(1, 2).contiguous()  # B x C x T
         for i in range(2):
             w = self.sd[f"encoder.subsample.conv_layers.{i}.weight"]
             b = self.sd[f"encoder.subsample.conv_layers.{i}.bias"]
@@ -256,17 +293,7 @@ class StreamSpeechOracle:
         v = _lin(xb, self.sd, p + ".linear_v").view(B, -1, H, dk).transpose(1, 2)
         pe = pos_emb.transpose(0, 1)  # [1, 2T-1, C]
         pp = F.linear(pe, self.sd[p + ".linear_pos.weight"]).view(pe.size(0), -1, H, dk).transpose(1, 2)
-        qu = (q + self.sd[p + ".pos_bias_u"]).transpose(1, 2)
-        qv = (q + self.sd[p + ".pos_bias_v"]).transpose(1, 2)
-        ac = torch.matmul(qu, k.transpose(-2, -1))
-        bd = rel_shift(torch.matmul(qv, pp.transpose(-2, -1)))
-        scores = (ac + bd) / math.sqrt(dk)
-        if mask is not None:
-            scores = scores.masked_fill(mask[None, None], NEG_INF)
-        if key_padding_mask is not None:
-            scores = scores.masked_fill(key_padding_mask[:, None, None, :], NEG_INF)
-        attn = torch.softmax(scores, dim=-1)
-        o = torch.matmul(attn, v).transpose(1, 2).contiguous().view(B, -1, C)
+        o = rel_attention_core(q, k, v, pp, self.sd[p + ".pos_bias_u"], self.sd[p + ".pos_bias_v"], mask, key_padding_mask)
         return _lin(o, self.sd, p + ".linear_out").transpose(0, 1)
 
     # ---- E5 ConvolutionModule.forward (conformer_layer.py:94-119)
@@ -274,14 +301,9 @@ class StreamSpeechOracle:
         y = _ln(x, self.sd, p + ".layer_norm").transpose(1, 2)  # B C T
         y = F.conv1d(y, self.sd[p + ".pointwise_conv1.weight"])
         y = F.glu(y, dim=1)
-        w = self.sd[p + ".depthwise_conv.weight"]
-        if self.conv_chunk_size is None:
-            y = F.conv1d(y, w, None, padding=(w.shape[-1] - 1) // 2, groups=w.shape[0])
-        else:
-            y = chunk_causal_conv1d(y, w, None, 1, w.shape[0], self.conv_chunk_size)
-        y = F.batch_norm(y, self.sd[p + ".batch_norm.running_mean"], self.sd[p + ".batch_norm.running_var"],
-                         self.sd[p + ".batch_norm.weight"], self.sd[p + ".batch_norm.bias"], False, 0.0, 1e-5)
-        y = F.silu(y)
+        y = depthwise_bn_silu_core(y, self.sd[p + ".depthwise_conv.weight"], self.sd[p + ".batch_norm.running_mean"],
+                                   self.sd[p + ".batch_norm.running_var"], self.sd[p + ".batch_norm.weight"], self.sd[p + ".batch_norm.bias"],
+                                   self.conv_chunk_size)
         y = F.conv1d(y, self.sd[p + ".pointwise_conv2.weight"])
         return y.transpose(1, 2)
 
@@ -305,7 +327,7 @@ class StreamSpeechOracle:
         T, B, C = x.shape
         pad_mask = torch.arange(T).unsqueeze(0) >= out_len.unsqueeze(1)  # lengths_to_padding_mask
         x = math.sqrt(C) * x
-        pos = rel_positional_encoding(T, C).unsqueeze(1)  # [2T-1,1,C]
+        pos = rel_positional_encoding(T, C).to(self.dtype).unsqueeze(1)  # [2T-1,1,C]
         x = _lin(x, self.sd, "encoder.linear")
         mask = chunk_mask(T, self.chunk_size) if self.chunk_size is not None else None
         layers = []
@@ -318,10 +340,10 @@ class StreamSpeechOracle:
 
     # ---- C1 CTCDecoder.generate (agent/ctc_decoder.py:40-111)
     def ctc_logits(self, name: str, enc_out: torch.Tensor) -> torch.Tensor:
-        return _lin(enc_out, self.sd, f"{name}_decoder.proj").transpose(0, 1)  # B x T x V
+        return _lin(enc_out.to(self.dtype), self.sd, f"{name}_decoder.proj").transpose(0, 1)  # B x T x V
 
     def ctc_greedy(self, name: str, enc_out: torch.Tensor):
-        lprobs = F.log_softmax(self.ctc_logits(name, enc_out).float(), dim=-1)
+        lprobs = F.log_softmax(self.ctc_logits(name, enc_out), dim=-1)
         lprobs[:, :, self.cfg.pad] = NEG_INF
         lprobs[:, :, self.cfg.unk] = NEG_INF
         _, pred = torch.max(lprobs, dim=2)
@@ -351,7 +373,8 @@ class StreamSpeechOracle:
         c = self.cfg
         B, L = prev_tokens.shape
         pfx = "target_unigram_decoder"
-        table = sinusoidal_table(max(1024, c.pad + 1 + L + 1), c.mt_dim, c.pad)
+        enc_out = enc_out.to(self.dtype)
+        table = sinusoidal_table(max(1024, c.pad + 1 + L + 1), c.mt_dim, c.pad).to(self.dtype)
         pos = table.index_select(0, make_positions(prev_tokens, c.pad).view(-1)).view(B, L, -1)
         x = math.sqrt(c.mt_dim) * F.embedding(prev_tokens, self.sd[pfx + ".embed_tokens.weight"]) + pos
         x = x.transpose(0, 1)
@@ -382,7 +405,7 @@ class StreamSpeechOracle:
         score = 0.0
         for step in range(start, max_len + 1):
             logits = self.mt_logits(torch.tensor([tokens], dtype=torch.long), enc_out)[:, -1, :]
-            lprobs = F.log_softmax(logits.float(), dim=-1)[0]
+            lprobs = F.log_softmax(logits, dim=-1)[0]
             lprobs[lprobs != lprobs] = NEG_INF
             lprobs[c.pad] = NEG_INF
             if step >= max_len:
@@ -413,7 +436,8 @@ class StreamSpeechOracle:
         prev_key length and concatenates (transformer_layer.py:492-505, static_kv otherwise).  Returns logits [vocab]."""
         c = self.cfg
         pfx = "target_unigram_decoder"
-        table = sinusoidal_table(max(1024, c.pad + 1 + step + 2), c.mt_dim, c.pad)
+        enc_out = enc_out.to(self.dtype)
+        table = sinusoidal_table(max(1024, c.pad + 1 + step + 2), c.mt_dim, c.pad).to(self.dtype)
         p = c.pad if token == c.pad else c.pad + 1 + step
         x = math.sqrt(c.mt_dim) * self.sd[pfx + ".embed_tokens.weight"][token] + table[p]
         x = x.view(1, 1, -1)
@@ -465,7 +489,7 @@ class StreamSpeechOracle:
         tokens = [c.eos] + prefix
         for step in range(start, max_len + 1):
             logits = self._mt_step_incremental(state, tokens[step], step, enc_out)
-            lprobs = F.log_softmax(logits.float(), dim=-1)
+            lprobs = F.log_softmax(logits, dim=-1)
             lprobs[lprobs != lprobs] = NEG_INF
             lprobs[c.pad] = NEG_INF
             if step >= max_len:
@@ -483,6 +507,7 @@ class StreamSpeechOracle:
     def t2u_encoder(self, x: torch.Tensor, pad_mask: Optional[torch.Tensor]) -> torch.Tensor:
         """x [S,B,512] -> [S,B,512]."""
         c = self.cfg
+        x = x.to(self.dtype)
         S = x.size(0)
         causal = torch.triu(torch.ones(S, S, dtype=torch.bool), 1) if c.uni_encoder else None
         for i in range(c.t2u_layers):
@@ -500,12 +525,13 @@ class StreamSpeechOracle:
     def unit_decoder_logits(self, t2u_out: torch.Tensor, pad_mask: Optional[torch.Tensor]) -> torch.Tensor:
         """t2u_out [S,B,512] -> logits [B, 25*S, 1005]."""
         c = self.cfg
+        t2u_out = t2u_out.to(self.dtype)
         S, B, E = t2u_out.shape
         R = c.ctc_upsample_rate
         x = t2u_out.unsqueeze(1).repeat(1, R, 1, 1).contiguous().view(S * R, B, E)
         # N1: positions are computed from x[:, :, 0] viewed as [bsz=T', seq=B]
         first = x[:, :, 0]
-        table = sinusoidal_table(max(1200, c.pad + 1 + B + 1), E, c.pad)
+        table = sinusoidal_table(max(1200, c.pad + 1 + B + 1), E, c.pad).to(self.dtype)
         pos = table.index_select(0, make_positions(first, c.pad).view(-1)).view(S * R, B, -1)
         x = x + pos
         self_pad = None
@@ -522,7 +548,7 @@ class StreamSpeechOracle:
     # ---- U2 CTCSequenceGenerator.generate (agent/ctc_generator.py:41-123); offline variant also masks eos (N3)
     def unit_ctc_greedy(self, logits: torch.Tensor, mask_eos: bool = False):
         c = self.cfg
-        lprobs = F.log_softmax(logits.float(), dim=-1)
+        lprobs = F.log_softmax(logits.to(self.dtype), dim=-1)
         lprobs[:, :, c.pad] = NEG_INF
         lprobs[:, :, c.unk] = NEG_INF
         if mask_eos:

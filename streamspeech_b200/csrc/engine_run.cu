@@ -1695,4 +1695,193 @@ int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, i
 
 }  // extern "C"
 
+namespace {
+
+// Host arrays of one parity-test launch, copied to device memory that lives until the launch has finished.
+struct OpUploads {
+  std::vector<void*> ptrs;
+  template <class T>
+  const T* put(const T* host, size_t n) {
+    if (!host || n == 0) return nullptr;
+    void* d = nullptr;
+    if (cudaMalloc(&d, n * sizeof(T)) != cudaSuccess) throw std::runtime_error("cudaMalloc failed");
+    ptrs.push_back(d);
+    if (cudaMemcpy(d, host, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) throw std::runtime_error("cudaMemcpy failed");
+    return static_cast<const T*>(d);
+  }
+  // checks the launch, waits for it and frees the copies
+  int finish(ss_engine* h, cudaStream_t st, const char* where) {
+    const int rc = check_launch(h, where);
+    if (rc != SS_OK) return rc;
+    const cudaError_t e = cudaStreamSynchronize(st);
+    return e == cudaSuccess ? SS_OK : h->fail(SS_ERR_CUDA, std::string(where) + ": " + cudaGetErrorString(e));
+  }
+  ~OpUploads() {
+    for (void* p : ptrs) cudaFree(p);
+  }
+};
+
+bool row_stride_ok(int ld, int D) { return ld >= D && ld % 4 == 0; }
+
+// every length in [1, T]
+bool lengths_ok(const int32_t* len, int B, int T) {
+  for (int b = 0; len && b < B; ++b)
+    if (len[b] < 1 || len[b] > T) return false;
+  return true;
+}
+
+constexpr size_t ROW_KERNEL_SMEM = 160 * 1024;  // kernels_attn.cu: the row kernel keeps T scores in shared memory
+
+}  // namespace
+
+extern "C" {
+
+int ss_op_relpos_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv,
+                           const float* pos_dev, int Tpos, const float* bias_u_dev, const float* bias_v_dev, float* out_dev, int B, int nQ,
+                           int q_offset, int T, int H, int D, int chunk, const int32_t* lengths_host, int kernel) {
+  if (!h) return SS_ERR_INVALID;
+  if (!q_dev || !k_dev || !v_dev || !pos_dev || !bias_u_dev || !bias_v_dev || !out_dev) return h->fail(SS_ERR_INVALID, "ss_op_relpos_attention: null pointer");
+  if (B < 1 || nQ < 1 || T < 1 || H < 1 || D != H * 64 || T > Tpos || q_offset < 0 || q_offset + nQ > T || chunk < 0 || kernel < 0 || kernel > 2 ||
+      !row_stride_ok(ldq, D) || !row_stride_ok(ldk, D) || !row_stride_ok(ldv, D))
+    return h->fail(SS_ERR_INVALID, "ss_op_relpos_attention: bad shape");
+  if (!lengths_ok(lengths_host, B, T)) return h->fail(SS_ERR_INVALID, "ss_op_relpos_attention: a length outside [1, T]");
+  if (kernel == 1 && (size_t)T * sizeof(float) > ROW_KERNEL_SMEM) return h->fail(SS_ERR_INVALID, "ss_op_relpos_attention: T too long for the row kernel");
+  try {
+    OpUploads up;
+    relpos_attention(q_dev, ldq, k_dev, ldk, v_dev, ldv, pos_dev, Tpos, bias_u_dev, bias_v_dev, out_dev, B, nQ, q_offset, T, H, D, chunk,
+                     up.put(lengths_host, B), S(stream), kernel);
+    return up.finish(h, S(stream), "ss_op_relpos_attention");
+  } catch (const std::exception& e) {
+    return h->fail(SS_ERR_CUDA, e.what());
+  }
+}
+
+int ss_op_mha_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv, float* out_dev,
+                        int ldo, int B, int Tq, int Tk, int H, float scale, int causal, int causal_offset, const int32_t* kv_len_host, int kernel) {
+  if (!h) return SS_ERR_INVALID;
+  if (!q_dev || !k_dev || !v_dev || !out_dev) return h->fail(SS_ERR_INVALID, "ss_op_mha_attention: null pointer");
+  const int D = H * 64;
+  if (B < 1 || Tq < 1 || Tk < 1 || H < 1 || causal < 0 || causal > 1 || causal_offset < 0 || kernel < 0 || kernel > 2 || !row_stride_ok(ldq, D) ||
+      !row_stride_ok(ldk, D) || !row_stride_ok(ldv, D) || !row_stride_ok(ldo, D))
+    return h->fail(SS_ERR_INVALID, "ss_op_mha_attention: bad shape");
+  if (!lengths_ok(kv_len_host, B, Tk)) return h->fail(SS_ERR_INVALID, "ss_op_mha_attention: a key length outside [1, Tk]");
+  if (kernel == 1 && (size_t)Tk * sizeof(float) > ROW_KERNEL_SMEM) return h->fail(SS_ERR_INVALID, "ss_op_mha_attention: Tk too long for the row kernel");
+  try {
+    OpUploads up;
+    mha_attention(q_dev, ldq, k_dev, ldk, v_dev, ldv, out_dev, ldo, B, Tq, Tk, H, scale, causal, causal_offset, up.put(kv_len_host, B), S(stream),
+                  kernel);
+    return up.finish(h, S(stream), "ss_op_mha_attention");
+  } catch (const std::exception& e) {
+    return h->fail(SS_ERR_CUDA, e.what());
+  }
+}
+
+int ss_op_grouped_causal_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* k_dev, int ldk, const float* v_dev, int ldv,
+                                   float* out_dev, int ldo, int S_, int R, int H, float scale, int B, const int32_t* kv_len_host) {
+  if (!h) return SS_ERR_INVALID;
+  if (!q_dev || !k_dev || !v_dev || !out_dev) return h->fail(SS_ERR_INVALID, "ss_op_grouped_causal_attention: null pointer");
+  const int D = H * 64;
+  // the kernel keeps S scores in the default 48 KB of dynamic shared memory
+  if (B < 1 || S_ < 1 || S_ > 12 * 1024 || R < 1 || H < 1 || !row_stride_ok(ldq, D) || !row_stride_ok(ldk, D) || !row_stride_ok(ldv, D) ||
+      ldo < D)
+    return h->fail(SS_ERR_INVALID, "ss_op_grouped_causal_attention: bad shape");
+  if (!lengths_ok(kv_len_host, B, S_)) return h->fail(SS_ERR_INVALID, "ss_op_grouped_causal_attention: a key length outside [1, S]");
+  try {
+    OpUploads up;
+    grouped_causal_attention(q_dev, ldq, k_dev, ldk, v_dev, ldv, out_dev, ldo, S_, R, H, scale, up.put(kv_len_host, B), B, S(stream));
+    return up.finish(h, S(stream), "ss_op_grouped_causal_attention");
+  } catch (const std::exception& e) {
+    return h->fail(SS_ERR_CUDA, e.what());
+  }
+}
+
+int ss_op_depthwise_bn_silu(ss_engine* h, void* stream, const float* x_dev, int ldx, const float* w_dev, const float* scale_dev, const float* shift_dev,
+                            float* y_dev, int ldy, int B, int T, int t0, int n, int C, int k, int chunk) {
+  if (!h) return SS_ERR_INVALID;
+  if (!x_dev || !w_dev || !scale_dev || !shift_dev || !y_dev) return h->fail(SS_ERR_INVALID, "ss_op_depthwise_bn_silu: null pointer");
+  if (B < 1 || T < 1 || t0 < 0 || n < 1 || t0 + n > T || C < 1 || ldx < C || ldy < C || k < 1 || k % 2 == 0 || chunk < 0)
+    return h->fail(SS_ERR_INVALID, "ss_op_depthwise_bn_silu: bad shape");
+  depthwise_bn_silu(x_dev, ldx, w_dev, scale_dev, shift_dev, y_dev, ldy, B, T, t0, n, C, k, chunk, S(stream));
+  return check_launch(h, "ss_op_depthwise_bn_silu");
+}
+
+}  // extern "C"
+
+namespace {
+
+// MsStream descriptors of a multi-stream parity-test launch; false when a stream is out of range: a slot outside [0, n_slots), T outside
+// [1, T_cap], a0 < 0, nA outside [0, T - a0], a chunk < 0, or output rows outside [0, rows)
+bool ms_streams(int n, const int32_t* slot, const int32_t* a0, const int32_t* nA, const int32_t* T, const int32_t* chunk, const int32_t* row0,
+                int n_slots, int T_cap, int rows, bool conv, std::vector<MsStream>& out, int& max_nA, int& Tmax) {
+  out.assign(n, MsStream{});
+  max_nA = 0;
+  Tmax = 0;
+  for (int b = 0; b < n; ++b) {
+    MsStream& s = out[b];
+    s.slot = slot[b]; s.a0 = a0[b]; s.nA = nA[b]; s.T = T[b]; s.row0 = row0[b];
+    (conv ? s.conv_chunk : s.attn_chunk) = chunk[b];
+    if (s.slot < 0 || s.slot >= n_slots || s.T < 1 || s.T > T_cap || s.a0 < 0 || s.nA < 0 || s.nA > s.T - s.a0 || chunk[b] < 0 || s.row0 < 0 ||
+        s.row0 + s.nA > rows)
+      return false;
+    max_nA = std::max(max_nA, s.nA);
+    Tmax = std::max(Tmax, s.T);
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ss_op_ms_relpos_attention(ss_engine* h, void* stream, const float* q_dev, int ldq, const float* kc_dev, const float* vc_dev, int64_t slot_stride,
+                              int n_slots, const float* pos_dev, int Tpos, const float* bias_u_dev, const float* bias_v_dev, float* out_dev, int ldo,
+                              int rows, int H, int n, const int32_t* slot_host, const int32_t* a0_host, const int32_t* nA_host, const int32_t* T_host,
+                              const int32_t* attn_chunk_host, const int32_t* row0_host) {
+  if (!h) return SS_ERR_INVALID;
+  if (!q_dev || !kc_dev || !vc_dev || !pos_dev || !bias_u_dev || !bias_v_dev || !out_dev || !slot_host || !a0_host || !nA_host || !T_host ||
+      !attn_chunk_host || !row0_host)
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_relpos_attention: null pointer");
+  const int D = H * 64;
+  if (n < 1 || H < 1 || n_slots < 1 || rows < 1 || Tpos < 1 || slot_stride < (int64_t)D || !row_stride_ok(ldq, D) || !row_stride_ok(ldo, D))
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_relpos_attention: bad shape");
+  // keys of a stream: T rows of D floats inside its slot; the row kernel keeps T scores in shared memory
+  const int T_cap = (int)std::min<int64_t>({(int64_t)Tpos, slot_stride / D, (int64_t)(ROW_KERNEL_SMEM / sizeof(float))});
+  std::vector<MsStream> st_host;
+  int max_nA = 0, Tmax = 0;
+  if (!ms_streams(n, slot_host, a0_host, nA_host, T_host, attn_chunk_host, row0_host, n_slots, T_cap, rows, false, st_host, max_nA, Tmax))
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_relpos_attention: a stream's slot, rows or chunk is out of range");
+  try {
+    OpUploads up;
+    ms_relpos_attention(q_dev, ldq, kc_dev, vc_dev, slot_stride, D, pos_dev, Tpos, bias_u_dev, bias_v_dev, out_dev, ldo, up.put(st_host.data(), n), n,
+                        max_nA, H, Tmax, S(stream));
+    return up.finish(h, S(stream), "ss_op_ms_relpos_attention");
+  } catch (const std::exception& e) {
+    return h->fail(SS_ERR_CUDA, e.what());
+  }
+}
+
+int ss_op_ms_depthwise(ss_engine* h, void* stream, const float* x_dev, int64_t slot_stride, int n_slots, const float* w_dev, const float* scale_dev,
+                       const float* shift_dev, float* y_dev, int ldy, int rows, int C, int k, int n, const int32_t* slot_host, const int32_t* a0_host,
+                       const int32_t* nA_host, const int32_t* T_host, const int32_t* conv_chunk_host, const int32_t* row0_host) {
+  if (!h) return SS_ERR_INVALID;
+  if (!x_dev || !w_dev || !scale_dev || !shift_dev || !y_dev || !slot_host || !a0_host || !nA_host || !T_host || !conv_chunk_host || !row0_host)
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_depthwise: null pointer");
+  if (n < 1 || C < 1 || k < 1 || k % 2 == 0 || n_slots < 1 || rows < 1 || slot_stride < (int64_t)C || ldy < C)
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_depthwise: bad shape");
+  std::vector<MsStream> st_host;
+  int max_nA = 0, Tmax = 0;
+  const int T_cap = (int)std::min<int64_t>(slot_stride / C, 1 << 30);
+  if (!ms_streams(n, slot_host, a0_host, nA_host, T_host, conv_chunk_host, row0_host, n_slots, T_cap, rows, true, st_host, max_nA, Tmax))
+    return h->fail(SS_ERR_INVALID, "ss_op_ms_depthwise: a stream's slot, rows or chunk is out of range");
+  try {
+    OpUploads up;
+    ms_depthwise(x_dev, slot_stride, w_dev, scale_dev, shift_dev, y_dev, ldy, up.put(st_host.data(), n), n, max_nA, C, k, S(stream));
+    return up.finish(h, S(stream), "ss_op_ms_depthwise");
+  } catch (const std::exception& e) {
+    return h->fail(SS_ERR_CUDA, e.what());
+  }
+}
+
+}  // extern "C"
+
 #include "engine_pool.inc"

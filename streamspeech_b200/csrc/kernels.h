@@ -150,16 +150,18 @@ void fbank_cmvn_tma(const float* samples, int f0, int nf, const float* melT, con
 // q: [B*nQ][ldq] rows for absolute query positions q_offset .. q_offset+nQ-1; k, v: [B*T][ld] rows for absolute
 // key positions 0..T-1; pos: [2*Tpos-1][D] rows indexed by (i-j) + Tpos-1; out: [B*nQ][D].
 // Full recompute: q = qkv, k = qkv + D, v = qkv + 2D, ld* = 3D, q_offset = 0, nQ = T.
+// kernel: 0 = row or tile kernel by the shape rule of kernels_attn.cu; 1 = row kernel (T * 4 bytes <= 160 KB), 2 = tile kernel
+// (the forced choices exist for the parity tests)
 void relpos_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* pos, int Tpos,
                       const float* bias_u, const float* bias_v, float* out, int B, int nQ, int q_offset, int T, int H, int D,
-                      int chunk /*0 = full*/, const int* lengths_dev, cudaStream_t st);
+                      int chunk /*0 = full*/, const int* lengths_dev, cudaStream_t st, int kernel = 0);
 
 // Standard multi-head attention, head_dim 64.  q rows = b*Tq + t, k / v rows = b*Tk + j.  kv_len[b] (device, optional) masks
 // keys >= len.  causal: key j visible to query i iff j <= i + causal_offset.  Each sample gets the same kernel and arithmetic
-// as a call with B = 1.
+// as a call with B = 1.  kernel: as relpos_attention's.
 void mha_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int B,
                    int Tq, int Tk, int H, float scale, int causal, int causal_offset, const int* kv_len_dev,
-                   cudaStream_t st);
+                   cudaStream_t st, int kernel = 0);
 
 // Causal self-attention over S groups of R identical consecutive rows (unit decoder layer 1, see kernels_attn.cu), for B samples:
 // q / k / v hold each sample's S distinct rows (rows b*S + g), out gets S*R rows per sample (rows (b*S + g)*R + r).

@@ -344,11 +344,12 @@ __global__ void __launch_bounds__(ATT_NT) grouped_causal_attn_kernel(const float
 template <bool RELPOS>
 void launch_attn(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* pos, int Tpos, int ldp,
                  const float* bias_u, const float* bias_v, float* out, int ldo, int B, int nQ, int q_offset, int T, int H, float scale,
-                 int chunk, int causal, int causal_offset, const int* lengths, int B_choice, cudaStream_t st) {
+                 int chunk, int causal, int causal_offset, const int* lengths, int B_choice, int kernel, cudaStream_t st) {
   // row or tile kernel, chosen from B_choice samples of this shape (1: from one sample, so that batching never switches a
-  // sample's arithmetic to the other kernel)
+  // sample's arithmetic to the other kernel); kernel = 1 / 2 forces the row / tile kernel (parity tests; the caller checks that
+  // T fits the row kernel's shared memory)
   const long tiles = (long)((nQ + QT - 1) / QT) * H * B_choice;
-  if (tiles < 96 && (size_t)T * sizeof(float) <= 160 * 1024) {
+  if (kernel == 1 || (kernel == 0 && tiles < 96 && (size_t)T * sizeof(float) <= 160 * 1024)) {
     size_t smem_row = (size_t)((T + 3) & ~3) * sizeof(float);
     if (smem_row > 40 * 1024 && first_time_on_device((const void*)attn_row_kernel<RELPOS>))
       cudaFuncSetAttribute(attn_row_kernel<RELPOS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
@@ -367,10 +368,11 @@ void launch_attn(const float* q, int ldq, const float* k, int ldk, const float* 
 
 void relpos_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* pos, int Tpos,
                       const float* bias_u, const float* bias_v, float* out, int B, int nQ, int q_offset, int T, int H, int D,
-                      int chunk, const int* lengths_dev, cudaStream_t st) {
+                      int chunk, const int* lengths_dev, cudaStream_t st, int kernel) {
   ++g_launches;
   if (B <= 0 || T <= 0 || nQ <= 0) return;
-  launch_attn<true>(q, ldq, k, ldk, v, ldv, pos, Tpos, D, bias_u, bias_v, out, D, B, nQ, q_offset, T, H, 0.125f, chunk, 0, 0, lengths_dev, B, st);
+  launch_attn<true>(q, ldq, k, ldk, v, ldv, pos, Tpos, D, bias_u, bias_v, out, D, B, nQ, q_offset, T, H, 0.125f, chunk, 0, 0, lengths_dev, B, kernel,
+                    st);
 }
 
 void grouped_causal_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int S, int R,
@@ -383,11 +385,11 @@ void grouped_causal_attention(const float* q, int ldq, const float* k, int ldk, 
 
 void mha_attention(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int B,
                    int Tq, int Tk, int H, float scale, int causal, int causal_offset, const int* kv_len_dev,
-                   cudaStream_t st) {
+                   cudaStream_t st, int kernel) {
   ++g_launches;
   if (B <= 0 || Tq <= 0 || Tk <= 0) return;
   launch_attn<false>(q, ldq, k, ldk, v, ldv, nullptr, 0, 0, nullptr, nullptr, out, ldo, B, Tq, 0, Tk, H, scale, 0, causal, causal_offset,
-                     kv_len_dev, 1, st);
+                     kv_len_dev, 1, kernel, st);
 }
 
 }  // namespace ss

@@ -108,6 +108,13 @@ def load_library() -> ctypes.CDLL:
     lib.ss_pool_step.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp]
     lib.ss_pool_mt_greedy.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32]
     lib.ss_t2u_unit_decode_ragged.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i32, vp, vp]
+    f32 = ctypes.c_float
+    lib.ss_op_relpos_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32]
+    lib.ss_op_mha_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, f32, i32, i32, vp, i32]
+    lib.ss_op_grouped_causal_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, f32, i32, vp]
+    lib.ss_op_depthwise_bn_silu.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32]
+    lib.ss_op_ms_relpos_attention.argtypes = [vp, vp, vp, i32, vp, vp, i64, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.ss_op_ms_depthwise.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     _lib = lib
     return lib
 
@@ -118,8 +125,13 @@ EXPORTED_SYMBOLS = [
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
-    "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_t2u_unit_decode_ragged",
+    "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
+    "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
 ]
+
+
+def _i32_array(xs: Optional[Sequence[int]]):
+    return None if xs is None else (ctypes.c_int32 * max(len(xs), 1))(*[int(x) for x in xs])
 
 
 def make_ss_config(cfg: ModelConfig, max_enc_frames: int, max_mt_positions: int = 1024) -> SSConfig:
@@ -692,3 +704,68 @@ class Engine:
         out = torch.empty_like(x)
         self._check(self.lib.ss_op_layer_norm(self._h, self._stream(), x.data_ptr(), x.shape[0], x.shape[1], g.data_ptr(), b.data_ptr(), out.data_ptr()))
         return out
+
+    # Attention / depthwise-conv parity hooks (ss_op_*_attention, ss_op_*depthwise*).  Matrices are 2-D device fp32 tensors whose rows
+    # may be strided (column slices of a fused buffer); kernel: 0 = the engine's choice, 1 = row kernel, 2 = tile kernel.
+    @staticmethod
+    def _ld(t: torch.Tensor) -> int:
+        assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1, (t.shape, t.stride())
+        return t.stride(0)
+
+    def op_relpos_attention(self, q, k, v, pos, bias_u, bias_v, B: int, nQ: int, q_offset: int, T: int, H: int, chunk: int,
+                            lengths: Optional[Sequence[int]] = None, kernel: int = 0) -> torch.Tensor:
+        """q [B*nQ, >=D] (absolute positions q_offset ..), k / v [B*T, >=D], pos [2*Tpos-1, D] -> out [B*nQ, D]"""
+        D = H * 64
+        Tpos = (pos.shape[0] + 1) // 2
+        out = self._f32(B * nQ, D)
+        self._check(self.lib.ss_op_relpos_attention(self._h, self._stream(), q.data_ptr(), self._ld(q), k.data_ptr(), self._ld(k), v.data_ptr(),
+                                                    self._ld(v), pos.data_ptr(), Tpos, bias_u.data_ptr(), bias_v.data_ptr(), out.data_ptr(), B,
+                                                    nQ, q_offset, T, H, D, chunk, _i32_array(lengths), kernel))
+        return out
+
+    def op_mha_attention(self, q, k, v, B: int, Tq: int, Tk: int, H: int, scale: float, causal: bool = False, causal_offset: int = 0,
+                         kv_len: Optional[Sequence[int]] = None, kernel: int = 0) -> torch.Tensor:
+        """q [B*Tq, >=D], k / v [B*Tk, >=D] -> out [B*Tq, D]"""
+        out = self._f32(B * Tq, H * 64)
+        self._check(self.lib.ss_op_mha_attention(self._h, self._stream(), q.data_ptr(), self._ld(q), k.data_ptr(), self._ld(k), v.data_ptr(),
+                                                 self._ld(v), out.data_ptr(), self._ld(out), B, Tq, Tk, H, float(scale), int(causal),
+                                                 causal_offset, _i32_array(kv_len), kernel))
+        return out
+
+    def op_grouped_causal_attention(self, q, k, v, B: int, S: int, R: int, H: int, scale: float,
+                                    kv_len: Optional[Sequence[int]] = None) -> torch.Tensor:
+        """q / k / v [B*S, >=D] (one row per group) -> out [B*S*R, D]"""
+        out = self._f32(B * S * R, H * 64)
+        self._check(self.lib.ss_op_grouped_causal_attention(self._h, self._stream(), q.data_ptr(), self._ld(q), k.data_ptr(), self._ld(k),
+                                                            v.data_ptr(), self._ld(v), out.data_ptr(), self._ld(out), S, R, H, float(scale), B,
+                                                            _i32_array(kv_len)))
+        return out
+
+    def op_depthwise_bn_silu(self, x, w, scale, shift, B: int, T: int, t0: int, n: int, chunk: int) -> torch.Tensor:
+        """x [B*T, >=C], w [k, C] -> y [B*n, C] for positions t0 .. t0+n-1"""
+        k, C = w.shape
+        y = self._f32(B * n, C)
+        self._check(self.lib.ss_op_depthwise_bn_silu(self._h, self._stream(), x.data_ptr(), self._ld(x), w.data_ptr(), scale.data_ptr(),
+                                                     shift.data_ptr(), y.data_ptr(), C, B, T, t0, n, C, k, chunk))
+        return y
+
+    @staticmethod
+    def _ms_args(streams: Sequence[dict], chunk_key: str):
+        return [_i32_array([s[f] for s in streams]) for f in ("slot", "a0", "nA", "T", chunk_key, "row0")]
+
+    def op_ms_relpos_attention(self, q, kc, vc, pos, bias_u, bias_v, out, H: int, streams: Sequence[dict]):
+        """kc / vc [n_slots, slot_rows, D] key / value caches; streams: dicts of slot, a0, nA, T, attn_chunk, row0; writes the rows of
+        out [rows, >=D] the streams own (the others are left as they are)"""
+        n_slots = kc.shape[0]
+        self._check(self.lib.ss_op_ms_relpos_attention(self._h, self._stream(), q.data_ptr(), self._ld(q), kc.data_ptr(), vc.data_ptr(),
+                                                       kc.stride(0), n_slots, pos.data_ptr(), (pos.shape[0] + 1) // 2, bias_u.data_ptr(),
+                                                       bias_v.data_ptr(), out.data_ptr(), self._ld(out), out.shape[0], H, len(streams),
+                                                       *self._ms_args(streams, "attn_chunk")))
+
+    def op_ms_depthwise(self, x, w, scale, shift, y, streams: Sequence[dict]):
+        """x [n_slots, slot_rows, C] conv-input caches; streams: dicts of slot, a0, nA, T, conv_chunk, row0; writes the rows of
+        y [rows, >=C] the streams own"""
+        k, C = w.shape
+        self._check(self.lib.ss_op_ms_depthwise(self._h, self._stream(), x.data_ptr(), x.stride(0), x.shape[0], w.data_ptr(), scale.data_ptr(),
+                                                shift.data_ptr(), y.data_ptr(), self._ld(y), y.shape[0], C, k, len(streams),
+                                                *self._ms_args(streams, "conv_chunk")))

@@ -91,6 +91,48 @@ def test_decoder_fixtures(gold):
     assert lgp[0].argmax(-1).tolist() == g["unit_argmax_pad"].tolist()
 
 
+def test_float64_oracle_reproduces_fixtures(gold):
+    """The float64 oracle is the reference of the fp64 kernel tests (test_attention_ops.py, test_long_utterance_fp64.py): it must
+    reproduce the fixtures of the real reference modules within the bars the fp32 oracle meets, so that it cannot drift with a kernel."""
+    cfg = golden_cfg()
+    sd = synth.make_model_state_dict(cfg, seed=0)
+    g = gold["encoder"]
+    feats = torch.from_numpy(g["feats"])
+    for chunk, conv in ((4, 8), (16, 16), (None, None)):
+        o = StreamSpeechOracle(cfg, sd, None, None, chunk_size=chunk, conv_chunk_size=conv, dtype=torch.float64)
+        out = o.encoder(feats.unsqueeze(0), torch.tensor([feats.size(0)]), return_layers=True)
+        assert out["encoder_out"][0].dtype == torch.float64
+        assert np.abs(out["encoder_out"][0][:, 0].numpy() - g[f"out_c{chunk}"]).max() < 2e-5, chunk
+        assert np.abs(out["encoder_states"][0][:, 0].numpy() - g[f"layer0_c{chunk}"]).max() < 2e-5, chunk
+    o = StreamSpeechOracle(cfg, sd, None, None, chunk_size=8, conv_chunk_size=8, dtype=torch.float64)
+    fb = torch.zeros(2, feats.size(0), 80)
+    fb[0] = feats
+    fb[1, :150] = feats[:150]
+    assert np.abs(o.encoder(fb, torch.from_numpy(g["batched_lens"]))["encoder_out"][0].numpy() - g["batched_out"]).max() < 2e-5
+    g = gold["decoders"]
+    eo = torch.from_numpy(g["enc_out"]).unsqueeze(1)
+    for name in ("source_unigram", "ctc_target_unigram"):
+        assert o.ctc_greedy(name, eo)[0]["org_tokens"] == g[f"ctc_{name}_argmax"].tolist()
+    toks = torch.from_numpy(g["mt_tokens"])
+    feats64 = o.mt_features(toks, eo)
+    assert feats64.dtype == torch.float64
+    # |features| reaches 240, where an fp32 ulp is 1.5e-5: the fixture's own rounding (measured 5.3e-5 from fp64) is held to the
+    # 2e-4 bar the fp32 kernels meet on this fixture (test_gpu_parity.py FP_TOL)
+    assert np.abs(feats64[0].numpy() - g["mt_feats"]).max() < 2e-4
+    assert np.abs(o.mt_logits(toks, eo)[0, -1].numpy() - g["mt_logits_last"]).max() < 5e-5
+    tp = torch.from_numpy(g["mt_tokens_pad"])
+    fp = o.mt_features(tp, eo)
+    assert np.abs(fp[0].numpy() - g["mt_feats_pad"]).max() < 2e-4
+    t2u = o.t2u_encoder(torch.from_numpy(g["mt_feats"]).unsqueeze(1), None)
+    assert np.abs(t2u[:, 0].numpy() - g["t2u_out"]).max() < 2e-5
+    lg = o.unit_decoder_logits(t2u, None)
+    assert np.abs(lg[0, :4].numpy() - g["unit_logits_first"]).max() < 1e-4
+    assert o.unit_ctc_greedy(lg)[0]["org_tokens"] == g["unit_argmax"].tolist()
+    pm = tp.eq(1)
+    lgp = o.unit_decoder_logits(o.t2u_encoder(fp.transpose(0, 1), pm), pm)
+    assert lgp[0].argmax(-1).tolist() == g["unit_argmax_pad"].tolist()
+
+
 def test_vocoder_fixture(gold):
     g = gold["vocoder"]
     cfg = golden_cfg()
