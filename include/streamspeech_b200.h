@@ -308,6 +308,28 @@ int ss_pool_step(ss_engine* h, void* stream, int n, const int32_t* slots_host, i
 int ss_pool_mt_greedy(ss_engine* h, void* stream, int n, const int32_t* slots_host, const int64_t* prefix_host, const int32_t* n_prefix_host,
                       const int32_t* max_new_tokens_host, int max_len_b, int64_t* tokens_out_host, int max_out, int32_t* n_out_host,
                       float* feats_out_dev, int feats_ld);
+/* ss_mt_greedy_incremental (the S2TT agent's MT search with the reference's incremental states, N12) for n pool streams at once,
+ * each on its slot's own state: stream i (slot slots_host[i]) gets exactly what ss_mt_greedy_incremental(enc, T_i, prefix_i,
+ * n_prefix_host[i], max_new_tokens_host[i], max_len_host[i]) gives on a handle holding that slot's state, with enc the slot's
+ * encoder rows [0, T_i) of its last ss_pool_step.  max_len_host[i] is the stream's max_len for max_new_tokens == -1.  The state
+ * lives in the pool until ss_pool_reset: per slot a self-attention cache [mt_layers][max_mt_positions][mt_dim] (K and V; allocated by
+ * the first call for every slot) with its entry count, and the cross-attention K / V of the encoder rows seen so far.  As in the
+ * single-stream call, each call re-feeds the last prefix token (one duplicate self-attention entry per call: the prefix's entry of
+ * position p is p + kv_off with kv_off = entries - n_prefix) and projects only encoder rows that earlier calls had not seen; those are
+ * never refreshed.  Prefix tokens are not fed again (their K / V are in the cache).  prefix_host holds the n prefixes concatenated;
+ * tokens_out_host [n][max_out] gets each hypothesis without eos (prefix included), n_out_host[i] its length.
+ * Up to 32 streams form a group: the new encoder rows of the whole group are projected at once, then groups of at least
+ * mt_batch_min_rows streams decode together on the batched MT kernel and smaller ones stream by stream on the single-token kernel,
+ * both over the same slot state.  The handle's single-stream MT state is neither read nor written.  A slot's cross K / V serve either
+ * this call or ss_pool_mt_greedy (which re-projects rows above T_final) between resets: the other one returns SS_ERR_STATE.
+ * Synchronises `stream` once per group for the uploads and once per burst of 16 steps.
+ * Errors, all before any launch or state change: SS_ERR_INVALID for a bad or repeated slot, a slot without encoder rows, a null
+ * pointer, a prefix token outside the vocabulary, max_len < 1 or a prefix longer than max_len; SS_ERR_STATE when kv_off < 0 (a prefix
+ * the state did not produce), the persistent MT kernel is off or does not support the shape, or ss_pool_mt_greedy owns the slot;
+ * SS_ERR_CAPACITY when max_len + kv_off + 2 > max_mt_positions or max_len > max_out.  A refused cooperative launch is SS_ERR_CUDA. */
+int ss_pool_mt_greedy_incremental(ss_engine* h, void* stream, int n, const int32_t* slots_host, const int64_t* prefix_host,
+                                  const int32_t* n_prefix_host, const int32_t* max_new_tokens_host, const int32_t* max_len_host,
+                                  int64_t* tokens_out_host, int max_out, int32_t* n_out_host);
 
 /* ---- single ops exported for the parity tests (same kernels the entry points above launch) ------------- */
 int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N,

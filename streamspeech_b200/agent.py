@@ -534,11 +534,17 @@ class StreamSpeechS2TTAgent(_EngineAgentMixin, SpeechToTextAgent):
         self.tgt_text = ""
         self.states.reset()
         self._reset_caches()
+
+    def _reset_caches(self):
+        """new utterance: the mixin's caches and the handle's incremental MT state"""
+        super()._reset_caches()
         if hasattr(self, "engine"):
             self.engine.mt_incremental_reset()
 
     @torch.inference_mode()
     def policy(self):
+        """The body of the reference policy().  The host stages around the MT call are methods of their own (_gate, _after_mt), which
+        the pooled agent (scheduler.PooledS2TTAgent) calls around its batched MT call."""
         tr = self.trace = {}
         feature = self._features()
         if feature.size(0) == 0 and not self.states.source_finished:
@@ -546,27 +552,42 @@ class StreamSpeechS2TTAgent(_EngineAgentMixin, SpeechToTextAgent):
         enc = self._encode(feature)
         (src_ctc_indices, _), (tgt_ctc_indices, _) = self._ctc_pair(enc)
         tr["asr_tokens"], tr["st_tokens"] = src_ctc_indices, tgt_ctc_indices
+        new_subword_tokens = self._gate(src_ctc_indices, tgt_ctc_indices)
+        if new_subword_tokens is None:
+            return ReadAction()
+        tokens = self.engine.mt_greedy_incremental(enc, self.tgt_subwords_indices, new_subword_tokens, self._max_len(feature.size(0)))
+        return self._after_mt(tokens, new_subword_tokens)
+
+    def _max_len(self, n_frames: int) -> int:
+        """generator_mt: max_len_a = 1, max_len_b = 200 (:161-179); src_len = src_tokens.size(1) = fbank frames"""
+        return min(int(n_frames + 200), self.max_decoder_positions - 1)
+
+    def _gate(self, src_ctc_indices, tgt_ctc_indices) -> Optional[int]:
+        """READ / WRITE gate on the CTC prefixes (:437-465): None = READ, else the MT call's new_subword_tokens (-1 once the source is
+        finished)."""
         if not self.states.source_finished:  # :437-465
             src_ctc_prefix_length, tgt_ctc_prefix_length = len(src_ctc_indices), len(tgt_ctc_indices)
             self.src_ctc_indices = src_ctc_indices
             if (src_ctc_prefix_length < self.src_ctc_prefix_length + self.stride_n
                     or tgt_ctc_prefix_length < self.tgt_ctc_prefix_length + self.stride_n):
-                return ReadAction()
+                return None
             self.src_ctc_prefix_length = max(src_ctc_prefix_length, self.src_ctc_prefix_length)
             self.tgt_ctc_prefix_length = max(tgt_ctc_prefix_length, self.tgt_ctc_prefix_length)
             subword_tokens = ((tgt_ctc_prefix_length - self.lagging_k1) // self.stride_n) * self.stride_n
             new_subword_tokens = (subword_tokens - len(self.tgt_subwords_indices)) if self.tgt_subwords_indices is not None else subword_tokens
             if new_subword_tokens < 1:
-                return ReadAction()
+                return None
         else:
             self.src_ctc_indices = src_ctc_indices
             new_subword_tokens = -1
         new_subword_tokens = int(new_subword_tokens)
-        tr["new_subword_tokens"] = new_subword_tokens
-        # generator_mt: max_len_a = 1, max_len_b = 200 (:161-179); src_len = src_tokens.size(1) = fbank frames
-        max_len_full = min(int(feature.size(0) + 200), self.max_decoder_positions - 1)
-        tokens = self.engine.mt_greedy_incremental(enc, self.tgt_subwords_indices, new_subword_tokens, max_len_full)
-        tr["mt_tokens"] = list(tokens)
+        self.trace["new_subword_tokens"] = new_subword_tokens
+        return new_subword_tokens
+
+    def _after_mt(self, tokens: List[int], new_subword_tokens: int):
+        """From the MT hypothesis (without eos) to the action (:519-545): the "same hypothesis" check, the text delta and the reset
+        quirk at the end of the utterance."""
+        self.trace["mt_tokens"] = list(tokens)
         if self.tgt_subwords_indices is not None and self.tgt_subwords_indices == tokens:  # :519-529
             if not self.states.source_finished:
                 return ReadAction()

@@ -224,6 +224,15 @@ struct ss_engine {
     // [0, mt_cross_rows[slot]) were projected from final encoder rows and are not projected again until ss_pool_reset
     float* mt_cross = nullptr;
     std::vector<int> mt_cross_rows;
+    // ss_pool_mt_greedy_incremental: the reference's incremental MT decoder state per slot, as the handle keeps it for one stream
+    // (mt_inc_self_len / mt_inc_cross_rows).  Self-attention K then V, each [slot][mt_layers][max_mt_positions][mt_dim] (allocated
+    // by its first call): a slot's block is MtDecodeParams' self_k / self_v, and its block of mt_cross is cross_kv with cross_cap = Tcap.
+    float* mt_self_kv = nullptr;
+    std::vector<int> mt_inc_self_len, mt_inc_cross_rows;
+    // which search owns the slot's block of mt_cross since its last reset: ss_pool_mt_greedy re-projects rows at or above T_final,
+    // the incremental search keeps every row it projected, so a slot serves one of them until ss_pool_reset
+    enum MtOwner : char { kMtNone, kMtGreedy, kMtIncremental };
+    std::vector<char> mt_owner;
   } pool;
 
   int fail(int code, const std::string& msg) {

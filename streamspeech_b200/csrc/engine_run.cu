@@ -1083,6 +1083,44 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
   return check_launch(h, "ss_mt_greedy_batch");
 }
 
+}  // extern "C"
+
+namespace {
+
+// The incremental search of one stream on the single-token kernel: P holds the stream's state (self_k / self_v / cross_kv, kv_off)
+// and P.tok[start] its first token; positions start .. max_len over Tk cross rows, `burst` steps per launch and synchronisation.
+// The new tokens go to tokens_out_host[*n_tok ...]; *self_len follows the entries the self-attention cache holds.
+int mt_incremental_bursts(ss_engine* h, cudaStream_t st, const MtDecodeParams& P, int start, int max_len, int Tk, int burst, int64_t* tokens_out_host,
+                          int* n_tok, int* self_len, const char* where) {
+  int step = start;
+  bool done = false;
+  while (!done) {
+    const int cnt = std::min(max_len - step + 1, burst);
+    if (mt_decode_persistent(P, h->mt_persist_layers, step, cnt, max_len, Tk, h->persist_bar, &h->persist_bar_target, st) != 0) {
+      cudaGetLastError();
+      return h->fail(SS_ERR_CUDA, std::string(where) + ": cooperative launch of the persistent MT kernel was refused");
+    }
+    const int readable = std::min(cnt, max_len - step);  // the forced-eos step writes no token
+    const int rc = sync_burst(h, st, h->mt_next_pinned, P.tok + step + 1, readable, readable, 1, where);
+    if (rc) return rc;
+    for (int i = 0; i < cnt && !done; ++i) {
+      const int sidx = step + i;            // this step fed the token at position sidx (one more cache entry)
+      *self_len = sidx + P.kv_off + 1;
+      if (sidx >= max_len) { done = true; break; }   // eos forced (sequence_generator.py:362-364)
+      const int64_t next = h->mt_next_pinned[i];
+      if (next == h->cfg.eos) { done = true; break; }
+      tokens_out_host[(*n_tok)++] = next;
+    }
+    step += cnt;
+    if (step > max_len) done = true;
+  }
+  return SS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 int ss_mt_incremental_reset(ss_engine* h) {
   if (!h) return SS_ERR_INVALID;
   h->mt_inc_self_len = 0;
@@ -1140,29 +1178,9 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
   int n_tok = start;
   for (int i = 0; i < start; ++i) tokens_out_host[i] = prefix_host[i];
   const int burst = (max_new_tokens >= 0) ? std::max(1, max_new_tokens + 1) : 32;
-  int step = start;
-  bool done = false;
-  while (!done) {
-    const int cnt = std::min(max_len - step + 1, burst);
-    const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats, kv_off);
-    if (mt_decode_persistent(P, h->mt_persist_layers, step, cnt, max_len, Tk, h->persist_bar, &h->persist_bar_target, st) != 0) {
-      cudaGetLastError();
-      return h->fail(SS_ERR_CUDA, "cooperative launch of the persistent MT kernel was refused");
-    }
-    const int readable = std::min(cnt, max_len - step);  // the forced-eos step writes no token
-    rc = sync_burst(h, st, h->mt_next_pinned, h->mt_tok_dev + step + 1, readable, readable, 1, "ss_mt_greedy_incremental");
-    if (rc) return rc;
-    for (int i = 0; i < cnt && !done; ++i) {
-      const int sidx = step + i;            // this step fed the token at position sidx (one more cache entry)
-      h->mt_inc_self_len = sidx + kv_off + 1;
-      if (sidx >= max_len) { done = true; break; }   // eos forced (sequence_generator.py:362-364)
-      const int64_t next = h->mt_next_pinned[i];
-      if (next == c.eos) { done = true; break; }
-      tokens_out_host[n_tok++] = next;
-    }
-    step += cnt;
-    if (step > max_len) done = true;
-  }
+  const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats, kv_off);
+  rc = mt_incremental_bursts(h, st, P, start, max_len, Tk, burst, tokens_out_host, &n_tok, &h->mt_inc_self_len, "ss_mt_greedy_incremental");
+  if (rc) return rc;
   *n_out = n_tok;
   return check_launch(h, "ss_mt_greedy_incremental");
 }

@@ -122,6 +122,12 @@ struct MtBatchParams {
   const int* cross_row = nullptr;   // [rows] cross_kv is [.][layers][cross_cap][2 * dim] and row r reads block cross_row[r]
   float* feats = nullptr;           // [rows][feats_ld][dim]: the final-LN row of every position a row feeds
   int feats_ld = 0;
+  // The incremental search (ss_pool_mt_greedy_incremental) sets these two on top of the four above (feats may then be null; a third
+  // instantiation reads them): self_k / self_v are then [.][layers][self_ld][dim], row r's block is self_row[r], and the
+  // position-p entry of row r is p + kv_off[r] (self-attention spans p + kv_off[r] + 1 entries), as MtDecodeParams' kv_off.
+  const int* self_row = nullptr;
+  const int* kv_off = nullptr;
+  int self_ld = 0;
 };
 // enqueue steps step0 .. step0 + nsteps - 1 for every unfinished row (without P.max_len, all < the host's max_len: the forced-eos
 // step needs no work); returns 0, or < 0 if the launch was refused

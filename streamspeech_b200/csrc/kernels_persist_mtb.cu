@@ -7,6 +7,9 @@
 // The stream pool's search (ss_pool_mt_greedy) continues each row after a forced prefix: with MtBatchParams' per-row fields a row
 // feeds position start + step (position embedding, cache row, self-attention length and the position-0 eos ban follow), stops at
 // its own max_len with eos forced, reads its slot's cross K / V and writes its final-LN rows as features.
+// The incremental search (ss_pool_mt_greedy_incremental) runs a third instantiation on the same per-row fields plus two more: row r
+// keeps its self-attention cache in a block of its own that lives across calls (self_row[r], [layers][self_ld][dim] as
+// MtDecodeParams' self_k / self_v), and the position-p entry of that cache is p + kv_off[r] (the single-token kernel's kv_off).
 // Every CTA keeps the residual rows of all samples in shared memory (32 x 2 KB); the LayerNorm outputs share a second
 // 64 KB buffer with the FFN hidden rows, which do not fit at once (8 KB each) and are staged 8 rows at a time.
 //
@@ -147,9 +150,18 @@ __device__ __forceinline__ void attend_rows(MtSmem& sm, MtbSmem& sb, const float
   }
 }
 
-// position row r feeds at step s (kRows: a search that continues a forced prefix, MtBatchParams' per-row fields set)
-template <bool kRows>
-__device__ __forceinline__ int row_pos(const MtBatchParams& P, int r, int s) { return kRows ? P.start[r] + s : s; }
+// the three searches: offline (no per-row fields), a forced prefix continued (start / max_len / cross_row / feats), and the
+// incremental search on slot-resident self-attention caches (those fields plus self_row / kv_off, feats optional)
+enum MtbMode { kMtbOffline, kMtbPrefix, kMtbIncremental };
+
+// position row r feeds at step s
+template <int kMode>
+__device__ __forceinline__ int row_pos(const MtBatchParams& P, int r, int s) { return kMode != kMtbOffline ? P.start[r] + s : s; }
+
+// kMtbIncremental: offset of row r's layer-l block in the slot-resident self-attention cache (K and V alike)
+__device__ __forceinline__ size_t self_block(const MtBatchParams& P, int r, int l) {
+  return ((size_t)P.self_row[r] * P.n_layers + l) * P.self_ld * DIM;
+}
 
 __device__ __forceinline__ void load_active(MtbSmem& sb, const int* fin, int rows) {
   if (threadIdx.x == 0) {
@@ -161,8 +173,8 @@ __device__ __forceinline__ void load_active(MtbSmem& sb, const int* fin, int row
   __syncthreads();
 }
 
-// kRows = false: the per-row fields are null and compiled out (the offline generator's search as before they existed)
-template <bool kRows>
+// kMtbOffline: the per-row fields are null and compiled out (the offline generator's search as before they existed)
+template <int kMode>
 __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P, const MtLayerP* __restrict__ layers, int step0, int nsteps,
                                                                  unsigned* bar_ctr, unsigned bar_target) {
   __shared__ __align__(16) MtSmem sm;
@@ -189,7 +201,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     for (int e = tid; e < sb.nact * DIM; e += MTT) {
       const int r = sb.act[e / DIM], c = e % DIM;
       const int64_t tok = P.tok[(size_t)r * P.tok_ld + s];
-      const int p = (tok == P.pad) ? P.pad : P.pad + 1 + row_pos<kRows>(P, r, s);
+      const int p = (tok == P.pad) ? P.pad : P.pad + 1 + row_pos<kMode>(P, r, s);
       xs[r * DIM + c] = emb_scale * P.emb[tok * DIM + c] + P.pos[(int64_t)p * DIM + c];
     }
     __syncthreads();
@@ -212,9 +224,14 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       ln_rows(sb, xs, vb, L.self_g, L.self_b);
       for (int i = 0; i < sb.nact; ++i) {
         const int r = sb.act[i];
-        const int pos = row_pos<kRows>(P, r, s);
+        const int pos = row_pos<kMode>(P, r, s);
         float* kc = kl + ((size_t)r * P.tok_ld + pos) * DIM;
         float* vc = vl + ((size_t)r * P.tok_ld + pos) * DIM;
+        if constexpr (kMode == kMtbIncremental) {
+          const size_t e = self_block(P, r, l) + (size_t)(pos + P.kv_off[r]) * DIM;
+          kc = P.self_k + e;
+          vc = P.self_v + e;
+        }
         gemv_finish_b(w_qkv, vb + r * DIM, 3 * DIM, [&](int col, float y) {
           if (col < DIM) P.q[(size_t)r * DIM + col] = y;
           else if (col < 2 * DIM) kc[col - DIM] = y;
@@ -226,10 +243,17 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       // (2) self-attention over positions 0..s of each row's cache + partial out-projections
       if (in_group)
         attend_rows(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
-          kb = kl + (size_t)r * P.tok_ld * DIM;
-          vbs = vl + (size_t)r * P.tok_ld * DIM;
           ld = DIM;
-          n = row_pos<kRows>(P, r, s) + 1;
+          if constexpr (kMode == kMtbIncremental) {
+            const size_t b = self_block(P, r, l);
+            kb = P.self_k + b;
+            vbs = P.self_v + b;
+            n = row_pos<kMode>(P, r, s) + P.kv_off[r] + 1;
+          } else {
+            kb = kl + (size_t)r * P.tok_ld * DIM;
+            vbs = vl + (size_t)r * P.tok_ld * DIM;
+            n = row_pos<kMode>(P, r, s) + 1;
+          }
         }, L.wo, grp_h, grp_j, P.part);
       ARRIVE();
       GemvW<DIM, 1> w_cq;
@@ -247,7 +271,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       // (4) cross-attention over the first cross_len[r] encoder rows of each sample + partial out-projections
       if (in_group)
         attend_rows(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
-          const size_t blk = kRows ? (size_t)P.cross_row[r] * P.n_layers + l : (size_t)l * MAXR + r;
+          const size_t blk = kMode != kMtbOffline ? (size_t)P.cross_row[r] * P.n_layers + l : (size_t)l * MAXR + r;
           kb = P.cross_kv + blk * P.cross_cap * 2 * DIM;
           vbs = kb + DIM;
           ld = 2 * DIM;
@@ -292,10 +316,10 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     gemv_issue(w_out, P.emb, P.vocab);
     add_delta_rows(sb, xs, P.delta);
     ln_rows(sb, xs, vb, P.out_g, P.out_b);
-    if (kRows && blockIdx.x == 0)
+    if (kMode != kMtbOffline && (kMode != kMtbIncremental || P.feats) && blockIdx.x == 0)
       for (int e = tid; e < sb.nact * DIM; e += MTT) {
         const int r = sb.act[e / DIM], c = e % DIM;
-        P.feats[((size_t)r * P.feats_ld + row_pos<kRows>(P, r, s)) * DIM + c] = vb[r * DIM + c];
+        P.feats[((size_t)r * P.feats_ld + row_pos<kMode>(P, r, s)) * DIM + c] = vb[r * DIM + c];
       }
     for (int i = 0; i < sb.nact; ++i) {
       const int r = sb.act[i];
@@ -305,8 +329,8 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     // ---- arg-max: unfinished row i on CTA i (eos forced at the row's max_len)
     for (int i = blockIdx.x; i < sb.nact; i += gridDim.x) {
       const int r = sb.act[i];
-      const int pos = row_pos<kRows>(P, r, s);
-      const int tk = (kRows && pos >= P.max_len[r]) ? P.eos : masked_argmax(sm, P.logits + (size_t)r * P.vocab, P.vocab, P.pad, P.eos, pos);
+      const int pos = row_pos<kMode>(P, r, s);
+      const int tk = (kMode != kMtbOffline && pos >= P.max_len[r]) ? P.eos : masked_argmax(sm, P.logits + (size_t)r * P.vocab, P.vocab, P.pad, P.eos, pos);
       if (tid == 0) {
         P.tok[(size_t)r * P.tok_ld + s + 1] = tk;
         if (tk == P.eos) P.fin[r] = 1;
@@ -329,9 +353,12 @@ int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step
                     cudaStream_t st) {
   ++g_launches;
   if (P.rows < 1 || P.rows > MAXR) return -1;
-  const bool rows = P.start != nullptr;
-  if (rows && (!P.max_len || !P.cross_row || !P.feats)) return -1;  // the per-row fields come together
-  const void* kernel = rows ? (const void*)mt_decode_batch_kernel<true> : (const void*)mt_decode_batch_kernel<false>;
+  const bool rows = P.start != nullptr, inc = P.self_row != nullptr;
+  if (rows && (!P.max_len || !P.cross_row || (!P.feats && !inc))) return -1;  // the per-row fields come together
+  if (inc && (!rows || !P.kv_off || P.self_ld < 1)) return -1;
+  const void* kernel = inc    ? (const void*)mt_decode_batch_kernel<kMtbIncremental>
+                       : rows ? (const void*)mt_decode_batch_kernel<kMtbPrefix>
+                              : (const void*)mt_decode_batch_kernel<kMtbOffline>;
   if (first_time_on_device(kernel)) {  // cooperative launch needs one resident CTA per SM
     cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDynSmem);
     int occ = 0;

@@ -107,6 +107,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_pool_info.argtypes = [vp, i32, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     lib.ss_pool_step.argtypes = [vp, vp, i32, vp, i32, vp, i64, vp, vp, vp]
     lib.ss_pool_mt_greedy.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32]
+    lib.ss_pool_mt_greedy_incremental.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.ss_t2u_unit_decode_ragged.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i32, vp, vp]
     f32 = ctypes.c_float
     lib.ss_op_relpos_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32]
@@ -125,7 +126,7 @@ EXPORTED_SYMBOLS = [
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
-    "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
+    "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
     "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
 ]
 
@@ -687,6 +688,27 @@ class Engine:
         self._check(self.lib.ss_pool_mt_greedy(self._h, self._stream(), n, sl, cat, npf, mnt, int(max_len_b), out, cap, n_out, feats.data_ptr(),
                                                feats_ld))
         return [[int(out[i * cap + k]) for k in range(n_out[i])] for i in range(n)], feats[:n]
+
+    def pool_mt_greedy_incremental(self, slots: Sequence[int], prefixes: Sequence[Optional[Sequence[int]]], max_new_tokens: Sequence[int],
+                                   max_lens: Sequence[int]) -> List[List[int]]:
+        """mt_greedy_incremental of several pool streams at once (ss_pool_mt_greedy_incremental), each on its slot's own incremental
+        state (kept until pool_reset) and its encoder rows of the last pool_step: stream i continues prefixes[i] (None = empty) with
+        max_new_tokens[i] (-1 = source finished, then max_lens[i] is the generator's max_len).  Returns hypotheses without eos."""
+        n = len(slots)
+        if len(prefixes) != n or len(max_new_tokens) != n or len(max_lens) != n:
+            raise EngineError(f"{len(prefixes)} prefixes, {len(max_new_tokens)} token limits and {len(max_lens)} max_lens for {n} streams")
+        pfx = [list(p) if p is not None else [] for p in prefixes]
+        cap = self.max_mt_positions
+        flat = [int(t) for p in pfx for t in p]
+        sl = (ctypes.c_int32 * max(n, 1))(*[int(x) for x in slots])
+        cat = (ctypes.c_int64 * max(len(flat), 1))(*flat)
+        npf = (ctypes.c_int32 * max(n, 1))(*[len(p) for p in pfx])
+        mnt = (ctypes.c_int32 * max(n, 1))(*[int(m) for m in max_new_tokens])
+        mls = (ctypes.c_int32 * max(n, 1))(*[int(m) for m in max_lens])
+        out = (ctypes.c_int64 * (max(n, 1) * cap))()
+        n_out = (ctypes.c_int32 * max(n, 1))()
+        self._check(self.lib.ss_pool_mt_greedy_incremental(self._h, self._stream(), n, sl, cat, npf, mnt, mls, out, cap, n_out))
+        return [[int(out[i * cap + k]) for k in range(n_out[i])] for i in range(n)]
 
     def pool_encoder_rows(self, slot: int, T: int) -> torch.Tensor:
         """the slot's first T encoder rows [T, enc_dim] as a tensor over the pool's device memory (a view: valid until the next pool_step)"""

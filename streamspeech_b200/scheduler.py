@@ -11,6 +11,11 @@ of the round finds its result ready.  A harness that feeds the agents round-robi
 MT search (ss_pool_mt_greedy) for every stream whose policy gate says WRITE and ONE T2U + unit-decoder call
 (ss_t2u_unit_decode_ragged) for every stream that still has something to say; the vocoder stays one call per stream.  The host
 stages around those calls are the single agent's own methods (StreamSpeechS2STAgent._gate / _after_mt / _after_t2u).
+
+`PooledS2TTAgent` does the same for simultaneous speech-to-text translation: ONE incremental MT search
+(ss_pool_mt_greedy_incremental) for every writing stream, each on its slot's own incremental decoder state, between the single
+agent's host stages (StreamSpeechS2TTAgent._gate / _after_mt).  S2ST and S2TT agents can share one pool: a flush runs the decode
+round of each kind for its own streams.
 """
 from __future__ import annotations
 
@@ -18,7 +23,7 @@ from typing import Dict, List, Optional, Sequence
 
 import torch
 
-from streamspeech_b200.agent import READ, SAMPLE_RATE, StreamSpeechS2STAgent
+from streamspeech_b200.agent import READ, SAMPLE_RATE, StreamSpeechS2STAgent, StreamSpeechS2TTAgent
 from streamspeech_b200.engine import Engine
 from streamspeech_b200.simuleval_compat import ReadAction, SpeechToSpeechAgent, SpeechToTextAgent, WriteAction
 
@@ -38,8 +43,13 @@ class StreamPool:
         self.results: Dict[int, dict] = {}       # slot -> result of the last step that included it
         self.steps = 0                           # batched steps run (for tests / bench)
         self.rows_per_step: List[int] = []
-        self.s2st: Dict[int, "PooledS2STAgent"] = {}  # slot -> its S2ST agent: a flush also runs the decoders of these slots
+        self.decoders: Dict[int, "_PooledDecoder"] = {}  # slot -> its S2ST / S2TT agent: a flush also runs the decoders of these slots
         self.stage_ms: Optional[Dict[str, float]] = None  # a dict: device time per stage of every flush is added to it (CUDA events)
+
+    @property
+    def s2st(self) -> Dict[int, "PooledS2STAgent"]:
+        """the S2ST agents among the decoding agents, by slot"""
+        return {s: a for s, a in self.decoders.items() if isinstance(a, PooledS2STAgent)}
 
     def acquire(self) -> int:
         if not self.free:
@@ -55,7 +65,7 @@ class StreamPool:
         self.engine.pool_set_chunk(slot, 0, 0)
         self.pending.pop(slot, None)
         self.results.pop(slot, None)
-        self.s2st.pop(slot, None)
+        self.decoders.pop(slot, None)
         self.free.append(slot)
 
     def set_chunk(self, slot: int, attn_chunk: int, conv_chunk: int):
@@ -80,7 +90,8 @@ class StreamPool:
         self.results.pop(slot, None)
 
     def flush(self):
-        """one batched step for every stream with pending input (and the decoders of its S2ST streams)"""
+        """one batched step for every stream with pending input, then the decode round of its S2ST streams and that of its S2TT
+        streams"""
         slots = sorted(self.pending)
         if not slots:
             return
@@ -92,9 +103,12 @@ class StreamPool:
         self.pending.clear()
         self.steps += 1
         self.rows_per_step.append(len(slots))
-        agents = [self.s2st[s] for s in slots if s in self.s2st]
-        if agents:
-            PooledS2STAgent.decode_round(self, agents, clock)
+        rounds: Dict[type, list] = {}  # agent class -> its agents of this flush, in slot order
+        for s in slots:
+            if s in self.decoders:
+                rounds.setdefault(type(self.decoders[s]), []).append(self.decoders[s])
+        for kind, agents in rounds.items():
+            kind.decode_round(self, agents, clock)
         clock.close()
 
     def result(self, slot: int) -> dict:
@@ -178,7 +192,19 @@ class PooledASRAgent(_PooledSource, SpeechToTextAgent):
         return WriteAction(new_text, finished=self.states.target_finished)
 
 
-class PooledS2STAgent(_PooledSource, StreamSpeechS2STAgent):
+class _PooledDecoder(_PooledSource):
+    """an agent whose policy() result is computed by its pool's flush (decode_round of its class) and kept until it is asked for"""
+
+    def _policy_impl(self):
+        if self._action is None:
+            self.pool.flush()  # this agent's segment is pending: the round computes the action of every pending agent
+        action, self._action = self._action, None
+        if action is None:
+            raise RuntimeError("policy() of a pooled agent needs a pushed segment first")
+        return action
+
+
+class PooledS2STAgent(_PooledDecoder, StreamSpeechS2STAgent):
     """StreamSpeechS2STAgent (agent/speech_to_speech.streamspeech.agent.py:101-770) bound to a slot of a shared StreamPool: same
     push() / pop() / policy() contract and WriteAction(SpeechSegment) output, the same policy code (the single agent's host stages),
     but the tensor work of all agents of a round runs as one pool step, one batched MT search and one T2U + unit-decoder call.
@@ -212,7 +238,7 @@ class PooledS2STAgent(_PooledSource, StreamSpeechS2STAgent):
         self.slot = pool.acquire()
         chunk_size = args.source_segment_size // 40  # agent:395-413
         pool.set_chunk(self.slot, chunk_size, 16 if chunk_size >= 16 else 8)  # once: it survives the reset between utterances
-        pool.s2st[self.slot] = self
+        pool.decoders[self.slot] = self
         SpeechToSpeechAgent.__init__(self, args)  # states + reset()
 
     def _reset_caches(self):
@@ -220,14 +246,6 @@ class PooledS2STAgent(_PooledSource, StreamSpeechS2STAgent):
         if hasattr(self, "slot"):
             self.pool.reset(self.slot)
         self._action = None
-
-    def _policy_impl(self):
-        if self._action is None:
-            self.pool.flush()  # this agent's segment is pending: the round computes the action of every pending agent
-        action, self._action = self._action, None
-        if action is None:
-            raise RuntimeError("policy() of a pooled agent needs a pushed segment first")
-        return action
 
     @staticmethod
     @torch.inference_mode()
@@ -285,6 +303,76 @@ class PooledS2STAgent(_PooledSource, StreamSpeechS2STAgent):
         clock.mark("vocoder")
         for (a, new, _, _, _, _), u in zip(going, units):
             a._action = a._after_t2u(u, new)
+
+
+class PooledS2TTAgent(_PooledDecoder, StreamSpeechS2TTAgent):
+    """StreamSpeechS2TTAgent (agent/speech_to_text.s2tt.streamspeech.agent.py:101-545) bound to a slot of a shared StreamPool: same
+    push() / pop() / policy() contract and text output, the same policy code (the single agent's host stages), but the tensor work of
+    all agents of a round runs as one pool step and one incremental MT search.  The reference's incremental MT decoder state (N12) lives
+    in the slot (ss_pool_mt_greedy_incremental) and is cleared with it by reset(), as the single agent clears the handle's.  The pool
+    needs both CTC heads (StreamPool(..., ctc_heads=2)).  The slot takes the S2TT agent's latency rule: chunk c = source_segment_size //
+    40, conv chunk min(c, 16) (:359-366).  dictionary: the target subword dictionary (the single agent's dict["target_unigram"]);
+    args: the single agent's flags (lagging_k1, stride_n, ...); the model comes from the pool's engine."""
+
+    def __init__(self, pool: StreamPool, dictionary, args):
+        if pool.ctc_heads != 2:
+            raise ValueError("a pooled S2TT agent needs a stream pool with both CTC heads (ctc_heads=2)")
+        self.pool = pool
+        self.engine = pool.engine
+        self.cfg = pool.engine.cfg
+        self.torch_device = pool.engine.device
+        self.dict = {"target_unigram": dictionary}
+        self.lagging_k1 = args.lagging_k1
+        self.lagging_k2 = args.lagging_k2
+        self.segment_size = args.segment_size
+        self.stride_n = args.stride_n
+        self.unit_per_subword = args.unit_per_subword
+        self.stride_n2 = args.stride_n2
+        self.max_decoder_positions = getattr(args, "max_decoder_positions", 1200)
+        self.trace = {}
+        self._action = None
+        self.slot = pool.acquire()
+        chunk_size = args.source_segment_size // 40  # :359-366
+        pool.set_chunk(self.slot, chunk_size, min(chunk_size, 16))  # once: it survives the reset between utterances
+        pool.decoders[self.slot] = self
+        SpeechToTextAgent.__init__(self, args)  # states + reset()
+
+    def _reset_caches(self):
+        """new utterance: the slot starts over (audio, encoder state, incremental MT state)"""
+        if hasattr(self, "slot"):
+            self.pool.reset(self.slot)
+        self._action = None
+
+    def policy(self):
+        return self._policy_impl()
+
+    @staticmethod
+    @torch.inference_mode()
+    def decode_round(pool: StreamPool, agents: Sequence["PooledS2TTAgent"], clock: _StageClock):
+        """The S2TT stages of a flush for the agents whose slots the pool step just ran: the gate per stream, one incremental MT
+        search for the writing streams, then the text delta per stream."""
+        eng = pool.engine
+        writing = []
+        for a in agents:
+            a.trace = {}
+            r = pool.results[a.slot]
+            if r["T"] == 0 and not a.states.source_finished:  # no fbank frame yet
+                a._action = ReadAction()
+                continue
+            (src, _), (tgt, _) = r["ctc"]
+            a.trace["asr_tokens"], a.trace["st_tokens"] = src, tgt
+            new = a._gate(src, tgt)
+            if new is None:
+                a._action = ReadAction()
+            else:
+                writing.append((a, new))
+        if not writing:
+            return
+        clock.mark("mt_incremental")
+        hyps = eng.pool_mt_greedy_incremental([a.slot for a, _ in writing], [a.tgt_subwords_indices for a, _ in writing],
+                                              [new for _, new in writing], [a._max_len(eng.pool_info(a.slot)["n_feat"]) for a, _ in writing])
+        for (a, new), tokens in zip(writing, hyps):
+            a._action = a._after_mt(tokens, new)
 
 
 def pushpop_many(agents: Sequence, segments: Sequence) -> list:
