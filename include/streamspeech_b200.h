@@ -253,6 +253,24 @@ int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, i
  * (the agent always emits the tail).  enqueue only */
 int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0, int n_frames, int left_context,
                         float* wav_out_dev);
+/* ---- V1 + V2 of n sequences at once (ss_vocoder_durations / ss_vocoder_generate are these calls with n = 1).
+ * Durations: codes_dev holds the n code sequences concatenated (U_host[n] units each); dur_out_dev receives the durations
+ * packed the same way, and cumsum_out_dev (optional) one cumsum of U_s + 1 frame offsets per sequence, packed in sequence order.
+ * The duration predictor runs over groups of up to 32 sequences (and as many padded rows as its split-K scratch holds) in a fixed
+ * number of launches per group, each sequence seeing its own zero padding; every sequence's durations and cumsum equal those of a
+ * call with that sequence alone.  The expanded sequences stay
+ * cached in the handle for ss_vocoder_generate_ragged.
+ * Generate: sequence s does what ss_vocoder_generate(total_frames_host[s], frame0_host[s], n_frames_host[s],
+ * left_context_host[s]) does, bit for bit, and its n_frames_s * hop samples are written packed in sequence order to wav_out_dev.
+ * n must equal the last durations call's n.  Sequences of up to 1024 frames (after the left context) run together in one
+ * cooperative launch of the fused generator kernel per group (up to 32 sequences and 3072 frames), after one frame-expansion
+ * launch; longer ones, and every sequence when the cooperative launch is refused or option vocoder_fused = 0, take the
+ * multi-launch path.  Errors: SS_ERR_INVALID for n <= 0, a U_s <= 0, a frame range that is not the tail or a null pointer;
+ * SS_ERR_STATE without vocoder weights, or for a generate call without a durations call of the same n.  enqueue only */
+int ss_vocoder_durations_ragged(ss_engine* h, void* stream, int n, const int64_t* codes_dev, const int32_t* U_host, int dur_prediction,
+                                int64_t* dur_out_dev, int32_t* cumsum_out_dev);
+int ss_vocoder_generate_ragged(ss_engine* h, void* stream, int n, const int32_t* total_frames_host, const int32_t* frame0_host,
+                               const int32_t* n_frames_host, const int32_t* left_context_host, float* wav_out_dev);
 int ss_vocoder_hop(const ss_engine* h);
 int ss_vocoder_receptive_field(const ss_engine* h);
 

@@ -19,7 +19,7 @@ import array
 import json
 import os
 import sys
-from typing import List, Optional
+from typing import List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -329,7 +329,7 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
     @torch.inference_mode()
     def _policy_impl(self):
         """The body of the reference policy(); returns (kind, wav on the device, SpeechSegment.finished, WriteAction.finished).
-        The host stages between the engine calls are methods of their own (_gate, _after_mt, _after_t2u), which the pooled agent
+        The host stages between the engine calls are methods of their own (_gate, _after_mt, _before_vocoder, _after_vocoder), which the pooled agent
         (scheduler.PooledS2STAgent) calls between its batched engine calls."""
         eng = self.engine
         tr = self.trace = {}
@@ -422,13 +422,21 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
         return None, (prev_output_tokens_mt, n_pad_tail)
 
     def _after_t2u(self, tmp: List[int], new_subword_tokens: int):
-        """From the collapsed unit indices of the T2U + unit-decoder call to the action (agent:690-770): unit dictionary mapping,
-        the new units (cur_unit), the vocoder on them (one engine call per stream), the wav tail and the reset quirk."""
-        eng = self.engine
+        """From the collapsed unit indices of the T2U + unit-decoder call to the action (agent:690-770), as a batch of one of the
+        three stages the pooled agent runs for all of its streams: _before_vocoder, _vocode, _after_vocoder."""
+        action, unit = self._before_vocoder(tmp)
+        if action is not None:
+            return action
+        new_wav = self._vocode(self.engine, [self], [unit])[0]
+        return self._after_vocoder(unit, new_wav, new_subword_tokens)
+
+    def _before_vocoder(self, tmp: List[int]):
+        """Unit dictionary mapping and the new units (cur_unit) (agent:690-742).  Returns (action, None) when the call ends here,
+        else (None, unit): the vocoder's input, the whole unit sequence so far."""
         if len(tmp) == 0:
             if not self.states.source_finished:
-                return READ
-            return self._finished_write_tuple()
+                return READ, None
+            return self._finished_write_tuple(), None
         if tmp[-1] == self.eos:
             tmp = tmp[:-1]
         unit = []
@@ -440,21 +448,43 @@ class StreamSpeechS2STAgent(_EngineAgentMixin, SpeechToSpeechAgent):
         cur_unit = unit if self.unit is None else unit[len(self.unit):]
         if len(unit) < 1 or len(cur_unit) < 1:
             if not self.states.source_finished:
-                return READ
-            return self._finished_write_tuple()
+                return READ, None
+            return self._finished_write_tuple(), None
+        return None, unit
 
-        # 4. vocoder (agent:743-753): wav tail of the new units
-        codes = torch.tensor(unit, dtype=torch.long, device=self.torch_device)
-        dur, cum = eng.vocoder_durations(codes, self.dur_prediction)
-        cum_h = cum.tolist()
-        total = cum_h[-1]
-        new_frames = total - cum_h[len(unit) - len(cur_unit)]
-        self.trace["dur"] = [cum_h[i + 1] - cum_h[i] for i in range(len(unit))]
-        if self.vocoder_context == "full":
-            wav_all = eng.vocoder_generate(total, 0, total, 0)
-            new_wav = wav_all[-new_frames * eng.hop:]
-        else:
-            new_wav = eng.vocoder_generate(total, total - new_frames, new_frames, -1)
+    @staticmethod
+    def _vocode(eng, agents: Sequence["StreamSpeechS2STAgent"], units: Sequence[List[int]]) -> List[torch.Tensor]:
+        """4. vocoder (agent:743-753): the wav of each agent's new units, for all agents in one durations call, one host read of the
+        cumsums and one generate call per dur_prediction setting.  Each agent's wav equals that of a call of its own, bit for bit."""
+        if len(agents) == 1:  # a batch of one: the single-sequence calls (the n = 1 case of the same entry points), one cumsum read
+            a, unit = agents[0], units[0]
+            _, cum = eng.vocoder_durations(torch.tensor(unit, dtype=torch.long, device=eng.device), a.dur_prediction)
+            cum_h = cum.tolist()
+            total = cum_h[-1]
+            new = total - cum_h[0 if a.unit is None else len(a.unit)]
+            a.trace["dur"] = [cum_h[j + 1] - cum_h[j] for j in range(len(unit))]
+            if a.vocoder_context == "full":
+                return [eng.vocoder_generate(total, 0, total, 0)[-new * eng.hop:]]
+            return [eng.vocoder_generate(total, total - new, new, -1)]
+        out: List[Optional[torch.Tensor]] = [None] * len(agents)
+        for dp in sorted({bool(a.dur_prediction) for a in agents}):
+            idx = [i for i, a in enumerate(agents) if bool(a.dur_prediction) == dp]
+            _, cums, _ = eng.vocoder_durations_ragged([units[i] for i in idx], dp)
+            args, new_frames = [], []  # (total_frames, frame0, n_frames, left_context) per stream; its new frames
+            for i, cum_h in zip(idx, cums):
+                a, unit = agents[i], units[i]
+                total = cum_h[-1]
+                a.trace["dur"] = [cum_h[j + 1] - cum_h[j] for j in range(len(unit))]
+                new = total - cum_h[0 if a.unit is None else len(a.unit)]
+                new_frames.append(new)
+                args.append((total, 0, total, 0) if a.vocoder_context == "full" else (total, total - new, new, -1))
+            wavs = eng.vocoder_generate_ragged(*zip(*args))
+            for i, w, new in zip(idx, wavs, new_frames):
+                out[i] = w[-new * eng.hop:]  # ("full": the tail of the whole-sequence pass)
+        return out
+
+    def _after_vocoder(self, unit: List[int], new_wav: torch.Tensor, new_subword_tokens: int):
+        """The wav tail, unfinished_wav and the reset quirk (agent:754-770)."""
         if self.unfinished_wav is not None and len(self.unfinished_wav) > 0:
             new_wav = torch.cat((self.unfinished_wav, new_wav), dim=0)
         self.unit = unit

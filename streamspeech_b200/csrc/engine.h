@@ -100,7 +100,10 @@ struct ss_engine {
   // whole generator as one persistent kernel (kernels_umma2.cu vocoder_fused): -1 = when the frame count is at most
   // voc_fused_max_frames, 0 = never (multi-launch path), 1 = whenever the shapes allow it
   int vocoder_fused = -1;
-  std::map<std::pair<int, uintptr_t>, ss::VocFusedParams> voc_fused;  // kernel parameters per (frames, arena)
+  // job / phase templates of the fused kernel per (frame capacity, arena): the packed-weight pointers of each tile width are filled
+  // in by the first call that uses them
+  std::map<std::pair<int, uintptr_t>, ss::VocFusedParams> voc_fused;
+  ss::VocFusedParams voc_call{};  // the templates with one call's sequences filled in
   float* persist_ffn_scratch = nullptr;  // [enc_ffn / 16][16][enc_dim] partial sums of the fused FFN phases
   float* cl_blobs = nullptr;             // [enc_layers][16][624][256] weight blobs of the cluster encoder kernel (allocated when the option is set)
   int cluster_cooperative = 1;           // cooperative launch attribute of the cluster kernel (0 only under a serialising profiler)
@@ -171,10 +174,12 @@ struct ss_engine {
   int64_t* mt_tok_dev = nullptr;  // [max_pos]
   int64_t* mt_next_dev = nullptr;
   int64_t* mt_next_pinned = nullptr;
-  // vocoder cached frame sequence
-  float* voc_unit_emb = nullptr;  // [Ucap][emb]
-  int* voc_cumsum = nullptr;      // [Ucap+1]
-  int voc_ucap = 0, voc_U = 0;
+  // vocoder: the unit sequences of the last ss_vocoder_durations_ragged call, cached for ss_vocoder_generate_ragged
+  float* voc_unit_emb = nullptr;  // [voc_ucap][emb]: sequence s at rows u0 .. u0 + U - 1
+  int* voc_cumsum = nullptr;      // [voc_ccap]: sequence s's U + 1 frame offsets at c0 (packed in sequence order)
+  int voc_ucap = 0, voc_ccap = 0;
+  struct VocSeq { int u0, U, c0; };
+  std::vector<VocSeq> voc_seqs;
   // streaming encoder state (one utterance per handle)
   int st_T_final = 0;
   float* st_k = nullptr;    // [enc_layers][Tpos][enc_dim]

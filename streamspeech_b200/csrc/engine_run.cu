@@ -155,85 +155,73 @@ bool ws_begin(ss_engine* h, size_t bytes) {
 // at 52 (the streaming agent's calls: new frames plus the receptive field), 180 and 750 frames (the offline leg); longer sequences,
 // which were not measured, keep the multi-launch path.
 constexpr int kVocFusedMaxFrames = 1024;
+// Frames of one ragged generate group: its sequences share the workspace buffers (~14 x 20 KB per frame at the default
+// generator), so a group of 3072 frames holds four 750-frame utterances in 0.9 GB (one 750-frame call alone: 0.2 GB).
+constexpr int kVocGroupFrames = 3072;
+// k-tiles (16 columns each) per split-K slice of the duration predictor's GEMMs: fixed, so that a row's sums do not depend on the
+// call's row count
+constexpr int kVocDurTilesPerSplit = 4;
 
-// Job / phase tables of the fused generator for N input frames with the arena's buffers (built once per (N, arena) and kept on
-// the device).  nullptr when a shape is outside what the kernel supports or memory runs out.
-VocFusedParams* vocoder_fused_table(ss_engine* h, int N, const float* frames, float* bufX, float* bufY, const std::vector<float*>& rbA,
-                                                    const std::vector<float*>& rbB, const std::vector<float*>& rbT, const std::vector<float*>& rbO,
-                                                    cudaStream_t st) {
-  const auto key = std::make_pair(N, (uintptr_t)h->ws.base);
+// Job / phase templates of the fused generator over `cap` frames of the arena's buffers (built once per (cap, arena) and kept on
+// the handle).  nullptr when a shape is outside what the kernel supports.
+VocFusedParams* vocoder_fused_table(ss_engine* h, int cap, const float* frames, float* bufX, float* bufY, const std::vector<float*>& rbA,
+                                    const std::vector<float*>& rbB, const std::vector<float*>& rbT, const std::vector<float*>& rbO) {
+  const auto key = std::make_pair(cap, (uintptr_t)h->ws.base);
   auto it = h->voc_fused.find(key);
   if (it != h->voc_fused.end()) return &it->second;
   const ss_config& c = h->cfg;
-  const int grid = vocoder_fused_grid();
-  if (grid <= 0) return nullptr;
   std::vector<VocJob> jobs;
   std::vector<VocPhase> phases;
-  int a_stride = 0, b_stride = 0;
+  int a_stride = 0;
   bool ok = true;
-  auto job = [&](const float* x0, const float* x1, const float* x2, int L_in, int M, int C_in, int k, int dil, int pad_left, float slope,
-                 const float* W, const float* bias, float* out, int Nout, int stride, int offset, const float* residual, float alpha, float res_scale) {
+  auto job = [&](const float* x0, const float* x1, const float* x2, int in_mult, int C_in, int k, int dil, int pad_left, float slope,
+                 const float* W, const float* bias, float* out, int Nout, int stride, int offset, int m_adj, const float* residual,
+                 float alpha, float res_scale) {
     VocJob j{};
-    j.x0 = x0; j.x1 = x1; j.x2 = x2; j.L_in = L_in; j.M = M; j.C_in = C_in; j.ksize = k; j.dil = dil; j.pad_left = pad_left; j.slope = slope;
-    j.wp = reinterpret_cast<const unsigned char*>(W);  // replaced by the packed copy once the phase's tile width is known
-    j.bias = bias; j.out = out; j.N = Nout; j.out_row_stride = stride; j.out_row_offset = offset; j.residual = residual; j.alpha = alpha;
-    j.res_scale = res_scale;
+    j.x0 = x0; j.x1 = x1; j.x2 = x2; j.in_mult = in_mult; j.C_in = C_in; j.ksize = k; j.dil = dil; j.pad_left = pad_left; j.slope = slope;
+    j.wp = reinterpret_cast<const unsigned char*>(W);  // the fp32 weights: packed per tile width by the calls (vocoder_fused_fill)
+    j.bias = bias; j.out = out; j.N = Nout; j.out_row_stride = stride; j.out_row_offset = offset; j.m_adj = m_adj;
+    j.residual = residual; j.alpha = alpha; j.res_scale = res_scale;
     j.CK = (C_in % 32 == 0) ? 32 : 16;
-    j.m_tiles = (M + VOC_FUSED_BM - 1) / VOC_FUSED_BM;
     if (C_in % 16 != 0 || Nout % 16 != 0 || k < 1 || (k - 1) * dil > 50 || bias == nullptr) ok = false;
+    const int rs_pad = ((VOC_FUSED_BM + (k - 1) * dil + 7) & ~7) + 4;
+    a_stride = std::max(a_stride, 2 * (j.CK / 8) * rs_pad * 16);
     jobs.push_back(j);
   };
-  // closes the phase of jobs [first, end): tile width, packed weights, longest jobs first
+  // closes the phase of jobs [first, end): longest jobs first
   auto phase = [&](int first) {
-    const int n_jobs = (int)jobs.size() - first;
-    int items32 = 0;
-    for (int i = first; i < (int)jobs.size(); ++i) items32 += jobs[i].N % 32 == 0 ? jobs[i].m_tiles * (jobs[i].N / 32) : 0;
-    const bool bn32 = items32 >= grid;  // 16-column tiles when 32-column ones would leave SMs idle
-    VocPhase p{first, n_jobs, 0};
-    for (int i = first; i < (int)jobs.size(); ++i) {
-      VocJob& j = jobs[i];
-      j.BN = (bn32 && j.N % 32 == 0) ? 32 : 16;
-      j.n_tiles = j.N / j.BN;
-      j.wp = umma2_packed_weights(h->umma2_cache, reinterpret_cast<const float*>(j.wp), j.N, j.C_in, j.ksize, j.BN, j.CK, 2, st);
-      if (j.wp == nullptr) ok = false;
-      const int rs_pad = ((VOC_FUSED_BM + (j.ksize - 1) * j.dil + 7) & ~7) + 4;
-      a_stride = std::max(a_stride, 2 * (j.CK / 8) * rs_pad * 16);
-      b_stride = std::max(b_stride, j.ksize * 2 * j.BN * j.CK * 2);
-      p.n_items += j.m_tiles * j.n_tiles;
-    }
     std::stable_sort(jobs.begin() + first, jobs.end(), [](const VocJob& a, const VocJob& b) { return a.ksize > b.ksize; });
-    phases.push_back(p);
+    phases.push_back(VocPhase{first, (int)jobs.size() - first, 0});
   };
   jobs.reserve(1 + c.voc_n_ups * (8 + 2 * c.voc_n_rb * c.voc_rb_ndil));
-  job(frames, nullptr, nullptr, N, N, c.voc_in_dim, 7, 1, 3, 1.0f, h->conv_pre.lin.w, h->conv_pre.lin.b, bufX, c.voc_init_channels, 1, 0, nullptr,
-      1.0f, 1.0f);
+  job(frames, nullptr, nullptr, 1, c.voc_in_dim, 7, 1, 3, 1.0f, h->conv_pre.lin.w, h->conv_pre.lin.b, bufX, c.voc_init_channels, 1, 0, 0,
+      nullptr, 1.0f, 1.0f);
   phase(0);
   const int nrb = c.voc_n_rb, nd = c.voc_rb_ndil;
-  int L = N;
+  int mult = 1;  // rows per frame of the stage input
   for (int i = 0; i < c.voc_n_ups; ++i) {
     const UpsampleW& U = h->ups[i];
-    const int Lout = L * U.u;
     // stage input: conv_pre's output, or the previous stage's three resblock outputs summed while loading
     const float* x0 = i == 0 ? bufX : rbO[0];
     const float* x1 = i == 0 ? nullptr : rbO[1];
     const float* x2 = i == 0 ? nullptr : rbO[2];
     int first = (int)jobs.size();
+    // output phase phi owns rows q0 .. (L * u - 1 - phi + pad) / u of its phase: M = L + floor((pad - 1 - phi) / u) - (q0 - 1)
     for (int phi = 0; phi < U.u; ++phi) {
-      const int J = U.phase_J[phi], q0 = U.phase_q0[phi];
-      const int nrows = (Lout - 1 - phi + U.pad) / U.u - q0 + 1;
-      if (nrows <= 0) continue;
-      job(x0, x1, x2, L, nrows, U.cin, J, 1, (J - 1) - q0, 0.1f, U.phase_w[phi].w, U.bias, bufY, U.cout, U.u, q0 * U.u + phi - U.pad, nullptr,
+      const int J = U.phase_J[phi], q0 = U.phase_q0[phi], a = U.pad - 1 - phi;
+      const int m_adj = (a >= 0 ? a / U.u : -((-a + U.u - 1) / U.u)) - (q0 - 1);
+      job(x0, x1, x2, mult, U.cin, J, 1, (J - 1) - q0, 0.1f, U.phase_w[phi].w, U.bias, bufY, U.cout, U.u, q0 * U.u + phi - U.pad, m_adj, nullptr,
           1.0f, 1.0f);
     }
     phase(first);
-    L = Lout;
+    mult *= U.u;
     const int ch = U.cout;
     for (int m = 0; m < nd; ++m) {
       first = (int)jobs.size();
       for (int j = 0; j < nrb; ++j) {
         const ConvW& w1 = h->rb1[i][j][m];
         const float* cur = m == 0 ? bufY : (m == 1 ? rbA[j] : rbB[j]);
-        job(cur, nullptr, nullptr, L, L, ch, w1.ksize, w1.dil, (w1.ksize * w1.dil - w1.dil) / 2, 0.1f, w1.lin.w, w1.lin.b, rbT[j], ch, 1, 0,
+        job(cur, nullptr, nullptr, mult, ch, w1.ksize, w1.dil, (w1.ksize * w1.dil - w1.dil) / 2, 0.1f, w1.lin.w, w1.lin.b, rbT[j], ch, 1, 0, 0,
             nullptr, 1.0f, 1.0f);
       }
       phase(first);
@@ -243,20 +231,94 @@ VocFusedParams* vocoder_fused_table(ss_engine* h, int N, const float* frames, fl
         const float* cur = m == 0 ? bufY : (m == 1 ? rbA[j] : rbB[j]);
         float* out = m + 1 < nd ? (m == 0 ? rbA[j] : rbB[j]) : rbO[j];
         const float s = m + 1 < nd ? 1.0f : 1.0f / nrb;  // last pair of the block: (xt + x) / num_kernels
-        job(rbT[j], nullptr, nullptr, L, L, ch, w2.ksize, 1, (w2.ksize - 1) / 2, 0.1f, w2.lin.w, w2.lin.b, out, ch, 1, 0, cur, s, s);
+        job(rbT[j], nullptr, nullptr, mult, ch, w2.ksize, 1, (w2.ksize - 1) / 2, 0.1f, w2.lin.w, w2.lin.b, out, ch, 1, 0, 0, cur, s, s);
       }
       phase(first);
     }
   }
-  if (!ok || jobs.size() > VOC_MAX_JOBS || phases.size() > VOC_MAX_PHASES || vocoder_fused_smem(a_stride, b_stride) > 200 * 1024) return nullptr;
+  if (!ok || jobs.size() > VOC_MAX_JOBS || phases.size() > VOC_MAX_PHASES) return nullptr;
   if (h->voc_fused.size() >= 64) h->voc_fused.clear();
   VocFusedParams& p = h->voc_fused[key];
   std::copy(jobs.begin(), jobs.end(), p.jobs);
   std::copy(phases.begin(), phases.end(), p.phases);
   p.n_phases = (int)phases.size();
   p.a_stride = a_stride;
-  p.b_stride = b_stride;
+  p.post.x0 = rbO[0]; p.post.x1 = rbO[1]; p.post.x2 = rbO[2];
+  p.post.w = h->conv_post_w; p.post.bias = h->conv_post_b; p.post.slope = 0.01f;  // leaky_relu(x) [slope 0.01, hifigan.py:166]
+  p.post.hop = h->hop; p.post.C = h->conv_post_c; p.post.k = h->conv_post_k;
   return &p;
+}
+
+// One fused-kernel sequence of a ragged generate call: N frames at row0 of the group's frame buffer, the new samples from frame
+// ctx on, written to wav_out + dst.
+struct VocFusedSeq {
+  int N, row0, ctx, dst;
+};
+
+// Fills h->voc_call from template T for the sequences `seqs`.  Each sequence gets the tile widths and tiles a call with that
+// sequence alone takes: the 32-column width in a phase when its own 32-column items would fill the grid.  False when the packed
+// weights cannot be made or shared memory would exceed what the kernel is set up for.
+bool vocoder_fused_fill(ss_engine* h, VocFusedParams& T, const std::vector<VocFusedSeq>& seqs, float* wav_out, cudaStream_t st) {
+  const int grid = vocoder_fused_grid();
+  if (grid <= 0 || seqs.empty() || (int)seqs.size() > VOC_MAX_STREAMS) return false;
+  VocFusedParams& p = h->voc_call;
+  std::copy(T.jobs, T.jobs + VOC_MAX_JOBS, p.jobs);
+  std::copy(T.phases, T.phases + VOC_MAX_PHASES, p.phases);
+  p.n_phases = T.n_phases;
+  p.a_stride = T.a_stride;
+  p.post = T.post;
+  p.post.out = wav_out;
+  p.n_streams = (int)seqs.size();
+  int out0 = 0;
+  for (size_t s = 0; s < seqs.size(); ++s) {
+    VocStreamGeo& G = p.streams[s];
+    G.bn32 = 0;
+    G.N = seqs[s].N; G.row0 = seqs[s].row0; G.t0 = seqs[s].ctx * h->hop; G.out0 = out0; G.dst = seqs[s].dst;
+    out0 += (G.N - seqs[s].ctx) * h->hop;
+  }
+  p.post.total = out0;
+  auto m_tiles = [](const VocJob& J, int N) {
+    const int M = N * J.in_mult + J.m_adj;
+    return M > 0 ? (M + VOC_FUSED_BM - 1) / VOC_FUSED_BM : 0;
+  };
+  int b_stride = 0;
+  for (int ph = 0; ph < p.n_phases; ++ph) {
+    const VocPhase& P = p.phases[ph];
+    int items = 0;
+    bool use16[VOC_MAX_JOBS] = {}, use32[VOC_MAX_JOBS] = {};
+    for (size_t s = 0; s < seqs.size(); ++s) {
+      VocStreamGeo& G = p.streams[s];
+      int items32 = 0;
+      for (int jb = P.first_job; jb < P.first_job + P.n_jobs; ++jb)
+        items32 += p.jobs[jb].N % 32 == 0 ? m_tiles(p.jobs[jb], G.N) * (p.jobs[jb].N / 32) : 0;
+      const bool bn32 = items32 >= grid;  // 16-column tiles when 32-column ones would leave SMs idle
+      if (bn32) G.bn32 |= 1ull << ph;
+      p.item0[ph][s] = items;
+      for (int jb = P.first_job; jb < P.first_job + P.n_jobs; ++jb) {
+        const VocJob& J = p.jobs[jb];
+        const int mt = m_tiles(J, G.N);
+        if (mt == 0) continue;
+        const int BN = (bn32 && J.N % 32 == 0) ? 32 : 16;
+        (BN == 32 ? use32 : use16)[jb] = true;
+        items += mt * (J.N / BN);
+      }
+    }
+    p.phases[ph].n_items = items;
+    for (int jb = P.first_job; jb < P.first_job + P.n_jobs; ++jb) {
+      VocJob& J = T.jobs[jb];
+      const float* W = reinterpret_cast<const float*>(J.wp);
+      for (int BN : {16, 32}) {
+        if (!(BN == 32 ? use32 : use16)[jb]) continue;
+        const unsigned char*& wp = BN == 32 ? J.wp32 : J.wp16;
+        if (!wp) wp = umma2_packed_weights(h->umma2_cache, W, J.N, J.C_in, J.ksize, BN, J.CK, 2, st);
+        if (!wp) return false;
+        (BN == 32 ? p.jobs[jb].wp32 : p.jobs[jb].wp16) = wp;
+        b_stride = std::max(b_stride, J.ksize * 2 * BN * J.CK * 2);
+      }
+    }
+  }
+  p.b_stride = b_stride;
+  return vocoder_fused_smem(p.a_stride, p.b_stride) <= 200 * 1024;
 }
 
 struct DecScratch {
@@ -1325,125 +1387,13 @@ int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_d
   return ss_t2u_unit_decode_ragged(h, stream, mt_feats_dev, B, Slen, nullptr, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev);
 }
 
-int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, int U, int dur_prediction, int64_t* dur_out_dev,
-                         int32_t* cumsum_out_dev) {
-  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
-  if (!h->has_vocoder) return h->fail(SS_ERR_STATE, "no vocoder weights were loaded");
-  if (U <= 0) return h->fail(SS_ERR_INVALID, "empty code sequence");
+// The generator of one sequence as one launch per convolution (the reference path for the fused kernel, and the path of
+// sequences it does not take): frames [N][in_dim] -> the n = N - ctx new frames' samples at out.
+static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* frames, int N, int ctx, float* bufX, float* bufY, const std::vector<float*>& rbA,
+                          const std::vector<float*>& rbB, const std::vector<float*>& rbT, const std::vector<float*>& rbO, float* wav, bool fan_out,
+                          float* out) {
   const ss_config& c = h->cfg;
-  cudaStream_t st = S(stream);
-  const int E = c.voc_embedding_dim, Hd = c.voc_dur_hidden;
-  if (U > h->voc_ucap) {
-    if (h->voc_unit_emb) cudaFree(h->voc_unit_emb);
-    if (h->voc_cumsum) cudaFree(h->voc_cumsum);
-    h->voc_unit_emb = nullptr;
-    h->voc_cumsum = nullptr;
-    h->voc_ucap = 0;
-    const int cap = std::max(2 * U, 1024);
-    if (cudaMalloc((void**)&h->voc_unit_emb, (size_t)cap * E * sizeof(float)) != cudaSuccess ||
-        cudaMalloc((void**)&h->voc_cumsum, (size_t)(cap + 1) * sizeof(int)) != cudaSuccess)
-      return h->fail(SS_ERR_CUDA, "cudaMalloc(vocoder unit cache) failed");
-    h->voc_ucap = cap;
-  }
-  h->voc_U = U;
-  if (!ws_begin(h, ((size_t)U * (2 * Hd + 2) + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
-  gather_rows(codes_dev, U, 0, h->voc_dict, E, h->voc_unit_emb, st);
-  float* a = h->ws.f32((size_t)U * Hd);
-  float* b = h->ws.f32((size_t)U * Hd);
-  float* ld = h->ws.f32(U);
-  if (dur_prediction) {
-    // VariancePredictor.forward (fairseq/models/text_to_speech/fastspeech2.py:144-151)
-    ConvA c1;
-    c1.x = h->voc_unit_emb; c1.B = 1; c1.L_in = U; c1.L_rows = U; c1.C_in = E; c1.ldx = E;
-    c1.ksize = h->dur_conv1.ksize; c1.pad_left = (h->dur_conv1.ksize - 1) / 2;
-    Epilogue e1 = ep_out(a, Hd, ACT_RELU);
-    e1.bias = h->dur_conv1.lin.b;
-    gemm_conv(c1, h->dur_conv1.lin.w, Hd, e1, st);
-    layer_norm(a, Hd, a, Hd, h->dur_ln1.g, h->dur_ln1.b, U, Hd, st);
-    ConvA c2;
-    c2.x = a; c2.B = 1; c2.L_in = U; c2.L_rows = U; c2.C_in = Hd; c2.ldx = Hd;
-    c2.ksize = h->dur_conv2.ksize; c2.pad_left = 1;  // padding=1 is hard-coded for conv2 (fastspeech2.py:137)
-    Epilogue e2 = ep_out(b, Hd, ACT_RELU);
-    e2.bias = h->dur_conv2.lin.b;
-    gemm_conv(c2, h->dur_conv2.lin.w, Hd, e2, st);
-    layer_norm(b, Hd, b, Hd, h->dur_ln2.g, h->dur_ln2.b, U, Hd, st);
-    linear(b, Hd, U, h->dur_proj, ep_out(ld, 1), st);
-  } else {
-    // no duration prediction: every code is one frame; log(2) rounds to dur 1
-    std::vector<float> v(U, 0.6931472f);
-    cudaMemcpyAsync(ld, v.data(), U * sizeof(float), cudaMemcpyHostToDevice, st);
-    cudaStreamSynchronize(st);
-  }
-  duration_from_log(ld, U, dur_out_dev, h->voc_cumsum, st);
-  if (cumsum_out_dev) cudaMemcpyAsync(cumsum_out_dev, h->voc_cumsum, (U + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st);
-  return check_launch(h, "ss_vocoder_durations");
-}
-
-int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0, int n_frames, int left_context, float* wav_out_dev) {
-  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
-  if (!h->has_vocoder || h->voc_U <= 0) return h->fail(SS_ERR_STATE, "ss_vocoder_durations must run first");
-  if (n_frames <= 0 || frame0 < 0 || frame0 + n_frames != total_frames) return h->fail(SS_ERR_INVALID, "vocoder frame range must be the tail of the sequence");
-  const ss_config& c = h->cfg;
-  cudaStream_t st = S(stream);
-  route_from(h);
-  g_umma_conv = h->umma_vocoder;
-  int ctx = left_context < 0 ? h->receptive_field : left_context;
-  ctx = std::min(ctx, frame0);
-  const int f_lo = frame0 - ctx;
-  const int N = n_frames + ctx;
-  // workspace: input frames + per-stage buffers
-  size_t maxbuf = 0;
-  {
-    int ch = c.voc_init_channels;
-    size_t L = N;
-    maxbuf = L * ch;
-    for (int i = 0; i < c.voc_n_ups; ++i) {
-      L *= c.voc_up_rates[i];
-      ch /= 2;
-      maxbuf = std::max(maxbuf, L * ch);
-    }
-  }
   const int nrb = c.voc_n_rb;
-  size_t total = ((size_t)N * c.voc_in_dim + (size_t)(2 + 4 * nrb) * maxbuf + (size_t)N * h->hop + 8192) * sizeof(float) + 64 * 256;
-  if (!ws_begin(h, total)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
-  float* frames = h->ws.f32((size_t)N * c.voc_in_dim);
-  float* bufX = h->ws.f32(maxbuf);   // stage input / output
-  float* bufY = h->ws.f32(maxbuf);   // upsampled stage activation
-  // per resblock (they run concurrently): ping-pong pair, conv1 output, block output
-  std::vector<float*> rbA(nrb), rbB(nrb), rbT(nrb), rbO(nrb);
-  bool ok = frames && bufX && bufY;
-  for (int j = 0; j < nrb; ++j) {
-    rbA[j] = h->ws.f32(maxbuf); rbB[j] = h->ws.f32(maxbuf); rbT[j] = h->ws.f32(maxbuf); rbO[j] = h->ws.f32(maxbuf);
-    ok = ok && rbA[j] && rbB[j] && rbT[j] && rbO[j];
-  }
-  float* wav = h->ws.f32((size_t)N * h->hop);
-  if (!ok || !wav) return h->fail(SS_ERR_CUDA, "workspace too small");
-  // The resblocks of a stage are independent until their outputs are averaged (hifigan.py:158-165).  Each one is a chain of
-  // small latency-bound convs, so they run on separate streams (block 0 on the caller's) and overlap on the GPU.
-  const bool fan_out = h->vocoder_streams && nrb == 3 && (g_umma_conv == 0 || g_umma_conv >= 12);
-  if (fan_out && !h->fork_event) {
-    bool made = cudaEventCreateWithFlags(&h->fork_event, cudaEventDisableTiming) == cudaSuccess;
-    for (int i = 0; i < 2 && made; ++i)
-      made = cudaStreamCreateWithFlags(&h->aux_stream[i], cudaStreamNonBlocking) == cudaSuccess &&
-             cudaEventCreateWithFlags(&h->join_event[i], cudaEventDisableTiming) == cudaSuccess;
-    if (!made) return h->fail(SS_ERR_CUDA, "cannot create the vocoder's auxiliary streams");
-  }
-  // V1 tail: repeat_interleave(x, dur) for the frame window (agent/tts/codehifigan.py:66)
-  expand_frames(h->voc_unit_emb, h->voc_cumsum, h->voc_U, f_lo, N, c.voc_embedding_dim, frames, st);
-  // Short sequences (the streaming calls): conv_pre .. conv_post as one persistent kernel whose phases are separated by grid
-  // barriers.  A shape it does not support or a refused cooperative launch falls through to the multi-launch path below.
-  const bool fused = h->vocoder_fused != 0 && (h->vocoder_fused == 1 || N <= kVocFusedMaxFrames) && g_umma_conv == 12 && nrb == 3;
-  if (fused) {
-    VocFusedParams* P = vocoder_fused_table(h, N, frames, bufX, bufY, rbA, rbB, rbT, rbO, st);
-    if (P) {
-      VocPost& post = P->post;
-      post.x0 = rbO[0]; post.x1 = rbO[1]; post.x2 = rbO[2];
-      post.w = h->conv_post_w; post.bias = h->conv_post_b; post.slope = 0.01f;  // leaky_relu(x) [slope 0.01, hifigan.py:166]
-      post.L = N * h->hop; post.C = h->conv_post_c; post.k = h->conv_post_k; post.t0 = ctx * h->hop;
-      post.out = wav_out_dev;
-      if (vocoder_fused(*P, h->persist_bar, &h->persist_bar_target, st) == 0) return check_launch(h, "ss_vocoder_generate");
-    }
-  }
   // conv_pre
   {
     ConvA a;
@@ -1537,8 +1487,232 @@ int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0
   }
   // x = leaky_relu(x) [slope 0.01, hifigan.py:166]; conv_post; tanh
   conv_post_tanh(bufX, L, ch, h->conv_post_w, h->conv_post_b, h->conv_post_k, 0.01f, wav, st);
-  copy_f32(wav + (size_t)ctx * h->hop, wav_out_dev, (int64_t)n_frames * h->hop, st);
-  return check_launch(h, "ss_vocoder_generate");
+  copy_f32(wav + (size_t)ctx * h->hop, out, (int64_t)(N - ctx) * h->hop, st);
+}
+
+int ss_vocoder_durations_ragged(ss_engine* h, void* stream, int n, const int64_t* codes_dev, const int32_t* U_host, int dur_prediction,
+                                int64_t* dur_out_dev, int32_t* cumsum_out_dev) {
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (!h->has_vocoder) return h->fail(SS_ERR_STATE, "no vocoder weights were loaded");
+  if (n <= 0 || !codes_dev || !U_host || !dur_out_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_vocoder_durations_ragged");
+  for (int s = 0; s < n; ++s)
+    if (U_host[s] <= 0) return h->fail(SS_ERR_INVALID, "empty code sequence");
+  const ss_config& c = h->cfg;
+  cudaStream_t st = S(stream);
+  const int E = c.voc_embedding_dim, Hd = c.voc_dur_hidden;
+  // Padded rows of one group: the split-K partial sums of its GEMMs (conv1, conv2: Hd columns; projection: 1) must fit the split-K
+  // scratch, or the GEMM would run unsplit and the group's rows would not equal those of a call of their own.  A sequence longer than
+  // this runs alone, as in a call of its own.
+  auto slices = [](int K) { return ((K + 15) / 16 + kVocDurTilesPerSplit - 1) / kVocDurTilesPerSplit; };
+  const size_t per_row = (size_t)std::max({slices(h->dur_conv1.ksize * E) * Hd, slices(h->dur_conv2.ksize * Hd) * Hd, slices(Hd)}) * sizeof(float);
+  const size_t dur_rows = splitk_workspace_bytes() / per_row;
+  // groups of consecutive sequences, each padded to its longest one: [count][Umax] rows
+  struct Group { int s0, count, Umax, row0; };
+  std::vector<Group> groups;
+  int rows = 0, max_rows = 0, n_cum = 0;
+  for (int s = 0; s < n; ++s) {
+    const int U = U_host[s];
+    n_cum += U + 1;
+    if (!groups.empty()) {
+      Group& g = groups.back();
+      const int um = std::max(g.Umax, U);
+      if (g.count < VOC_MAX_STREAMS && (size_t)(g.count + 1) * um <= dur_rows) {
+        ++g.count;
+        g.Umax = um;
+        continue;
+      }
+      rows += g.count * g.Umax;
+      max_rows = std::max(max_rows, g.count * g.Umax);
+    }
+    groups.push_back(Group{s, 1, U, rows});
+  }
+  rows += groups.back().count * groups.back().Umax;
+  max_rows = std::max(max_rows, groups.back().count * groups.back().Umax);
+  if (rows > h->voc_ucap || n_cum > h->voc_ccap) {
+    if (h->voc_unit_emb) cudaFree(h->voc_unit_emb);
+    if (h->voc_cumsum) cudaFree(h->voc_cumsum);
+    h->voc_unit_emb = nullptr;
+    h->voc_cumsum = nullptr;
+    h->voc_ucap = h->voc_ccap = 0;
+    h->voc_seqs.clear();
+    const int ucap = std::max(2 * rows, 1024), ccap = std::max(2 * n_cum, 1024);
+    if (cudaMalloc((void**)&h->voc_unit_emb, (size_t)ucap * E * sizeof(float)) != cudaSuccess ||
+        cudaMalloc((void**)&h->voc_cumsum, (size_t)ccap * sizeof(int)) != cudaSuccess)
+      return h->fail(SS_ERR_CUDA, "cudaMalloc(vocoder unit cache) failed");
+    h->voc_ucap = ucap;
+    h->voc_ccap = ccap;
+  }
+  if (!ws_begin(h, ((size_t)max_rows * (2 * Hd + 1) + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  float* a = h->ws.f32((size_t)max_rows * Hd);
+  float* b = h->ws.f32((size_t)max_rows * Hd);
+  float* ld = h->ws.f32(max_rows);
+  if (!a || !b || !ld) return h->fail(SS_ERR_CUDA, "workspace too small");
+  h->voc_seqs.assign(n, ss_engine::VocSeq{});
+  int packed = 0;  // units of the sequences before the group
+  for (const Group& g : groups) {
+    // group-local geometry: unit rows of the padded [count][Umax] block, packed codes / durations / cumsums from the group's first
+    VocSeqs q{};
+    q.n = g.count;
+    int pu = 0;
+    for (int i = 0; i < g.count; ++i) {
+      const int s = g.s0 + i;
+      q.s[i].u0 = i * g.Umax;
+      q.s[i].U = U_host[s];
+      q.s[i].c0 = pu + i;
+      h->voc_seqs[s] = ss_engine::VocSeq{g.row0 + i * g.Umax, U_host[s], packed + pu + g.s0 + i};
+      pu += U_host[s];
+    }
+    const int M = g.count * g.Umax;
+    float* emb = h->voc_unit_emb + (size_t)g.row0 * E;
+    gather_codes_ragged(codes_dev + packed, q, g.Umax, h->voc_dict, E, emb, st);
+    if (dur_prediction) {
+      // VariancePredictor.forward (fairseq/models/text_to_speech/fastspeech2.py:144-151) on every sequence of the group.  Each
+      // sequence sees zeros past its end, as alone: its pad rows are zero in the embeddings and re-zeroed after LayerNorm 1.
+      // The split-K slices are fixed, so that a row's sums do not depend on the group's row count.
+      ConvA c1;
+      c1.x = emb; c1.B = g.count; c1.L_in = g.Umax; c1.L_rows = g.Umax; c1.C_in = E; c1.ldx = E;
+      c1.ksize = h->dur_conv1.ksize; c1.pad_left = (h->dur_conv1.ksize - 1) / 2; c1.k_tiles_per_split = kVocDurTilesPerSplit;
+      Epilogue e1 = ep_out(a, Hd, ACT_RELU);
+      e1.bias = h->dur_conv1.lin.b;
+      gemm_conv(c1, h->dur_conv1.lin.w, Hd, e1, st);
+      layer_norm(a, Hd, a, Hd, h->dur_ln1.g, h->dur_ln1.b, M, Hd, st);
+      if (g.count > 1) zero_pad_rows(a, q, g.Umax, Hd, st);
+      ConvA c2;
+      c2.x = a; c2.B = g.count; c2.L_in = g.Umax; c2.L_rows = g.Umax; c2.C_in = Hd; c2.ldx = Hd;
+      c2.ksize = h->dur_conv2.ksize; c2.pad_left = 1;  // padding=1 is hard-coded for conv2 (fastspeech2.py:137)
+      c2.k_tiles_per_split = kVocDurTilesPerSplit;
+      Epilogue e2 = ep_out(b, Hd, ACT_RELU);
+      e2.bias = h->dur_conv2.lin.b;
+      gemm_conv(c2, h->dur_conv2.lin.w, Hd, e2, st);
+      layer_norm(b, Hd, b, Hd, h->dur_ln2.g, h->dur_ln2.b, M, Hd, st);
+      ConvA pr;
+      pr.x = b; pr.L_in = M; pr.L_rows = M; pr.C_in = Hd; pr.ldx = Hd; pr.k_tiles_per_split = kVocDurTilesPerSplit;
+      Epilogue e3 = ep_out(ld, 1);
+      e3.bias = h->dur_proj.b;
+      gemm_conv(pr, h->dur_proj.w, 1, e3, st);
+    }
+    // no duration prediction: every code is one frame
+    duration_from_log_ragged(dur_prediction ? ld : nullptr, q, dur_out_dev + packed, h->voc_cumsum + packed + g.s0, st);
+    packed += pu;
+  }
+  if (cumsum_out_dev) cudaMemcpyAsync(cumsum_out_dev, h->voc_cumsum, (size_t)n_cum * sizeof(int), cudaMemcpyDeviceToDevice, st);
+  return check_launch(h, "ss_vocoder_durations_ragged");
+}
+
+int ss_vocoder_durations(ss_engine* h, void* stream, const int64_t* codes_dev, int U, int dur_prediction, int64_t* dur_out_dev,
+                         int32_t* cumsum_out_dev) {
+  const int32_t U_host = U;
+  return ss_vocoder_durations_ragged(h, stream, 1, codes_dev, &U_host, dur_prediction, dur_out_dev, cumsum_out_dev);
+}
+
+int ss_vocoder_generate_ragged(ss_engine* h, void* stream, int n, const int32_t* total_frames_host, const int32_t* frame0_host,
+                               const int32_t* n_frames_host, const int32_t* left_context_host, float* wav_out_dev) {
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (!h->has_vocoder) return h->fail(SS_ERR_STATE, "no vocoder weights were loaded");
+  if (n <= 0 || !total_frames_host || !frame0_host || !n_frames_host || !left_context_host || !wav_out_dev)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_vocoder_generate_ragged");
+  if ((size_t)n != h->voc_seqs.size())
+    return h->fail(SS_ERR_STATE, "ss_vocoder_generate_ragged needs an ss_vocoder_durations_ragged call with the same n first");
+  for (int s = 0; s < n; ++s)
+    if (n_frames_host[s] <= 0 || frame0_host[s] < 0 || frame0_host[s] + n_frames_host[s] != total_frames_host[s])
+      return h->fail(SS_ERR_INVALID, "vocoder frame range must be the tail of the sequence");
+  const ss_config& c = h->cfg;
+  cudaStream_t st = S(stream);
+  route_from(h);
+  g_umma_conv = h->umma_vocoder;
+  const int nrb = c.voc_n_rb;
+  std::vector<int> ctx(n), N(n), dst(n);
+  int n_out = 0;
+  for (int s = 0; s < n; ++s) {
+    ctx[s] = std::min(left_context_host[s] < 0 ? h->receptive_field : (int)left_context_host[s], (int)frame0_host[s]);
+    N[s] = n_frames_host[s] + ctx[s];
+    dst[s] = n_out;
+    n_out += n_frames_host[s] * h->hop;
+  }
+  // groups of consecutive sequences that share the workspace buffers, sequence s at frame row row0[s] of its group
+  std::vector<int> g_first, row0(n);
+  int cap = 0, rows = 0;
+  for (int s = 0; s < n; ++s) {
+    if (s == 0 || s - g_first.back() >= VOC_MAX_STREAMS || rows + N[s] > kVocGroupFrames) {
+      g_first.push_back(s);
+      rows = 0;
+    }
+    row0[s] = rows;
+    rows += N[s];
+    cap = std::max(cap, rows);
+  }
+  g_first.push_back(n);
+  cap = (cap + 63) & ~63;  // (a stable capacity keeps the fused kernel's templates cached across calls)
+  // workspace: the group's frames + per-stage buffers; per frame each buffer holds max over stages of rows x channels
+  size_t per_frame = c.voc_init_channels;
+  {
+    size_t L = 1, ch = c.voc_init_channels;
+    for (int i = 0; i < c.voc_n_ups; ++i) {
+      L *= c.voc_up_rates[i];
+      ch /= 2;
+      per_frame = std::max(per_frame, L * ch);
+    }
+  }
+  const size_t maxbuf = (size_t)cap * per_frame;
+  size_t total = ((size_t)cap * c.voc_in_dim + (size_t)(2 + 4 * nrb) * maxbuf + (size_t)cap * h->hop + 8192) * sizeof(float) + 64 * 256;
+  if (!ws_begin(h, total)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  float* frames = h->ws.f32((size_t)cap * c.voc_in_dim);
+  float* bufX = h->ws.f32(maxbuf);   // stage input / output
+  float* bufY = h->ws.f32(maxbuf);   // upsampled stage activation
+  // per resblock (they run concurrently): ping-pong pair, conv1 output, block output
+  std::vector<float*> rbA(nrb), rbB(nrb), rbT(nrb), rbO(nrb);
+  bool ok = frames && bufX && bufY;
+  for (int j = 0; j < nrb; ++j) {
+    rbA[j] = h->ws.f32(maxbuf); rbB[j] = h->ws.f32(maxbuf); rbT[j] = h->ws.f32(maxbuf); rbO[j] = h->ws.f32(maxbuf);
+    ok = ok && rbA[j] && rbB[j] && rbT[j] && rbO[j];
+  }
+  float* wav = h->ws.f32((size_t)cap * h->hop);
+  if (!ok || !wav) return h->fail(SS_ERR_CUDA, "workspace too small");
+  // The resblocks of a stage are independent until their outputs are averaged (hifigan.py:158-165).  Each one is a chain of
+  // small latency-bound convs, so the multi-launch path runs them on separate streams (block 0 on the caller's) and they overlap.
+  const bool fan_out = h->vocoder_streams && nrb == 3 && (g_umma_conv == 0 || g_umma_conv >= 12);
+  if (fan_out && !h->fork_event) {
+    bool made = cudaEventCreateWithFlags(&h->fork_event, cudaEventDisableTiming) == cudaSuccess;
+    for (int i = 0; i < 2 && made; ++i)
+      made = cudaStreamCreateWithFlags(&h->aux_stream[i], cudaStreamNonBlocking) == cudaSuccess &&
+             cudaEventCreateWithFlags(&h->join_event[i], cudaEventDisableTiming) == cudaSuccess;
+    if (!made) return h->fail(SS_ERR_CUDA, "cannot create the vocoder's auxiliary streams");
+  }
+  const bool fused_on = h->vocoder_fused != 0 && g_umma_conv == 12 && nrb == 3;
+  for (size_t g = 0; g + 1 < g_first.size(); ++g) {
+    const int s0 = g_first[g], s1 = g_first[g + 1];
+    // V1 tail: repeat_interleave(x, dur) for each sequence's frame window (agent/tts/codehifigan.py:66), one launch
+    VocSeqs q{};
+    q.n = s1 - s0;
+    for (int s = s0; s < s1; ++s) {
+      const ss_engine::VocSeq& v = h->voc_seqs[s];
+      q.s[s - s0] = {v.u0, v.U, v.c0, frame0_host[s] - ctx[s], N[s], row0[s]};
+    }
+    expand_frames_ragged(h->voc_unit_emb, h->voc_cumsum, q, row0[s1 - 1] + N[s1 - 1], c.voc_in_dim, frames, st);
+    // Sequences of up to kVocFusedMaxFrames frames: conv_pre .. conv_post as one persistent kernel whose phases are separated by
+    // grid barriers.  Longer ones, a shape the kernel does not support or a refused cooperative launch take the multi-launch path.
+    std::vector<VocFusedSeq> fs;
+    std::vector<char> in_fused(s1 - s0, 0);
+    for (int s = s0; s < s1; ++s) {
+      in_fused[s - s0] = fused_on && (h->vocoder_fused == 1 || N[s] <= kVocFusedMaxFrames);
+      if (in_fused[s - s0]) fs.push_back(VocFusedSeq{N[s], row0[s], ctx[s], dst[s]});
+    }
+    bool launched = false;
+    if (!fs.empty()) {
+      VocFusedParams* T = vocoder_fused_table(h, cap, frames, bufX, bufY, rbA, rbB, rbT, rbO);
+      launched = T && vocoder_fused_fill(h, *T, fs, wav_out_dev, st) && vocoder_fused(h->voc_call, h->persist_bar, &h->persist_bar_target, st) == 0;
+    }
+    for (int s = s0; s < s1; ++s)
+      if (!(launched && in_fused[s - s0]))
+        vocoder_multi_launch(h, st, frames + (size_t)row0[s] * c.voc_in_dim, N[s], ctx[s], bufX, bufY, rbA, rbB, rbT, rbO, wav, fan_out,
+                             wav_out_dev + dst[s]);
+  }
+  return check_launch(h, "ss_vocoder_generate_ragged");
+}
+
+int ss_vocoder_generate(ss_engine* h, void* stream, int total_frames, int frame0, int n_frames, int left_context, float* wav_out_dev) {
+  const int32_t t = total_frames, f0 = frame0, nf = n_frames, lc = left_context;
+  return ss_vocoder_generate_ragged(h, stream, 1, &t, &f0, &nf, &lc, wav_out_dev);
 }
 
 int ss_set_option(ss_engine* h, const char* name, int value) {

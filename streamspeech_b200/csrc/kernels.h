@@ -34,6 +34,9 @@ struct ConvA {
   int t_offset = 0;
   int x_row0 = 0;
   int x_rows = 0;
+  // > 0 (gemm_conv): split-K slices of this many k-tiles whatever M is, so that a row's sum does not depend on how many rows the
+  // call has (0: the slice count is chosen to fill the GPU)
+  int k_tiles_per_split = 0;
 };
 
 struct Epilogue {
@@ -67,6 +70,7 @@ void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaSt
 
 // split-K scratch (one per process; launches of a handle are stream-ordered) and its fixed-order reduce + epilogue
 float* splitk_workspace(size_t bytes);
+size_t splitk_workspace_bytes();  // capacity of one split-K scratch region
 // split-K scratch region (0..2) used by the GEMM launches of the calling thread from now on; 0 is the default
 void set_splitk_slot(int slot);
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st);
@@ -85,48 +89,89 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
 // packed copy of W[N][ksize*C_in] in the kernels' tiling (made once per weight matrix and tiling; nullptr when out of memory)
 const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int N, int C_in, int ksize, int BN, int CK, int NP, cudaStream_t st);
 
-// ---- the whole vocoder generator of one call as one persistent cooperative wgmma kernel (kernels_umma2.cu, bf16x3)
-// One job = one stride-1 convolution of the generator, tiled into 128-row x BN-column work items:
+// ---- the vocoder generator of up to VOC_MAX_STREAMS sequences as one persistent cooperative wgmma kernel (kernels_umma2.cu, bf16x3)
+// One job = one stride-1 convolution of the generator, tiled per sequence into 128-row x BN-column work items:
 //   out[m * out_row_stride + out_row_offset][n] = alpha * (sum_{j, ci} pre(x[m + j*dil - pad_left][ci]) * W[n][j][ci] + bias[n])
 //                                                + res_scale * residual[same index]
 // with x = x0, or x2 + (x1 + x0) when x1 != nullptr (the sum of a stage's three resblock outputs), pre = leaky_relu(slope).
+// The job table holds each convolution once.  Sequence s of N_s frames owns rows [row0_s * in_mult, (row0_s + N_s) * in_mult) of
+// the job's input buffer and the matching rows (x out_row_stride) of its output: the kernel resolves L_in, M, the row bases and the
+// tile width of (job, sequence) from the sequence's VocStreamGeo, so every sequence gets the tiles a call of its own would run.
 struct VocJob {
   const float *x0, *x1, *x2;
-  int L_in, M, C_in, ksize, dil, pad_left;
+  int C_in, ksize, dil, pad_left;
   float slope;
-  const unsigned char* wp;  // umma2_packed_weights(W, N, C_in, ksize, BN, CK, 2)
+  const unsigned char* wp;              // the fp32 weights W (the host packs them per tile width into wp16 / wp32 when first used)
+  const unsigned char *wp16, *wp32;     // umma2_packed_weights(W, N, C_in, ksize, BN = 16 / 32, CK, 2) (nullptr when unused)
   const float* bias;
   float* out;
   int N, out_row_stride, out_row_offset;
   const float* residual;
   float alpha, res_scale;
-  int BN, CK, m_tiles, n_tiles;
+  int CK;
+  // per sequence: L_in = N_s * in_mult, M = L_in + m_adj (upsample phases skip the rows their output phase does not own); output
+  // rows start at row0_s * in_mult * out_row_stride
+  int in_mult, m_adj;
 };
-struct VocPhase {  // jobs [first_job, first_job + n_jobs) are independent; items of the phase = sum of m_tiles * n_tiles
+struct VocPhase {  // jobs [first_job, first_job + n_jobs) are independent; items of the phase = sum over sequences of m_tiles * n_tiles
   int first_job, n_jobs, n_items;
 };
-// last phase: out[t - t0] = tanh(bias + sum_{j, c} w[j][c] * leaky_relu(x2 + (x1 + x0))[t + j - (k-1)/2][c]) for t in [t0, L)
+// per sequence: N frames at row0 of the packed frame buffer; conv_post computes samples [t0, N * hop), numbered from out0 among
+// all sequences' samples, into out[dst ..); bit ph of bn32 = the 32-column tile width in phase ph (the choice a call with this
+// sequence alone makes)
+struct VocStreamGeo {
+  unsigned long long bn32;
+  int N, row0, t0, out0, dst;
+};
+// last phase, per sequence: out[t - t0] = tanh(bias + sum_{j, c} w[j][c] * leaky_relu(x2 + (x1 + x0))[t + j - (k-1)/2][c])
+// for t in [t0, L = N * hop), with x rows counted from row0 * hop
 struct VocPost {
   const float *x0, *x1, *x2;
   const float* w;  // [k][C]
   float bias, slope;
-  int L, C, k, t0;
+  int hop, C, k, total;  // total = samples written by all sequences
   float* out;
 };
 constexpr int VOC_FUSED_BM = 128;
-constexpr int VOC_MAX_JOBS = 128, VOC_MAX_PHASES = 48;
-struct VocFusedParams {  // passed by value in the kernel's parameter space (~17 KB): no per-call upload
+constexpr int VOC_MAX_JOBS = 128, VOC_MAX_PHASES = 40, VOC_MAX_STREAMS = 32;
+struct VocFusedParams {  // passed by value in the kernel's parameter space (< 32 KB): no per-call upload
   VocJob jobs[VOC_MAX_JOBS];
   VocPhase phases[VOC_MAX_PHASES];
-  int n_phases;
+  int n_phases, n_streams;
   int a_stride, b_stride;  // shared-memory bytes of one A stage (rows x channels x pieces) / one B stage (all taps of a chunk)
   VocPost post;
+  VocStreamGeo streams[VOC_MAX_STREAMS];
+  int item0[VOC_MAX_PHASES][VOC_MAX_STREAMS];  // first work item of sequence s in phase ph
 };
+static_assert(VOC_MAX_PHASES <= 64, "VocStreamGeo::bn32 has one bit per phase");
+static_assert(sizeof(VocFusedParams) <= 32000, "the fused vocoder parameters must fit the 32 KB kernel parameter space");
 // CTAs of the cooperative launch on the current device (0: the kernel cannot be made resident)
 int vocoder_fused_grid();
 size_t vocoder_fused_smem(int a_stride, int b_stride);
 // returns 0 (enqueued; the barrier target advanced by grid x n_phases) or < 0 (launch refused)
 int vocoder_fused(const VocFusedParams& p, unsigned* bar_ctr, unsigned* bar_target_host, cudaStream_t st);
+
+// Per-sequence geometry of the vocoder's ragged front end (kernels_misc.cu), passed by value.
+struct VocSeqs {
+  int n;
+  struct {
+    int u0;     // first unit row of the sequence in the unit-embedding / log-duration buffers
+    int U;      // units
+    int c0;     // first entry of its cumsum [U + 1] in the packed cumsum buffer (durations: also dur_out[c0 - s ..])
+    int f_lo;   // expand: first frame
+    int N;      // expand: frames
+    int row0;   // expand: first output row
+  } s[VOC_MAX_STREAMS];
+};
+// emb rows u0_s + [0, U_max) = table[codes[packed offset of s + i]] for i < U_s, zero rows for i in [U_s, rows_per_seq)
+void gather_codes_ragged(const int64_t* codes, const VocSeqs& q, int rows_per_seq, const float* table, int C, float* emb, cudaStream_t st);
+// zero rows [U_s, rows_per_seq) of sequence s (rows u0_s ..) of x [.][C]
+void zero_pad_rows(float* x, const VocSeqs& q, int rows_per_seq, int C, cudaStream_t st);
+// per sequence: dur = clamp(round(exp(logdur) - 1), min 1) (round half to even like torch.round; logdur == nullptr: every
+// duration is 1) into dur[c0_s - s ..], and its inclusive prefix sum into cumsum[c0_s .. c0_s + U_s] (one CTA per sequence)
+void duration_from_log_ragged(const float* logdur, const VocSeqs& q, int64_t* dur, int* cumsum, cudaStream_t st);
+// out rows row0_s + i = emb[u0_s + unit of frame f_lo_s + i] for i < N_s (repeat_interleave via the cumsum at c0_s)
+void expand_frames_ragged(const float* emb, const int* cumsum, const VocSeqs& q, int total_rows, int C, float* out, cudaStream_t st);
 
 // Weight-streaming GEMM for M <= 64 rows (plain row-major A): one warp per output column, see kernels_skinny.cu.
 bool skinny_gemm_supported(int M, int N, int K, const Epilogue& ep);
@@ -194,11 +239,6 @@ void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, i
 void ctc_argmax_collapse_pair(const float* logits, int ld, int V, int n_new, int row0, int n_rows, const int* masked, int n_masked, int blank,
                               int pad, int64_t* am0, int64_t* am1, int64_t* out, int out_stride, unsigned* ticket, cudaStream_t st);
 void gather_rows(const int64_t* idx, int n, int idx_offset, const float* table, int C, float* out, cudaStream_t st);
-// dur = clamp(round(exp(x) - 1), min 1) (round half to even like torch.round); also inclusive prefix sum (single CTA)
-void duration_from_log(const float* logdur, int n, int64_t* dur, int* cumsum /*[n+1]*/, cudaStream_t st);
-// out[f] = emb[unit of frame f] for f in [f0, f0+nf): expands repeat_interleave via the cumsum
-void expand_frames(const float* emb /*[U][C]*/, const int* cumsum /*[U+1]*/, int U, int f0, int nf, int C, float* out,
-                   cudaStream_t st);
 // conv_post (C_in -> 1, k taps, "same" padding) + leaky_relu(slope) on the input + tanh
 void conv_post_tanh(const float* x, int L, int C, const float* w /*[k][C]*/, float bias, int k, float pre_slope, float* out,
                     cudaStream_t st);

@@ -287,6 +287,8 @@ float* splitk_workspace(size_t bytes) {
   return splitk_region();
 }
 
+size_t splitk_workspace_bytes() { return SPLITK_WS_BYTES; }
+
 void set_splitk_slot(int slot) { g_splitk_slot = (slot >= 0 && slot < SPLITK_SLOTS) ? slot : 0; }
 
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st) {
@@ -304,7 +306,10 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
   const int nk = (K + BK - 1) / BK;
   int splits = 1;
   const long sms = std::max(1, current_device_sms());
-  if (ctas < sms && nk >= 8) {
+  if (a.k_tiles_per_split > 0) {
+    splits = (nk + a.k_tiles_per_split - 1) / a.k_tiles_per_split;
+    if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
+  } else if (ctas < sms && nk >= 8) {
     splits = (int)std::min<long>((sms + ctas - 1) / ctas, nk / 4);  // >= 4 k-tiles (64 columns) per slice
     if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
   }

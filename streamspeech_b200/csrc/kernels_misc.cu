@@ -196,35 +196,68 @@ __global__ void gather_rows_kernel(const int64_t* __restrict__ idx, int idx_offs
   for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = table[t * C + c];
 }
 
-__global__ void duration_kernel(const float* __restrict__ logdur, int n, int64_t* __restrict__ dur, int* __restrict__ cumsum) {
+__global__ void gather_codes_ragged_kernel(const int64_t* __restrict__ codes, VocSeqs q, int rows_per_seq, const float* __restrict__ table,
+                                           int C, float* __restrict__ emb) {
   pdl_trigger();
   pdl_wait();
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const int s = blockIdx.y, i = blockIdx.x;
+  const bool valid = i < q.s[s].U;
+  const int64_t t = valid ? codes[q.s[s].c0 - s + i] : 0;
+  float* o = emb + (int64_t)(q.s[s].u0 + i) * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) o[c] = valid ? table[t * C + c] : 0.f;
+}
+
+__global__ void zero_pad_rows_kernel(float* __restrict__ x, VocSeqs q, int rows_per_seq, int C) {
+  pdl_trigger();
+  pdl_wait();
+  const int s = blockIdx.y, i = blockIdx.x;
+  if (i < q.s[s].U) return;
+  float* o = x + (int64_t)(q.s[s].u0 + i) * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) o[c] = 0.f;
+}
+
+__global__ void duration_ragged_kernel(const float* __restrict__ logdur, VocSeqs q, int64_t* __restrict__ dur, int* __restrict__ cumsum) {
+  pdl_trigger();
+  pdl_wait();
+  if (threadIdx.x != 0) return;
+  const int s = blockIdx.x;
+  const int n = q.s[s].U;
+  const float* ld = logdur ? logdur + q.s[s].u0 : nullptr;
+  int64_t* d = dur + (q.s[s].c0 - s);
+  int* cs = cumsum + q.s[s].c0;
   int acc = 0;
-  cumsum[0] = 0;
+  cs[0] = 0;
   for (int i = 0; i < n; ++i) {
     // torch.clamp(torch.round(torch.exp(x) - 1).long(), min=1)  (agent/tts/codehifigan.py:63-65); round = half-to-even
-    float d = rintf(expf(logdur[i]) - 1.0f);
-    long long di = (long long)d;
-    if (di < 1) di = 1;
-    if (di > 100000) di = 100000;
-    dur[i] = di;
+    long long di = 1;
+    if (ld) {
+      float f = rintf(expf(ld[i]) - 1.0f);
+      di = (long long)f;
+      if (di < 1) di = 1;
+      if (di > 100000) di = 100000;
+    }
+    d[i] = di;
     acc += (int)di;
-    cumsum[i + 1] = acc;
+    cs[i + 1] = acc;
   }
 }
 
-__global__ void expand_frames_kernel(const float* __restrict__ emb, const int* __restrict__ cumsum, int U, int f0, int C,
-                                     float* __restrict__ out) {
+__global__ void expand_frames_ragged_kernel(const float* __restrict__ emb, const int* __restrict__ cumsum, VocSeqs q, int C,
+                                            float* __restrict__ out) {
   pdl_trigger();
   pdl_wait();
-  int f = f0 + blockIdx.x;
-  int lo = 0, hi = U;  // find u with cumsum[u] <= f < cumsum[u+1]
+  const int r = blockIdx.x;  // output row
+  int s = 0;
+  while (s + 1 < q.n && r >= q.s[s + 1].row0) ++s;
+  const int* cs = cumsum + q.s[s].c0;
+  const int f = q.s[s].f_lo + (r - q.s[s].row0);
+  int lo = 0, hi = q.s[s].U;  // find u with cumsum[u] <= f < cumsum[u+1]
   while (hi - lo > 1) {
     int mid = (lo + hi) >> 1;
-    if (cumsum[mid] <= f) lo = mid; else hi = mid;
+    if (cs[mid] <= f) lo = mid; else hi = mid;
   }
-  for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)blockIdx.x * C + c] = emb[(int64_t)lo * C + c];
+  const float* e = emb + (int64_t)(q.s[s].u0 + lo) * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) out[(int64_t)r * C + c] = e[c];
 }
 
 __global__ void conv_post_tanh_kernel(const float* __restrict__ x, int L, int C, const float* __restrict__ w, float bias, int k,
@@ -361,15 +394,28 @@ void gather_rows(const int64_t* idx, int n, int idx_offset, const float* table, 
   launch_pdl(gather_rows_kernel, dim3(n), dim3(128), 0, st, idx, idx_offset, table, C, out);
 }
 
-void duration_from_log(const float* logdur, int n, int64_t* dur, int* cumsum, cudaStream_t st) {
+void gather_codes_ragged(const int64_t* codes, const VocSeqs& q, int rows_per_seq, const float* table, int C, float* emb, cudaStream_t st) {
   ++g_launches;
-  launch_pdl(duration_kernel, dim3(1), dim3(32), 0, st, logdur, n, dur, cumsum);
+  if (q.n <= 0 || rows_per_seq <= 0) return;
+  launch_pdl(gather_codes_ragged_kernel, dim3(rows_per_seq, q.n), dim3(128), 0, st, codes, q, rows_per_seq, table, C, emb);
 }
 
-void expand_frames(const float* emb, const int* cumsum, int U, int f0, int nf, int C, float* out, cudaStream_t st) {
+void zero_pad_rows(float* x, const VocSeqs& q, int rows_per_seq, int C, cudaStream_t st) {
   ++g_launches;
-  if (nf <= 0) return;
-  launch_pdl(expand_frames_kernel, dim3(nf), dim3(128), 0, st, emb, cumsum, U, f0, C, out);
+  if (q.n <= 0 || rows_per_seq <= 0) return;
+  launch_pdl(zero_pad_rows_kernel, dim3(rows_per_seq, q.n), dim3(128), 0, st, x, q, rows_per_seq, C);
+}
+
+void duration_from_log_ragged(const float* logdur, const VocSeqs& q, int64_t* dur, int* cumsum, cudaStream_t st) {
+  ++g_launches;
+  if (q.n <= 0) return;
+  launch_pdl(duration_ragged_kernel, dim3(q.n), dim3(32), 0, st, logdur, q, dur, cumsum);
+}
+
+void expand_frames_ragged(const float* emb, const int* cumsum, const VocSeqs& q, int total_rows, int C, float* out, cudaStream_t st) {
+  ++g_launches;
+  if (q.n <= 0 || total_rows <= 0) return;
+  launch_pdl(expand_frames_ragged_kernel, dim3(total_rows), dim3(128), 0, st, emb, cumsum, q, C, out);
 }
 
 void conv_post_tanh(const float* x, int L, int C, const float* w, float bias, int k, float pre_slope, float* out,

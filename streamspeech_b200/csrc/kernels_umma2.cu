@@ -604,9 +604,16 @@ __device__ __forceinline__ void vf_cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
+// a job template resolved for one sequence: its rows, the packed weights of its tile width and its row bases (in floats)
+struct VocSeqJob {
+  int L_in, M, m_tiles, n_tiles, BN;
+  const unsigned char* wp;
+  int64_t in_off, out_off;
+};
+
 template <int BN, bool ADD3>
-__device__ __forceinline__ void vf_item(const VocJob& J, int mt, int nt, unsigned char* a_smem, unsigned char* b_smem, float* tile,
-                                        uint32_t a_stride, uint32_t b_stride) {
+__device__ __forceinline__ void vf_item(const VocJob& J, const VocSeqJob& Q, int mt, int nt, unsigned char* a_smem, unsigned char* b_smem,
+                                        float* tile, uint32_t a_stride, uint32_t b_stride) {
   constexpr int NACC = BN / 2;
   constexpr int TP = BN + 8;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
@@ -620,7 +627,7 @@ __device__ __forceinline__ void vf_item(const VocJob& J, int mt, int nt, unsigne
   const uint32_t b_piece = (uint32_t)BN * CK * 2u;
   const uint32_t b_unit = 2u * b_piece;
   const uint32_t b_chunk = (uint32_t)k * b_unit;
-  const unsigned char* wsrc = J.wp + (size_t)nt * n_chunks * b_chunk;
+  const unsigned char* wsrc = Q.wp + (size_t)nt * n_chunks * b_chunk;
 
   const int upr_shift = (CK == 32) ? 3 : 2;
   const int upr = 1 << upr_shift;
@@ -632,8 +639,8 @@ __device__ __forceinline__ void vf_item(const VocJob& J, int mt, int nt, unsigne
     const int idx = tid + i * VF_THREADS;
     const int r = idx >> upr_shift, q = idx & (upr - 1);
     const int pos = m0 + r - J.pad_left;
-    const bool inb = idx < n_a && pos >= 0 && pos < J.L_in;
-    goff[i] = inb ? (int64_t)pos * C_in + q * 4 : (int64_t)-1;
+    const bool inb = idx < n_a && pos >= 0 && pos < Q.L_in;
+    goff[i] = inb ? Q.in_off + (int64_t)pos * C_in + q * 4 : (int64_t)-1;
     soff[i] = (uint32_t)(q >> 1) * a_plane + (uint32_t)r * 16u + (uint32_t)(q & 1) * 8u;
   }
   // activations are written by earlier phases of this kernel: L2 loads (.cg), never the non-coherent read-only path
@@ -721,16 +728,31 @@ __device__ __forceinline__ void vf_item(const VocJob& J, int mt, int nt, unsigne
     }
   }
   __syncthreads();
-  const int rows = min(VOC_FUSED_BM, J.M - m0);
+  const int rows = min(VOC_FUSED_BM, Q.M - m0);
   for (int idx = tid; idx < rows * BN; idx += VF_THREADS) {
     const int r = idx / BN, cc = idx - r * BN;
     const int n = n0 + cc;
-    const int64_t o = ((int64_t)(m0 + r) * J.out_row_stride + J.out_row_offset) * J.N + n;
+    const int64_t o = Q.out_off + ((int64_t)(m0 + r) * J.out_row_stride + J.out_row_offset) * J.N + n;
     const float v = tile[r * TP + cc] + J.bias[n];
     const float res = J.residual != nullptr ? J.res_scale * __ldcg(J.residual + o) : 0.f;
     J.out[o] = J.alpha * v + res;
   }
   __syncthreads();  // the tile and the operand stages are reused by the next item
+}
+
+// job template T resolved for one sequence (see VocJob)
+__device__ __forceinline__ VocSeqJob vf_resolve(const VocJob& T, const VocStreamGeo& G, bool bn32) {
+  VocSeqJob Q;
+  Q.L_in = G.N * T.in_mult;
+  Q.M = Q.L_in + T.m_adj;
+  Q.m_tiles = Q.M > 0 ? (Q.M + VOC_FUSED_BM - 1) / VOC_FUSED_BM : 0;
+  const bool w32 = bn32 && (T.N & 31) == 0;
+  Q.BN = w32 ? 32 : 16;
+  Q.wp = w32 ? T.wp32 : T.wp16;
+  Q.n_tiles = w32 ? T.N >> 5 : T.N >> 4;
+  Q.in_off = (int64_t)G.row0 * T.in_mult * T.C_in;
+  Q.out_off = (int64_t)G.row0 * T.in_mult * T.out_row_stride * T.N;
+  return Q;
 }
 
 __global__ void __launch_bounds__(VF_THREADS, 1)
@@ -742,42 +764,65 @@ __global__ void __launch_bounds__(VF_THREADS, 1)
   float* tile = reinterpret_cast<float*>(b_smem + 2 * (size_t)b_stride);
   const VocJob* jobs = p.jobs;
   const VocPost& post = p.post;
+  // Items are numbered sequence by sequence, job by job, and this CTA's i only grows: (s, jb) is a cursor that moves forward,
+  // with the items of (s, jb) from `base` on, so a job is resolved once per CTA and sequence, not once per item.  The cursor of a
+  // phase is set up before the grid barrier that precedes it, so its parameter loads overlap the wait.
+  int s = 0, jb = 0, base = 0;
+  VocSeqJob Q = vf_resolve(jobs[p.phases[0].first_job], p.streams[0], p.streams[0].bn32 & 1ull);
   for (int ph = 0; ph < p.n_phases; ++ph) {
     const VocPhase P = p.phases[ph];
+    s = 0;
+    jb = P.first_job;
+    base = 0;
     for (int i = blockIdx.x; i < P.n_items; i += gridDim.x) {
-      int jb = P.first_job, rest = i;
-      while (rest >= jobs[jb].m_tiles * jobs[jb].n_tiles) {
-        rest -= jobs[jb].m_tiles * jobs[jb].n_tiles;
-        ++jb;
+      if (s + 1 < p.n_streams && i >= p.item0[ph][s + 1]) {
+        do ++s; while (s + 1 < p.n_streams && i >= p.item0[ph][s + 1]);
+        jb = P.first_job;
+        base = p.item0[ph][s];
+        Q = vf_resolve(jobs[jb], p.streams[s], (p.streams[s].bn32 >> ph) & 1ull);
+      }
+      while (i - base >= Q.m_tiles * Q.n_tiles) {
+        base += Q.m_tiles * Q.n_tiles;
+        Q = vf_resolve(jobs[++jb], p.streams[s], (p.streams[s].bn32 >> ph) & 1ull);
       }
       const VocJob& J = jobs[jb];
-      const int nt = rest % J.n_tiles, mt = rest / J.n_tiles;  // neighbouring CTAs share activation rows
+      const int rest = i - base;
+      const int nt = rest % Q.n_tiles, mt = rest / Q.n_tiles;  // neighbouring CTAs share activation rows
       const bool add3 = J.x1 != nullptr;
-      if (J.BN == 32) {
-        if (add3) vf_item<32, true>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
-        else vf_item<32, false>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+      if (Q.BN == 32) {
+        if (add3) vf_item<32, true>(J, Q, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+        else vf_item<32, false>(J, Q, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
       } else {
-        if (add3) vf_item<16, true>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
-        else vf_item<16, false>(J, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+        if (add3) vf_item<16, true>(J, Q, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
+        else vf_item<16, false>(J, Q, mt, nt, a_smem, b_smem, tile, a_stride, b_stride);
       }
     }
+    if (ph + 1 < p.n_phases) Q = vf_resolve(jobs[p.phases[ph + 1].first_job], p.streams[0], (p.streams[0].bn32 >> (ph + 1)) & 1ull);
     grid_barrier(bar_ctr, bar_target);
   }
-  // conv_post + tanh on the new samples only, straight into the caller's buffer (same arithmetic order as conv_post_tanh_kernel)
+  // conv_post + tanh on each sequence's new samples only, straight into the caller's buffer (same arithmetic order as
+  // conv_post_tanh_kernel); sample o of the output belongs to the sequence whose [out0, out0 + (N * hop - t0)) holds it
   const int half = (post.k - 1) >> 1;
-  for (int t = post.t0 + blockIdx.x * VF_THREADS + threadIdx.x; t < post.L; t += gridDim.x * VF_THREADS) {
+  s = 0;
+  for (int o = blockIdx.x * VF_THREADS + threadIdx.x; o < post.total; o += gridDim.x * VF_THREADS) {
+    while (s + 1 < p.n_streams && o >= p.streams[s + 1].out0) ++s;
+    const VocStreamGeo& G = p.streams[s];
+    const int L = G.N * post.hop, t = o - G.out0 + G.t0;
+    const float* x0 = post.x0 + (int64_t)G.row0 * post.hop * post.C;
+    const float* x1 = post.x1 + (int64_t)G.row0 * post.hop * post.C;
+    const float* x2 = post.x2 + (int64_t)G.row0 * post.hop * post.C;
     float acc = post.bias;
     for (int j = 0; j < post.k; ++j) {
       const int p = t - half + j;
-      if (p < 0 || p >= post.L) continue;
+      if (p < 0 || p >= L) continue;
       const int64_t row = (int64_t)p * post.C;
       for (int c = 0; c < post.C; ++c) {
-        float v = __ldcg(post.x2 + row + c) + (__ldcg(post.x1 + row + c) + __ldcg(post.x0 + row + c));
+        float v = __ldcg(x2 + row + c) + (__ldcg(x1 + row + c) + __ldcg(x0 + row + c));
         v = v > 0.f ? v : v * post.slope;
         acc = fmaf(post.w[j * post.C + c], v, acc);
       }
     }
-    post.out[t - post.t0] = tanhf(acc);
+    post.out[G.dst + (o - G.out0)] = tanhf(acc);
   }
 }
 

@@ -84,6 +84,8 @@ def load_library() -> ctypes.CDLL:
     lib.ss_unit_position_row.argtypes = [vp, vp]
     lib.ss_vocoder_durations.argtypes = [vp, vp, vp, i32, i32, vp, vp]
     lib.ss_vocoder_generate.argtypes = [vp, vp, i32, i32, i32, i32, vp]
+    lib.ss_vocoder_durations_ragged.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp]
+    lib.ss_vocoder_generate_ragged.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     lib.ss_vocoder_hop.argtypes = [vp]
     lib.ss_vocoder_receptive_field.argtypes = [vp]
     lib.ss_op_linear.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, vp]
@@ -123,7 +125,7 @@ def load_library() -> ctypes.CDLL:
 EXPORTED_SYMBOLS = [
     "ss_create", "ss_destroy", "ss_last_error", "ss_version", "ss_load_tensor", "ss_finalize", "ss_set_chunk",
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
-    "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_hop",
+    "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_durations_ragged", "ss_vocoder_generate_ragged", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
     "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
@@ -562,6 +564,52 @@ class Engine:
         wav = self._f32(n_frames * self.hop)
         self._check(self.lib.ss_vocoder_generate(self._h, self._stream(), total_frames, frame0, n_frames, left_context, wav.data_ptr()))
         return wav
+
+    def vocoder_durations_ragged(self, codes_list: Sequence, dur_prediction: bool = True):
+        """vocoder_durations of every code sequence in codes_list (1-D int64 tensors or lists) in one call
+        (ss_vocoder_durations_ragged).  Returns (durations per sequence, cumsum per sequence (U_s + 1 frame offsets), as host lists
+        from ONE device->host copy, and {"dur": packed durations, "cumsum": packed cumsums} device tensors).  The sequences stay
+        cached for vocoder_generate_ragged."""
+        n = len(codes_list)
+        if n == 0:
+            raise EngineError("vocoder_durations_ragged needs at least one code sequence")
+        if all(isinstance(c, torch.Tensor) for c in codes_list):
+            U = [int(c.numel()) for c in codes_list]
+            codes = torch.cat([c.reshape(-1).to(self.device, torch.int64) for c in codes_list])
+        else:  # host lists: one host->device copy
+            U = [len(c) for c in codes_list]
+            codes = torch.tensor([int(u) for c in codes_list for u in c], dtype=torch.int64, device=self.device)
+        n_dur, n_cum = sum(U), sum(U) + n
+        buf = torch.empty(n_dur + (n_cum + 1) // 2, dtype=torch.int64, device=self.device)  # [durations | cumsums (int32)]
+        dur, cum = buf[:n_dur], buf[n_dur:].view(torch.int32)[:n_cum]
+        lens = (ctypes.c_int32 * n)(*U)
+        self._check(self.lib.ss_vocoder_durations_ragged(self._h, self._stream(), n, codes.data_ptr(), lens, int(dur_prediction),
+                                                         dur.data_ptr(), cum.data_ptr()))
+        host = buf.cpu()
+        h_dur, h_cum = host[:n_dur].tolist(), host[n_dur:].view(torch.int32)[:n_cum].tolist()
+        durs, cums, o = [], [], 0
+        for s, u in enumerate(U):
+            durs.append(h_dur[o:o + u])
+            cums.append(h_cum[o + s:o + s + u + 1])
+            o += u
+        return durs, cums, {"dur": dur, "cumsum": cum}
+
+    def vocoder_generate_ragged(self, totals: Sequence[int], frame0s: Sequence[int], n_frames: Sequence[int],
+                                left_contexts: Sequence[int]) -> List[torch.Tensor]:
+        """vocoder_generate of every sequence of the last vocoder_durations_ragged call in one call (ss_vocoder_generate_ragged).
+        Returns each sequence's n_frames[s] * hop samples as views of one device buffer."""
+        n = len(totals)
+        if not (len(frame0s) == len(n_frames) == len(left_contexts) == n) or n == 0:
+            raise EngineError("vocoder_generate_ragged needs one total, frame0, n_frames and left context per sequence")
+        arr = lambda v: (ctypes.c_int32 * n)(*[int(x) for x in v])
+        wav = self._f32(sum(int(x) for x in n_frames) * self.hop)
+        self._check(self.lib.ss_vocoder_generate_ragged(self._h, self._stream(), n, arr(totals), arr(frame0s), arr(n_frames),
+                                                        arr(left_contexts), wav.data_ptr()))
+        out, o = [], 0
+        for nf in n_frames:
+            out.append(wav[o:o + int(nf) * self.hop])
+            o += int(nf) * self.hop
+        return out
 
     # single ops (parity tests)
     def op_linear(self, x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], act: int = 0) -> torch.Tensor:

@@ -2,7 +2,8 @@
 
 Front door of the reference's offline pipeline after `fairseq-generate`
 (fairseq/examples/speech_to_speech/generate_waveform_from_code.py:40-111, used by
-researches/ctc_unity/test_scripts/pred.offline-s2st.sh): one unit sequence per line in, `<i>_pred.wav` (16 kHz) per line out.
+researches/ctc_unity/test_scripts/pred.offline-s2st.sh): one unit sequence per line in, `<i>_pred.wav` (16 kHz) per line out.  Lines are synthesised
+32 at a time, each group in one vocoder call.
 Same flags; `--cpu` is refused (there is no CPU path), multi-speaker vocoders are not part of StreamSpeech's unit vocoder.
 
     python -m streamspeech_b200.generate_waveform_from_code --in-code-file unit.txt --vocoder g_00500000 \\
@@ -16,7 +17,7 @@ import os
 import sys
 import wave
 from pathlib import Path
-from typing import List
+from typing import List, Sequence
 
 import numpy as np
 import torch
@@ -28,6 +29,9 @@ if _REPO not in sys.path:
 from streamspeech_b200 import synth  # noqa: E402
 from streamspeech_b200.config import ModelConfig, VocoderConfig  # noqa: E402
 from streamspeech_b200.engine import Engine  # noqa: E402
+from streamspeech_b200.offline import vocode_whole  # noqa: E402
+
+LINES_PER_CALL = 32  # code lines synthesised by one vocoder call (one generator kernel per group of the engine's ragged call)
 
 
 def load_code(in_file: str) -> List[List[int]]:
@@ -58,13 +62,13 @@ class VocoderOnly:
         cfg.vocoder = vc
         self.engine = Engine(cfg, synth.make_model_state_dict(cfg, 0), sd, None, device=device)
 
-    @torch.inference_mode()
     def __call__(self, code: List[int], dur_prediction: bool = False) -> torch.Tensor:
-        eng = self.engine
-        codes = torch.tensor([c for c in code if c >= 0], dtype=torch.long, device=eng.device)  # "remove invalid code" (vocoder.py:52-54)
-        _, cum = eng.vocoder_durations(codes, dur_prediction)
-        total = int(cum[-1].item())
-        return eng.vocoder_generate(total, 0, total, 0)
+        return self.batch([code], dur_prediction)[0]
+
+    @torch.inference_mode()
+    def batch(self, codes: Sequence[List[int]], dur_prediction: bool = False) -> List[torch.Tensor]:
+        """__call__ of every code line in one vocoder call; each waveform equals __call__'s bit for bit"""
+        return vocode_whole(self.engine, [[c for c in code if c >= 0] for code in codes], dur_prediction)  # "remove invalid code" (vocoder.py:52-54)
 
 
 def main(args):
@@ -75,9 +79,9 @@ def main(args):
     vocoder = VocoderOnly(args.vocoder, vocoder_cfg)
     data = load_code(args.in_code_file)
     Path(args.results_path).mkdir(exist_ok=True, parents=True)
-    for i, d in enumerate(data):
-        wav = vocoder(d, args.dur_prediction)
-        write_wav(f"{args.results_path}/{i}_pred.wav", wav.detach().cpu().numpy())
+    for g in range(0, len(data), LINES_PER_CALL):
+        for i, wav in enumerate(vocoder.batch(data[g:g + LINES_PER_CALL], args.dur_prediction), start=g):
+            write_wav(f"{args.results_path}/{i}_pred.wav", wav.detach().cpu().numpy())
     return len(data)
 
 

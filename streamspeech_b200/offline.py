@@ -75,11 +75,19 @@ class OfflineS2STGenerator:
         n = self.cfg.vocoder.num_embeddings
         return [int(u) - 4 for u in units if 4 <= int(u) < 4 + n]
 
-    @torch.inference_mode()
     def synthesize(self, codes: Sequence[int], dur_prediction: bool = True) -> torch.Tensor:
         """generate_waveform_from_code.py:58-71: one utterance, whole sequence.  `codes` are vocoder code indices (0..999)."""
-        eng = self.engine
-        codes = torch.tensor([int(u) for u in codes], dtype=torch.long, device=eng.device)
-        _, cum = eng.vocoder_durations(codes, dur_prediction)
-        total = int(cum[-1].item())
-        return eng.vocoder_generate(total, 0, total, 0)
+        return self.synthesize_batch([codes], dur_prediction)[0]
+
+    @torch.inference_mode()
+    def synthesize_batch(self, codes_list: Sequence[Sequence[int]], dur_prediction: bool = True) -> List[torch.Tensor]:
+        """synthesize() of every utterance in one vocoder durations call and one generate call; each waveform equals synthesize()'s
+        bit for bit (views of one device buffer)."""
+        return vocode_whole(self.engine, codes_list, dur_prediction)
+
+
+def vocode_whole(eng, codes_list: Sequence[Sequence[int]], dur_prediction: bool) -> List[torch.Tensor]:
+    """Whole-sequence vocoder passes of the code sequences: one durations call, one host read of the cumsums, one generate call."""
+    _, cums, _ = eng.vocoder_durations_ragged([[int(u) for u in c] for c in codes_list], dur_prediction)
+    totals = [c[-1] for c in cums]
+    return eng.vocoder_generate_ragged(totals, [0] * len(totals), totals, [0] * len(totals))

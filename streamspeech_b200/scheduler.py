@@ -9,8 +9,9 @@ of the round finds its result ready.  A harness that feeds the agents round-robi
 
 `PooledS2STAgent` extends this to simultaneous speech-to-speech translation: the flush that serves its streams also runs ONE batched
 MT search (ss_pool_mt_greedy) for every stream whose policy gate says WRITE and ONE T2U + unit-decoder call
-(ss_t2u_unit_decode_ragged) for every stream that still has something to say; the vocoder stays one call per stream.  The host
-stages around those calls are the single agent's own methods (StreamSpeechS2STAgent._gate / _after_mt / _after_t2u).
+(ss_t2u_unit_decode_ragged) for every stream that still has something to say, then ONE vocoder durations call and ONE generate call
+(ss_vocoder_durations_ragged / ss_vocoder_generate_ragged) for every stream that has new units.  The host stages around those calls
+are the single agent's own methods (StreamSpeechS2STAgent._gate / _after_mt / _before_vocoder / _after_vocoder).
 
 `PooledS2TTAgent` does the same for simultaneous speech-to-text translation: ONE incremental MT search
 (ss_pool_mt_greedy_incremental) for every writing stream, each on its slot's own incremental decoder state, between the single
@@ -252,7 +253,8 @@ class PooledS2STAgent(_PooledDecoder, StreamSpeechS2STAgent):
     def decode_round(pool: StreamPool, agents: Sequence["PooledS2STAgent"], clock: _StageClock):
         """Stages 2-7 of a flush for the agents whose slots the pool step just ran: the gate per stream, one batched MT search for
         the writing streams, the post-MT checks per stream, teacher-forced features for finishing whole-word streams (once per
-        utterance, N2 pad tail), one T2U + unit-decoder call for every stream that goes on, then the vocoder stream by stream."""
+        utterance, N2 pad tail), one T2U + unit-decoder call for every stream that goes on, then one vocoder call (durations, one host
+        read of the cumsums, generate) for every stream with new units."""
         eng = pool.engine
         writing = []
         for a in agents:
@@ -300,9 +302,19 @@ class PooledS2STAgent(_PooledDecoder, StreamSpeechS2STAgent):
                 x[j, :lengths[j]] = pf[m, :lengths[j]]
         clock.mark("t2u")
         units, _, _ = eng.t2u_unit_decode_ragged(x, lengths, [g[5] for g in going])
-        clock.mark("vocoder")
+        clock.mark("vocoder")  # (unit mapping included, as in the single agent's post-T2U stage)
+        voc = []  # (agent, new_subword_tokens, unit)
         for (a, new, _, _, _, _), u in zip(going, units):
-            a._action = a._after_t2u(u, new)
+            action, unit = a._before_vocoder(u)
+            if action is not None:
+                a._action = action
+            else:
+                voc.append((a, new, unit))
+        if not voc:
+            return
+        wavs = StreamSpeechS2STAgent._vocode(eng, [a for a, _, _ in voc], [unit for _, _, unit in voc])
+        for (a, new, unit), w in zip(voc, wavs):
+            a._action = a._after_vocoder(unit, w, new)
 
 
 class PooledS2TTAgent(_PooledDecoder, StreamSpeechS2TTAgent):

@@ -10,7 +10,8 @@ compared with the 1e-3 bar).  Then the two arms run alternately (--reps times ea
 synchronisation and is timed on the host clock.  Reported per workload: audio seconds per wall second of both arms; the pooled
 arm's device time per flush stage (CUDA events at the stage boundaries, so each stage includes the host work between its
 engine calls); kernel launches per flush; host synchronisations per flush, counted from the engine calls the flush makes (one per
-upload or read-back, one per 16-step MT burst); the card's name and power limit, read in the same run.
+upload or read-back, one per 16-step MT burst; the vocoder: one read of all cumsums, and one for the waveforms the agents then read);
+the card's name and power limit, read in the same run.
 
     python tools/pool_s2st_bench.py [--streams 1 8 32] [--reps 2] [--out results/pool_s2st_bench.json]
 """
@@ -91,8 +92,8 @@ class SyncCounter:
 
     def __init__(self, eng):
         self.n = 0
-        for name, fixed in (("pool_step", 2), ("mt_features_batch", 1), ("t2u_unit_decode_ragged", 2), ("vocoder_durations", 1),
-                            ("vocoder_generate", 1)):
+        for name, fixed in (("pool_step", 2), ("mt_features_batch", 1), ("t2u_unit_decode_ragged", 2),
+                            ("vocoder_durations_ragged", 1), ("vocoder_generate_ragged", 1)):
             self._wrap(eng, name, fixed)
         f = eng.pool_mt_greedy
 
