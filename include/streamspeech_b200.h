@@ -49,17 +49,29 @@ typedef struct ss_config {
   int32_t t2u_layers, unit_dim, unit_ffn, unit_heads, unit_layers, unit_vocab, ctc_upsample_rate;
   int32_t bos, pad, eos, unk, uni_encoder;
   int32_t max_enc_frames;   /* longest encoder sequence (40 ms frames) the rel-pos tables cover */
-  int32_t max_mt_positions; /* MT decoder max positions (1024) */
+  int32_t max_mt_positions; /* entries of every MT self-attention cache, 3 .. SS_MAX_MT_POSITIONS (see below) */
   /* CodeHiFiGAN */
   int32_t voc_n_ups, voc_up_rates[SS_MAX_UPS], voc_up_kernels[SS_MAX_UPS], voc_init_channels;
   int32_t voc_n_rb, voc_rb_kernels[SS_MAX_RB], voc_rb_ndil, voc_rb_dils[SS_MAX_RB][SS_MAX_DIL];
   int32_t voc_num_embeddings, voc_embedding_dim, voc_in_dim, voc_dur_hidden, voc_dur_kernel;
 } ss_config;
 
+/* max_mt_positions sizes everything the MT searches index by position: the handle's self-attention K / V caches
+ * [mt_layers][max_mt_positions][mt_dim], its token and feature buffers, the position table the host loads as "__const__.mt_pos_table"
+ * (max_mt_positions + pad + 2 rows) and, per stream-pool slot, the incremental search's K / V caches (2 x mt_layers x max_mt_positions
+ * x mt_dim floats, allocated for every slot by the first ss_pool_mt_greedy_incremental: with mt_layers = 4 and mt_dim = 512, 16 MB
+ * per slot at 1024 and 32 MB at 2048, so 1 GB for 32 slots at 2048).  A search needs max_len + 2 entries and is refused with
+ * SS_ERR_CAPACITY before any launch otherwise.  The incremental searches keep one more entry per call of the utterance (max_len +
+ * kv_off + 2), so the S2TT agents, whose generator allows max_decoder_positions - 1 tokens once the source is finished, need
+ * max_decoder_positions + (MT calls of the utterance) + 2: 2048 covers every utterance that max_enc_frames = 1024 admits (1200
+ * positions; a 41 s utterance in 160 ms segments makes 256 calls).  The self-attention of the persistent MT kernels takes any number
+ * of entries; ss_create refuses a value outside [3, SS_MAX_MT_POSITIONS] with SS_ERR_INVALID. */
+#define SS_MAX_MT_POSITIONS 8192
+
 /* ---- lifecycle --------------------------------------------------------------------------------------- */
 int ss_create(ss_engine** out, int device, const ss_config* cfg);
 int ss_destroy(ss_engine* h);
-const char* ss_last_error(const ss_engine* h);
+const char* ss_last_error(const ss_engine* h); /* h == NULL: why this thread's last ss_create was refused */
 const char* ss_version(void);
 
 /* Load one fp32 tensor of the checkpoint by its fairseq state-dict key (host memory, row-major).

@@ -32,7 +32,7 @@ if _REPO not in sys.path:
 
 from streamspeech_b200.config import ModelConfig, VocoderConfig  # noqa: E402
 from streamspeech_b200.dictionary import Dictionary  # noqa: E402
-from streamspeech_b200.engine import Engine, EngineError  # noqa: E402
+from streamspeech_b200.engine import SS_ERR_CAPACITY, Engine, EngineError  # noqa: E402
 from streamspeech_b200.simuleval_compat import (ReadAction, SpeechSegment, SpeechToSpeechAgent, SpeechToTextAgent, WriteAction)  # noqa: E402
 from streamspeech_b200 import synth  # noqa: E402
 
@@ -164,7 +164,8 @@ class _EngineAgentMixin:
         self.cfg = cfg
         self.dict = dicts
         dev = getattr(args, "device_index", 0)
-        self.engine = Engine(cfg, sd, vsd, gcmvn, device=dev, max_enc_frames=getattr(args, "max_enc_frames", 1024))
+        self.engine = Engine(cfg, sd, vsd, gcmvn, device=dev, max_enc_frames=getattr(args, "max_enc_frames", 1024),
+                             max_mt_positions=getattr(args, "max_mt_positions", 1024))
         self.torch_device = self.engine.device
         self.audio = _DeviceAudio(self.torch_device, engine=self.engine, sample_rate=args.sample_rate)
         self.feat_cache = torch.zeros(6000, cfg.feat_dim, dtype=torch.float32, device=self.torch_device)
@@ -585,8 +586,21 @@ class StreamSpeechS2TTAgent(_EngineAgentMixin, SpeechToTextAgent):
         new_subword_tokens = self._gate(src_ctc_indices, tgt_ctc_indices)
         if new_subword_tokens is None:
             return ReadAction()
-        tokens = self.engine.mt_greedy_incremental(enc, self.tgt_subwords_indices, new_subword_tokens, self._max_len(feature.size(0)))
+        tokens = self._mt_capacity_named(lambda: self.engine.mt_greedy_incremental(enc, self.tgt_subwords_indices, new_subword_tokens,
+                                                                                     self._max_len(feature.size(0))))
         return self._after_mt(tokens, new_subword_tokens)
+
+    def _mt_capacity_named(self, search):
+        """Runs the incremental MT search; its SS_ERR_CAPACITY (refused before any launch: the cache must hold max_len + 2 entries plus
+        one per earlier call of the utterance, wherever eos would fall) comes back as an error that says what to change."""
+        try:
+            return search()
+        except EngineError as e:
+            if e.code != SS_ERR_CAPACITY:
+                raise
+            raise EngineError(f"utterance too long for this agent's MT decoder cache (max_mt_positions = {self.engine.max_mt_positions}): "
+                              f"{e.detail}.  Build the agent with a larger args.max_mt_positions; 2048 covers every utterance the encoder "
+                              f"admits") from e
 
     def _max_len(self, n_frames: int) -> int:
         """generator_mt: max_len_a = 1, max_len_b = 200 (:161-179); src_len = src_tokens.size(1) = fbank frames"""

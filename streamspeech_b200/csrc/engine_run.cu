@@ -1149,6 +1149,12 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
 
 namespace {
 
+// why an incremental search is refused for capacity: the entries it needs against those every self-attention cache has
+std::string mt_incremental_capacity_message(int max_len, int kv_off, int max_mt_positions) {
+  return "MT hypothesis longer than capacity: the incremental search needs " + std::to_string(max_len + kv_off + 2) + " self-attention entries (max_len " +
+         std::to_string(max_len) + " + " + std::to_string(kv_off) + " kept from earlier calls + 2), max_mt_positions = " + std::to_string(max_mt_positions);
+}
+
 // The incremental search of one stream on the single-token kernel: P holds the stream's state (self_k / self_v / cross_kv, kv_off)
 // and P.tok[start] its first token; positions start .. max_len over Tk cross rows, `burst` steps per launch and synchronisation.
 // The new tokens go to tokens_out_host[*n_tok ...]; *self_len follows the entries the self-attention cache holds.
@@ -1205,7 +1211,8 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
   // re-feeds the last prefix token on top of the entry the previous call's final step left (kv_off grows by one per call)
   const int kv_off = h->mt_inc_self_len - start;
   if (kv_off < 0) return h->fail(SS_ERR_STATE, "incremental MT state is shorter than the prefix (reset missing, or a prefix that this state did not produce)");
-  if (max_len + kv_off + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
+  if (max_len + kv_off + 2 > c.max_mt_positions) return h->fail(SS_ERR_CAPACITY, mt_incremental_capacity_message(max_len, kv_off, c.max_mt_positions));
+  if (max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
   if (!h->persistent_mt || !mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, std::max(T, h->mt_inc_cross_rows)))
     return h->fail(SS_ERR_STATE, "incremental MT decoding runs on the persistent MT kernel, which is off or does not support this shape");
   int rc = ensure_mt_cross(h, std::max(T, h->mt_inc_cross_rows), h->mt_inc_cross_rows);

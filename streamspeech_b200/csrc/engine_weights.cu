@@ -322,7 +322,8 @@ void finalize_impl(ss_engine* h) {
     expect_shape(e, "target_unigram_decoder.embed_tokens.weight", {c.tgt_vocab, c.mt_dim});
     h->mt_emb = upload(h, e.data);
     const HostTensor& pt = get(h, "__const__.mt_pos_table");
-    if (pt.shape.size() != 2 || pt.shape[1] != c.mt_dim) throw std::runtime_error("bad __const__.mt_pos_table");
+    if (pt.shape.size() != 2 || pt.shape[1] != c.mt_dim || pt.shape[0] < (int64_t)c.max_mt_positions + c.pad + 2)
+      throw std::runtime_error("bad __const__.mt_pos_table (needs max_mt_positions + pad + 2 rows of mt_dim)");
     h->mt_pos_rows = (int)pt.shape[0];
     h->mt_pos = upload(h, pt.data);
     for (int i = 0; i < c.mt_layers; ++i)
@@ -458,6 +459,9 @@ void finalize_impl(ss_engine* h) {
 
 }  // namespace
 
+// what ss_last_error(NULL) returns: the reason of this thread's last refused ss_create (which leaves no handle to ask)
+static thread_local std::string g_create_err = "null handle";
+
 extern "C" {
 
 const char* ss_version(void) { return "streamspeech_b200 0.1 (sm_90a)"; }
@@ -465,9 +469,14 @@ const char* ss_version(void) { return "streamspeech_b200 0.1 (sm_90a)"; }
 int ss_create(ss_engine** out, int device, const ss_config* cfg) {
   if (!out || !cfg) return SS_ERR_INVALID;
   *out = nullptr;
+  g_create_err = "null handle";
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device >= n) return SS_ERR_CUDA;
   if (cudaSetDevice(device) != cudaSuccess) return SS_ERR_CUDA;
+  if (cfg->max_mt_positions < 3 || cfg->max_mt_positions > SS_MAX_MT_POSITIONS) {  // (max_len >= 1 needs max_len + 2 entries)
+    g_create_err = "ss_create: max_mt_positions = " + std::to_string(cfg->max_mt_positions) + " is outside [3, " + std::to_string(SS_MAX_MT_POSITIONS) + "]";
+    return SS_ERR_INVALID;
+  }
   ss_engine* h = new ss_engine();
   h->device = device;
   h->cfg = *cfg;
@@ -510,7 +519,7 @@ int ss_destroy(ss_engine* h) {
   return SS_OK;
 }
 
-const char* ss_last_error(const ss_engine* h) { return h ? h->err.c_str() : "null handle"; }
+const char* ss_last_error(const ss_engine* h) { return h ? h->err.c_str() : g_create_err.c_str(); }
 
 int ss_load_tensor(ss_engine* h, const char* key, const float* data_host, int ndim, const int64_t* shape) {
   if (!h || !key || !data_host || ndim < 0 || ndim > 8) return SS_ERR_INVALID;

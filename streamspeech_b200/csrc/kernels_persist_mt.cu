@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_persistent_kernel_v2(MtDecod
       STAMP(2);
       // (2) self-attention of head grp_h (every CTA of the group) + partial out-projection of this CTA's 32 columns
       if (in_group) {
-        attend_head_early(sm, P.q + grp_h * MHD, P.self_k + (size_t)l * P.max_pos * DIM + grp_h * MHD, P.self_v + (size_t)l * P.max_pos * DIM + grp_h * MHD,
+        attend_head_self(sm, P.q + grp_h * MHD, P.self_k + (size_t)l * P.max_pos * DIM + grp_h * MHD, P.self_v + (size_t)l * P.max_pos * DIM + grp_h * MHD,
                           DIM, s + P.kv_off + 1, att_h);
         __syncthreads();
         head_partial_proj_w(att_h, hw, grp_j, part + grp_h * DIM);
@@ -213,8 +213,9 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_persistent_kernel_v2(MtDecod
 }  // namespace
 
 bool mt_decode_persistent_supported(int dim, int ffn, int heads, int vocab, int max_pos, int T) {
-  // (one round of columns per phase: vocab <= 6 columns x 8 warps x #SMs, checked against the smallest supported grid)
-  return vocab <= 6 * MW * 132 && dim == 512 && ffn == 2048 && heads * MHD == dim && vocab >= 1 && max_pos <= 1024 && T >= 1 && T <= 1024;
+  // (one round of columns per phase: vocab <= 6 columns x 8 warps x #SMs, checked against the smallest supported grid; the
+  // self-attention cache may hold any number of entries, the cross-attention of T encoder rows keeps its scores in MtSmem::S)
+  return vocab <= 6 * MW * 132 && dim == 512 && ffn == 2048 && heads * MHD == dim && vocab >= 1 && max_pos >= 1 && T >= 1 && T <= MSC;
 }
 
 int mt_decode_persistent(const MtDecodeParams& P, const MtLayerP* layers_dev, int step0, int nsteps, int max_len, int T, unsigned* bar_ctr,

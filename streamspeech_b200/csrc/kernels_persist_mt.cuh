@@ -12,6 +12,7 @@ namespace {
 constexpr int MW = 8;
 constexpr int MTT = MW * 32;
 constexpr int MHD = 64;
+constexpr int MSC = 1024;  // attention scores a CTA holds at once (MtSmem::S)
 
 __device__ __forceinline__ float4 ldw(const float* p) {
   float4 r;
@@ -22,7 +23,7 @@ __device__ __forceinline__ float4 ldw(const float* p) {
 struct MtSmem {
   float x[512];     // residual stream of the token (model dim <= 512)
   float v[2048];    // GEMV input vector (LN(x), attention output or FFN hidden)
-  float S[1024];    // attention scores
+  float S[MSC];     // attention scores (of one block of keys in attend_head_long)
   float qh[MHD];
   float pv[16][MHD];
   float red[MW];
@@ -216,7 +217,7 @@ constexpr int GRP = 16;                 // CTAs per head group (8 heads x 16 = 1
 constexpr int PCOLS = 512 / GRP;        // out-projection columns per CTA of a group
 constexpr int PCOLS_PER_WARP = PCOLS / MW;
 
-// softmax(q . K^T * scale) V for one head by one CTA: q[64], K/V rows at kbase/vbase + j * ld, n keys; out[64].
+// softmax(q . K^T * scale) V for one head by one CTA: q[64], K/V rows at kbase/vbase + j * ld, n <= MSC keys; out[64].
 // Every independent load is issued up front: the key row of this thread, the first 8 value rows of its part and the
 // query are all in flight together (one L2 round trip instead of three dependent ones); n <= 256 keys take a single pass.
 // Thread (part, q) sums keys j = part (mod 16) over dims [4q, 4q + 4), 8 keys (8 independent 16-byte loads) in flight per thread.
@@ -293,6 +294,93 @@ __device__ void attend_head_early(MtSmem& sm, const float* q, const float* kbase
     for (int x = 0; x < 16; ++x) t += sm.pv[x][tid];
     out[tid] = t / sum;
   }
+}
+
+// The same attention over any number of keys, for n > MSC (the incremental search's self-attention cache of a long utterance): the
+// keys go through sm.S in blocks of MSC.  Per block: the scores and their maximum, then exp and the P.V partial sums with
+// attend_head_early's thread mapping; between blocks the running maximum m, each thread's part of the sum and its accumulator are
+// rescaled by exp(m_old - m_new).  Inlined on purpose: as a call it costs the single-token kernel 16 more bytes of register spill
+// (live weights saved around the call), inlined none.
+__device__ __forceinline__ void attend_head_long(MtSmem& sm, const float* q, const float* kbase, const float* vbase, int ld, int n, float* out) {
+  const int tid = threadIdx.x;
+  const int q4 = (tid & 15) * 4, part = tid >> 4;
+  __syncthreads();
+  if (tid < MHD) sm.qh[tid] = q[tid] * 0.125f;
+  __syncthreads();
+  float m = -INFINITY, sum = 0.f;
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+  for (int b0 = 0; b0 < n; b0 += MSC) {
+    const int nb = min(MSC, n - b0);
+    const float* kb = kbase + (int64_t)b0 * ld;
+    const float* vb = vbase + (int64_t)b0 * ld + q4;
+    float mx = -INFINITY;
+    for (int j = tid; j < nb; j += MTT) {
+      const float* kr = kb + (int64_t)j * ld;
+      float4 kk[MHD / 4];
+#pragma unroll
+      for (int d = 0; d < MHD / 4; ++d) kk[d] = *reinterpret_cast<const float4*>(kr + 4 * d);
+      float s = 0.f;
+#pragma unroll
+      for (int d = 0; d < MHD / 4; ++d) {
+        s = fmaf(sm.qh[4 * d], kk[d].x, s);
+        s = fmaf(sm.qh[4 * d + 1], kk[d].y, s);
+        s = fmaf(sm.qh[4 * d + 2], kk[d].z, s);
+        s = fmaf(sm.qh[4 * d + 3], kk[d].w, s);
+      }
+      sm.S[j] = s;
+      mx = fmaxf(mx, s);
+    }
+    const float m_new = fmaxf(m, block_reduce_max(sm, mx));
+    const float rescale = expf(m - m_new);  // (0 at the first block: m = -inf)
+    m = m_new;
+    sum *= rescale;
+    a.x *= rescale;
+    a.y *= rescale;
+    a.z *= rescale;
+    a.w *= rescale;
+    for (int j = tid; j < nb; j += MTT) {
+      const float e = expf(sm.S[j] - m);
+      sm.S[j] = e;
+      sum += e;
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int j0 = part; j0 < nb; j0 += 16 * 8) {
+      float4 vv[8];
+      float pp[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int j = j0 + 16 * u;
+        const bool ok = j < nb;
+        vv[u] = ok ? *reinterpret_cast<const float4*>(vb + (int64_t)j * ld) : make_float4(0.f, 0.f, 0.f, 0.f);
+        pp[u] = ok ? sm.S[j] : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        a.x = fmaf(pp[u], vv[u].x, a.x);
+        a.y = fmaf(pp[u], vv[u].y, a.y);
+        a.z = fmaf(pp[u], vv[u].z, a.z);
+        a.w = fmaf(pp[u], vv[u].w, a.w);
+      }
+    }
+    __syncthreads();  // the next block's scores overwrite sm.S
+  }
+  sum = block_reduce_sum(sm, sum);
+  *reinterpret_cast<float4*>(&sm.pv[part][q4]) = a;
+  __syncthreads();
+  if (tid < MHD) {
+    float t = 0.f;
+#pragma unroll
+    for (int x = 0; x < 16; ++x) t += sm.pv[x][tid];
+    out[tid] = t / sum;
+  }
+}
+
+// self-attention of one head over a cache of any length: the key count selects the form (the same for every thread of the CTA)
+__device__ __forceinline__ void attend_head_self(MtSmem& sm, const float* q, const float* kbase, const float* vbase, int ld, int n, float* out) {
+  if (n <= MSC) attend_head_early(sm, q, kbase, vbase, ld, n, out);
+  else attend_head_long(sm, q, kbase, vbase, ld, n, out);
 }
 
 // x[c] += sum_h part[h][c] + bias[c]   (every CTA, identical order); x is a 512-float residual row in shared memory,

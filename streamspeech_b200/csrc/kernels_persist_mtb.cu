@@ -104,8 +104,9 @@ __device__ __forceinline__ void add_delta_rows(const MtbSmem& sb, float* xs, con
 }
 
 // attention of head h for this CTA's rows (unfinished rows i = j, j + 16, ...) and their partial out-projections over all 512
-// columns: part[r][h][col] = sum_{i < 64} a[i] * W[col][64 h + i], warp w owning columns [64 w, 64 w + 64)
-template <typename KV>
+// columns: part[r][h][col] = sum_{i < 64} a[i] * W[col][64 h + i], warp w owning columns [64 w, 64 w + 64).  kSelf: the rows' key
+// counts are cache lengths, which may exceed MSC (attend_head_self, as the single-token kernel); cross-attention has at most MSC keys
+template <bool kSelf, typename KV>
 __device__ __forceinline__ void attend_rows(MtSmem& sm, MtbSmem& sb, const float* q, KV&& kv, const float* __restrict__ W, int h, int j,
                                             float* part) {
   int nloc = 0;
@@ -115,7 +116,8 @@ __device__ __forceinline__ void attend_rows(MtSmem& sm, MtbSmem& sb, const float
     const float* vbase;
     int ld, n;
     kv(r, kb, vbase, ld, n);
-    attend_head_early(sm, q + (size_t)r * DIM + h * MHD, kb + h * MHD, vbase + h * MHD, ld, n, sb.att[nloc]);
+    if constexpr (kSelf) attend_head_self(sm, q + (size_t)r * DIM + h * MHD, kb + h * MHD, vbase + h * MHD, ld, n, sb.att[nloc]);
+    else attend_head_early(sm, q + (size_t)r * DIM + h * MHD, kb + h * MHD, vbase + h * MHD, ld, n, sb.att[nloc]);
   }
   __syncthreads();
   if (nloc == 0) return;
@@ -242,7 +244,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       WAIT();
       // (2) self-attention over positions 0..s of each row's cache + partial out-projections
       if (in_group)
-        attend_rows(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
+        attend_rows<true>(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
           ld = DIM;
           if constexpr (kMode == kMtbIncremental) {
             const size_t b = self_block(P, r, l);
@@ -270,7 +272,7 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
       WAIT();
       // (4) cross-attention over the first cross_len[r] encoder rows of each sample + partial out-projections
       if (in_group)
-        attend_rows(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
+        attend_rows<false>(sm, sb, P.q, [&](int r, const float*& kb, const float*& vbs, int& ld, int& n) {
           const size_t blk = kMode != kMtbOffline ? (size_t)P.cross_row[r] * P.n_layers + l : (size_t)l * MAXR + r;
           kb = P.cross_kv + blk * P.cross_cap * 2 * DIM;
           vbs = kb + DIM;

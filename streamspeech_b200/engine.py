@@ -35,8 +35,15 @@ class SSConfig(ctypes.Structure):
     )
 
 
+SS_ERR_CAPACITY = -5
+
+
 class EngineError(RuntimeError):
-    pass
+    """code: the ss_status of a failed library call (None for errors raised on the host side); detail: the library's message"""
+
+    def __init__(self, message: str, code: Optional[int] = None, detail: str = ""):
+        super().__init__(message)
+        self.code, self.detail = code, detail
 
 
 _lib = None
@@ -198,7 +205,7 @@ class Engine:
         sc = make_ss_config(cfg, max_enc_frames, max_mt_positions)
         rc = self.lib.ss_create(ctypes.byref(self._h), device, ctypes.byref(sc))
         if rc != 0:
-            raise EngineError(f"ss_create failed with {rc}")
+            raise EngineError(f"ss_create failed with {rc}: {self.lib.ss_last_error(None).decode()}")
         try:
             for k, v in model_sd.items():
                 if v.is_floating_point():
@@ -257,7 +264,8 @@ class Engine:
 
     def _check(self, rc: int):
         if rc != 0:
-            raise EngineError(f"libstreamspeech_b200 error {rc}: {self.lib.ss_last_error(self._h).decode()}")
+            detail = self.lib.ss_last_error(self._h).decode()
+            raise EngineError(f"libstreamspeech_b200 error {rc}: {detail}", rc, detail)
 
     def _load(self, key: str, t: torch.Tensor):
         t = t.detach().to(torch.float32).cpu().contiguous()

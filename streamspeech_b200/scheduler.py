@@ -381,8 +381,9 @@ class PooledS2TTAgent(_PooledDecoder, StreamSpeechS2TTAgent):
         if not writing:
             return
         clock.mark("mt_incremental")
-        hyps = eng.pool_mt_greedy_incremental([a.slot for a, _ in writing], [a.tgt_subwords_indices for a, _ in writing],
-                                              [new for _, new in writing], [a._max_len(eng.pool_info(a.slot)["n_feat"]) for a, _ in writing])
+        hyps = writing[0][0]._mt_capacity_named(lambda: eng.pool_mt_greedy_incremental(
+            [a.slot for a, _ in writing], [a.tgt_subwords_indices for a, _ in writing], [new for _, new in writing],
+            [a._max_len(eng.pool_info(a.slot)["n_feat"]) for a, _ in writing]))
         for (a, new), tokens in zip(writing, hyps):
             a._action = a._after_mt(tokens, new)
 

@@ -1,10 +1,12 @@
 """Concurrent simultaneous S2TT streams: PooledS2TTAgents on one stream pool vs the same utterances through one single-stream
 StreamSpeechS2TTAgent, one after another, on the same engine (synthetic 12-layer model).
 
-Workloads: N in {1, 8, 16, 32} concurrent 6.4 s utterances (synth.make_audio, seeds 9000 + j) at 320 ms segments, and a mixed set of
-16 streams, every other one at 640 ms.  6.4 s keeps the finishing call inside the MT kernels' 1024 self-attention entries: the
-synthetic model never emits eos, so that call decodes to max_len = fbank frames + 200.  The pooled arm feeds all streams round by
-round through pushpop_many (a 640 ms stream every second 320 ms round); the single arm plays each utterance to its end before the next.
+Workloads: N in {1, 8, 16, 32} concurrent utterances of --seconds (default 6.4; synth.make_audio, seeds 9000 + j) at 320 ms segments,
+and a mixed set of 16 streams, every other one at 640 ms.  The finishing call of an utterance reserves max_len = fbank frames + 200
+self-attention entries plus one per earlier MT call, whatever the length of the hypothesis: 6.4 s fits the engine's default
+max_mt_positions = 1024, a 10 s utterance needs --max-mt-positions 2048 (32 MB of incremental MT cache per pool slot instead of 16 MB).
+The pool is sized from --seconds.  The pooled arm feeds all streams round by round through pushpop_many (a 640 ms stream every
+second 320 ms round); the single arm plays each utterance to its end before the next.
 
 Before timing, both arms must emit identical actions, text deltas and CTC / MT tokens on every call.  Then the two arms run
 alternately (--reps times each); every run ends with a device synchronisation and is timed on the host clock.  Reported per
@@ -13,10 +15,11 @@ boundaries, so each stage includes the host work between its engine calls); kern
 flush, counted from the engine calls the flush makes (one per upload or read-back, one per 16-step MT burst); the card's name, power
 limit and max SM clock, read in the same run.
 
-    python tools/pool_s2tt_bench.py [--streams 1 8 16 32] [--reps 2] [--out results/pool_s2tt_bench.json]
+    python tools/pool_s2tt_bench.py [--streams 1 8 16 32] [--seconds 6.4] [--max-mt-positions 1024] [--reps 2] [--out results/pool_s2tt_bench.json]
 """
 import argparse
 import json
+import math
 import os
 import subprocess
 import sys
@@ -32,7 +35,6 @@ from streamspeech_b200.agent import StreamSpeechS2TTAgent  # noqa: E402
 from streamspeech_b200.scheduler import PooledS2TTAgent, StreamPool, pushpop_many  # noqa: E402
 from streamspeech_b200.simuleval_compat import SpeechSegment  # noqa: E402
 
-SECONDS = 6.4
 KEYS = ("asr_tokens", "st_tokens", "mt_tokens")
 
 
@@ -41,8 +43,8 @@ def gpu_info():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown (nvidia-smi unavailable)"
 
 
-def args_for(seg):
-    return argparse.Namespace(model_path="synthetic", data_bin=".", config_yaml=None, multitask_config_yaml=None, sample_rate=16000, max_len=200,
+def args_for(seg, max_mt_positions=1024):
+    return argparse.Namespace(max_mt_positions=max_mt_positions, model_path="synthetic", data_bin=".", config_yaml=None, multitask_config_yaml=None, sample_rate=16000, max_len=200,
                               force_finish=False, lagging_k1=0, lagging_k2=0, segment_size=seg, stride_n=1, stride_n2=1, unit_per_subword=15,
                               source_segment_size=seg, device_index=0)
 
@@ -73,6 +75,8 @@ def run_pooled(pool, agents, wavs, segs):
         due = [j for j, s in enumerate(segs) if rnd % (s // 320) == 0 and pos[j] < len(wavs[j])]
         chunks = []
         for j in due:
+            if pos[j] == 0 and agents[j].states.source_finished:  # its previous utterance ended on an unchanged hypothesis: no reset quirk
+                agents[j].reset()
             n = 16 * segs[j]
             chunks.append(SpeechSegment(content=wavs[j][pos[j]:pos[j] + n].tolist(), sample_rate=16000, finished=pos[j] + n >= len(wavs[j])))
             pos[j] += n
@@ -112,21 +116,23 @@ class SyncCounter:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, nargs="+", default=[1, 8, 16, 32])
+    ap.add_argument("--seconds", type=float, default=6.4, help="length of every utterance")
+    ap.add_argument("--max-mt-positions", type=int, default=1024, help="the engine's MT cache entries (2048 for utterances above about 8 s)")
     ap.add_argument("--reps", type=int, default=2)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
-    single = StreamSpeechS2TTAgent(args_for(320))
+    single = StreamSpeechS2TTAgent(args_for(320, a.max_mt_positions))
     eng = single.engine
     n_max = max(max(a.streams), 16)
-    pool = StreamPool(eng, n_slots=n_max, max_seconds=8, ctc_heads=2)
+    pool = StreamPool(eng, n_slots=n_max, max_seconds=math.ceil(a.seconds) + 1, ctc_heads=2)
     syncs = SyncCounter(eng)
     workloads = [(f"{n}x320ms", [320] * n) for n in a.streams] + [("16x_mixed_320_640ms", [320 if j % 2 == 0 else 640 for j in range(16)])]
-    result = {"gpu": gpu_info(), "utterance_seconds": SECONDS, "rows": []}
+    result = {"gpu": gpu_info(), "utterance_seconds": a.seconds, "max_mt_positions": a.max_mt_positions, "rows": []}
     dictionary = single.dict["target_unigram"]
     for name, segs in workloads:
-        wavs = [synth.make_audio(SECONDS, seed=9000 + j) for j in range(len(segs))]
+        wavs = [synth.make_audio(a.seconds, seed=9000 + j) for j in range(len(segs))]
         agents = [PooledS2TTAgent(pool, dictionary, args_for(s)) for s in segs]
         ref = run_single(single, wavs, segs)
         got = run_pooled(pool, agents, wavs, segs)
@@ -147,7 +153,7 @@ def main():
             if r == 0:
                 pool.stage_ms = None
                 flushes, launches, n_sync = pool.steps - steps0, eng.launch_count() - l0, syncs.n - s0
-        audio = SECONDS * len(segs)
+        audio = a.seconds * len(segs)
         best = {k: min(v) for k, v in times.items()}
         row = {"workload": name, "streams": len(segs), "audio_s_per_s": {k: audio / v for k, v in best.items()},
                "speedup_pooled_vs_single": best["single"] / best["pooled"], "seconds_all": times, "flushes": flushes,
@@ -158,7 +164,7 @@ def main():
         result["rows"].append(row)
         for ag in agents:
             pool.release(ag.slot)
-    print(json.dumps({"gpu": result["gpu"]}))
+    print(json.dumps({k: result[k] for k in ("gpu", "utterance_seconds", "max_mt_positions")}))
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:
