@@ -1880,6 +1880,9 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
 int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N, int act,
                  float* out_dev) {
   if (!h) return SS_ERR_INVALID;
+  // the plain linear (skinny / fp32 CUDA-core kernels; ss_op_linear_umma is the wgmma hook), whatever routing the last entry point
+  // of any handle left on this thread: that handle, and the weight cache the routing points to, may have been destroyed since
+  g_umma_linear = 0;
   Linear l;
   l.w = const_cast<float*>(w_dev); l.b = const_cast<float*>(bias_dev); l.N = N; l.K = K;
   linear(x_dev, K, M, l, ep_out(out_dev, N, act), S(stream));
