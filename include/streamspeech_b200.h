@@ -13,8 +13,8 @@
  *  - `stream` is a cudaStream_t (as void*).  Work is enqueued on it; functions documented as
  *    "enqueue only" never synchronise, the others synchronise that stream where stated;
  *  - one handle may be used from one host thread at a time; distinct handles share no device state (weights, caches,
- *    workspaces, barrier counters are per handle).  Process-wide: the launch counter (ss_launch_count), the tuning options
- *    "umma2_split_below" / "umma2_min_units" / "prefer_shared", and the per-device kernel attribute cache.
+ *    workspaces, split-K scratch, barrier counters, options are per handle).  Process-wide are only the launch counter
+ *    (ss_launch_count) and the per-device kernel attribute cache.
  */
 #ifndef STREAMSPEECH_B200_H_
 #define STREAMSPEECH_B200_H_

@@ -17,12 +17,6 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 // ... and the matching wait: everything the previous kernels of the stream wrote is visible after it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// Shared-memory carve-out: the wgmma kernels need > 100 KB of shared memory per CTA, the SIMT kernels a few KB.  An SM
-// holds ONE carve-out at a time, so kernels that ask for different ones cannot share an SM and every change drains it
-// -- which is what the vocoder's three concurrent streams of alternating conv / reduce kernels would do.  With the option on
-// (default) every kernel of the library asks for the maximum shared-memory carve-out, once per kernel function.
-extern int g_prefer_shared;
-
 // Function attributes (cudaFuncSetAttribute) belong to the CURRENT DEVICE: a process that holds handles on several devices
 // must configure every kernel once per device, not once per process.  true the first time (device, key) is seen.
 inline bool first_time_on_device(const void* key) {
@@ -45,18 +39,11 @@ inline int current_device_sms() {
   return sms[dev];
 }
 
-inline void prefer_shared_once(const void* fn) {
-  if (!g_prefer_shared) return;
-  // (key fn + 1: a key space distinct from the max-shared-memory configuration of the same function)
-  if (first_time_on_device((const char*)fn + 1)) cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-}
-
 // launch with programmatic stream serialization: the grid may be scheduled while its predecessor is still running; every
 // kernel launched this way calls pdl_wait() before it touches memory (so semantics equal a normal launch, minus the
 // launch / scheduling latency that now overlaps the predecessor)
 template <typename... KArgs, typename... Args>
 inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  prefer_shared_once((const void*)kernel);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -76,7 +63,6 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 // same, unconditionally (kernels that do real work before pdl_wait(): the skinny GEMM's weight prefetch)
 template <typename... KArgs, typename... Args>
 inline void launch_pdl_always(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  prefer_shared_once((const void*)kernel);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;

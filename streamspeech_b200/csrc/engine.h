@@ -93,7 +93,10 @@ struct ss_engine {
   int unit_grouped = 1;         // unit decoder layer 1: self-attention over the S distinct rows instead of the 25*S copies
   int umma_min_rows = 128;      // GEMMs with fewer rows stay on the fp32 CUDA-core kernels
   int umma_min_channels = 16;   // convs with fewer input channels stay on the fp32 CUDA-core kernel
-  ss::Umma2Cache* umma2_cache = nullptr;  // packed bf16-split weights of kernels_umma2.cu
+  ss::Umma2Cache* umma2_cache = nullptr;  // packed bf16-split weights of kernels_umma2.cu (created by ss_create)
+  // split-K scratch regions of the GEMMs (ss::splitk_workspace, allocated by the first split into each): region 0 serves every GEMM
+  // on the caller's stream, regions 1 / 2 the vocoder's auxiliary streams
+  float* splitk[3] = {nullptr, nullptr, nullptr};
   int vocoder_streams = 1;     // 1: the parallel resblocks of a vocoder stage run on three streams, 0: one stream
   cudaStream_t aux_stream[2] = {nullptr, nullptr};
   cudaEvent_t fork_event = nullptr, join_event[2] = {nullptr, nullptr};

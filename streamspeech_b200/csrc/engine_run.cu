@@ -19,54 +19,35 @@ int check_launch(ss_engine* h, const char* where) {
   return SS_OK;
 }
 
-// tensor-core routing of the current entry point (set from the handle at the top of each entry point)
-thread_local int g_umma_linear = 0;
-thread_local int g_umma_conv = 0;
-thread_local int g_umma_min_rows = 128;
-thread_local int g_umma_min_channels = 16;
-thread_local Umma2Cache* g_umma2_cache = nullptr;
-// Batched calls that stack g_route_samples samples of equal row counts into one GEMM decide the tensor-core routing from one
-// sample's rows (M / g_route_samples), so that a sample's GEMMs take the same class of kernel (fp32 or wgmma) as in the
-// single-sample call: the batch then reproduces the single-sample rounding instead of adding the split-bf16 error.
-thread_local int g_route_samples = 1;
-struct RouteSamples {  // scope of one such group
-  explicit RouteSamples(int n) { g_route_samples = n; }
-  ~RouteSamples() { g_route_samples = 1; }
-};
-
-void route_from(ss_engine* h) {
-  g_umma_linear = h->umma_linear;
-  g_umma_min_rows = h->umma_min_rows;
-  g_umma_min_channels = h->umma_min_channels;
-  if (!h->umma2_cache) h->umma2_cache = umma2_cache_create();
-  g_umma2_cache = h->umma2_cache;
-}
-
-// conv-as-GEMM dispatch: the wgmma split-bf16 kernel (kernels_umma2.cu; mode 12 / 13 = 2 / 3 bf16 pieces per operand) when enabled and
-// the shape fits, the fp32 CUDA-core kernel otherwise
-void conv_gemm(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaStream_t st) {
+// conv-as-GEMM dispatch of the vocoder: the wgmma split-bf16 kernel (kernels_umma2.cu; umma_vocoder 12 / 13 = 2 / 3 bf16 pieces per
+// operand) when enabled and the shape fits, the fp32 CUDA-core kernel otherwise.  lane: the split-K region of the launching stream.
+void conv_gemm(ss_engine* h, const ConvA& a, const float* W, int N, const Epilogue& ep, int lane, cudaStream_t st) {
   const int rows = a.B * a.L_rows;
-  if (g_umma_conv >= 12 && g_umma2_cache && rows >= g_umma_min_rows && a.C_in >= g_umma_min_channels && umma2_supported(a, N, ep))
-    umma2_conv(g_umma2_cache, a, W, N, ep, g_umma_conv - 10, st);
+  if (h->umma_vocoder >= 12 && rows >= h->umma_min_rows && a.C_in >= h->umma_min_channels && umma2_supported(a, N, ep))
+    umma2_conv(h->umma2_cache, a, W, N, ep, h->umma_vocoder - 10, &h->splitk[lane], st);
   else
-    gemm_conv(a, W, N, ep, st);
+    gemm_conv(a, W, N, ep, &h->splitk[lane], st);
 }
 
-// plain linear: out[M][N] = epilogue(x[M][K] @ W^T)
-void linear(const float* x, int ldx, int M, const Linear& l, Epilogue ep, cudaStream_t st) {
+// plain linear: out[M][N] = epilogue(x[M][K] @ W^T).
+// samples > 1: x stacks that many samples of equal row counts.  The tensor-core routing is decided from one sample's rows
+// (M / samples), so that a sample's GEMMs take the same class of kernel (fp32 or wgmma) as in the single-sample call: the batch
+// then reproduces the single-sample rounding instead of adding the split-bf16 error.
+void linear(ss_engine* h, const float* x, int ldx, int M, const Linear& l, Epilogue ep, cudaStream_t st, int samples = 1) {
   ConvA a;
   a.x = x; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = l.K; a.ldx = ldx;
   ep.bias = l.b;
   if (skinny_gemm_supported(M, l.N, l.K, ep) && (ldx & 3) == 0)
     skinny_gemm(x, ldx, l.w, M, l.N, l.K, ep, st);
-  else if (g_umma_linear >= 12 && g_umma2_cache && M / g_route_samples >= g_umma_min_rows && umma2_supported(a, l.N, ep))
-    umma2_conv(g_umma2_cache, a, l.w, l.N, ep, g_umma_linear - 10, st);
+  else if (h->umma_linear >= 12 && M / samples >= h->umma_min_rows && umma2_supported(a, l.N, ep))
+    umma2_conv(h->umma2_cache, a, l.w, l.N, ep, h->umma_linear - 10, &h->splitk[0], st);
   else
-    gemm_conv(a, l.w, l.N, ep, st);
+    gemm_conv(a, l.w, l.N, ep, &h->splitk[0], st);
 }
 // out = epilogue(LayerNorm(x) @ W^T).  The LN is fused into the skinny kernel's A load when the shape allows it,
 // otherwise it is a separate launch into `scratch` [M][K].
-void ln_linear(const float* x, int ldx, int M, const LNorm& ln, const Linear& l, Epilogue ep, float* scratch, cudaStream_t st) {
+void ln_linear(ss_engine* h, const float* x, int ldx, int M, const LNorm& ln, const Linear& l, Epilogue ep, float* scratch, cudaStream_t st,
+               int samples = 1) {
   ep.bias = l.b;
   Epilogue fused = ep;
   fused.ln_gamma = ln.g;
@@ -76,13 +57,13 @@ void ln_linear(const float* x, int ldx, int M, const LNorm& ln, const Linear& l,
     return;
   }
   layer_norm(x, ldx, scratch, l.K, ln.g, ln.b, M, l.K, st);
-  linear(scratch, l.K, M, l, ep, st);
+  linear(h, scratch, l.K, M, l, ep, st, samples);
 }
 
 // q | k | v = LayerNorm(x) @ Wqkv^T with the three column blocks routed to their own buffers (query scratch, K cache
 // rows, V cache rows).  One launch on the skinny path; LN + three GEMMs otherwise.
-void ln_qkv_routed(const float* x, int ldx, int M, const LNorm& ln, const Linear& qkv, int dim, float* q, int ldq, float* k, int ldk,
-                   float* v, int ldv, float* scratch, cudaStream_t st) {
+void ln_qkv_routed(ss_engine* h, const float* x, int ldx, int M, const LNorm& ln, const Linear& qkv, int dim, float* q, int ldq, float* k, int ldk,
+                   float* v, int ldv, float* scratch, cudaStream_t st, int samples = 1) {
   Epilogue ep;
   ep.out = q; ep.ldo = ldq; ep.out2 = k; ep.ldo2 = ldk; ep.out3 = v; ep.ldo3 = ldv; ep.split_n = dim;
   ep.bias = qkv.b; ep.ln_gamma = ln.g; ep.ln_beta = ln.b;
@@ -100,7 +81,7 @@ void ln_qkv_routed(const float* x, int ldx, int M, const LNorm& ln, const Linear
     part.b = qkv.b + p * dim;
     Epilogue e;
     e.out = outs[p]; e.ldo = lds[p];
-    linear(scratch, qkv.K, M, part, e, st);
+    linear(h, scratch, qkv.K, M, part, e, st, samples);
   }
 }
 
@@ -328,10 +309,9 @@ struct DecScratch {
 // pre-LN transformer layer over x[n][dim] (TransformerDecoderLayerBase.forward / TransformerEncoderLayerBase.forward,
 // ctc_unity/modules/transformer_layer.py:165-230,388-551).  Self-attention keys/values come either from the
 // layer's own fused qkv (full sequence, cache == nullptr) or from an external KV cache that already holds `past` rows.
-// nb > 1 (no cache): x holds nb samples of n / nb rows each; sample b attends to its own rows, cross_kv rows b*Tk .., and the
-// key-length arrays are indexed by sample.
-void dec_layer(const DecLayerW& L, float* x, int n, int dim, int ffn, int heads, bool causal, int self_kv_len_limit,
-               const int* self_kv_len_dev, float* cache_k, float* cache_v, int past, const float* cross_kv, int Tk,
+// nb > 1 (no cache): x holds nb samples of n / nb rows each; sample b attends to its own rows, cross_kv rows b*Tk .., the
+// key-length arrays are indexed by sample, and the GEMMs are routed by one sample's rows (linear's `samples`).
+void dec_layer(ss_engine* h, const DecLayerW& L, float* x, int n, int dim, int ffn, int heads, bool causal, const int* self_kv_len_dev, float* cache_k, float* cache_v, int past, const float* cross_kv, int Tk,
                const int* cross_len_dev, DecScratch& s, cudaStream_t st, int group_R = 0, const int* group_len_dev = nullptr, int nb = 1) {
   const float scale = 0.125f;  // head_dim ** -0.5, head_dim = 64
   const int rows = n / nb;       // per sample
@@ -339,26 +319,25 @@ void dec_layer(const DecLayerW& L, float* x, int n, int dim, int ffn, int heads,
     // rows come in groups of group_R identical consecutive rows (unit decoder layer 1): project the n / group_R distinct
     // rows only and collapse the causal softmax over the copies analytically (grouped_causal_attn_kernel)
     const int S = n / group_R;
-    ln_linear(x, dim * group_R, S, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st);
+    ln_linear(h, x, dim * group_R, S, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st, nb);
     grouped_causal_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, S / nb, group_R, heads, scale,
                              group_len_dev, nb, st);
   } else if (cache_k) {
-    ln_qkv_routed(x, dim, n, L.self_ln, L.qkv, dim, s.q, dim, cache_k + (size_t)past * dim, dim, cache_v + (size_t)past * dim, dim, s.y, st);
+    ln_qkv_routed(h, x, dim, n, L.self_ln, L.qkv, dim, s.q, dim, cache_k + (size_t)past * dim, dim, cache_v + (size_t)past * dim, dim, s.y, st, nb);
     mha_attention(s.q, dim, cache_k, dim, cache_v, dim, s.attn, dim, 1, n, past + n, heads, scale, 1, past, self_kv_len_dev, st);
   } else {
-    ln_linear(x, dim, n, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st);
+    ln_linear(h, x, dim, n, L.self_ln, L.qkv, ep_out(s.qkv, 3 * dim), s.y, st, nb);
     mha_attention(s.qkv, 3 * dim, s.qkv + dim, 3 * dim, s.qkv + 2 * dim, 3 * dim, s.attn, dim, nb, rows, rows, heads, scale,
                   causal ? 1 : 0, 0, self_kv_len_dev, st);
   }
-  (void)self_kv_len_limit;
-  linear(s.attn, dim, n, L.out, ep_residual(x, dim), st);
+  linear(h, s.attn, dim, n, L.out, ep_residual(x, dim), st, nb);
   if (L.has_cross) {
-    ln_linear(x, dim, n, L.cross_ln, L.cq, ep_out(s.q, dim), s.y, st);
+    ln_linear(h, x, dim, n, L.cross_ln, L.cq, ep_out(s.q, dim), s.y, st, nb);
     mha_attention(s.q, dim, cross_kv, 2 * dim, cross_kv + dim, 2 * dim, s.attn, dim, nb, rows, Tk, heads, scale, 0, 0, cross_len_dev, st);
-    linear(s.attn, dim, n, L.cout, ep_residual(x, dim), st);
+    linear(h, s.attn, dim, n, L.cout, ep_residual(x, dim), st, nb);
   }
-  ln_linear(x, dim, n, L.final_ln, L.fc1, ep_out(s.hid, ffn, ACT_RELU), s.y, st);
-  linear(s.hid, ffn, n, L.fc2, ep_residual(x, dim), st);
+  ln_linear(h, x, dim, n, L.final_ln, L.fc1, ep_out(s.hid, ffn, ACT_RELU), s.y, st, nb);
+  linear(h, s.hid, ffn, n, L.fc2, ep_residual(x, dim), st, nb);
 }
 
 // keep_rows > 0: rows [0, keep_rows) of every layer survive a reallocation (incremental-state decoding keeps cross K / V across calls)
@@ -391,7 +370,7 @@ void mt_forward(ss_engine* h, int past, int n, int T, const int* self_kv_len_dev
     float* ck = h->mt_self_k + (size_t)l * c.max_mt_positions * dim;
     float* cv = h->mt_self_v + (size_t)l * c.max_mt_positions * dim;
     const float* cross = h->mt_cross_kv + (size_t)l * h->mt_cross_cap * 2 * dim;
-    dec_layer(h->mt[l], x, n, dim, c.mt_ffn, c.mt_heads, true, 0, self_kv_len_dev, ck, cv, past, cross, T, nullptr, s, st);
+    dec_layer(h, h->mt[l], x, n, dim, c.mt_ffn, c.mt_heads, true, self_kv_len_dev, ck, cv, past, cross, T, nullptr, s, st);
   }
   layer_norm(x, dim, feats, dim, h->mt_ln.g, h->mt_ln.b, n, dim, st);
 }
@@ -405,7 +384,7 @@ void mt_begin(ss_engine* h, const float* enc_dev, int T, cudaStream_t st) {
   if (T > from) {
     for (int l = 0; l < c.mt_layers; ++l) {
       float* cross = h->mt_cross_kv + (size_t)l * h->mt_cross_cap * 2 * c.mt_dim;
-      linear(enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * c.mt_dim, 2 * c.mt_dim), st);
+      linear(h, enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * c.mt_dim, 2 * c.mt_dim), st);
     }
   }
   h->mt_cross_final = std::min(h->mt_stable_hint, T);
@@ -486,7 +465,7 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
   // cross K / V: the same projection call as mt_begin with the sample's own row count (the GEMM routing depends on M)
   for (int b = 0; b < Bg; ++b)
     for (int l = 0; l < c.mt_layers; ++l)
-      linear(enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, c.enc_dim, T_host[g0 + b], h->mt[l].ckv,
+      linear(h, enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, c.enc_dim, T_host[g0 + b], h->mt[l].ckv,
              ep_out(h->mtb_cross_kv + ((size_t)l * R + b) * h->mtb_cross_cap * 2 * dim, 2 * dim), st);
   const size_t floats = (size_t)Bg * (dim * 11 + c.mt_ffn + c.tgt_vocab);
   if (!ws_begin(h, floats * sizeof(float) + (size_t)Bg * ld * sizeof(int64_t) + (size_t)Bg * 2 * sizeof(int) + 16 * 256))
@@ -585,7 +564,6 @@ int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, in
   outp.w = h->unit_emb; outp.b = nullptr; outp.N = c.unit_vocab; outp.K = dim;
   for (int g0 = 0; g0 < B; g0 += G) {
     const int Bg = std::min(G, B - g0);
-    RouteSamples route(Bg);
     const int n = Bg * Slen, rows = Bg * L;
     const int* s_len = padded ? lens_dev + g0 : nullptr;       // T2U key lengths, unit cross-attention key lengths, valid groups of layer 1
     const int* up_len = padded ? lens_dev + B + g0 : nullptr;  // unit self-attention key lengths
@@ -593,19 +571,19 @@ int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, in
     // ---- T1: UniTransformerEncoderNoEmb.forward on the group's samples
     copy_f32(mt_feats_dev + (size_t)g0 * Slen * dim, x, (int64_t)n * dim, st);
     for (int l = 0; l < c.t2u_layers; ++l)
-      dec_layer(h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, 0, s_len, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st, 0,
+      dec_layer(h, h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, s_len, nullptr, nullptr, 0, nullptr, 0, nullptr, s1, st, 0,
                 nullptr, Bg);
     layer_norm(x, dim, t2u, dim, h->t2u_ln.g, h->t2u_ln.b, n, dim, st);
     // ---- U1: CTCTransformerUnitDecoder: x R upsample + (quirky) positional row of each sample (N1), 2 layers, out-proj
     repeat_rows_add(t2u, Slen, R, dim, pos_rows_dev + (size_t)g0 * dim, xu, Bg, st);
     for (int l = 0; l < c.unit_layers; ++l) {
-      linear(t2u, dim, n, h->unit[l].ckv, ep_out(ckv, 2 * dim), st);
+      linear(h, t2u, dim, n, h->unit[l].ckv, ep_out(ckv, 2 * dim), st, Bg);
       // layer 0 sees R identical copies of every T2U state (same positional row for every step, N1): grouped self-attention
       const int gR = (l == 0 && h->unit_grouped) ? R : 0;
-      dec_layer(h->unit[l], xu, rows, dim, c.unit_ffn, c.unit_heads, true, 0, up_len, nullptr, nullptr, 0, ckv, Slen, s_len, s2, st, gR, s_len, Bg);
+      dec_layer(h, h->unit[l], xu, rows, dim, c.unit_ffn, c.unit_heads, true, up_len, nullptr, nullptr, 0, ckv, Slen, s_len, s2, st, gR, s_len, Bg);
     }
     layer_norm(xu, dim, xu, dim, h->unit_ln.g, h->unit_ln.b, rows, dim, st);
-    linear(xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st);
+    linear(h, xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st, Bg);
     // ---- U2: never select pad, unk (agent version) [+ eos: offline version], then each sample's collapse
     int64_t* am = argmax_dev + (size_t)g0 * L;
     argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, st);
@@ -671,7 +649,6 @@ int ss_resample_48k_to_16k(ss_engine* h, void* stream, const float* in_dev, int6
 }
 
 int ss_encoder_forward(ss_engine* h, void* stream, const float* feats_dev, const int32_t* lengths_host, int B, int F, float* out_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (B <= 0 || F <= 0) return h->fail(SS_ERR_INVALID, "empty encoder input");
   const ss_config& c = h->cfg;
@@ -727,40 +704,40 @@ int ss_encoder_forward(ss_engine* h, void* stream, const float* feats_dev, const
     a.ksize = c.conv_kernel; a.stride = 2; a.pad_left = c.conv_kernel / 2; a.chunk = cc;
     Epilogue ep = ep_out(c1, c.conv_channels / 2);
     ep.bias = h->sub_conv[0].b; ep.glu = 1;
-    gemm_conv(a, h->sub_conv[0].w, h->sub_conv[0].N, ep, st);
+    gemm_conv(a, h->sub_conv[0].w, h->sub_conv[0].N, ep, &h->splitk[0], st);
     ConvA a2;
     a2.x = c1; a2.B = B; a2.L_in = T1; a2.L_rows = T; a2.C_in = c.conv_channels / 2; a2.ldx = c.conv_channels / 2;
     a2.ksize = c.conv_kernel; a2.stride = 2; a2.pad_left = c.conv_kernel / 2; a2.chunk = cc;
     Epilogue ep2 = ep_out(x0, D);
     ep2.bias = h->sub_conv[1].b; ep2.glu = 1; ep2.alpha = sqrtf((float)D);  // x = embed_scale * x (s2t_conformer.py:127)
-    gemm_conv(a2, h->sub_conv[1].w, h->sub_conv[1].N, ep2, st);
+    gemm_conv(a2, h->sub_conv[1].w, h->sub_conv[1].N, ep2, &h->splitk[0], st);
   }
-  linear(x0, D, (int)rows, h->enc_linear, ep_out(x, D), st);  // s2t_conformer.py:139
+  linear(h, x0, D, (int)rows, h->enc_linear, ep_out(x, D), st);  // s2t_conformer.py:139
   for (int i = 0; i < c.enc_layers; ++i) {
     const ConformerLayerW& L = h->enc[i];
     // x = x + 0.5 * ffn1(x)
     layer_norm(x, D, y, D, L.ffn1_ln.g, L.ffn1_ln.b, (int)rows, D, st);
-    linear(y, D, (int)rows, L.ffn1_w1, ep_out(hid, c.enc_ffn, ACT_SILU), st);
-    linear(hid, c.enc_ffn, (int)rows, L.ffn1_w2, ep_residual(x, D, 0.5f), st);
+    linear(h, y, D, (int)rows, L.ffn1_w1, ep_out(hid, c.enc_ffn, ACT_SILU), st);
+    linear(h, hid, c.enc_ffn, (int)rows, L.ffn1_w2, ep_residual(x, D, 0.5f), st);
     // x = x + self_attn(LN(x))
     layer_norm(x, D, y, D, L.attn_ln.g, L.attn_ln.b, (int)rows, D, st);
-    linear(y, D, (int)rows, L.qkv, ep_out(qkv, 3 * D), st);
+    linear(h, y, D, (int)rows, L.qkv, ep_out(qkv, 3 * D), st);
     relpos_attention(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, L.pos_proj, h->Tpos, L.pos_u, L.pos_v, att, B, T, 0, T, c.enc_heads, D,
                      h->attn_chunk, len_dev, st);
-    linear(att, D, (int)rows, L.attn_out, ep_residual(x, D), st);
+    linear(h, att, D, (int)rows, L.attn_out, ep_residual(x, D), st);
     // x = x + conv_module(x)
     layer_norm(x, D, y, D, L.conv_ln.g, L.conv_ln.b, (int)rows, D, st);
     {
       Epilogue ep = ep_out(glu, D);
       ep.glu = 1;
-      linear(y, D, (int)rows, L.pw1, ep, st);
+      linear(h, y, D, (int)rows, L.pw1, ep, st);
     }
     depthwise_bn_silu(glu, D, L.dw_w, L.bn_scale, L.bn_shift, dw, D, B, T, 0, T, D, c.dw_kernel, cc, st);
-    linear(dw, D, (int)rows, L.pw2, ep_residual(x, D), st);
+    linear(h, dw, D, (int)rows, L.pw2, ep_residual(x, D), st);
     // x = LN(x + 0.5 * ffn2(x))
     layer_norm(x, D, y, D, L.ffn2_ln.g, L.ffn2_ln.b, (int)rows, D, st);
-    linear(y, D, (int)rows, L.ffn2_w1, ep_out(hid, c.enc_ffn, ACT_SILU), st);
-    linear(hid, c.enc_ffn, (int)rows, L.ffn2_w2, ep_residual(x, D, 0.5f), st);
+    linear(h, y, D, (int)rows, L.ffn2_w1, ep_out(hid, c.enc_ffn, ACT_SILU), st);
+    linear(h, hid, c.enc_ffn, (int)rows, L.ffn2_w2, ep_residual(x, D, 0.5f), st);
     layer_norm(x, D, x, D, L.final_ln.g, L.final_ln.b, (int)rows, D, st);
   }
   return check_launch(h, "ss_encoder_forward");
@@ -781,7 +758,6 @@ int ss_mt_stable_rows(ss_engine* h, int rows) {
 }
 
 int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, int F, float* enc_out_dev, int32_t* T_out, int32_t* T_final_out) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (h->attn_chunk <= 0 || h->conv_chunk <= 0) return h->fail(SS_ERR_STATE, "streaming encoder needs a chunked model (ss_set_chunk)");
   const ss_config& c = h->cfg;
@@ -827,16 +803,16 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
       a.ksize = c.conv_kernel; a.stride = 2; a.pad_left = c.conv_kernel / 2; a.chunk = cc; a.t_offset = t1_lo;
       Epilogue ep = ep_out(c1, c.conv_channels / 2);
       ep.bias = h->sub_conv[0].b; ep.glu = 1;
-      gemm_conv(a, h->sub_conv[0].w, h->sub_conv[0].N, ep, st);
+      gemm_conv(a, h->sub_conv[0].w, h->sub_conv[0].N, ep, &h->splitk[0], st);
       ConvA a2;
       a2.x = c1; a2.B = 1; a2.L_in = T1; a2.L_rows = nA; a2.C_in = c.conv_channels / 2; a2.ldx = c.conv_channels / 2;
       a2.ksize = c.conv_kernel; a2.stride = 2; a2.pad_left = c.conv_kernel / 2; a2.chunk = cc;
       a2.t_offset = a0; a2.x_row0 = t1_lo; a2.x_rows = n1;
       Epilogue ep2 = ep_out(x0, D);
       ep2.bias = h->sub_conv[1].b; ep2.glu = 1; ep2.alpha = sqrtf((float)D);
-      gemm_conv(a2, h->sub_conv[1].w, h->sub_conv[1].N, ep2, st);
+      gemm_conv(a2, h->sub_conv[1].w, h->sub_conv[1].N, ep2, &h->splitk[0], st);
     }
-    linear(x0, D, nA, h->enc_linear, ep_out(x, D), st);
+    linear(h, x0, D, nA, h->enc_linear, ep_out(x, D), st);
     bool persistent = h->persistent_encoder && encoder_layers_persistent_supported(nA, D, c.enc_ffn, c.enc_heads, T, c.dw_kernel);
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     if (persistent && h->persistent_time) {  // bench: CUDA events on the launching stream around the dominant kernel
@@ -874,21 +850,21 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
       float* kc = h->st_k + (size_t)i * h->Tpos * D;
       float* vc = h->st_v + (size_t)i * h->Tpos * D;
       float* gc = h->st_glu + (size_t)i * h->Tpos * D;
-      ln_linear(x, D, nA, L.ffn1_ln, L.ffn1_w1, ep_out(hid, c.enc_ffn, ACT_SILU), y, st);
-      linear(hid, c.enc_ffn, nA, L.ffn1_w2, ep_residual(x, D, 0.5f), st);
+      ln_linear(h, x, D, nA, L.ffn1_ln, L.ffn1_w1, ep_out(hid, c.enc_ffn, ACT_SILU), y, st);
+      linear(h, hid, c.enc_ffn, nA, L.ffn1_w2, ep_residual(x, D, 0.5f), st);
       // q -> scratch, k / v -> cache rows a0.. (provisional tail rows are overwritten next call)
-      ln_qkv_routed(x, D, nA, L.attn_ln, L.qkv, D, qb, D, kc + (size_t)a0 * D, D, vc + (size_t)a0 * D, D, y, st);
+      ln_qkv_routed(h, x, D, nA, L.attn_ln, L.qkv, D, qb, D, kc + (size_t)a0 * D, D, vc + (size_t)a0 * D, D, y, st);
       relpos_attention(qb, D, kc, D, vc, D, L.pos_proj, h->Tpos, L.pos_u, L.pos_v, att, 1, nA, a0, T, c.enc_heads, D, h->attn_chunk, nullptr, st);
-      linear(att, D, nA, L.attn_out, ep_residual(x, D), st);
+      linear(h, att, D, nA, L.attn_out, ep_residual(x, D), st);
       {
         Epilogue ep = ep_out(gc + (size_t)a0 * D, D);
         ep.glu = 1;
-        ln_linear(x, D, nA, L.conv_ln, L.pw1, ep, y, st);
+        ln_linear(h, x, D, nA, L.conv_ln, L.pw1, ep, y, st);
       }
       depthwise_bn_silu(gc, D, L.dw_w, L.bn_scale, L.bn_shift, dw, D, 1, T, a0, nA, D, c.dw_kernel, cc, st);
-      linear(dw, D, nA, L.pw2, ep_residual(x, D), st);
-      ln_linear(x, D, nA, L.ffn2_ln, L.ffn2_w1, ep_out(hid, c.enc_ffn, ACT_SILU), y, st);
-      linear(hid, c.enc_ffn, nA, L.ffn2_w2, ep_residual(x, D, 0.5f), st);
+      linear(h, dw, D, nA, L.pw2, ep_residual(x, D), st);
+      ln_linear(h, x, D, nA, L.ffn2_ln, L.ffn2_w1, ep_out(hid, c.enc_ffn, ACT_SILU), y, st);
+      linear(h, hid, c.enc_ffn, nA, L.ffn2_w2, ep_residual(x, D, 0.5f), st);
       layer_norm(x, D, x, D, L.final_ln.g, L.final_ln.b, nA, D, st);
     }
   }
@@ -899,7 +875,6 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
 
 int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_dev, int rows, int row0, int64_t* argmax_dev,
                        int64_t* tokens_dev, int32_t* index_dev, int32_t* count_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (head < 0 || head > 1 || rows <= 0 || row0 < 0 || row0 > rows) return h->fail(SS_ERR_INVALID, "bad ctc head / rows");
   const Linear& l = h->ctc_head[head];
@@ -908,7 +883,7 @@ int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_de
   if (nr > 0) {
     if (!ws_begin(h, (size_t)nr * l.N * sizeof(float) + 4096)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
     float* logits = h->ws.f32((size_t)nr * l.N);
-    linear(enc_dev + (size_t)row0 * h->cfg.enc_dim, h->cfg.enc_dim, nr, l, ep_out(logits, l.N), st);
+    linear(h, enc_dev + (size_t)row0 * h->cfg.enc_dim, h->cfg.enc_dim, nr, l, ep_out(logits, l.N), st);
     argmax_rows(logits, l.N, nr, l.N, h->mask_pad_unk, 2, argmax_dev + row0, st);  // never select pad, unk
   }
   // <s> is the CTC blank (agent/ctc_decoder.py:72-76)
@@ -918,7 +893,6 @@ int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_de
 
 int ss_ctc_greedy_pair(ss_engine* h, void* stream, const float* enc_dev, int rows, int row0, int64_t* argmax0_dev, int64_t* argmax1_dev,
                        int64_t* packed_out_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (rows <= 0 || row0 < 0 || row0 > rows) return h->fail(SS_ERR_INVALID, "bad ctc rows");
   cudaStream_t st = S(stream);
@@ -938,7 +912,7 @@ int ss_ctc_greedy_pair(ss_engine* h, void* stream, const float* enc_dev, int row
   if (nr > 0) {
     if (!ws_begin(h, (size_t)nr * 2 * V * sizeof(float) + 4096)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
     logits = h->ws.f32((size_t)nr * 2 * V);
-    linear(enc_dev + (size_t)row0 * h->cfg.enc_dim, h->cfg.enc_dim, nr, h->ctc_pair, ep_out(logits, 2 * V), st);
+    linear(h, enc_dev + (size_t)row0 * h->cfg.enc_dim, h->cfg.enc_dim, nr, h->ctc_pair, ep_out(logits, 2 * V), st);
   }
   ctc_argmax_collapse_pair(logits, 2 * V, V, nr, row0, rows, h->mask_pad_unk, 2, 0 /* <s> = CTC blank */, h->cfg.pad, argmax0_dev, argmax1_dev,
                            packed_out_dev, W, h->ctc_ticket, st);
@@ -952,7 +926,6 @@ int ss_ctc_greedy(ss_engine* h, void* stream, int head, const float* enc_dev, in
 
 int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* tokens_host, int n, float* feats_out_dev,
                    float* logits_last_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (n <= 0 || n > c.max_mt_positions || T <= 0) return h->fail(SS_ERR_INVALID, "bad MT sequence length");
@@ -979,14 +952,13 @@ int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, cons
   if (logits_last_dev) {
     Linear out;
     out.w = h->mt_emb; out.b = nullptr; out.N = c.tgt_vocab; out.K = dim;
-    linear(feats_out_dev + (size_t)(n - 1) * dim, dim, 1, out, ep_out(logits_last_dev, c.tgt_vocab), st);
+    linear(h, feats_out_dev + (size_t)(n - 1) * dim, dim, 1, out, ep_out(logits_last_dev, c.tgt_vocab), st);
   }
   return check_launch(h, "ss_mt_features");
 }
 
 int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* prefix_host, int n_prefix, int max_new_tokens,
                  int max_len_b, int64_t* tokens_out_host, int max_out, int* n_out, float* feats_out_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   cudaStream_t st = S(stream);
@@ -1069,7 +1041,7 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
         ++step;
         break;
       }
-      linear(feats_out_dev + (size_t)step * dim, dim, 1, outp, ep_out(logits, c.tgt_vocab), st);
+      linear(h, feats_out_dev + (size_t)step * dim, dim, 1, outp, ep_out(logits, c.tgt_vocab), st);
       // lprobs[pad] = -inf; eos banned while step < min_len (=1)
       if (step < 1)
         argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_eos, 2, h->mt_tok_dev + step + 1, st);
@@ -1101,7 +1073,6 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
 
 int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int max_len_b,
                        int64_t* tokens_out_host, int max_out, int32_t* n_out_host) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (B <= 0 || T_stride <= 0 || !enc_dev || !T_host || !tokens_out_host || !n_out_host)
@@ -1198,7 +1169,6 @@ int ss_mt_incremental_reset(ss_engine* h) {
 
 int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* prefix_host, int n_prefix,
                              int max_new_tokens, int max_len_b, int64_t* tokens_out_host, int max_out, int* n_out) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   cudaStream_t st = S(stream);
@@ -1234,7 +1204,7 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
     const int from = h->mt_inc_cross_rows;
     for (int l = 0; l < c.mt_layers; ++l) {
       float* cross = h->mt_cross_kv + (size_t)l * h->mt_cross_cap * 2 * dim;
-      linear(enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * dim, 2 * dim), st);
+      linear(h, enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * dim, 2 * dim), st);
     }
     h->mt_inc_cross_rows = T;
   }
@@ -1256,7 +1226,6 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
 
 int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, int Slen, int n_pad_tail, int mask_eos, int64_t* argmax_dev,
                        int64_t* units_dev, int32_t* count_dev, float* t2u_out_dev, float* logits_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (Slen <= 0 || n_pad_tail < 0 || n_pad_tail >= Slen) return h->fail(SS_ERR_INVALID, "bad T2U sequence length");
   const int32_t np = n_pad_tail;
@@ -1273,7 +1242,6 @@ int ss_unit_position_row(ss_engine* h, const float* row_host) {
 }
 
 int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T, int64_t* packed_out_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   if (B <= 0 || T <= 0 || !enc_dev || !packed_out_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_ctc_greedy_batch");
   const ss_config& c = h->cfg;
@@ -1284,7 +1252,6 @@ int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B,
   const int G = std::max(1, SS_CTC_BATCH_ROWS / T);
   for (int g0 = 0; g0 < B; g0 += G) {
     const int Bg = std::min(G, B - g0);
-    RouteSamples route(Bg);
     const int rows = Bg * T;
     if (!ws_begin(h, (size_t)rows * 2 * Vmax * sizeof(float) + (size_t)rows * 2 * sizeof(int64_t) + 4 * 256))
       return h->fail(SS_ERR_CUDA, "workspace allocation failed");
@@ -1295,14 +1262,14 @@ int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B,
     int64_t* out = packed_out_dev + (size_t)g0 * 2 * W;
     if (pair) {
       // [rows][2V] logits = 2 * rows arg-max rows of V (head-minor); sequence s = 2 b + head is sample b's head, at out + s * W
-      linear(x, c.enc_dim, rows, h->ctc_pair, ep_out(logits, 2 * c.src_vocab), st);
+      linear(h, x, c.enc_dim, rows, h->ctc_pair, ep_out(logits, 2 * c.src_vocab), st, Bg);
       argmax_rows(logits, c.src_vocab, 2 * rows, c.src_vocab, h->mask_pad_unk, 2, am, st);  // never select pad, unk
       ctc_collapse_segments(am, T, 2, 2 * Bg, 0 /* <s> = CTC blank */, c.pad, out + 1, reinterpret_cast<int*>(out + 1 + T),
                             reinterpret_cast<int*>(out), W, st);
     } else {
       for (int hd = 0; hd < 2; ++hd) {
         const Linear& l = h->ctc_head[hd];
-        linear(x, c.enc_dim, rows, l, ep_out(logits, l.N), st);
+        linear(h, x, c.enc_dim, rows, l, ep_out(logits, l.N), st, Bg);
         argmax_rows(logits, l.N, rows, l.N, h->mask_pad_unk, 2, am, st);
         int64_t* o = out + hd * W;
         ctc_collapse_segments(am, T, 1, Bg, 0, c.pad, o + 1, reinterpret_cast<int*>(o + 1 + T), reinterpret_cast<int*>(o), 2 * W, st);
@@ -1314,7 +1281,6 @@ int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B,
 
 int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, const int64_t* tokens_host,
                          int Slen, float* feats_out_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (B <= 0 || T_stride <= 0 || Slen <= 0 || Slen > c.max_mt_positions || !enc_dev || !T_host || !tokens_host || !feats_out_dev)
@@ -1361,14 +1327,13 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
   const int* cross_len_dev = self_len_dev + B;
   for (int g0 = 0; g0 < B; g0 += G) {
     const int Bg = std::min(G, B - g0);
-    RouteSamples route(Bg);
     const int n = Bg * Slen;
     embed_tokens_pos(tok_dev + (size_t)g0 * Slen, pos_dev + (size_t)g0 * Slen, 0, h->mt_emb, h->mt_pos, sqrtf((float)dim), x, n, dim, c.pad, st);
     for (int l = 0; l < c.mt_layers; ++l) {
       // this layer's cross K / V of every row of the group's samples (rows past T_b are masked by cross_len)
-      linear(enc_dev + (size_t)g0 * T_stride * c.enc_dim, c.enc_dim, Bg * T_stride, h->mt[l].ckv, ep_out(ckv, 2 * dim), st);
-      dec_layer(h->mt[l], x, n, dim, c.mt_ffn, c.mt_heads, true, 0, self_len_dev + g0, nullptr, nullptr, 0, ckv, T_stride, cross_len_dev + g0, s, st,
-                0, nullptr, Bg);
+      linear(h, enc_dev + (size_t)g0 * T_stride * c.enc_dim, c.enc_dim, Bg * T_stride, h->mt[l].ckv, ep_out(ckv, 2 * dim), st, Bg);
+      dec_layer(h, h->mt[l], x, n, dim, c.mt_ffn, c.mt_heads, true, self_len_dev + g0, nullptr, nullptr, 0, ckv, T_stride, cross_len_dev + g0, s, st, 0,
+                nullptr, Bg);
     }
     layer_norm(x, dim, feats_out_dev + (size_t)g0 * Slen * dim, dim, h->mt_ln.g, h->mt_ln.b, n, dim, st);
   }
@@ -1377,7 +1342,6 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
 
 int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
                               const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
-  if (h) route_from(h);
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (B <= 0 || S_stride <= 0 || S_stride > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev ||
@@ -1407,7 +1371,7 @@ static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* fra
     a.x = frames; a.B = 1; a.L_in = N; a.L_rows = N; a.C_in = c.voc_in_dim; a.ldx = c.voc_in_dim; a.ksize = 7; a.pad_left = 3;
     Epilogue e = ep_out(bufX, c.voc_init_channels);
     e.bias = h->conv_pre.lin.b;
-    conv_gemm(a, h->conv_pre.lin.w, c.voc_init_channels, e, st);
+    conv_gemm(h, a, h->conv_pre.lin.w, c.voc_init_channels, e, 0, st);
   }
   int L = N, ch = c.voc_init_channels;
   for (int i = 0; i < c.voc_n_ups; ++i) {
@@ -1427,16 +1391,14 @@ static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* fra
       if (nrows <= 0) continue;
       const int lane = fan_up ? phi % 3 : 0;
       cudaStream_t sp = lane > 0 ? h->aux_stream[lane - 1] : st;
-      set_splitk_slot(lane);
       ConvA a;
       a.x = bufX; a.B = 1; a.L_in = L; a.L_rows = nrows; a.C_in = U.cin; a.ldx = U.cin; a.ksize = J; a.pad_left = (J - 1) - q0;
       a.pre_lrelu = 0.1f;
       Epilogue e = ep_out(bufY, U.cout);
       e.bias = U.bias;
       e.out_L = Lout; e.out_row_stride = U.u; e.out_row_offset = q0 * U.u + phi - U.pad;
-      conv_gemm(a, U.phase_w[phi].w, U.cout, e, sp);
+      conv_gemm(h, a, U.phase_w[phi].w, U.cout, e, lane, sp);
     }
-    set_splitk_slot(0);
     if (fan_up)
       for (int q = 0; q < 2; ++q) {
         cudaEventRecord(h->join_event[q], h->aux_stream[q]);
@@ -1450,8 +1412,8 @@ static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* fra
       for (int q = 0; q < 2; ++q) cudaStreamWaitEvent(h->aux_stream[q], h->fork_event, 0);
     }
     for (int j = 0; j < nrb; ++j) {
-      cudaStream_t sj = (fan_out && j > 0) ? h->aux_stream[j - 1] : st;
-      set_splitk_slot(fan_out ? j : 0);
+      const int lane = fan_out ? j : 0;
+      cudaStream_t sj = lane > 0 ? h->aux_stream[lane - 1] : st;
       const float* cur = bufY;
       float* pingpong[2] = {rbA[j], rbB[j]};
       int nd = c.voc_rb_ndil;
@@ -1463,7 +1425,7 @@ static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* fra
         a1.pad_left = (w1.ksize * w1.dil - w1.dil) / 2; a1.pre_lrelu = 0.1f;
         Epilogue e1 = ep_out(rbT[j], ch);
         e1.bias = w1.lin.b;
-        conv_gemm(a1, w1.lin.w, ch, e1, sj);
+        conv_gemm(h, a1, w1.lin.w, ch, e1, lane, sj);
         ConvA a2;
         a2.x = rbT[j]; a2.B = 1; a2.L_in = L; a2.L_rows = L; a2.C_in = ch; a2.ldx = ch; a2.ksize = w2.ksize; a2.dil = 1;
         a2.pad_left = (w2.ksize - 1) / 2; a2.pre_lrelu = 0.1f;
@@ -1481,12 +1443,11 @@ static void vocoder_multi_launch(ss_engine* h, cudaStream_t st, const float* fra
           e2.res_scale = 1.0f / nrb;
           e2.accumulate = nrb != 3 && j > 0;  // (other block counts: accumulate in place, single stream)
         }
-        conv_gemm(a2, w2.lin.w, ch, e2, sj);
+        conv_gemm(h, a2, w2.lin.w, ch, e2, lane, sj);
         cur = e2.out;
       }
-      if (fan_out && j > 0) cudaEventRecord(h->join_event[j - 1], sj);
+      if (lane > 0) cudaEventRecord(h->join_event[lane - 1], sj);
     }
-    set_splitk_slot(0);
     if (fan_out)
       for (int q = 0; q < 2; ++q) cudaStreamWaitEvent(st, h->join_event[q], 0);
     // stage output in the reference's summation order: block 0, then + block 1, then + block 2
@@ -1581,7 +1542,7 @@ int ss_vocoder_durations_ragged(ss_engine* h, void* stream, int n, const int64_t
       c1.ksize = h->dur_conv1.ksize; c1.pad_left = (h->dur_conv1.ksize - 1) / 2; c1.k_tiles_per_split = kVocDurTilesPerSplit;
       Epilogue e1 = ep_out(a, Hd, ACT_RELU);
       e1.bias = h->dur_conv1.lin.b;
-      gemm_conv(c1, h->dur_conv1.lin.w, Hd, e1, st);
+      gemm_conv(c1, h->dur_conv1.lin.w, Hd, e1, &h->splitk[0], st);
       layer_norm(a, Hd, a, Hd, h->dur_ln1.g, h->dur_ln1.b, M, Hd, st);
       if (g.count > 1) zero_pad_rows(a, q, g.Umax, Hd, st);
       ConvA c2;
@@ -1590,13 +1551,13 @@ int ss_vocoder_durations_ragged(ss_engine* h, void* stream, int n, const int64_t
       c2.k_tiles_per_split = kVocDurTilesPerSplit;
       Epilogue e2 = ep_out(b, Hd, ACT_RELU);
       e2.bias = h->dur_conv2.lin.b;
-      gemm_conv(c2, h->dur_conv2.lin.w, Hd, e2, st);
+      gemm_conv(c2, h->dur_conv2.lin.w, Hd, e2, &h->splitk[0], st);
       layer_norm(b, Hd, b, Hd, h->dur_ln2.g, h->dur_ln2.b, M, Hd, st);
       ConvA pr;
       pr.x = b; pr.L_in = M; pr.L_rows = M; pr.C_in = Hd; pr.ldx = Hd; pr.k_tiles_per_split = kVocDurTilesPerSplit;
       Epilogue e3 = ep_out(ld, 1);
       e3.bias = h->dur_proj.b;
-      gemm_conv(pr, h->dur_proj.w, 1, e3, st);
+      gemm_conv(pr, h->dur_proj.w, 1, e3, &h->splitk[0], st);
     }
     // no duration prediction: every code is one frame
     duration_from_log_ragged(dur_prediction ? ld : nullptr, q, dur_out_dev + packed, h->voc_cumsum + packed + g.s0, st);
@@ -1625,8 +1586,6 @@ int ss_vocoder_generate_ragged(ss_engine* h, void* stream, int n, const int32_t*
       return h->fail(SS_ERR_INVALID, "vocoder frame range must be the tail of the sequence");
   const ss_config& c = h->cfg;
   cudaStream_t st = S(stream);
-  route_from(h);
-  g_umma_conv = h->umma_vocoder;
   const int nrb = c.voc_n_rb;
   std::vector<int> ctx(n), N(n), dst(n);
   int n_out = 0;
@@ -1677,7 +1636,7 @@ int ss_vocoder_generate_ragged(ss_engine* h, void* stream, int n, const int32_t*
   if (!ok || !wav) return h->fail(SS_ERR_CUDA, "workspace too small");
   // The resblocks of a stage are independent until their outputs are averaged (hifigan.py:158-165).  Each one is a chain of
   // small latency-bound convs, so the multi-launch path runs them on separate streams (block 0 on the caller's) and they overlap.
-  const bool fan_out = h->vocoder_streams && nrb == 3 && (g_umma_conv == 0 || g_umma_conv >= 12);
+  const bool fan_out = h->vocoder_streams && nrb == 3 && (h->umma_vocoder == 0 || h->umma_vocoder >= 12);
   if (fan_out && !h->fork_event) {
     bool made = cudaEventCreateWithFlags(&h->fork_event, cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; i < 2 && made; ++i)
@@ -1685,7 +1644,7 @@ int ss_vocoder_generate_ragged(ss_engine* h, void* stream, int n, const int32_t*
              cudaEventCreateWithFlags(&h->join_event[i], cudaEventDisableTiming) == cudaSuccess;
     if (!made) return h->fail(SS_ERR_CUDA, "cannot create the vocoder's auxiliary streams");
   }
-  const bool fused_on = h->vocoder_fused != 0 && g_umma_conv == 12 && nrb == 3;
+  const bool fused_on = h->vocoder_fused != 0 && h->umma_vocoder == 12 && nrb == 3;
   for (size_t g = 0; g + 1 < g_first.size(); ++g) {
     const int s0 = g_first[g], s1 = g_first[g + 1];
     // V1 tail: repeat_interleave(x, dur) for each sequence's frame window (agent/tts/codehifigan.py:66), one launch
@@ -1733,20 +1692,18 @@ int ss_set_option(ss_engine* h, const char* name, int value) {
     umma2_cache_clear(h->umma2_cache);
     clear_voc_fused(h);
   }
-  else if (n == "umma2_split_below") { g_umma2_split_below = value; clear_voc_fused(h); }
-  else if (n == "umma2_min_units") { g_umma2_min_units = value; clear_voc_fused(h); }
   else if (n == "umma2_debug") {
-    if (value && !g_umma2_dbg) {
-      if (cudaMalloc(&g_umma2_dbg, 16 * sizeof(unsigned long long)) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");
-      cudaMemset(g_umma2_dbg, 0, 16 * sizeof(unsigned long long));
+    unsigned long long*& dbg = h->umma2_cache->dbg;
+    if (value && !dbg) {
+      if (cudaMalloc(&dbg, 16 * sizeof(unsigned long long)) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMalloc failed");
+      cudaMemset(dbg, 0, 16 * sizeof(unsigned long long));
     }
-    if (!value && g_umma2_dbg) {
+    if (!value && dbg) {
       cudaDeviceSynchronize();
-      cudaFree(g_umma2_dbg);
-      g_umma2_dbg = nullptr;
+      cudaFree(dbg);
+      dbg = nullptr;
     }
   }
-  else if (n == "prefer_shared") g_prefer_shared = value;  // takes effect for kernels that have not been launched yet
   else if (n == "unit_grouped") h->unit_grouped = value;
   else if (n == "vocoder_fused") h->vocoder_fused = value;
   else if (n == "fbank_tma") h->fbank_tma = value;
@@ -1790,8 +1747,9 @@ int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes) 
     return SS_OK;
   }
   if (n == "umma2_ts") {
-    if (!g_umma2_dbg || bytes > 16 * sizeof(unsigned long long)) return h->fail(SS_ERR_STATE, "no stamps (set option umma2_debug)");
-    if (cudaMemcpy(host_dst, g_umma2_dbg, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMemcpy failed");
+    const unsigned long long* dbg = h->umma2_cache->dbg;
+    if (!dbg || bytes > 16 * sizeof(unsigned long long)) return h->fail(SS_ERR_STATE, "no stamps (set option umma2_debug)");
+    if (cudaMemcpy(host_dst, dbg, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return h->fail(SS_ERR_CUDA, "cudaMemcpy failed");
     return SS_OK;
   }
   if (n == "cluster_steps") {  // long long: encoder steps taken by the cluster kernel so far
@@ -1846,21 +1804,19 @@ int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes) 
 int ss_op_linear_umma(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N, int act,
                       int pieces, float* out_dev) {
   if (!h) return SS_ERR_INVALID;
-  route_from(h);
   if (pieces != 2 && pieces != 3) return h->fail(SS_ERR_INVALID, "pieces must be 2 (bf16x3) or 3 (bf16x6)");
   ConvA a;
   a.x = x_dev; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = K; a.ldx = K;
   Epilogue ep = ep_out(out_dev, N, act);
   ep.bias = bias_dev;
   if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the wgmma kernel");
-  umma2_conv(h->umma2_cache, a, w_dev, N, ep, pieces, S(stream));
+  umma2_conv(h->umma2_cache, a, w_dev, N, ep, pieces, &h->splitk[0], S(stream));
   return check_launch(h, "ss_op_linear_umma");
 }
 
 int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in, const float* w_dev, const float* bias_dev, int N, int ksize,
                  int dil, int pad_left, float pre_lrelu, int mode, float* out_dev) {
   if (!h) return SS_ERR_INVALID;
-  route_from(h);
   ConvA a;
   a.x = x_dev; a.B = 1; a.L_in = L; a.L_rows = L; a.C_in = C_in; a.ldx = C_in; a.ksize = ksize; a.dil = dil; a.pad_left = pad_left;
   a.pre_lrelu = pre_lrelu;
@@ -1868,11 +1824,11 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
   ep.bias = bias_dev;
   if (mode >= 12) {
     if (!umma2_supported(a, N, ep)) return h->fail(SS_ERR_INVALID, "shape not supported by the wgmma conv kernel");
-    umma2_conv(h->umma2_cache, a, w_dev, N, ep, mode - 10, S(stream));
+    umma2_conv(h->umma2_cache, a, w_dev, N, ep, mode - 10, &h->splitk[0], S(stream));
   } else if (mode >= 2) {
     return h->fail(SS_ERR_INVALID, "modes 2 / 3 (first-generation tensor-core kernel) were removed: use 12 / 13");
   } else {
-    gemm_conv(a, w_dev, N, ep, S(stream));
+    gemm_conv(a, w_dev, N, ep, &h->splitk[0], S(stream));
   }
   return check_launch(h, "ss_op_conv1d");
 }
@@ -1880,12 +1836,16 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
 int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, const float* w_dev, const float* bias_dev, int N, int act,
                  float* out_dev) {
   if (!h) return SS_ERR_INVALID;
-  // the plain linear (skinny / fp32 CUDA-core kernels; ss_op_linear_umma is the wgmma hook), whatever routing the last entry point
-  // of any handle left on this thread: that handle, and the weight cache the routing points to, may have been destroyed since
-  g_umma_linear = 0;
-  Linear l;
-  l.w = const_cast<float*>(w_dev); l.b = const_cast<float*>(bias_dev); l.N = N; l.K = K;
-  linear(x_dev, K, M, l, ep_out(out_dev, N, act), S(stream));
+  // the plain linear: skinny / fp32 CUDA-core kernels whatever the handle's routing (ss_op_linear_umma is the wgmma hook)
+  Epilogue ep = ep_out(out_dev, N, act);
+  ep.bias = bias_dev;
+  if (skinny_gemm_supported(M, N, K, ep) && (K & 3) == 0) {
+    skinny_gemm(x_dev, K, w_dev, M, N, K, ep, S(stream));
+  } else {
+    ConvA a;
+    a.x = x_dev; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = K; a.ldx = K;
+    gemm_conv(a, w_dev, N, ep, &h->splitk[0], S(stream));
+  }
   return check_launch(h, "ss_op_linear");
 }
 

@@ -238,7 +238,7 @@ void finalize_impl(ss_engine* h) {
     a.x = pe_dev; a.B = 1; a.L_in = P; a.L_rows = P; a.C_in = D; a.ldx = D;
     Epilogue ep;
     ep.out = L.pos_proj; ep.ldo = D;
-    gemm_conv(a, lp.w, D, ep, 0);
+    gemm_conv(a, lp.w, D, ep, &h->splitk[0], 0);
     L.conv_ln = make_ln(h, p + ".conv_module.layer_norm", D);
     ConvW pw1 = make_conv(h, p + ".conv_module.pointwise_conv1", 2 * D, D, 1, 1, true, false);
     L.pw1 = pw1.lin;
@@ -484,6 +484,7 @@ int ss_create(ss_engine** out, int device, const ss_config* cfg) {
     delete h;
     return SS_ERR_INVALID;
   }
+  h->umma2_cache = new ss::Umma2Cache();
   *out = h;
   return SS_OK;
 }
@@ -494,6 +495,8 @@ int ss_destroy(ss_engine* h) {
   cudaDeviceSynchronize();
   for (void* p : h->dev_allocs) cudaFree(p);
   ss::umma2_cache_destroy(h->umma2_cache);
+  for (float* p : h->splitk)
+    if (p) cudaFree(p);
   if (h->ws.base) cudaFree(h->ws.base);
   if (h->mt_cross_kv) cudaFree(h->mt_cross_kv);
   if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);

@@ -4,10 +4,13 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <map>
+#include <tuple>
+#include <vector>
+
 namespace ss {
 
 extern unsigned long long g_launches;  // kernels launched by this library (process-wide)
-extern int g_prefer_shared;            // 1: every kernel asks for the maximum shared-memory carve-out (see common.cuh)
 
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3 };
 
@@ -66,26 +69,29 @@ struct Epilogue {
 };
 
 // C[M,N] = epilogue( A[M,K] * W[N,K]^T ), K = ksize*C_in, W row-major with K contiguous.
-void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaStream_t st);
+// splitk: the caller's split-K scratch region (nullptr: never split), see splitk_workspace.
+void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, float** splitk, cudaStream_t st);
 
-// split-K scratch (one per process; launches of a handle are stream-ordered) and its fixed-order reduce + epilogue
-float* splitk_workspace(size_t bytes);
+// Split-K scratch: *splitk is a region of splitk_workspace_bytes() that the first GEMM splitting into it allocates and its owner
+// frees; the launches that share a region must be stream-ordered.  Returns the region when `bytes` fit it (nullptr: no region,
+// request too large or out of memory).
+float* splitk_workspace(float** splitk, size_t bytes);
 size_t splitk_workspace_bytes();  // capacity of one split-K scratch region
-// split-K scratch region (0..2) used by the GEMM launches of the calling thread from now on; 0 is the default
-void set_splitk_slot(int slot);
+// fixed-order reduce of the split-K partial sums + epilogue
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st);
 
 // wgmma path (kernels_umma2.cu): stride-1 convolutions / linears over one sequence (B = 1) with
 // pre-packed bf16-split weights streamed by cp.async.bulk and activations converted once per channel chunk (taps are
 // descriptor row shifts).  The cache owns the packed weight copies (keyed by weight pointer and tiling).
-struct Umma2Cache;
-extern int g_umma2_split_below, g_umma2_min_units;  // split heuristics (tuning knobs)
-extern unsigned long long* g_umma2_dbg;             // optional %globaltimer stamps of CTA (0,0,0)
-Umma2Cache* umma2_cache_create();
-void umma2_cache_clear(Umma2Cache* c);
+struct Umma2Cache {
+  std::map<std::tuple<const float*, int, int, int, int, int, int>, unsigned char*> packed;
+  std::vector<void*> allocs;
+  unsigned long long* dbg = nullptr;  // optional device buffer of 16 %globaltimer stamps of CTA (0,0,0) (freed by umma2_cache_destroy)
+};
+void umma2_cache_clear(Umma2Cache* c);  // frees the packed weights
 void umma2_cache_destroy(Umma2Cache* c);
 bool umma2_supported(const ConvA& a, int N, const Epilogue& ep);
-void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, cudaStream_t st);
+void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, float** splitk, cudaStream_t st);
 // packed copy of W[N][ksize*C_in] in the kernels' tiling (made once per weight matrix and tiling; nullptr when out of memory)
 const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int N, int C_in, int ksize, int BN, int CK, int NP, cudaStream_t st);
 

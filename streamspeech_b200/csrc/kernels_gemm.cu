@@ -261,35 +261,20 @@ __global__ void splitk_epilogue_kernel(const float* __restrict__ ws, int splits,
   *op = y;
 }
 
-// scratch for split-K partial sums: one process-wide buffer of SPLITK_SLOTS independent regions.  Launches of a handle
-// are stream-ordered; an entry point that fans work out over several streams (the vocoder's three parallel resblocks)
-// gives each stream its own region with set_splitk_slot().
-float* g_splitk_base = nullptr;
 constexpr size_t SPLITK_WS_BYTES = 32u << 20;
-constexpr int SPLITK_SLOTS = 3;
-thread_local int g_splitk_slot = 0;
-
-float* splitk_region() {
-  if (!g_splitk_base) {
-    if (cudaMalloc((void**)&g_splitk_base, SPLITK_WS_BYTES * SPLITK_SLOTS) != cudaSuccess) {
-      g_splitk_base = nullptr;
-      cudaGetLastError();
-      return nullptr;
-    }
-  }
-  return g_splitk_base + (size_t)g_splitk_slot * (SPLITK_WS_BYTES / sizeof(float));
-}
 
 }  // namespace
 
-float* splitk_workspace(size_t bytes) {
-  if (bytes > SPLITK_WS_BYTES) return nullptr;
-  return splitk_region();
+float* splitk_workspace(float** splitk, size_t bytes) {
+  if (!splitk || bytes > SPLITK_WS_BYTES) return nullptr;
+  if (!*splitk && cudaMalloc((void**)splitk, SPLITK_WS_BYTES) != cudaSuccess) {
+    *splitk = nullptr;
+    cudaGetLastError();
+  }
+  return *splitk;
 }
 
 size_t splitk_workspace_bytes() { return SPLITK_WS_BYTES; }
-
-void set_splitk_slot(int slot) { g_splitk_slot = (slot >= 0 && slot < SPLITK_SLOTS) ? slot : 0; }
 
 void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, const Epilogue& ep, cudaStream_t st) {
   ++g_launches;
@@ -300,7 +285,7 @@ void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, cons
 namespace {
 
 template <int BM, int BN>
-void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue& ep, bool conv, cudaStream_t st) {
+void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue& ep, bool conv, float** splitk, cudaStream_t st) {
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   const long ctas = (long)grid.x * grid.y;
   const int nk = (K + BK - 1) / BK;
@@ -316,7 +301,7 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
   float* ws = nullptr;
   int tiles = nk;
   if (splits > 1) {
-    ws = splitk_region();
+    ws = splitk_workspace(splitk, (size_t)splits * M * N * sizeof(float));
     if (!ws) splits = 1;
   }
   if (splits > 1) {
@@ -324,7 +309,6 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
     splits = (nk + tiles - 1) / tiles;
     grid.z = splits;
   }
-  prefer_shared_once(conv ? (const void*)gemm_kernel<BM, BN, true> : (const void*)gemm_kernel<BM, BN, false>);
   if (conv)
     gemm_kernel<BM, BN, true><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws);  // tile GEMMs never launch early (see launch_pdl)
   else
@@ -338,7 +322,7 @@ void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue&
 
 }  // namespace
 
-void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaStream_t st) {
+void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, float** splitk, cudaStream_t st) {
   ++g_launches;
   const int M = a.B * a.L_rows;
   const int K = a.ksize * a.C_in;
@@ -348,23 +332,23 @@ void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, cudaSt
   auto ctas = [&](int bm, int bn) { return (long)((M + bm - 1) / bm) * ((N + bn - 1) / bn); };
   const long target = std::max(1, current_device_sms());  // one wave of SMs
   if (N <= 16 && !ep.glu) {
-    if (ctas(128, 16) >= target) launch<128, 16>(a, W, M, N, K, ep, conv, st);
-    else launch<32, 16>(a, W, M, N, K, ep, conv, st);
+    if (ctas(128, 16) >= target) launch<128, 16>(a, W, M, N, K, ep, conv, splitk, st);
+    else launch<32, 16>(a, W, M, N, K, ep, conv, splitk, st);
     return;
   }
   if (N <= 32) {
-    if (ctas(64, 32) >= target) launch<64, 32>(a, W, M, N, K, ep, conv, st);
-    else launch<32, 32>(a, W, M, N, K, ep, conv, st);
+    if (ctas(64, 32) >= target) launch<64, 32>(a, W, M, N, K, ep, conv, splitk, st);
+    else launch<32, 32>(a, W, M, N, K, ep, conv, splitk, st);
     return;
   }
   // Prefer the largest tile that still fills the GPU once split-K (slices of >= 8 k-tiles, at most 8 slices) is counted:
   // a long K walked by few small CTAs is latency-bound.
   const int nk = (K + BK - 1) / BK;
   const long max_splits = std::max(1, std::min(8, nk / 8));
-  if (ctas(128, 64) >= 2 * target) launch<128, 64>(a, W, M, N, K, ep, conv, st);
-  else if (ctas(64, 64) * max_splits >= target) launch<64, 64>(a, W, M, N, K, ep, conv, st);
-  else if (ctas(32, 64) * max_splits >= target) launch<32, 64>(a, W, M, N, K, ep, conv, st);
-  else launch<32, 32>(a, W, M, N, K, ep, conv, st);
+  if (ctas(128, 64) >= 2 * target) launch<128, 64>(a, W, M, N, K, ep, conv, splitk, st);
+  else if (ctas(64, 64) * max_splits >= target) launch<64, 64>(a, W, M, N, K, ep, conv, splitk, st);
+  else if (ctas(32, 64) * max_splits >= target) launch<32, 64>(a, W, M, N, K, ep, conv, splitk, st);
+  else launch<32, 32>(a, W, M, N, K, ep, conv, splitk, st);
 }
 
 }  // namespace ss

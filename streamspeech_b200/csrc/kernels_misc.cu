@@ -8,7 +8,6 @@
 
 namespace ss {
 unsigned long long g_launches = 0;
-int g_prefer_shared = 0;  // option prefer_shared (see common.cuh)
 namespace {
 
 // one warp per row; two-pass (mean, then centred sum of squares) like ATen's RowwiseMoments result

@@ -33,11 +33,6 @@
 
 namespace ss {
 
-struct Umma2Cache {
-  std::map<std::tuple<const float*, int, int, int, int, int, int>, unsigned char*> packed;
-  std::vector<void*> allocs;
-};
-
 namespace {
 
 constexpr int U2_BM = 128;
@@ -434,12 +429,9 @@ __global__ void umma2_pack_kernel(const float* __restrict__ W, int N, int C_in, 
   }
 }
 
-}  // namespace
-int g_umma2_split_below = 60;   // tile grids smaller than this are split over (chunk, tap) units (ss_set_option umma2_split_below:
-                                // below one wave, the extra reduce launch can cost more than the idle SMs)
-int g_umma2_min_units = 4;      // ... into slices of at least this many units
-unsigned long long* g_umma2_dbg = nullptr;  // device buffer of 16 stamps when the debug option is on
-namespace {
+constexpr int U2_SPLIT_BELOW = 60;  // tile grids smaller than this are split over (chunk, tap) units (below one wave, the extra
+                                    // reduce launch can cost more than the idle SMs)
+constexpr int U2_MIN_UNITS = 4;     // ... into slices of at least this many units
 
 int u2_bn(int N) { return N >= 128 ? 128 : N > 32 ? 64 : N > 16 ? 32 : 16; }
 
@@ -447,7 +439,6 @@ template <int BN, int NP, int UPT, int SETS>
 void u2_launch_v(const U2Params& p, dim3 grid, size_t smem, cudaStream_t st) {
   if (first_time_on_device((const void*)umma2_kernel<BN, NP, UPT, SETS>))
     cudaFuncSetAttribute(umma2_kernel<BN, NP, UPT, SETS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  prefer_shared_once((const void*)umma2_kernel<BN, NP, UPT, SETS>);
   umma2_kernel<BN, NP, UPT, SETS><<<grid, U2_THREADS, smem, st>>>(p);
 }
 
@@ -460,8 +451,6 @@ void u2_launch(const U2Params& p, dim3 grid, size_t smem, cudaStream_t st) {
 
 }  // namespace
 
-Umma2Cache* umma2_cache_create() { return new Umma2Cache(); }
-
 void umma2_cache_clear(Umma2Cache* c) {
   if (!c) return;
   cudaDeviceSynchronize();
@@ -473,6 +462,7 @@ void umma2_cache_clear(Umma2Cache* c) {
 void umma2_cache_destroy(Umma2Cache* c) {
   if (!c) return;
   umma2_cache_clear(c);
+  if (c->dbg) cudaFree(c->dbg);
   delete c;
 }
 
@@ -511,7 +501,7 @@ const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int
   return wp;
 }
 
-void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, cudaStream_t st) {
+void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, float** splitk, cudaStream_t st) {
   const int M = a.L_rows;
   if (M <= 0) {
     ++g_launches;
@@ -524,7 +514,7 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   // ---- packed weights (once per weight matrix and tiling)
   const unsigned char* wp = umma2_packed_weights(cache, W, N, a.C_in, k, BN, CK, NP, st);
   if (wp == nullptr) {
-    gemm_conv(a, W, N, ep, st);  // out of memory for the packed copy: exact fp32 path
+    gemm_conv(a, W, N, ep, splitk, st);  // out of memory for the packed copy: exact fp32 path
     return;
   }
   ++g_launches;
@@ -545,18 +535,17 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   // ---- split over (chunk, tap) units when the tile grid cannot fill the GPU
   const int m_tiles = (M + U2_BM - 1) / U2_BM;
   const long base = (long)m_tiles * n_tiles;
-  const int min_units = std::max(1, g_umma2_min_units);
   int splits = 1;
-  if (base < g_umma2_split_below && p.units_total >= 2 * min_units) {
+  if (base < U2_SPLIT_BELOW && p.units_total >= 2 * U2_MIN_UNITS) {
     const long sms = std::max(1, current_device_sms());
-    splits = (int)std::min<long>((sms + base - 1) / base, p.units_total / min_units);
+    splits = (int)std::min<long>((sms + base - 1) / base, p.units_total / U2_MIN_UNITS);
     while (splits > 1 && (size_t)splits * M * N * sizeof(float) > (32u << 20)) --splits;
   }
   int ups = (p.units_total + splits - 1) / splits;
   splits = (p.units_total + ups - 1) / ups;
   float* ws = nullptr;
   if (splits > 1) {
-    ws = splitk_workspace((size_t)splits * M * N * sizeof(float));
+    ws = splitk_workspace(splitk, (size_t)splits * M * N * sizeof(float));
     if (!ws) {
       splits = 1;
       ups = p.units_total;
@@ -564,7 +553,7 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   }
   p.units_per_split = ups;
   p.ws = ws;
-  p.dbg = g_umma2_dbg;
+  p.dbg = cache->dbg;
   const size_t a_bytes = (size_t)2 * NP * (CK >> 3) * p.rs_pad * 16;
   const size_t b_unit = (size_t)NP * BN * CK * 2;
   p.SB = (((a_bytes + 127) & ~(size_t)127) + 4 * b_unit <= 110 * 1024) ? 4 : 3;

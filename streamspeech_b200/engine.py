@@ -228,7 +228,6 @@ class Engine:
             raise
         # tensor-core routing (kernels_umma2.cu): vocoder convs tolerate the 3-MMA split (1e-3 waveform bar, measured 7e-6);
         # linears that feed an arg-max stay on the exact fp32 kernels unless explicitly switched on
-        self.set_option("prefer_shared", int(os.environ.get("SS_PREFER_SHARED", "0")))
         self.set_option("umma_vocoder", int(os.environ.get("SS_UMMA_VOCODER", "12")))
         self.set_option("umma_linear", int(os.environ.get("SS_UMMA_LINEAR", "13")))
         self.set_option("umma_min_rows", int(os.environ.get("SS_UMMA_MIN_ROWS", "128")))
@@ -245,8 +244,6 @@ class Engine:
         self.set_option("unit_grouped", int(os.environ.get("SS_UNIT_GROUPED", "1")))
         # vocoder generator as one persistent kernel: -1 (default) for short frame windows, 0 never (multi-launch path), 1 always
         self.set_option("vocoder_fused", int(os.environ.get("SS_VOCODER_FUSED", "-1")))
-        self.set_option("umma2_split_below", int(os.environ.get("SS_UMMA2_SPLIT_BELOW", "60")))
-        self.set_option("umma2_min_units", int(os.environ.get("SS_UMMA2_MIN_UNITS", "4")))
         self.hop = self.lib.ss_vocoder_hop(self._h)
         self.vocoder_receptive_field = self.lib.ss_vocoder_receptive_field(self._h)
 

@@ -377,9 +377,47 @@ def test_op_linear_ignores_routing_left_by_other_handles(voc):
     try:
         for umma_linear in (0, 13):
             voc.eng.set_option("umma_linear", umma_linear)
-            voc.eng.op_linear_umma(x, w, b)  # an entry point of another handle: it sets the thread's routing from that handle
+            voc.eng.op_linear_umma(x, w, b)  # an entry point of another handle with the tensor-core routing on or off
             outs.append(other.op_linear(x, w, b))
     finally:
         voc.eng.set_option("umma_linear", 13)
         other.close()
     assert torch.equal(outs[0], outs[1])
+
+
+def test_t2u_batch_routing_stays_with_its_handle():
+    """ss_t2u_unit_decode_batch alternating on one thread between two live handles with different tensor-core routing: each handle's
+    units and arg-max equal its run with the other handle absent (a call reads the routing of its own handle only)."""
+    from streamspeech_b200.engine import Engine
+
+    cfg = ModelConfig().tiny()
+    sd = synth.make_model_state_dict(cfg, 0)
+    feats = torch.randn(3, 20, cfg.unit_dim, generator=torch.Generator().manual_seed(6)).cuda()
+    pads = [0, 2, 5]
+    routes = [dict(umma_linear=13, umma_min_rows=64), dict(umma_linear=0, umma_min_rows=128)]
+
+    def make(r):
+        e = Engine(cfg, sd, None, None)
+        for k, v in r.items():
+            e.set_option(k, v)
+        return e
+
+    def decode(e):  # (units, arg-max) per sample: the rows the call writes
+        units, argmax, _ = e.t2u_unit_decode_batch(feats, pads)
+        return units, argmax
+
+    alone = []
+    for r in routes:
+        e = make(r)
+        try:
+            alone.append(decode(e))
+        finally:
+            e.close()
+    engines = [make(r) for r in routes]
+    try:
+        for _ in range(2):
+            for i, e in enumerate(engines):
+                assert decode(e) == alone[i], routes[i]
+    finally:
+        for e in engines:
+            e.close()
