@@ -159,7 +159,8 @@ int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B,
  * prefix_host[n_prefix] = tgt_subwords_indices; max_new_tokens as in the agent (-1 = source finished:
  * max_len = min(max_len_b, max_positions-1)).  Writes the finalized hypothesis WITHOUT the trailing eos to
  * tokens_out_host (capacity max_out) and the decoder features of [eos, tokens...] to feats_out_dev[(n_out+1)][mt_dim].
- * Synchronises `stream` once per generated token (the arg-max is needed on the host for the stop test). */
+ * Synchronises `stream` once per generated token (the arg-max is needed on the host for the stop test).
+ * Errors: SS_ERR_INVALID for a prefix token outside [0, tgt_vocab), before anything is launched or the handle's state changes. */
 int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* prefix_host, int n_prefix,
                  int max_new_tokens, int max_len_b, int64_t* tokens_out_host, int max_out, int* n_out,
                  float* feats_out_dev);
@@ -180,7 +181,8 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
  * Without the hint every call projects all rows (the reference recomputes everything, agent:520-538). */
 int ss_mt_stable_rows(ss_engine* h, int rows);
 /* teacher-forced features for tokens_host[n] (pads allowed only as a tail): TransformerDecoderBase.extract_features_scriptable
- * (ctc_unity/modules/transformer_decoder.py:257-403).  feats_out_dev [n][mt_dim]; logits_last_dev (optional) [tgt_vocab]. enqueue only */
+ * (ctc_unity/modules/transformer_decoder.py:257-403).  feats_out_dev [n][mt_dim]; logits_last_dev (optional) [tgt_vocab]. enqueue only.
+ * Errors: SS_ERR_INVALID for a token outside [0, tgt_vocab), before anything is launched or the handle's state changes. */
 int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* tokens_host, int n,
                    float* feats_out_dev, float* logits_last_dev);
 /* Samples per launch group of ss_mt_features_batch and ss_t2u_unit_decode_batch: at most max(1, SS_UNIT_BATCH_ROWS / (S * rate))
@@ -209,7 +211,8 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
  *    492-505) and never refreshed, i.e. early rows keep the projections of the then-provisional encoder output.
  * Both quirks change the hypothesis and are reproduced.  max_len_b = the caller's max_len for max_new_tokens == -1
  * (min(int(max_len_a * src_len + max_len_b), max_decoder_positions - 1), sequence_generator.py:205-215).  Requires the
- * persistent MT kernel (option persistent_mt = 1).  Synchronises `stream` once per burst. */
+ * persistent MT kernel (option persistent_mt = 1).  Synchronises `stream` once per burst.  A prefix token outside [0, tgt_vocab)
+ * is SS_ERR_INVALID, refused before anything is launched or the state changes. */
 int ss_mt_incremental_reset(ss_engine* h);
 int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, int T, const int64_t* prefix_host, int n_prefix,
                              int max_new_tokens, int max_len_b, int64_t* tokens_out_host, int max_out, int* n_out);
@@ -385,8 +388,8 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
  * "persistent_ffn_fused", "persistent_mt", "persistent_mt_prefix", "fbank_tma" = 1 (default): kernel variants of
  * round 2, each tested against the path it replaces;
  * "persistent_profile" = 1: the persistent kernels record %globaltimer stamps per phase; "persistent_time" = 1: CUDA events around
- * the encoder-stack kernel, the single-token MT kernel and the stream pool's resample kernel (read with ss_debug_copy "persist_time" /
- * "mt_time" / "pool_resample_time") */
+ * the encoder-stack kernel, every launch of the single-token MT kernel (ss_mt_greedy and the incremental searches) and the stream
+ * pool's resample kernel (read with ss_debug_copy "persist_time" / "mt_time" / "pool_resample_time") */
 int ss_set_option(ss_engine* h, const char* name, int value);
 /* synchronous copy of a diagnostic buffer to the host: "persist_ts" = uint64 ns stamps of the last persistent step;
  * "persist_time" / "mt_time" / "pool_resample_time" = double[3] {summed ms, launches, summed algorithmic bytes / executed steps /

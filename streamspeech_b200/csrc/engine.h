@@ -175,7 +175,6 @@ struct ss_engine {
                                      // feed the last prefix token again, speech_to_text.s2tt agent + sequence_generator.py:338-346)
   int mt_inc_cross_rows = 0;         // encoder rows whose cross K / V were appended (never refreshed, transformer_layer.py:492-505)
   int64_t* mt_tok_dev = nullptr;  // [max_pos]
-  int64_t* mt_next_dev = nullptr;
   int64_t* mt_next_pinned = nullptr;
   // vocoder: the unit sequences of the last ss_vocoder_durations_ragged call, cached for ss_vocoder_generate_ragged
   float* voc_unit_emb = nullptr;  // [voc_ucap][emb]: sequence s at rows u0 .. u0 + U - 1

@@ -375,18 +375,21 @@ void mt_forward(ss_engine* h, int past, int n, int T, const int* self_kv_len_dev
   layer_norm(x, dim, feats, dim, h->mt_ln.g, h->mt_ln.b, n, dim, st);
 }
 
+// cross-attention K | V of encoder rows [from, T) of enc into rows [from, T) of a cache whose layers are layer_rows rows apart: one
+// linear per MT layer over the T - from rows (the GEMM routing depends on that M)
+void mt_project_cross(ss_engine* h, const float* enc, int from, int T, float* cache, size_t layer_rows, cudaStream_t st) {
+  const ss_config& c = h->cfg;
+  if (T <= from) return;
+  for (int l = 0; l < c.mt_layers; ++l)
+    linear(h, enc + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cache + (l * layer_rows + from) * 2 * c.mt_dim, 2 * c.mt_dim), st);
+}
+
 // cross-attention K | V of the encoder rows.  Rows the caller declared final (ss_mt_stable_rows) at the previous call were
 // projected then and are not touched again; everything above is (re)computed.
 void mt_begin(ss_engine* h, const float* enc_dev, int T, cudaStream_t st) {
-  const ss_config& c = h->cfg;
   int from = (h->mt_cross_enc == enc_dev) ? std::min(h->mt_cross_final, T) : 0;
   if (from < 0) from = 0;
-  if (T > from) {
-    for (int l = 0; l < c.mt_layers; ++l) {
-      float* cross = h->mt_cross_kv + (size_t)l * h->mt_cross_cap * 2 * c.mt_dim;
-      linear(h, enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * c.mt_dim, 2 * c.mt_dim), st);
-    }
-  }
+  mt_project_cross(h, enc_dev, from, T, h->mt_cross_kv, h->mt_cross_cap, st);
   h->mt_cross_final = std::min(h->mt_stable_hint, T);
   h->mt_stable_hint = 0;
   h->mt_cross_enc = enc_dev;
@@ -415,6 +418,153 @@ MtDecodeParams mt_decode_params(ss_engine* h, const DecScratch& s, float* x, flo
   P.part = h->mt_part; P.delta = h->mt_part + (size_t)8 * c.mt_dim;
   if (h->persistent_profile) P.ts = h->persist_ts;
   return P;
+}
+
+// the single-token MT kernel runs a search over Tk cross rows on this handle (the batched kernel reproduces its rows: it runs there too)
+bool mt_single_token_runs(const ss_engine* h, int Tk) {
+  const ss_config& c = h->cfg;
+  return h->persistent_mt && mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, Tk);
+}
+
+// caller tokens index the embedding table: every one of tok[0 .. n) must be in [0, tgt_vocab)
+bool mt_tokens_in_vocab(const ss_engine* h, const int64_t* tok, int n) {
+  for (int i = 0; i < n; ++i)
+    if (tok[i] < 0 || tok[i] >= h->cfg.tgt_vocab) return false;
+  return true;
+}
+
+// max_len of a greedy search over a forced prefix of `start` tokens: max_len_b (capped by the positions) for max_new_tokens == -1,
+// else start + max_new_tokens.  The hypothesis must fit max_out tokens and, with feats_ld > 0, max_len + 1 feature rows.
+int mt_search_len(ss_engine* h, int start, int max_new_tokens, int max_len_b, int max_out, int feats_ld, int* max_len) {
+  const int P = h->cfg.max_mt_positions;
+  const int ml = (max_new_tokens == -1) ? std::min(max_len_b, P - 1) : start + max_new_tokens;
+  if (ml < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
+  if (start > ml) return h->fail(SS_ERR_INVALID, "prefix longer than max_len");
+  if (ml + 2 > P || ml > max_out || (feats_ld > 0 && ml + 1 > feats_ld)) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
+  *max_len = ml;
+  return SS_OK;
+}
+
+// max_len and kv_off of an incremental search (ss_mt_greedy_incremental, or pool slot `slot` >= 0) whose state holds self_len
+// self-attention entries.  The slot of the token at position s is s + kv_off: the first call starts with an empty cache (kv_off = 0),
+// every later call re-feeds the last prefix token on top of the entry the previous call's final step left (kv_off grows by one per
+// call).  kernel_runs: mt_single_token_runs over the state's cross rows.
+int mt_incremental_len(ss_engine* h, int slot, int start, int max_new_tokens, int max_len_b, int self_len, int max_out, bool kernel_runs,
+                       int* max_len, int* kv_off) {
+  const int P = h->cfg.max_mt_positions;
+  const int ml = (max_new_tokens == -1) ? max_len_b : start + max_new_tokens;
+  if (ml < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
+  if (start > ml) return h->fail(SS_ERR_INVALID, "prefix longer than max_len");
+  const int off = self_len - start;
+  if (off < 0)
+    return h->fail(SS_ERR_STATE, slot < 0 ? "incremental MT state is shorter than the prefix (reset missing, or a prefix that this state did not produce)"
+                                          : "the slot's incremental MT state is shorter than the prefix (a prefix that this state did not produce)");
+  if (ml + off + 2 > P) {
+    const std::string need = "MT hypothesis longer than capacity: the incremental search needs " + std::to_string(ml + off + 2) +
+                             " self-attention entries (max_len " + std::to_string(ml) + " + " + std::to_string(off) +
+                             " kept from earlier calls + 2), max_mt_positions = " + std::to_string(P);
+    return h->fail(SS_ERR_CAPACITY, slot < 0 ? need : "slot " + std::to_string(slot) + ": " + need);
+  }
+  if (ml > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
+  if (!kernel_runs) return h->fail(SS_ERR_STATE, "incremental MT decoding runs on the persistent MT kernel, which is off or does not support this shape");
+  *max_len = ml;
+  *kv_off = off;
+  return SS_OK;
+}
+
+// the token buffer of a single-stream search, [eos, prefix...] (eos is the decoder's bos), and the prefix as the first tokens of the
+// hypothesis
+void mt_put_prefix(ss_engine* h, cudaStream_t st, const int64_t* prefix_host, int start, int64_t* tokens_out_host) {
+  std::vector<int64_t> toks(start + 1);
+  toks[0] = h->cfg.eos;
+  for (int i = 0; i < start; ++i) toks[i + 1] = prefix_host[i];
+  cudaMemcpyAsync(h->mt_tok_dev, toks.data(), toks.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
+  cudaStreamSynchronize(st);  // (host vector)
+  for (int i = 0; i < start; ++i) tokens_out_host[i] = prefix_host[i];
+}
+
+// Burst loop of the single-token kernel.  P holds the search's state (self_k / self_v / cross_kv, kv_off) and P.tok the tokens of
+// positions <= *step; positions *step .. max_len run over Tk cross rows.  Tokens of positions *first + 1 .. *step were enqueued by the
+// caller and not read yet: they are read back with the first launch's, which runs `burst` minus those steps (every launch and its
+// read-back covers `burst` steps).  The kernel stops by itself at eos and at the forced eos of position max_len.  New tokens up to eos
+// go to tokens_out_host[*n_tok ...]; *self_len (optional) follows the entries the self-attention cache holds.  Returns SS_OK once the
+// search ended, an error code (reported), or -1 when a launch was refused: *first / *step then give the unread tokens and the position
+// of the refused launch, and nothing from it on was enqueued.
+int mt_single_token_bursts(ss_engine* h, cudaStream_t st, const MtDecodeParams& P, int* first, int* step, int max_len, int Tk, int burst,
+                           int64_t* tokens_out_host, int* n_tok, int* self_len, const char* where) {
+  bool done = false;
+  while (!done) {
+    const int f = *first, s = *step;
+    const int cnt = std::min(max_len - s + 1, burst - (s - f));
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    const bool timed = h->persistent_time && h->mt_time_events.size() < 4096 && cudaEventCreate(&ev0) == cudaSuccess && cudaEventCreate(&ev1) == cudaSuccess;
+    if (timed) cudaEventRecord(ev0, st);
+    const int rc_launch = mt_decode_persistent(P, h->mt_persist_layers, s, cnt, max_len, Tk, h->persist_bar, &h->persist_bar_target, st);
+    if (timed) {
+      cudaEventRecord(ev1, st);
+      h->mt_time_events.push_back({ev0, ev1, -1.0});  // steps executed: filled in below once the tokens are read
+    }
+    if (rc_launch != 0) {
+      cudaGetLastError();
+      return -1;
+    }
+    done = s + cnt > max_len;      // eos forced at max_len (sequence_generator.py:362-364): that step writes no token
+    int last = s + cnt - 1;        // the last position fed
+    const int produced = std::min(s + cnt, max_len) - f;
+    int steps_run = produced;
+    // an incremental search also waits for a launch that only ran the forced-eos step: a barrier timeout there is reported by the
+    // call that left the state's last entry
+    if (produced > 0 || self_len) {
+      const int rc = sync_burst(h, st, h->mt_next_pinned, P.tok + f + 1, produced, produced, 1, where);
+      if (rc) return rc;
+      for (int i = 0; i < produced; ++i) {
+        const int64_t next = h->mt_next_pinned[i];
+        if (next == h->cfg.eos) {
+          done = true;
+          steps_run = i + 1;  // (the kernel stops after the step that produced eos)
+          last = f + i;
+          break;
+        }
+        tokens_out_host[(*n_tok)++] = next;
+      }
+    }
+    if (timed && steps_run > 0) h->mt_time_events.back().bytes = (double)steps_run;  // (mt_time counts launches that produced a token)
+    if (self_len) *self_len = last + P.kv_off + 1;
+    *first = *step = s + cnt;
+  }
+  return SS_OK;
+}
+
+// Burst loop of the batched kernel: steps 0 .. steps - 1 of the P.rows rows, 16 per launch and host read-back; row b's tokens up to its
+// eos are appended at tokens_out_host[b * max_out + n_out_host[b]].  Returns SS_OK, an error code (reported), or -1 when the first
+// launch was refused (nothing written to the outputs yet: the caller decodes per sample).
+int mt_batch_bursts(ss_engine* h, cudaStream_t st, const MtBatchParams& P, int steps, int64_t* tokens_out_host, int max_out, int32_t* n_out_host,
+                    const char* where) {
+  std::vector<char> done(P.rows, 0);
+  int active = P.rows;
+  constexpr int kBurst = 16;  // the rows of h->mtb_tok_pinned
+  for (int step = 0; step < steps && active > 0; step += kBurst) {
+    const int cnt = std::min(kBurst, steps - step);
+    if (mt_decode_batch(P, h->mt_persist_layers, step, cnt, h->persist_bar, &h->persist_bar_target, st) != 0) {
+      cudaGetLastError();
+      if (step == 0) return -1;
+      return h->fail(SS_ERR_CUDA, "cooperative launch of the batched MT kernel was refused");
+    }
+    const int rc = sync_burst(h, st, h->mtb_tok_pinned, P.tok + step + 1, cnt, P.tok_ld, P.rows, where);
+    if (rc) return rc;
+    for (int b = 0; b < P.rows; ++b) {
+      for (int i = 0; i < cnt && !done[b]; ++i) {
+        const int64_t next = h->mtb_tok_pinned[(size_t)b * cnt + i];
+        if (next == P.eos) {
+          done[b] = 1;
+          --active;
+        } else {
+          tokens_out_host[(size_t)b * max_out + n_out_host[b]++] = next;
+        }
+      }
+    }
+  }
+  return SS_OK;
 }
 
 // device buffers of the batched greedy search, grown on demand: self K / V for tok_ld positions, cross K / V for Tmax rows per sample
@@ -462,11 +612,10 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
   int rc = ensure_mt_batch(h, max_len + 2, Tmax);
   if (rc) return rc;
   const int ld = h->mtb_tok_ld;
-  // cross K / V: the same projection call as mt_begin with the sample's own row count (the GEMM routing depends on M)
+  // cross K / V: the same projection as mt_begin with the sample's own row count (the GEMM routing depends on M)
   for (int b = 0; b < Bg; ++b)
-    for (int l = 0; l < c.mt_layers; ++l)
-      linear(h, enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, c.enc_dim, T_host[g0 + b], h->mt[l].ckv,
-             ep_out(h->mtb_cross_kv + ((size_t)l * R + b) * h->mtb_cross_cap * 2 * dim, 2 * dim), st);
+    mt_project_cross(h, enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, 0, T_host[g0 + b], h->mtb_cross_kv + (size_t)b * h->mtb_cross_cap * 2 * dim,
+                     R * h->mtb_cross_cap, st);
   const size_t floats = (size_t)Bg * (dim * 11 + c.mt_ffn + c.tgt_vocab);
   if (!ws_begin(h, floats * sizeof(float) + (size_t)Bg * ld * sizeof(int64_t) + (size_t)Bg * 2 * sizeof(int) + 16 * 256))
     return h->fail(SS_ERR_CUDA, "workspace allocation failed");
@@ -489,31 +638,32 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
   cudaMemcpyAsync(ints, ints0.data(), ints0.size() * sizeof(int), cudaMemcpyHostToDevice, st);
   cudaStreamSynchronize(st);  // (host vectors)
   for (int b = 0; b < Bg; ++b) n_out_host[g0 + b] = 0;
-  std::vector<char> done(Bg, 0);
-  int active = Bg;
-  constexpr int kBurst = 16;  // steps per launch, as ss_mt_greedy; the host reads the tokens back once per burst
-  for (int step = 0; step < max_len && active > 0; step += kBurst) {  // step max_len is the forced eos: no work
-    const int cnt = std::min(kBurst, max_len - step);
-    if (mt_decode_batch(P, h->mt_persist_layers, step, cnt, h->persist_bar, &h->persist_bar_target, st) != 0) {
-      cudaGetLastError();
-      if (step == 0) return -1;
-      return h->fail(SS_ERR_CUDA, "cooperative launch of the batched MT kernel was refused");
-    }
-    rc = sync_burst(h, st, h->mtb_tok_pinned, P.tok + step + 1, cnt, ld, Bg, "ss_mt_greedy_batch");
-    if (rc) return rc;
-    for (int b = 0; b < Bg; ++b) {
-      for (int i = 0; i < cnt && !done[b]; ++i) {
-        const int64_t next = h->mtb_tok_pinned[(size_t)b * cnt + i];
-        if (next == c.eos) {
-          done[b] = 1;
-          --active;
-        } else {
-          tokens_out_host[(size_t)(g0 + b) * max_out + n_out_host[g0 + b]++] = next;
-        }
-      }
-    }
+  // step max_len is the forced eos: no work
+  return mt_batch_bursts(h, st, P, max_len, tokens_out_host + (size_t)g0 * max_out, max_out, n_out_host + g0, "ss_mt_greedy_batch");
+}
+
+// Streams i0 .. i0 + n - 1 of a batched search one by one through ss_mt_greedy: stream i decodes encoder block enc_block[i] (nullptr:
+// block i) of enc, enc_ld floats apart, over its T[i] rows, after its n_prefix[i] tokens pfx[i] (nullptr: none) with max_new_tokens[i]
+// (nullptr: -1); its features (feats_out_dev non-null) go to rows i * feats_ld.  ss_mt_greedy uses the single-stream MT buffers, so
+// their cross K / V cache is marked invalid afterwards (a streaming call on this handle then projects every row again) and a pending
+// stable-rows hint is kept.
+int mt_greedy_per_stream(ss_engine* h, void* stream, int i0, int n, const float* enc, size_t enc_ld, const int32_t* enc_block, const int32_t* T,
+                         const int64_t* const* pfx, const int32_t* n_prefix, const int32_t* max_new_tokens, int max_len_b, int64_t* tokens_out_host,
+                         int max_out, int32_t* n_out_host, float* feats_out_dev, int feats_ld) {
+  const int hint = h->mt_stable_hint;
+  h->mt_stable_hint = 0;
+  int rc = SS_OK;
+  for (int i = i0; i < i0 + n && rc == SS_OK; ++i) {
+    int n_tok = 0;
+    rc = ss_mt_greedy(h, stream, enc + (enc_block ? enc_block[i] : i) * enc_ld, T[i], pfx ? pfx[i] : nullptr, n_prefix ? n_prefix[i] : 0,
+                      max_new_tokens ? max_new_tokens[i] : -1, max_len_b, tokens_out_host + (size_t)i * max_out, max_out, &n_tok,
+                      feats_out_dev ? feats_out_dev + (size_t)i * feats_ld * h->cfg.mt_dim : nullptr);
+    n_out_host[i] = n_tok;
   }
-  return SS_OK;
+  h->mt_cross_enc = nullptr;
+  h->mt_cross_final = 0;
+  h->mt_stable_hint = hint;
+  return rc;
 }
 
 // T2U encoder -> unit decoder -> unit CTC of B samples of Slen positions (mt_feats [B][Slen][dim]); sample b adds positional row
@@ -929,6 +1079,7 @@ int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, cons
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (n <= 0 || n > c.max_mt_positions || T <= 0) return h->fail(SS_ERR_INVALID, "bad MT sequence length");
+  if (!mt_tokens_in_vocab(h, tokens_host, n)) return h->fail(SS_ERR_INVALID, "ss_mt_features: token outside the vocabulary");
   cudaStream_t st = S(stream);
   int rc = ensure_mt_cross(h, T);
   if (rc) return rc;
@@ -964,11 +1115,11 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
   cudaStream_t st = S(stream);
   if (T <= 0 || n_prefix < 0 || !n_out) return h->fail(SS_ERR_INVALID, "bad arguments to ss_mt_greedy");
   const int start = n_prefix;
-  int max_len = (max_new_tokens == -1) ? std::min(max_len_b, c.max_mt_positions - 1) : start + max_new_tokens;
-  if (max_len < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
-  if (start > max_len) return h->fail(SS_ERR_INVALID, "prefix longer than max_len");
-  if (max_len + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
-  int rc = ensure_mt_cross(h, T);
+  if (!mt_tokens_in_vocab(h, prefix_host, start)) return h->fail(SS_ERR_INVALID, "ss_mt_greedy: prefix token outside the vocabulary");
+  int max_len = 0;
+  int rc = mt_search_len(h, start, max_new_tokens, max_len_b, max_out, 0, &max_len);
+  if (rc) return rc;
+  rc = ensure_mt_cross(h, T);
   if (rc) return rc;
   const int dim = c.mt_dim;
   const int nmax = std::max(start + 1, 1);
@@ -980,61 +1131,41 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
   if (!feats_out_dev) feats_out_dev = h->ws.f32(feat_floats);
   Linear outp;
   outp.w = h->mt_emb; outp.b = nullptr; outp.N = c.tgt_vocab; outp.K = dim;
-  // tokens buffer = [eos, prefix...]
-  std::vector<int64_t> toks(start + 1);
-  toks[0] = c.eos;
-  for (int i = 0; i < start; ++i) toks[i + 1] = prefix_host[i];
-  cudaMemcpyAsync(h->mt_tok_dev, toks.data(), toks.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
-  cudaStreamSynchronize(st);
+  mt_put_prefix(h, st, prefix_host, start, tokens_out_host);
   mt_begin(h, enc_dev, T, st);
   int fed = 0;  // rows in the KV cache
   int n_tok = start;  // hypothesis length so far (without eos)
-  for (int i = 0; i < start; ++i) tokens_out_host[i] = prefix_host[i];
   // The arg-max of step s is written straight into the device token buffer at s+1, so consecutive steps need no host
   // round trip.  Steps are enqueued in bursts; the host reads the burst's tokens back once and stops at the first eos
   // (steps enqueued past an eos only produce rows that are never read).
   const int burst = (max_new_tokens >= 0) ? std::max(1, max_new_tokens) : 16;
-  const bool persistent_mt = h->persistent_mt && mt_decode_persistent_supported(dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, T);
-  int step = start;
-  bool done = false;
-  if (persistent_mt && h->persistent_mt_prefix && start >= 1 && mt_prefix_persistent_supported(dim, c.mt_ffn, c.mt_heads, start, T)) {
+  bool single = mt_single_token_runs(h, T);
+  const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats_out_dev, 0);
+  if (single && h->persistent_mt_prefix && start >= 1 && mt_prefix_persistent_supported(dim, c.mt_ffn, c.mt_heads, start, T)) {
     // rows 0 .. start-1 ([eos, p1 .. p_{start-1}]) in one cooperative launch; the single-token kernel continues at position `start`
-    const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats_out_dev, 0);
     if (mt_prefix_persistent(P, h->mt_persist_layers, start, T, h->persist_bar, &h->persist_bar_target, st) == 0)
       fed = start;
     else
       cudaGetLastError();  // refused launch: per-kernel path
   }
+  int step = start;
+  bool done = false;
   while (!done) {
-    const int burst_first = step;
-    int enq = 0;
-    for (; step <= max_len && enq < burst; ++step, ++enq) {
-      // feed tokens[fed .. step]  (first iteration: the whole prefix; afterwards one token)
-      int n = step + 1 - fed;
-      if (n == 1 && persistent_mt) {
-        // the rest of the burst as ONE cooperative launch (it stops by itself at eos / max_len)
-        const int cnt = std::min(max_len - step + 1, burst - enq);
-        const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats_out_dev, 0);
-        cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-        if (h->persistent_time && h->mt_time_events.size() < 4096 && cudaEventCreate(&ev0) == cudaSuccess && cudaEventCreate(&ev1) == cudaSuccess)
-          cudaEventRecord(ev0, st);
-        else
-          ev0 = ev1 = nullptr;
-        const int rc_launch = mt_decode_persistent(P, h->mt_persist_layers, step, cnt, max_len, T, h->persist_bar, &h->persist_bar_target, st);
-        if (ev0 && ev1) {
-          cudaEventRecord(ev1, st);
-          h->mt_time_events.push_back({ev0, ev1, -1.0});  // steps executed: filled in below once the tokens are read
+    int burst_first = step;  // tokens of positions burst_first + 1 .. step are not read yet
+    for (; step <= max_len && step - burst_first < burst; ++step) {
+      if (single && step == fed) {
+        // the rest of the search on the single-token kernel, the rest of this burst in its first launch
+        rc = mt_single_token_bursts(h, st, P, &burst_first, &step, max_len, T, burst, tokens_out_host, &n_tok, nullptr, "ss_mt_greedy");
+        if (rc != -1) {
+          if (rc) return rc;
+          *n_out = n_tok;
+          return check_launch(h, "ss_mt_greedy");
         }
-        if (rc_launch == 0) {
-          fed = step + cnt;
-          if (step + cnt - 1 >= max_len) done = true;
-          step += cnt;
-          enq += cnt;
-          break;
-        }
-        cudaGetLastError();  // refused launch: per-kernel path below
+        single = false;  // refused launch: the per-kernel path below finishes the search from this step
+        fed = step;
       }
-      mt_forward(h, fed, n, T, nullptr, feats_out_dev + (size_t)fed * dim, s, x, st);
+      // feed tokens[fed .. step]  (first iteration: the whole prefix; afterwards one token)
+      mt_forward(h, fed, step + 1 - fed, T, nullptr, feats_out_dev + (size_t)fed * dim, s, x, st);
       fed = step + 1;
       if (step >= max_len) {  // eos is forced here (sequence_generator.py:362-364): no need for the logits
         done = true;
@@ -1049,21 +1180,18 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
         argmax_rows(logits, c.tgt_vocab, 1, c.tgt_vocab, h->mask_pad_unk, 1, h->mt_tok_dev + step + 1, st);
     }
     // tokens produced by this burst live at mt_tok_dev[burst_first+1 .. ]; the forced-eos step produced none
-    int produced = step - burst_first - (done ? 1 : 0);
+    const int produced = step - burst_first - (done ? 1 : 0);
     if (produced > 0) {
       rc = sync_burst(h, st, h->mt_next_pinned, h->mt_tok_dev + burst_first + 1, produced, produced, 1, "ss_mt_greedy");
       if (rc) return rc;
-      int steps_run = produced;
       for (int i = 0; i < produced; ++i) {
-        int64_t next = h->mt_next_pinned[i];
+        const int64_t next = h->mt_next_pinned[i];
         if (next == c.eos) {
           done = true;
-          steps_run = i + 1;  // (the kernel stops after the step that produced eos)
           break;
         }
         tokens_out_host[n_tok++] = next;
       }
-      if (!h->mt_time_events.empty() && h->mt_time_events.back().bytes < 0.0) h->mt_time_events.back().bytes = (double)steps_run;
     }
     if (step > max_len) done = true;
   }
@@ -1082,83 +1210,21 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
     if (T_host[b] < 1 || T_host[b] > T_stride) return h->fail(SS_ERR_INVALID, "ss_mt_greedy_batch: sample length outside [1, T_stride]");
     Tmax = std::max(Tmax, (int)T_host[b]);
   }
-  const int max_len = std::min(max_len_b, c.max_mt_positions - 1);
-  if (max_len < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
-  if (max_len + 2 > c.max_mt_positions || max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
+  int max_len = 0;
+  int rc = mt_search_len(h, 0, -1, max_len_b, max_out, 0, &max_len);
+  if (rc) return rc;
   cudaStream_t st = S(stream);
-  // the batched kernel reproduces the rows of the single-token kernel: it runs where ss_mt_greedy would run that one
-  const bool batched = h->persistent_mt && mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, Tmax);
+  const bool batched = mt_single_token_runs(h, Tmax);
   for (int g0 = 0; g0 < B; g0 += MT_BATCH_MAX_ROWS) {
     const int Bg = std::min(MT_BATCH_MAX_ROWS, B - g0);
-    if (batched && Bg >= h->mt_batch_min_rows) {
-      const int rc = mt_batch_group(h, st, enc_dev, g0, Bg, T_stride, T_host, max_len, tokens_out_host, max_out, n_out_host);
-      if (rc != -1) {
-        if (rc) return rc;
-        continue;
-      }
-    }
-    // sample by sample on ss_mt_greedy's path.  It uses the single-stream MT buffers, so their cross K / V cache is marked
-    // invalid afterwards (a streaming call on this handle then projects every row again) and a pending stable-rows hint is kept.
-    const int hint = h->mt_stable_hint;
-    h->mt_stable_hint = 0;
-    int rc = SS_OK;
-    for (int b = g0; b < g0 + Bg && rc == SS_OK; ++b) {
-      int n = 0;
-      rc = ss_mt_greedy(h, stream, enc_dev + (size_t)b * T_stride * c.enc_dim, T_host[b], nullptr, 0, -1, max_len_b,
-                        tokens_out_host + (size_t)b * max_out, max_out, &n, nullptr);
-      n_out_host[b] = n;
-    }
-    h->mt_cross_enc = nullptr;
-    h->mt_cross_final = 0;
-    h->mt_stable_hint = hint;
+    rc = batched && Bg >= h->mt_batch_min_rows ? mt_batch_group(h, st, enc_dev, g0, Bg, T_stride, T_host, max_len, tokens_out_host, max_out, n_out_host) : -1;
+    if (rc == -1)  // sample by sample on ss_mt_greedy's path
+      rc = mt_greedy_per_stream(h, stream, g0, Bg, enc_dev, (size_t)T_stride * c.enc_dim, nullptr, T_host, nullptr, nullptr, nullptr, max_len_b,
+                                tokens_out_host, max_out, n_out_host, nullptr, 0);
     if (rc) return rc;
   }
   return check_launch(h, "ss_mt_greedy_batch");
 }
-
-}  // extern "C"
-
-namespace {
-
-// why an incremental search is refused for capacity: the entries it needs against those every self-attention cache has
-std::string mt_incremental_capacity_message(int max_len, int kv_off, int max_mt_positions) {
-  return "MT hypothesis longer than capacity: the incremental search needs " + std::to_string(max_len + kv_off + 2) + " self-attention entries (max_len " +
-         std::to_string(max_len) + " + " + std::to_string(kv_off) + " kept from earlier calls + 2), max_mt_positions = " + std::to_string(max_mt_positions);
-}
-
-// The incremental search of one stream on the single-token kernel: P holds the stream's state (self_k / self_v / cross_kv, kv_off)
-// and P.tok[start] its first token; positions start .. max_len over Tk cross rows, `burst` steps per launch and synchronisation.
-// The new tokens go to tokens_out_host[*n_tok ...]; *self_len follows the entries the self-attention cache holds.
-int mt_incremental_bursts(ss_engine* h, cudaStream_t st, const MtDecodeParams& P, int start, int max_len, int Tk, int burst, int64_t* tokens_out_host,
-                          int* n_tok, int* self_len, const char* where) {
-  int step = start;
-  bool done = false;
-  while (!done) {
-    const int cnt = std::min(max_len - step + 1, burst);
-    if (mt_decode_persistent(P, h->mt_persist_layers, step, cnt, max_len, Tk, h->persist_bar, &h->persist_bar_target, st) != 0) {
-      cudaGetLastError();
-      return h->fail(SS_ERR_CUDA, std::string(where) + ": cooperative launch of the persistent MT kernel was refused");
-    }
-    const int readable = std::min(cnt, max_len - step);  // the forced-eos step writes no token
-    const int rc = sync_burst(h, st, h->mt_next_pinned, P.tok + step + 1, readable, readable, 1, where);
-    if (rc) return rc;
-    for (int i = 0; i < cnt && !done; ++i) {
-      const int sidx = step + i;            // this step fed the token at position sidx (one more cache entry)
-      *self_len = sidx + P.kv_off + 1;
-      if (sidx >= max_len) { done = true; break; }   // eos forced (sequence_generator.py:362-364)
-      const int64_t next = h->mt_next_pinned[i];
-      if (next == h->cfg.eos) { done = true; break; }
-      tokens_out_host[(*n_tok)++] = next;
-    }
-    step += cnt;
-    if (step > max_len) done = true;
-  }
-  return SS_OK;
-}
-
-}  // namespace
-
-extern "C" {
 
 int ss_mt_incremental_reset(ss_engine* h) {
   if (!h) return SS_ERR_INVALID;
@@ -1174,18 +1240,12 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
   cudaStream_t st = S(stream);
   if (T <= 0 || n_prefix < 0 || !n_out) return h->fail(SS_ERR_INVALID, "bad arguments to ss_mt_greedy_incremental");
   const int start = n_prefix;
-  const int max_len = (max_new_tokens == -1) ? max_len_b : start + max_new_tokens;
-  if (max_len < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
-  if (start > max_len) return h->fail(SS_ERR_INVALID, "prefix longer than max_len");
-  // slot of the token at position s = s + kv_off; the first call starts with an empty cache (kv_off = 0), every later call
-  // re-feeds the last prefix token on top of the entry the previous call's final step left (kv_off grows by one per call)
-  const int kv_off = h->mt_inc_self_len - start;
-  if (kv_off < 0) return h->fail(SS_ERR_STATE, "incremental MT state is shorter than the prefix (reset missing, or a prefix that this state did not produce)");
-  if (max_len + kv_off + 2 > c.max_mt_positions) return h->fail(SS_ERR_CAPACITY, mt_incremental_capacity_message(max_len, kv_off, c.max_mt_positions));
-  if (max_len > max_out) return h->fail(SS_ERR_CAPACITY, "MT hypothesis longer than capacity");
-  if (!h->persistent_mt || !mt_decode_persistent_supported(c.mt_dim, c.mt_ffn, c.mt_heads, c.tgt_vocab, c.max_mt_positions, std::max(T, h->mt_inc_cross_rows)))
-    return h->fail(SS_ERR_STATE, "incremental MT decoding runs on the persistent MT kernel, which is off or does not support this shape");
-  int rc = ensure_mt_cross(h, std::max(T, h->mt_inc_cross_rows), h->mt_inc_cross_rows);
+  if (!mt_tokens_in_vocab(h, prefix_host, start)) return h->fail(SS_ERR_INVALID, "ss_mt_greedy_incremental: prefix token outside the vocabulary");
+  const int Tk = std::max(T, h->mt_inc_cross_rows);
+  int max_len = 0, kv_off = 0;
+  int rc = mt_incremental_len(h, -1, start, max_new_tokens, max_len_b, h->mt_inc_self_len, max_out, mt_single_token_runs(h, Tk), &max_len, &kv_off);
+  if (rc) return rc;
+  rc = ensure_mt_cross(h, Tk, h->mt_inc_cross_rows);
   if (rc) return rc;
   const int dim = c.mt_dim;
   if (!ws_begin(h, ((size_t)(dim * 8 + c.mt_ffn) + c.tgt_vocab + (size_t)c.max_mt_positions * dim + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
@@ -1200,25 +1260,14 @@ int ss_mt_greedy_incremental(ss_engine* h, void* stream, const float* enc_dev, i
     h->mt_cross_final = 0;
     h->mt_cross_enc = nullptr;
   }
-  if (T > h->mt_inc_cross_rows) {
-    const int from = h->mt_inc_cross_rows;
-    for (int l = 0; l < c.mt_layers; ++l) {
-      float* cross = h->mt_cross_kv + (size_t)l * h->mt_cross_cap * 2 * dim;
-      linear(h, enc_dev + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cross + (size_t)from * 2 * dim, 2 * dim), st);
-    }
-    h->mt_inc_cross_rows = T;
-  }
-  const int Tk = h->mt_inc_cross_rows;
-  std::vector<int64_t> toks(start + 1);
-  toks[0] = c.eos;
-  for (int i = 0; i < start; ++i) toks[i + 1] = prefix_host[i];
-  cudaMemcpyAsync(h->mt_tok_dev, toks.data(), toks.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
-  cudaStreamSynchronize(st);
-  int n_tok = start;
-  for (int i = 0; i < start; ++i) tokens_out_host[i] = prefix_host[i];
+  mt_project_cross(h, enc_dev, h->mt_inc_cross_rows, T, h->mt_cross_kv, h->mt_cross_cap, st);
+  h->mt_inc_cross_rows = Tk;
+  mt_put_prefix(h, st, prefix_host, start, tokens_out_host);
+  int n_tok = start, first = start, step = start;
   const int burst = (max_new_tokens >= 0) ? std::max(1, max_new_tokens + 1) : 32;
   const MtDecodeParams P = mt_decode_params(h, s, x, logits, feats, kv_off);
-  rc = mt_incremental_bursts(h, st, P, start, max_len, Tk, burst, tokens_out_host, &n_tok, &h->mt_inc_self_len, "ss_mt_greedy_incremental");
+  rc = mt_single_token_bursts(h, st, P, &first, &step, max_len, Tk, burst, tokens_out_host, &n_tok, &h->mt_inc_self_len, "ss_mt_greedy_incremental");
+  if (rc == -1) return h->fail(SS_ERR_CUDA, "ss_mt_greedy_incremental: cooperative launch of the persistent MT kernel was refused");
   if (rc) return rc;
   *n_out = n_tok;
   return check_launch(h, "ss_mt_greedy_incremental");
@@ -1294,10 +1343,10 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
   for (int b = 0; b < B; ++b) {
     if (T_host[b] < 1 || T_host[b] > T_stride) return h->fail(SS_ERR_INVALID, "ss_mt_features_batch: sample length outside [1, T_stride]");
     const int64_t* t = tokens_host + (size_t)b * Slen;
+    if (!mt_tokens_in_vocab(h, t, Slen)) return h->fail(SS_ERR_INVALID, "ss_mt_features_batch: token outside the vocabulary");
     int n_valid = Slen;  // trailing pads are masked as keys (ss_mt_features)
     while (n_valid > 0 && t[n_valid - 1] == c.pad) --n_valid;
     for (int i = 0; i < Slen; ++i) {
-      if (t[i] < 0 || t[i] >= c.tgt_vocab) return h->fail(SS_ERR_INVALID, "ss_mt_features_batch: token outside the vocabulary");
       if (i < n_valid && t[i] == c.pad) return h->fail(SS_ERR_INVALID, "pads are only supported as a tail");
       pos[(size_t)b * Slen + i] = t[i] == c.pad ? c.pad : c.pad + 1 + i;  // make_positions, restarting for every sample
     }

@@ -333,7 +333,6 @@ void finalize_impl(ss_engine* h) {
     h->mt_self_k = dev_alloc<float>(h, cache);
     h->mt_self_v = dev_alloc<float>(h, cache);
     h->mt_tok_dev = dev_alloc<int64_t>(h, c.max_mt_positions + 8);
-    h->mt_next_dev = dev_alloc<int64_t>(h, 8);
     h->mt_part = dev_alloc<float>(h, (size_t)9 * c.mt_dim);
     cudaMallocHost((void**)&h->mt_next_pinned, (size_t)(c.max_mt_positions + 8) * sizeof(int64_t));
     std::vector<MtLayerP> ml(c.mt_layers);

@@ -202,6 +202,26 @@ def test_errors_leave_the_handle_usable(eng):
     rc = lib.ss_mt_greedy_batch(eng._h, eng._stream(), enc.data_ptr(), 2, T, tl, 60, out, 8, n)
     assert rc == -5  # SS_ERR_CAPACITY: a 60-token hypothesis does not fit 8 slots
     assert b"capacity" in lib.ss_last_error(eng._h)
+    # a token outside [0, tgt_vocab): SS_ERR_INVALID before any launch, the incremental state as it was
+    x = enc[0, : lens[0]].contiguous()
+    eng.mt_incremental_reset()
+    h1 = eng.mt_greedy_incremental(x, None, 2, 60)
+    toks, n_one = (ctypes.c_int64 * 64)(), ctypes.c_int32(0)
+    feats = torch.empty(2, eng.cfg.mt_dim, device="cuda")
+    torch.cuda.synchronize()
+    l0 = eng.launch_count()
+    for bad in (eng.cfg.tgt_vocab, -1):
+        pb = (ctypes.c_int64 * 2)(h1[0], bad)
+        assert lib.ss_mt_greedy(eng._h, eng._stream(), x.data_ptr(), x.shape[0], pb, 2, 3, 60, toks, 64, ctypes.byref(n_one), None) == -1
+        assert lib.ss_mt_greedy_incremental(eng._h, eng._stream(), x.data_ptr(), x.shape[0], pb, 2, 3, 60, toks, 64, ctypes.byref(n_one)) == -1
+        assert lib.ss_mt_features(eng._h, eng._stream(), x.data_ptr(), x.shape[0], (ctypes.c_int64 * 2)(eng.cfg.eos, bad), 2, feats.data_ptr(),
+                                  None) == -1
+        assert b"outside the vocabulary" in lib.ss_last_error(eng._h)
+    assert eng.launch_count() == l0
+    cont = eng.mt_greedy_incremental(x, h1, -1, 60)
+    eng.mt_incremental_reset()
+    assert eng.mt_greedy_incremental(x, eng.mt_greedy_incremental(x, None, 2, 60), -1, 60) == cont
+    eng.mt_incremental_reset()
     assert eng.mt_greedy_batch(enc, lens, 60) == per_sample(eng, enc, lens, 60)
 
 

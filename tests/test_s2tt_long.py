@@ -27,6 +27,7 @@ from streamspeech_b200.config import ModelConfig
 torch.set_grad_enabled(False)
 gpu = pytest.mark.gpu
 TRACE_KEYS = ("asr_tokens", "st_tokens", "mt_tokens")
+SS_ERR_INVALID = -1
 SS_ERR_CAPACITY = -5
 MARGIN = 1e-4
 LONG_POSITIONS = 2048
@@ -354,7 +355,8 @@ def test_searches_to_the_block_edges_vs_fp64_oracle(noeos):
 
 @gpu
 def test_capacity_is_checked_before_any_launch(noeos):
-    """max_len + kv_off + 2 > max_mt_positions: SS_ERR_CAPACITY with nothing launched, on the handle and in the pool, and the state as it was"""
+    """max_len + kv_off + 2 > max_mt_positions: SS_ERR_CAPACITY with nothing launched, on the handle and in the pool, and the state as it was;
+    the same for a token outside the vocabulary (SS_ERR_INVALID) in ss_mt_greedy_incremental, ss_mt_greedy and ss_mt_features"""
     cfg, e, o = noeos
     lib, h, st = e.lib, e._h, e._stream()
     I32, I64 = ctypes.c_int32, ctypes.c_int64
@@ -376,6 +378,16 @@ def test_capacity_is_checked_before_any_launch(noeos):
     assert lib.ss_pool_mt_greedy_incremental(h, st, 1, (I32 * 1)(1), pf, (I32 * 1)(3), (I32 * 1)(-1), (I32 * 1)(max_len), out, cap,
                                              n_out) == SS_ERR_CAPACITY
     assert b"max_mt_positions = %d" % cap in lib.ss_last_error(h)
+    # a caller token outside [0, tgt_vocab) would index the embedding table out of bounds: SS_ERR_INVALID, also before any launch
+    feats = torch.empty(2, cfg.mt_dim, device="cuda")
+    for bad in (cfg.tgt_vocab, -1):
+        pb = (I64 * 3)(h1[0], h1[1], bad)
+        assert lib.ss_mt_greedy_incremental(h, st, enc.data_ptr(), enc.shape[0], pb, 3, 3, 100, out, cap, ctypes.byref(n_one)) == SS_ERR_INVALID
+        assert b"outside the vocabulary" in lib.ss_last_error(h)
+        assert lib.ss_mt_greedy(h, st, enc.data_ptr(), enc.shape[0], pb, 3, 3, 100, out, cap, ctypes.byref(n_one), None) == SS_ERR_INVALID
+        assert b"outside the vocabulary" in lib.ss_last_error(h)
+        assert lib.ss_mt_features(h, st, enc.data_ptr(), enc.shape[0], (I64 * 2)(cfg.eos, bad), 2, feats.data_ptr(), None) == SS_ERR_INVALID
+        assert b"outside the vocabulary" in lib.ss_last_error(h)
     assert e.launch_count() == l0
     # both states are intact: the largest search that fits continues them and the two agree
     a = e.mt_greedy_incremental(enc, h1, -1, cap - 3)
