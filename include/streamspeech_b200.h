@@ -175,6 +175,23 @@ int ss_mt_greedy(ss_engine* h, void* stream, const float* enc_dev, int T, const 
  * Errors: SS_ERR_INVALID for B <= 0, a T_b outside [1, T_stride] or a null pointer; SS_ERR_CAPACITY when max_len > max_out. */
 int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int max_len_b,
                        int64_t* tokens_out_host, int max_out, int32_t* n_out_host);
+/* MT beam search of width `beam` (SequenceGenerator.generate_decoder with BeamSearch, beam_size = beam, min_len 1,
+ * normalize_scores, no prefix; the offline generator's --beam-mt K --lenpen len_penalty) for B independent samples.  enc_dev,
+ * T_stride, T_host and max_len_b as ss_mt_greedy_batch.  For sample b, hypothesis i < beam (sorted by score, highest first; on
+ * equal scores the one finalized first) is written to tokens_out_host[(b * beam + i) * max_out ...] without eos, its length to
+ * n_out_host[b * beam + i], its score (sum of log-probabilities, eos included, over (length + 1) ** len_penalty) to
+ * scores_out_host[b * beam + i], and its per-token scores, eos's last, to pos_scores_out_host[(b * beam + i) * (max_out + 1) ...].
+ * The candidates of a step are ranked by score; on exactly equal scores the lower index beam * tgt_vocab + token ranks first.
+ * Each launch of the batched MT kernel holds floor(32 / beam) samples of beam rows each, whose beams share one cross K / V
+ * projection; the search keeps all its state on the device and the host reads one done flag per sample per burst of 16 steps.
+ * Like ss_mt_greedy_batch it does not touch the handle's single-stream MT state.
+ * Errors, all before anything is launched: SS_ERR_INVALID for B <= 0, beam outside [2, 32] (beam 1 is ss_mt_greedy_batch), a
+ * non-finite len_penalty, a T_b outside [1, T_stride] or a null pointer; SS_ERR_CAPACITY when max_len > max_out; SS_ERR_CUDA
+ * when the persistent MT kernels are off (option persistent_mt) or do not support the shape.  A refused cooperative launch is
+ * SS_ERR_CUDA too (there is no other implementation of the beam search). */
+int ss_mt_beam_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int beam, int max_len_b,
+                     float len_penalty, int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host,
+                     float* pos_scores_out_host);
 /* Streaming hint for the NEXT ss_mt_greedy / ss_mt_features call: rows [0, rows) of the encoder output passed to it are
  * final, i.e. bit-identical in every later call with the same buffer until ss_encoder_stream_reset (ss_encoder_stream_step
  * reports that count as T_final).  Their cross-attention keys / values are then projected once instead of on every call.

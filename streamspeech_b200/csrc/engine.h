@@ -202,6 +202,7 @@ struct ss_engine {
   int persistent_mt_prefix = 1;                // ... and the forced-prefix pass (M <= 64 rows) as one cooperative kernel
   // batched greedy search (ss_mt_greedy_batch): caches of its own, so that a streaming agent's MT state on the handle survives it
   float* mtb_self_kv = nullptr;                // K then V: 2 x [mt_layers][MT_BATCH_MAX_ROWS][mtb_tok_ld][mt_dim]
+  float* mtb_self_kv2 = nullptr;               // the beam search's second buffer of the same shape (ss_mt_beam_batch)
   int mtb_tok_ld = 0;
   float* mtb_cross_kv = nullptr;               // [mt_layers][MT_BATCH_MAX_ROWS][mtb_cross_cap][2 * mt_dim]
   int mtb_cross_cap = 0;

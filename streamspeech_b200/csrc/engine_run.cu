@@ -567,20 +567,27 @@ int mt_batch_bursts(ss_engine* h, cudaStream_t st, const MtBatchParams& P, int s
   return SS_OK;
 }
 
-// device buffers of the batched greedy search, grown on demand: self K / V for tok_ld positions, cross K / V for Tmax rows per sample
-int ensure_mt_batch(ss_engine* h, int tok_ld, int Tmax) {
+// device buffers of the batched searches, grown on demand: self K / V for tok_ld positions (second_self_kv: a second such buffer,
+// the beam search's reorder target), cross K / V for Tmax rows per sample
+int ensure_mt_batch(ss_engine* h, int tok_ld, int Tmax, bool second_self_kv = false) {
   const ss_config& c = h->cfg;
   const size_t R = MT_BATCH_MAX_ROWS;
   if (tok_ld > h->mtb_tok_ld || Tmax > h->mtb_cross_cap) cudaDeviceSynchronize();  // earlier launches may still read the old buffers
   if (tok_ld > h->mtb_tok_ld) {
     if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);
-    h->mtb_self_kv = nullptr;
+    if (h->mtb_self_kv2) cudaFree(h->mtb_self_kv2);
+    h->mtb_self_kv = h->mtb_self_kv2 = nullptr;
     h->mtb_tok_ld = 0;
     if (cudaMalloc((void**)&h->mtb_self_kv, (size_t)2 * c.mt_layers * R * tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
       h->mtb_self_kv = nullptr;
       return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt self kv) failed");
     }
     h->mtb_tok_ld = tok_ld;
+  }
+  if (second_self_kv && !h->mtb_self_kv2 &&
+      cudaMalloc((void**)&h->mtb_self_kv2, (size_t)2 * c.mt_layers * R * h->mtb_tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
+    h->mtb_self_kv2 = nullptr;
+    return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt self kv, second buffer) failed");
   }
   if (Tmax > h->mtb_cross_cap) {
     const int cap = std::max(Tmax + Tmax / 2, 512);
@@ -640,6 +647,101 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
   for (int b = 0; b < Bg; ++b) n_out_host[g0 + b] = 0;
   // step max_len is the forced eos: no work
   return mt_batch_bursts(h, st, P, max_len, tokens_out_host + (size_t)g0 * max_out, max_out, n_out_host + g0, "ss_mt_greedy_batch");
+}
+
+// Beam search of samples g0 .. g0 + Sg - 1 (Sg * beam <= MT_BATCH_MAX_ROWS rows) on mt_decode_batch_kernel's beam instantiation.
+// The steps run in bursts of 16 per launch; after each burst the host reads one done flag per sample and stops once all are set.
+// The search ends with K finalized hypotheses per sample, read once at the end and sorted by score (stable: on equal scores the
+// earlier finalized first).  Returns SS_OK or an error code (reported).
+int mt_beam_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, int Sg, int beam, int T_stride, const int32_t* T_host,
+                  int max_len, float len_penalty, int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host,
+                  float* pos_scores_out_host) {
+  const ss_config& c = h->cfg;
+  const int dim = c.mt_dim, K = beam, rows = Sg * K, nh = Sg * K;
+  const size_t R = MT_BATCH_MAX_ROWS;
+  int Tmax = 0;
+  for (int b = 0; b < Sg; ++b) Tmax = std::max(Tmax, (int)T_host[g0 + b]);
+  int rc = ensure_mt_batch(h, max_len + 2, Tmax, true);
+  if (rc) return rc;
+  const int ld = h->mtb_tok_ld;
+  // cross K / V once per sample (its K beams read the same block), as ss_mt_greedy_batch projects it
+  for (int b = 0; b < Sg; ++b)
+    mt_project_cross(h, enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, 0, T_host[g0 + b], h->mtb_cross_kv + (size_t)b * h->mtb_cross_cap * 2 * dim,
+                     R * h->mtb_cross_cap, st);
+  const size_t floats = (size_t)rows * (dim * 11 + c.mt_ffn + c.tgt_vocab + 2 * ld + 2 * K) + (size_t)nh * (ld + 1);
+  const size_t i64s = (size_t)2 * rows * ld + (size_t)nh * ld;
+  const size_t ints = (size_t)rows * (4 + 2 * K) + (size_t)Sg * 2 + nh;
+  if (!ws_begin(h, floats * sizeof(float) + i64s * sizeof(int64_t) + ints * sizeof(int) + 32 * 256)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  MtBatchParams P;
+  P.n_layers = c.mt_layers; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
+  P.rows = rows; P.tok_ld = ld; P.cross_cap = h->mtb_cross_cap;
+  P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
+  P.self_k = h->mtb_self_kv; P.self_v = h->mtb_self_kv + (size_t)c.mt_layers * R * ld * dim; P.cross_kv = h->mtb_cross_kv;
+  P.q = h->ws.f32((size_t)rows * dim); P.part = h->ws.f32((size_t)rows * 8 * dim); P.delta = h->ws.f32((size_t)rows * dim);
+  P.hid = h->ws.f32((size_t)rows * c.mt_ffn); P.logits = h->ws.f32((size_t)rows * c.tgt_vocab);
+  P.tok = (int64_t*)h->ws.raw((size_t)rows * ld * sizeof(int64_t));
+  MtBeamParams Bm;
+  Bm.beam = K; Bm.max_len = max_len; Bm.len_penalty = len_penalty;
+  Bm.tok2 = (int64_t*)h->ws.raw((size_t)rows * ld * sizeof(int64_t));
+  Bm.self_k2 = h->mtb_self_kv2; Bm.self_v2 = h->mtb_self_kv2 + (size_t)c.mt_layers * R * ld * dim;
+  Bm.cum = h->ws.f32((size_t)2 * rows * ld); Bm.cand = h->ws.f32((size_t)rows * 2 * K);
+  Bm.cand_tok = (int*)h->ws.raw((size_t)rows * 2 * K * sizeof(int)); Bm.parent = (int*)h->ws.raw((size_t)rows * sizeof(int));
+  Bm.hyp_tok = (int64_t*)h->ws.raw((size_t)nh * ld * sizeof(int64_t)); Bm.hyp_pos = h->ws.f32((size_t)nh * ld);
+  Bm.hyp_score = h->ws.f32(nh); Bm.hyp_len = (int*)h->ws.raw((size_t)nh * sizeof(int));
+  int* init = (int*)h->ws.raw(((size_t)2 * rows + 2 * Sg) * sizeof(int));  // [fin | cross_len | n_fin | done]
+  if (!P.q || !P.part || !P.delta || !P.hid || !P.logits || !P.tok || !Bm.tok2 || !Bm.cum || !Bm.cand || !Bm.cand_tok || !Bm.parent ||
+      !Bm.hyp_tok || !Bm.hyp_pos || !Bm.hyp_score || !Bm.hyp_len || !init)
+    return h->fail(SS_ERR_CUDA, "workspace too small");
+  P.fin = init;
+  P.cross_len = init + rows;
+  Bm.n_fin = init + 2 * rows;
+  Bm.done = Bm.n_fin + Sg;
+  std::vector<int64_t> tok0((size_t)rows * ld, c.eos);  // column 0 = eos (the decoder's bos)
+  std::vector<int> init0(2 * rows + 2 * Sg, 0);
+  for (int r = 0; r < rows; ++r) {
+    init0[r] = r % K != 0;  // step 0 runs beam 0 only (lprobs[:, ::beam_size]); its selection starts every beam
+    init0[rows + r] = T_host[g0 + r / K];
+  }
+  // (no synchronisation here: tok0 / init0 outlive every burst of this function, whose first read-back synchronises the stream)
+  cudaMemcpyAsync(P.tok, tok0.data(), tok0.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(init, init0.data(), init0.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+  int* done_pinned = reinterpret_cast<int*>(h->mtb_tok_pinned);  // (MT_BATCH_MAX_ROWS * 16 int64 words)
+  constexpr int kBurst = 16;
+  for (int step = 0; step <= max_len; step += kBurst) {  // step max_len forces eos: it still scores and finalizes every beam
+    const int cnt = std::min(kBurst, max_len + 1 - step);
+    if (mt_decode_batch(P, h->mt_persist_layers, step, cnt, h->persist_bar, &h->persist_bar_target, st, &Bm) != 0) {
+      cudaGetLastError();
+      return h->fail(SS_ERR_CUDA, "ss_mt_beam_batch: the cooperative launch of the batched MT kernel's beam search was refused");
+    }
+    cudaMemcpyAsync(done_pinned, Bm.done, Sg * sizeof(int), cudaMemcpyDeviceToHost, st);
+    rc = sync_burst(h, st, nullptr, nullptr, 0, 0, 0, "ss_mt_beam_batch");
+    if (rc) return rc;
+    if (std::all_of(done_pinned, done_pinned + Sg, [](int d) { return d != 0; })) break;
+  }
+  std::vector<int64_t> toks((size_t)nh * ld);
+  std::vector<float> pos((size_t)nh * ld), score(nh);
+  std::vector<int> len(nh), nfin(Sg);
+  cudaMemcpyAsync(toks.data(), Bm.hyp_tok, toks.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(pos.data(), Bm.hyp_pos, pos.size() * sizeof(float), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(score.data(), Bm.hyp_score, nh * sizeof(float), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(len.data(), Bm.hyp_len, nh * sizeof(int), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(nfin.data(), Bm.n_fin, Sg * sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_mt_beam_batch: ") + cudaGetErrorString(cudaGetLastError()));
+  for (int j = 0; j < Sg; ++j) {
+    if (nfin[j] != K) return h->fail(SS_ERR_CUDA, "ss_mt_beam_batch: a sample ended with fewer than beam finalized hypotheses");
+    std::vector<int> order(K);
+    for (int i = 0; i < K; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return score[(size_t)j * K + a] > score[(size_t)j * K + b]; });
+    for (int i = 0; i < K; ++i) {
+      const size_t src = (size_t)j * K + order[i], dst = (size_t)(g0 + j) * K + i;
+      const int n = len[src];  // eos included
+      std::copy(toks.begin() + src * ld, toks.begin() + src * ld + n - 1, tokens_out_host + dst * max_out);
+      std::copy(pos.begin() + src * ld, pos.begin() + src * ld + n, pos_scores_out_host + dst * (max_out + 1));
+      n_out_host[dst] = n - 1;
+      scores_out_host[dst] = score[src];
+    }
+  }
+  return SS_OK;
 }
 
 // Streams i0 .. i0 + n - 1 of a batched search one by one through ss_mt_greedy: stream i decodes encoder block enc_block[i] (nullptr:
@@ -1224,6 +1326,37 @@ int ss_mt_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, 
     if (rc) return rc;
   }
   return check_launch(h, "ss_mt_greedy_batch");
+}
+
+int ss_mt_beam_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T_stride, const int32_t* T_host, int beam, int max_len_b,
+                     float len_penalty, int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host,
+                     float* pos_scores_out_host) {
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || T_stride <= 0 || !enc_dev || !T_host || !tokens_out_host || !n_out_host || !scores_out_host || !pos_scores_out_host)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_mt_beam_batch");
+  if (beam < 2 || beam > MT_BATCH_MAX_ROWS || 2 * beam > c.tgt_vocab)
+    return h->fail(SS_ERR_INVALID, "ss_mt_beam_batch: beam outside [2, 32] (beam 1 is ss_mt_greedy_batch)");
+  if (!std::isfinite(len_penalty)) return h->fail(SS_ERR_INVALID, "ss_mt_beam_batch: len_penalty is not finite");
+  int Tmax = 0;
+  for (int b = 0; b < B; ++b) {
+    if (T_host[b] < 1 || T_host[b] > T_stride) return h->fail(SS_ERR_INVALID, "ss_mt_beam_batch: sample length outside [1, T_stride]");
+    Tmax = std::max(Tmax, (int)T_host[b]);
+  }
+  int max_len = 0;
+  int rc = mt_search_len(h, 0, -1, max_len_b, max_out, 0, &max_len);
+  if (rc) return rc;
+  if (!mt_single_token_runs(h, Tmax))
+    return h->fail(SS_ERR_CUDA, "ss_mt_beam_batch: the beam search runs on the persistent MT kernels, which are off (option persistent_mt) "
+                                "or do not support this shape");
+  cudaStream_t st = S(stream);
+  const int S_launch = MT_BATCH_MAX_ROWS / beam;  // samples per launch
+  for (int g0 = 0; g0 < B; g0 += S_launch) {
+    rc = mt_beam_group(h, st, enc_dev, g0, std::min(S_launch, B - g0), beam, T_stride, T_host, max_len, len_penalty, tokens_out_host, max_out,
+                       n_out_host, scores_out_host, pos_scores_out_host);
+    if (rc) return rc;
+  }
+  return check_launch(h, "ss_mt_beam_batch");
 }
 
 int ss_mt_incremental_reset(ss_engine* h) {

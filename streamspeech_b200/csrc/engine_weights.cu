@@ -499,6 +499,7 @@ int ss_destroy(ss_engine* h) {
   if (h->ws.base) cudaFree(h->ws.base);
   if (h->mt_cross_kv) cudaFree(h->mt_cross_kv);
   if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);
+  if (h->mtb_self_kv2) cudaFree(h->mtb_self_kv2);
   if (h->mtb_cross_kv) cudaFree(h->mtb_cross_kv);
   if (h->mtb_tok_pinned) cudaFreeHost(h->mtb_tok_pinned);
   if (h->mt_next_pinned) cudaFreeHost(h->mt_next_pinned);

@@ -129,10 +129,32 @@ struct MtBatchParams {
   const int* kv_off = nullptr;
   int self_ld = 0;
 };
+// Beam search (ss_mt_beam_batch): passed to mt_decode_batch, it selects a fourth instantiation of the kernel, which excludes
+// MtBatchParams' per-row fields.  Row r is beam r % beam of sample r / beam; the rows of a sample read cross block r / beam, and
+// cross_len is per row.  The token rows, the cumulative-score rows and the self-attention cache come in two buffers each: step s
+// feeds and writes buffer s & 1 and its selection reorders the rows into buffer (s + 1) & 1.  fin is the host's initial state
+// (1 for every beam but 0 at step 0) and is then kept by the kernel.
+struct MtBeamParams {
+  int beam = 0;                   // K (2 .. MT_BATCH_MAX_ROWS)
+  int max_len = 0;                // eos forced at this step, which ends every sample still searching
+  float len_penalty = 1.f;        // finalized score = cumulative score / (step + 1) ** len_penalty
+  int64_t* tok2 = nullptr;        // second token buffer, as MtBatchParams::tok ([rows][tok_ld])
+  float *self_k2 = nullptr, *self_v2 = nullptr;  // second self-attention cache, as self_k / self_v
+  float* cum = nullptr;           // [2][rows][tok_ld] cumulative score of the row's hypothesis after each step
+  float* cand = nullptr;          // [rows][2 K] candidate scores of a row, best first
+  int* cand_tok = nullptr;        // [rows][2 K] their tokens
+  int* parent = nullptr;          // [rows] row whose hypothesis this row continues at the next step
+  int* n_fin = nullptr;           // [samples] finalized hypotheses
+  int* done = nullptr;            // [samples] the sample's search ended
+  int64_t* hyp_tok = nullptr;     // [samples][K][tok_ld] finalized tokens, eos last
+  float* hyp_pos = nullptr;       // [samples][K][tok_ld] their positional scores
+  float* hyp_score = nullptr;     // [samples][K] their normalized scores
+  int* hyp_len = nullptr;         // [samples][K] their lengths, eos included
+};
 // enqueue steps step0 .. step0 + nsteps - 1 for every unfinished row (without P.max_len, all < the host's max_len: the forced-eos
-// step needs no work); returns 0, or < 0 if the launch was refused
+// step needs no work; a beam search runs its step max_len); returns 0, or < 0 if the launch was refused
 int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step0, int nsteps, unsigned* barrier_counter_dev,
-                    unsigned* barrier_target_host, cudaStream_t st);
+                    unsigned* barrier_target_host, cudaStream_t st, const MtBeamParams* beam = nullptr);
 
 // ---- MT decoder, prefix pass over M <= 64 rows (kernels_persist_mtp.cu): fills self-attention cache rows 0 .. M-1 and feature
 // rows 0 .. M-1 from P.tok[0 .. M-1]; P.x / P.q / P.attn hold M x dim floats, P.hid M x ffn

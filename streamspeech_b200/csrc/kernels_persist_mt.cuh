@@ -160,17 +160,24 @@ __device__ __forceinline__ void gemv_finish(const GemvW<K, MAXC>& r, const float
   }
 }
 
-// arg-max of log_softmax(x[0 .. vocab)) with pad always masked and eos masked while s < 1 (min_len), first index wins on ties
-// (argmax_rows_kernel); the whole CTA computes it, every thread gets the index
-__device__ __forceinline__ int masked_argmax(MtSmem& sm, const float* x, int vocab, int pad, int eos, int s) {
+// max and log-sum-exp of x[0 .. vocab) about that max, so that log_softmax(x)[c] = (x[c] - mx) - lse; every thread gets both
+__device__ __forceinline__ void row_log_softmax_terms(MtSmem& sm, const float* x, int vocab, float& mx, float& lse) {
   const int tid = threadIdx.x;
-  float mx = -INFINITY;
+  mx = -INFINITY;
   for (int c = tid; c < vocab; c += MTT) mx = fmaxf(mx, x[c]);
   mx = block_reduce_max(sm, mx);
   float su = 0.f;
   for (int c = tid; c < vocab; c += MTT) su += expf(x[c] - mx);
   su = block_reduce_sum(sm, su);
-  const float lse = logf(su);
+  lse = logf(su);
+}
+
+// arg-max of log_softmax(x[0 .. vocab)) with pad always masked and eos masked while s < 1 (min_len), first index wins on ties
+// (argmax_rows_kernel); the whole CTA computes it, every thread gets the index
+__device__ __forceinline__ int masked_argmax(MtSmem& sm, const float* x, int vocab, int pad, int eos, int s) {
+  const int tid = threadIdx.x;
+  float mx, lse;
+  row_log_softmax_terms(sm, x, vocab, mx, lse);
   float best = -INFINITY;
   int bi = 0x7fffffff;
   for (int c = tid; c < vocab; c += MTT) {

@@ -80,6 +80,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_ctc_greedy_pair.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
     lib.ss_mt_greedy.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp, i32, ctypes.POINTER(i32), vp]
     lib.ss_mt_greedy_batch.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, i32, vp]
+    lib.ss_mt_beam_batch.argtypes = [vp, vp, vp, i32, i32, vp, i32, i32, ctypes.c_float, vp, i32, vp, vp, vp]
     lib.ss_mt_stable_rows.argtypes = [vp, i32]
     lib.ss_mt_incremental_reset.argtypes = [vp]
     lib.ss_mt_greedy_incremental.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp, i32, ctypes.POINTER(i32)]
@@ -134,7 +135,7 @@ EXPORTED_SYMBOLS = [
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_durations_ragged", "ss_vocoder_generate_ragged", "ss_vocoder_hop",
     "ss_vocoder_receptive_field", "ss_op_linear", "ss_op_linear_umma", "ss_op_conv1d", "ss_set_option", "ss_debug_copy", "ss_op_layer_norm", "ss_launch_count", "ss_async_error", "ss_mt_incremental_reset", "ss_mt_greedy_incremental", "ss_ctc_greedy_pair", "ss_resample_out_len", "ss_resample_48k_to_16k", "ss_pool_create", "ss_pool_reset", "ss_pool_push_audio", "ss_pool_info", "ss_pool_step",
-    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
+    "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_mt_beam_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
     "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
     "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
 ]
@@ -425,6 +426,36 @@ class Engine:
         n_out = (ctypes.c_int32 * max(B, 1))()
         self._check(self.lib.ss_mt_greedy_batch(self._h, self._stream(), enc.data_ptr(), B, T, lens, int(max_len_b), out, cap, n_out))
         return [[int(out[b * cap + i]) for i in range(n_out[b])] for b in range(B)]
+
+    def mt_beam_batch(self, enc: torch.Tensor, enc_lengths: Sequence[int], beam: int, max_len_b: int,
+                      len_penalty: float = 1.0) -> List[List[Dict[str, object]]]:
+        """MT beam search of width `beam` (>= 2) over every sample of a padded encoder batch enc [B, T, C] (ss_mt_beam_batch):
+        SequenceGenerator.generate_decoder with beam_size = beam, len_penalty and normalize_scores, max_len as mt_greedy_batch.
+        Returns per sample the `beam` finalized hypotheses in the order of the reference's finalized[b] (score, highest first),
+        each {"tokens": [...] without eos, "score": float, "positional_scores": [...] one per token, eos's last}."""
+        assert enc.is_cuda and enc.is_contiguous() and enc.dim() == 3
+        B, T = int(enc.shape[0]), int(enc.shape[1])
+        if len(enc_lengths) != B:
+            raise EngineError(f"{len(enc_lengths)} lengths for a batch of {B}")
+        K = int(beam)
+        lens = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in enc_lengths])
+        cap = self.max_mt_positions
+        n = max(B, 1) * max(K, 1)
+        out = (ctypes.c_int64 * (n * cap))()
+        n_out = (ctypes.c_int32 * n)()
+        scores = (ctypes.c_float * n)()
+        pos = (ctypes.c_float * (n * (cap + 1)))()
+        self._check(self.lib.ss_mt_beam_batch(self._h, self._stream(), enc.data_ptr(), B, T, lens, K, int(max_len_b), float(len_penalty),
+                                              out, cap, n_out, scores, pos))
+        res = []
+        for b in range(B):
+            hyps = []
+            for i in range(K):
+                h = b * K + i
+                hyps.append({"tokens": [int(out[h * cap + t]) for t in range(n_out[h])], "score": float(scores[h]),
+                             "positional_scores": [float(pos[h * (cap + 1) + t]) for t in range(n_out[h] + 1)]})
+            res.append(hyps)
+        return res
 
     def mt_incremental_reset(self):
         self._check(self.lib.ss_mt_incremental_reset(self._h))

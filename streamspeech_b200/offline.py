@@ -2,11 +2,12 @@
 
 Drop-in for the reference's `CTCMultiDecoderSequenceGenerator` as `fairseq-generate --task speech_to_speech_ctc` uses it
 (researches/ctc_unity/sequence_generator_multi_decoder_ctc.py:163-331, built by tasks/speech_to_speech_ctc.py:21-49) with
-`--beam-mt 1 --beam 1`, plus the batch-1 vocoder pass of `generate_waveform_from_code.py:40-78`:
+`--beam-mt K --lenpen L --beam 1`, plus the batch-1 vocoder pass of `generate_waveform_from_code.py:40-78`:
 
     batched padded encoder (offline model: chunk_size None)                       ss_encoder_forward(B, lengths)
     ASR / ST CTC prints over all T rows of every sample (:206-246)                ss_ctc_greedy_batch
-    MT greedy search of the batch, max_len = max_len_b_mt (:251-260)              ss_mt_greedy_batch
+    MT search of the batch, max_len = max_len_b_mt (:251-260): K = 1 greedy        ss_mt_greedy_batch
+      K >= 2 beam search, best finalized hypothesis finalized[b][0] (:262-279)    ss_mt_beam_batch
     prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum (:262-271) host
     mt_decoder(features_only) on the padded batch (:287-291)                      ss_mt_features_batch
     T2U encoder -> CTC unit decoder -> CTC generate (:293-330)                    ss_t2u_unit_decode_batch
@@ -18,10 +19,11 @@ reference, which the batched calls reproduce (oracle/offline_oracle.py is pinned
       -> Engine.t2u_unit_decode_batch passes every sample's row (Engine.unit_position_row(b))
   N2  hypotheses keep the tokens emitted at padded T2U positions -> the pad tail is decoded too (n_pad_tail)
   N3  pad, unk and eos are masked before the arg-max (researches/ctc_unity/ctc_generator.py:56-58) -> mask_eos
-Beam search over the MT decoder (beam_size_mt > 1) is not implemented: the constructor refuses it.
+The T2U beam (`--beam`) stays 1: the reference's CTC unit decoder does not search; max_len_a_mt stays 0.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, List, Optional, Sequence
 
 import torch
@@ -30,13 +32,20 @@ from .engine import Engine, EngineError
 
 
 class OfflineS2STGenerator:
-    def __init__(self, engine: Engine, beam_size_mt: int = 1, beam_size: int = 1, max_len_a_mt: float = 0.0, max_len_b_mt: int = 200):
-        if beam_size_mt != 1 or beam_size != 1:
-            raise NotImplementedError("the H100 offline generator implements beam_size_mt = beam_size = 1 (greedy) only")
+    def __init__(self, engine: Engine, beam_size_mt: int = 1, beam_size: int = 1, max_len_a_mt: float = 0.0, max_len_b_mt: int = 200,
+                 len_penalty: float = 1.0):
+        if beam_size != 1:
+            raise NotImplementedError("the H100 offline generator implements beam_size = 1 only (the CTC unit decoder does not search)")
+        if int(beam_size_mt) != beam_size_mt or not 1 <= beam_size_mt <= 32:
+            raise ValueError(f"beam_size_mt must be an integer in [1, 32], got {beam_size_mt}")
         if max_len_a_mt != 0.0:
             raise NotImplementedError("max_len_a_mt != 0 is not supported (the reference default is 0)")
+        if not math.isfinite(len_penalty):
+            raise ValueError(f"len_penalty must be finite, got {len_penalty}")
         self.engine = engine
         self.cfg = engine.cfg
+        self.beam_size_mt = int(beam_size_mt)
+        self.len_penalty = float(len_penalty)
         self.max_len_b_mt = int(max_len_b_mt)
         engine.set_chunk(None, None)  # offline model: full attention, symmetric convolutions (N10)
 
@@ -58,8 +67,11 @@ class OfflineS2STGenerator:
         hyps: List[List[int]]
         if forced_mt is not None:
             hyps = [list(h) for h in forced_mt]
-        else:
+        elif self.beam_size_mt == 1:
             hyps = eng.mt_greedy_batch(enc, out_len, self.max_len_b_mt)  # all samples in one search
+        else:
+            nbest = eng.mt_beam_batch(enc, out_len, self.beam_size_mt, self.max_len_b_mt, self.len_penalty)
+            hyps = [n[0]["tokens"] for n in nbest]
         max_tgt_len = max(len(h) for h in hyps) + 1  # hypothesis + eos (:262)
         n_pad = [max_tgt_len - (len(h) + 1) for h in hyps]
         prev = [[c.eos] + h + [c.pad] * n for h, n in zip(hyps, n_pad)]
