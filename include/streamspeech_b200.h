@@ -255,6 +255,13 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
  * Errors: SS_ERR_INVALID for B <= 0, S <= 0 or S > max_mt_positions, an n_pad_tail outside [0, S), or a null pointer. */
 int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
                              int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);
+/* ss_t2u_unit_decode_batch plus the unit hypothesis' positional scores (CTCSequenceGenerator.generate, ctc_generator.py:54-61):
+ * lprob_dev [B][S * rate] fp32, row r of sample b = log_softmax(logits[b][r])[argmax[b][r]] over all unit_vocab columns (the masked
+ * pad / unk / eos columns stay in the normaliser, as the reference masks after log_softmax), pad-tail rows included.  argmax_dev and
+ * packed_units_dev are bit-identical to ss_t2u_unit_decode_batch's.  Same synchronisation and groups as ss_t2u_unit_decode_batch.
+ * Errors: those of ss_t2u_unit_decode_batch, and SS_ERR_INVALID for a null lprob_dev. */
+int ss_t2u_unit_decode_batch_scored(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S, const int32_t* n_pad_tail_host,
+                                    const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev, float* lprob_dev);
 /* ss_t2u_unit_decode_batch over ragged lengths (the stream pool's S2ST agents: every writing stream has its own number of MT
  * positions).  mt_feats_dev [B][S_stride][mt_dim]; sample b has S_host[b] positions, 1 <= S_b <= S_stride (S_host NULL: all S_stride),
  * of which the last n_pad_tail_host[b] (in [0, S_b)) are N2 pad positions that are decoded; positions >= S_b are neither keys nor
@@ -415,6 +422,9 @@ int ss_set_option(ss_engine* h, const char* name, int value);
 int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes);
 int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev,
                      float* out_dev);
+/* The unit arg-max hook: logits_dev [rows][ld] -> idx_dev [rows] with the first n_masked (<= 3) of pad, unk, eos never selected,
+ * through argmax_rows (lprob_dev NULL) or argmax_lprob_rows (lprob_dev [rows]: each winner's log_softmax over all V columns). */
+int ss_op_argmax_rows(ss_engine* h, void* stream, const float* logits_dev, int rows, int V, int ld, int n_masked, int64_t* idx_dev, float* lprob_dev);
 /* Attention and depthwise-conv hooks: each launches the launch function the engine uses (kernels.h) on `stream`; the hooks that take host arrays
  * copy them to the device and synchronise `stream`.  head_dim is 64 and D = H * 64; row strides are in floats, >= D and multiples
  * of 4.  kernel: 0 = the row / tile kernel the engine would choose for this shape, 1 = row kernel, 2 = tile kernel.

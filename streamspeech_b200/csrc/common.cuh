@@ -106,8 +106,11 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 
 // arg-max of log_softmax(x[0 .. V)) with the columns masked[0 .. n_masked) excluded, first index wins on ties, for a block of 256
 // threads (CTCDecoder.generate, agent/ctc_decoder.py:53-62; F.log_softmax = (x - max) - log(sum(exp(x - max)))).  Every row of
-// every caller goes through this one reduction order, so all arg-maxes agree bit for bit.  The index is valid in thread 0.
-__device__ __forceinline__ int block_masked_argmax256(const float* __restrict__ x, int V, const int* __restrict__ masked, int n_masked) {
+// every caller goes through this one reduction order, so all arg-maxes agree bit for bit.  The index is valid in thread 0, and so is
+// `lprob`, the winner's log-probability (x[idx] - max) - log(sum_v exp(x[v] - max)): the value the reduction compares, with every
+// one of the V columns, masked ones included, in the normaliser (the reference masks after log_softmax, ctc_generator.py:54-58).
+__device__ __forceinline__ int block_masked_argmax_lprob256(const float* __restrict__ x, int V, const int* __restrict__ masked, int n_masked,
+                                                            float& lprob) {
   __shared__ float red[32];
   __shared__ float sval[8];
   __shared__ int sidx[8];
@@ -157,7 +160,13 @@ __device__ __forceinline__ int block_masked_argmax256(const float* __restrict__ 
         bi = sidx[i];
       }
   }
+  lprob = best;
   return bi;
+}
+
+__device__ __forceinline__ int block_masked_argmax256(const float* __restrict__ x, int V, const int* __restrict__ masked, int n_masked) {
+  float lprob;
+  return block_masked_argmax_lprob256(x, V, masked, n_masked, lprob);
 }
 
 // CTC collapse (CTCDecoder.generate, agent/ctc_decoder.py:64-111) of one arg-max sequence am[i * stride], i < n: repeats, then

@@ -775,9 +775,10 @@ int mt_greedy_per_stream(ss_engine* h, void* stream, int i0, int n, const float*
 // lengths are uploaded (one synchronisation) only when some sample has a pad tail or fewer than Slen positions; otherwise every
 // attention runs at full length.
 // t2u_out_dev / logits_dev (optional, B = 1): the T2U encoder output and the unit logits are written there.
+// lprob_dev (optional, [B][Slen * R]): each row's arg-max log-probability (argmax_lprob_rows instead of argmax_rows).
 int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, int B, int Slen, const int32_t* S_host, const int32_t* n_pad_tail_host,
                     const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* units_dev, int32_t* count_dev, int64_t seg_stride,
-                    float* t2u_out_dev, float* logits_dev, const char* where) {
+                    float* t2u_out_dev, float* logits_dev, float* lprob_dev, const char* where) {
   const ss_config& c = h->cfg;
   const int dim = c.unit_dim, R = c.ctc_upsample_rate, L = Slen * R;
   std::vector<int> lens(3 * (size_t)B);  // [valid T2U positions B | valid upsampled rows B | decoded upsampled rows B]
@@ -838,7 +839,10 @@ int t2u_unit_decode(ss_engine* h, cudaStream_t st, const float* mt_feats_dev, in
     linear(h, xu, dim, rows, outp, ep_out(logits, c.unit_vocab), st, Bg);
     // ---- U2: never select pad, unk (agent version) [+ eos: offline version], then each sample's collapse
     int64_t* am = argmax_dev + (size_t)g0 * L;
-    argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, st);
+    if (lprob_dev)
+      argmax_lprob_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, lprob_dev + (size_t)g0 * L, st);
+    else
+      argmax_rows(logits, c.unit_vocab, rows, c.unit_vocab, h->mask_pad_unk, mask_eos ? 3 : 2, am, st);
     ctc_collapse_segments(am, L, 1, Bg, c.unit_vocab - 1, c.pad, units_dev + g0 * seg_stride, nullptr, count_dev + 2 * g0 * seg_stride, seg_stride,
                           st, dec_len);
   }
@@ -1412,7 +1416,7 @@ int ss_t2u_unit_decode(ss_engine* h, void* stream, const float* mt_feats_dev, in
   if (Slen <= 0 || n_pad_tail < 0 || n_pad_tail >= Slen) return h->fail(SS_ERR_INVALID, "bad T2U sequence length");
   const int32_t np = n_pad_tail;
   return t2u_unit_decode(h, S(stream), mt_feats_dev, 1, Slen, nullptr, &np, h->unit_pos_row, mask_eos, argmax_dev, units_dev, count_dev, 0, t2u_out_dev,
-                         logits_dev, "ss_t2u_unit_decode");
+                         logits_dev, nullptr, "ss_t2u_unit_decode");
 }
 
 int ss_unit_position_row(ss_engine* h, const float* row_host) {
@@ -1522,17 +1526,32 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
   return check_launch(h, "ss_mt_features_batch");
 }
 
-int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
-                              const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
+// the checks and packed-output layout of ss_t2u_unit_decode_ragged / _batch_scored
+static int t2u_unit_decode_packed(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
+                                  const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev,
+                                  int64_t* packed_units_dev, float* lprob_dev, const char* where) {
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
   const ss_config& c = h->cfg;
   if (B <= 0 || S_stride <= 0 || S_stride > c.max_mt_positions || !mt_feats_dev || !n_pad_tail_host || !pos_rows_dev || !argmax_dev ||
       !packed_units_dev)
-    return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_ragged");
+    return h->fail(SS_ERR_INVALID, std::string("bad arguments to ") + where);
   // sample b's [count | units] row of packed_units_dev: L + 1 int64 words
   const int64_t W = (int64_t)S_stride * c.ctc_upsample_rate + 1;
   return t2u_unit_decode(h, S(stream), mt_feats_dev, B, S_stride, S_host, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev + 1,
-                         reinterpret_cast<int32_t*>(packed_units_dev), W, nullptr, nullptr, "ss_t2u_unit_decode_ragged");
+                         reinterpret_cast<int32_t*>(packed_units_dev), W, nullptr, nullptr, lprob_dev, where);
+}
+
+int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
+                              const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev) {
+  return t2u_unit_decode_packed(h, stream, mt_feats_dev, B, S_stride, S_host, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev,
+                                nullptr, "ss_t2u_unit_decode_ragged");
+}
+
+int ss_t2u_unit_decode_batch_scored(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host,
+                                    const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev, float* lprob_dev) {
+  if (h && !lprob_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_unit_decode_batch_scored");
+  return t2u_unit_decode_packed(h, stream, mt_feats_dev, B, Slen, nullptr, n_pad_tail_host, pos_rows_dev, mask_eos, argmax_dev, packed_units_dev,
+                                lprob_dev, "ss_t2u_unit_decode_batch_scored");
 }
 
 int ss_t2u_unit_decode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int Slen, const int32_t* n_pad_tail_host, const float* pos_rows_dev,
@@ -2035,6 +2054,15 @@ int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, i
   if (!h) return SS_ERR_INVALID;
   layer_norm(x_dev, C, out_dev, C, g_dev, b_dev, rows, C, S(stream));
   return check_launch(h, "ss_op_layer_norm");
+}
+
+int ss_op_argmax_rows(ss_engine* h, void* stream, const float* logits_dev, int rows, int V, int ld, int n_masked, int64_t* idx_dev, float* lprob_dev) {
+  if (!h || rows < 0 || V <= 0 || ld < V || n_masked < 0 || n_masked > 3 || !logits_dev || !idx_dev) return h ? h->fail(SS_ERR_INVALID, "bad arguments to ss_op_argmax_rows") : SS_ERR_INVALID;
+  if (lprob_dev)
+    argmax_lprob_rows(logits_dev, ld, rows, V, h->mask_pad_unk, n_masked, idx_dev, lprob_dev, S(stream));
+  else
+    argmax_rows(logits_dev, ld, rows, V, h->mask_pad_unk, n_masked, idx_dev, S(stream));
+  return check_launch(h, "ss_op_argmax_rows");
 }
 
 }  // extern "C"

@@ -233,6 +233,9 @@ void embed_tokens_pos(const int64_t* tokens, const int* positions_or_null, int p
 void repeat_rows_add(const float* x, int S, int R, int C, const float* addvec_or_null, float* out, int B, cudaStream_t st);
 // arg-max of log_softmax over V columns of every row, masked columns excluded, first index wins on ties
 void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx, cudaStream_t st);
+// argmax_rows (the same indices, bit for bit) plus each winner's log_softmax value over all V columns, masked ones included
+void argmax_lprob_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx, float* out_lprob,
+                       cudaStream_t st);
 // CTC collapse (dedup consecutive, drop blank/pad) of n_seg sequences of n entries, one CTA each.  Sequence s reads
 // argmax[((s / inner) * n + i) * inner + s % inner] (inner = 2: the arg-max rows of two heads interleaved) and writes
 // out_tokens + s * seg_stride, and out_index (optional) / out_count + 2 * s * seg_stride (seg_stride in int64 words, so that one

@@ -140,6 +140,20 @@ __global__ void argmax_rows_kernel(const float* __restrict__ logits, int ld, int
   if (threadIdx.x == 0) out_idx[blockIdx.x] = bi;
 }
 
+// argmax_rows_kernel plus the winner's log-probability over all V columns (the offline unit decoder's positional scores,
+// ctc_generator.py:54-61): the same reduction, so the index equals argmax_rows_kernel's bit for bit, and the same bytes read
+__global__ void argmax_lprob_rows_kernel(const float* __restrict__ logits, int ld, int V, const int* __restrict__ masked, int n_masked,
+                                         int64_t* __restrict__ out_idx, float* __restrict__ out_lprob) {
+  pdl_trigger();
+  pdl_wait();
+  float lp;
+  const int bi = block_masked_argmax_lprob256(logits + (int64_t)blockIdx.x * ld, V, masked, n_masked, lp);
+  if (threadIdx.x == 0) {
+    out_idx[blockIdx.x] = bi;
+    out_lprob[blockIdx.x] = lp;
+  }
+}
+
 // CTC collapse (block_ctc_collapse), one CTA of 1024 threads per sequence s = blockIdx.x: entries am[((s / inner) * n + i) * inner +
 // s % inner] for i < n (or < n_seq[s / inner]), outputs at s * seg_stride int64 words
 __global__ void ctc_collapse_kernel(const int64_t* __restrict__ am, int n, const int* __restrict__ n_seq, int inner, int blank, int pad,
@@ -340,6 +354,13 @@ void argmax_rows(const float* logits, int ld, int rows, int V, const int* masked
   ++g_launches;
   if (rows <= 0) return;
   launch_pdl(argmax_rows_kernel, dim3(rows), dim3(256), 0, st, logits, ld, V, masked_cols, n_masked, out_idx);
+}
+
+void argmax_lprob_rows(const float* logits, int ld, int rows, int V, const int* masked_cols, int n_masked, int64_t* out_idx, float* out_lprob,
+                       cudaStream_t st) {
+  ++g_launches;
+  if (rows <= 0) return;
+  launch_pdl(argmax_lprob_rows_kernel, dim3(rows), dim3(256), 0, st, logits, ld, V, masked_cols, n_masked, out_idx, out_lprob);
 }
 
 void ctc_collapse_segments(const int64_t* argmax, int n, int inner, int n_seg, int blank, int pad, int64_t* out_tokens, int* out_index,

@@ -89,6 +89,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_ctc_greedy_batch.argtypes = [vp, vp, vp, i32, i32, vp]
     lib.ss_mt_features_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, vp]
     lib.ss_t2u_unit_decode_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, vp, vp]
+    lib.ss_t2u_unit_decode_batch_scored.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, vp, vp, vp]
     lib.ss_unit_position_row.argtypes = [vp, vp]
     lib.ss_vocoder_durations.argtypes = [vp, vp, vp, i32, i32, vp, vp]
     lib.ss_vocoder_generate.argtypes = [vp, vp, i32, i32, i32, i32, vp]
@@ -101,6 +102,7 @@ def load_library() -> ctypes.CDLL:
     lib.ss_op_conv1d.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, ctypes.c_float, i32, vp]
     lib.ss_set_option.argtypes = [vp, ctypes.c_char_p, i32]
     lib.ss_op_layer_norm.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
+    lib.ss_op_argmax_rows.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp, vp]
     lib.ss_debug_copy.argtypes = [vp, ctypes.c_char_p, vp, ctypes.c_size_t]
     lib.ss_launch_count.argtypes = [vp]
     lib.ss_launch_count.restype = i64
@@ -138,6 +140,7 @@ EXPORTED_SYMBOLS = [
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_mt_beam_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
     "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
     "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
+    "ss_t2u_unit_decode_batch_scored", "ss_op_argmax_rows",
 ]
 
 
@@ -561,6 +564,30 @@ class Engine:
         units = [h_packed[b, 1:1 + int(h_packed[b, :1].view(torch.int32)[0])].tolist() for b in range(B)]
         return units, [h_am[b].tolist() for b in range(B)], {"argmax": am, "packed": packed}
 
+    def t2u_unit_decode_batch_scored(self, mt_feats: torch.Tensor, n_pad_tail: Sequence[int], mask_eos: bool = False):
+        """t2u_unit_decode_batch plus every upsampled row's arg-max log-probability (ss_t2u_unit_decode_batch_scored: the reference's
+        CTCSequenceGenerator positional scores, pad-tail rows included).  Returns (units per sample, arg-max per sample, lprob per
+        sample as fp32 [S*rate] host tensors, {"argmax", "packed", "lprob": [B, S*rate] device}); units, arg-max and lprob come from
+        ONE device->host copy."""
+        assert mt_feats.is_cuda and mt_feats.is_contiguous() and mt_feats.dim() == 3
+        B, S = int(mt_feats.shape[0]), int(mt_feats.shape[1])
+        if len(n_pad_tail) != B:
+            raise EngineError(f"{len(n_pad_tail)} pad-tail lengths for a batch of {B}")
+        L = S * self.cfg.ctc_upsample_rate
+        rows = torch.stack([self.unit_position_row(b) for b in range(B)]).to(self.device) if B else self._f32(0, self.cfg.unit_dim)
+        n_lp = (B * L + 1) // 2  # int64 words holding the fp32 scores
+        buf = torch.empty(B * (2 * L + 1) + n_lp, dtype=torch.int64, device=self.device)  # [argmax B*L | packed B*(L+1) | lprob]
+        am, packed = buf[:B * L].view(B, L), buf[B * L:B * (2 * L + 1)].view(B, L + 1)
+        lprob = buf[B * (2 * L + 1):].view(torch.float32)[:B * L].view(B, L)
+        pads = (ctypes.c_int32 * max(B, 1))(*[int(x) for x in n_pad_tail])
+        self._check(self.lib.ss_t2u_unit_decode_batch_scored(self._h, self._stream(), mt_feats.data_ptr(), B, S, pads, rows.data_ptr(),
+                                                             int(mask_eos), am.data_ptr(), packed.data_ptr(), lprob.data_ptr()))
+        host = buf.cpu()
+        h_am, h_packed = host[:B * L].view(B, L), host[B * L:B * (2 * L + 1)].view(B, L + 1)
+        h_lp = host[B * (2 * L + 1):].view(torch.float32)[:B * L].view(B, L)
+        units = [h_packed[b, 1:1 + int(h_packed[b, :1].view(torch.int32)[0])].tolist() for b in range(B)]
+        return units, [h_am[b].tolist() for b in range(B)], [h_lp[b] for b in range(B)], {"argmax": am, "packed": packed, "lprob": lprob}
+
     def t2u_unit_decode_ragged(self, mt_feats: torch.Tensor, lengths: Sequence[int], n_pad_tail: Sequence[int], pos_rows: Optional[torch.Tensor] = None,
                                mask_eos: bool = False):
         """t2u_unit_decode for every sample of mt_feats [B, S_stride, mt_dim] where sample b has only its first lengths[b] positions
@@ -810,6 +837,16 @@ class Engine:
         out = torch.empty_like(x)
         self._check(self.lib.ss_op_layer_norm(self._h, self._stream(), x.data_ptr(), x.shape[0], x.shape[1], g.data_ptr(), b.data_ptr(), out.data_ptr()))
         return out
+
+    def op_argmax_rows(self, logits: torch.Tensor, n_masked: int, scored: bool):
+        """ss_op_argmax_rows on a 2-D fp32 device tensor: (indices, log-probabilities or None)"""
+        assert logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+        rows, V = logits.shape
+        idx = torch.empty(rows, dtype=torch.int64, device=self.device)
+        lp = torch.empty(rows, dtype=torch.float32, device=self.device) if scored else None
+        self._check(self.lib.ss_op_argmax_rows(self._h, self._stream(), logits.data_ptr(), rows, V, logits.stride(0), n_masked, idx.data_ptr(),
+                                               self._ptr(lp)))
+        return idx, lp
 
     # Attention / depthwise-conv parity hooks (ss_op_*_attention, ss_op_*depthwise*).  Matrices are 2-D device fp32 tensors whose rows
     # may be strided (column slices of a fused buffer); kernel: 0 = the engine's choice, 1 = row kernel, 2 = tile kernel.

@@ -11,6 +11,7 @@ Drop-in for the reference's `CTCMultiDecoderSequenceGenerator` as `fairseq-gener
     prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum (:262-271) host
     mt_decoder(features_only) on the padded batch (:287-291)                      ss_mt_features_batch
     T2U encoder -> CTC unit decoder -> CTC generate (:293-330)                    ss_t2u_unit_decode_batch
+      with the unit hypothesis' scores (generate(scores=True))                    ss_t2u_unit_decode_batch_scored
 
 Each stage is one call for the whole batch (the entry points split batches larger than their workspace budget into groups
 themselves), so the host synchronisations of generate() do not grow with B.  Samples only interact through three quirks of the
@@ -50,11 +51,14 @@ class OfflineS2STGenerator:
         engine.set_chunk(None, None)  # offline model: full attention, symmetric convolutions (N10)
 
     @torch.inference_mode()
-    def generate(self, src_tokens: torch.Tensor, src_lengths: Sequence[int], forced_mt: Optional[List[List[int]]] = None) -> List[Dict[str, object]]:
+    def generate(self, src_tokens: torch.Tensor, src_lengths: Sequence[int], forced_mt: Optional[List[List[int]]] = None,
+                 scores: bool = False) -> List[Dict[str, object]]:
         """src_tokens [B, F, 80] fbank + CMVN features on the engine's device (zero padded), src_lengths [B].
         Returns one dict per sample: asr_tokens / st_tokens (CTC prints), mt_tokens (hypothesis without eos), units (the
         reference's `finalized[b][0]["tokens"]`), unit_argmax (per-position arg-max, padded positions included) and
-        mt_feats ([max_tgt_len, 512], device).  forced_mt: use these MT hypotheses instead of searching (tests)."""
+        mt_feats ([max_tgt_len, 512], device).  forced_mt: use these MT hypotheses instead of searching (tests).
+        scores: each result also gets the unit hypothesis' scores as `fairseq-generate` prints them (ctc_generator.py:54-61):
+        unit_positional_scores (fp32 [max_tgt_len * rate], pad-tail rows included) and unit_score (their fp32 sum)."""
         eng, c = self.engine, self.cfg
         if src_tokens.dim() != 3 or not src_tokens.is_cuda:
             raise EngineError("src_tokens must be a [B, F, feat_dim] CUDA tensor")
@@ -76,7 +80,12 @@ class OfflineS2STGenerator:
         n_pad = [max_tgt_len - (len(h) + 1) for h in hyps]
         prev = [[c.eos] + h + [c.pad] * n for h, n in zip(hyps, n_pad)]
         feats = eng.mt_features_batch(enc, out_len, prev)  # [B, max_tgt_len, mt_dim]
-        units, argmax, _ = eng.t2u_unit_decode_batch(feats, n_pad, mask_eos=True)  # N1, N2, N3
+        if scores:
+            units, argmax, lprob, _ = eng.t2u_unit_decode_batch_scored(feats, n_pad, mask_eos=True)  # N1, N2, N3
+            for b in range(B):
+                results[b].update(unit_positional_scores=lprob[b], unit_score=float(lprob[b].sum()))
+        else:
+            units, argmax, _ = eng.t2u_unit_decode_batch(feats, n_pad, mask_eos=True)  # N1, N2, N3
         for b in range(B):
             results[b].update(mt_tokens=hyps[b], units=units[b], unit_argmax=argmax[b], mt_feats=feats[b])
         return results
