@@ -226,7 +226,10 @@ int ss_mt_features_batch(ss_engine* h, void* stream, const float* enc_dev, int B
  *    305-308, and the previous call's final, eos-forcing step had already fed it), which leaves a duplicate cache entry per call;
  *  - cross-attention K / V are projected only for encoder rows beyond those cached by earlier calls (transformer_layer.py:
  *    492-505) and never refreshed, i.e. early rows keep the projections of the then-provisional encoder output.
- * Both quirks change the hypothesis and are reproduced.  max_len_b = the caller's max_len for max_new_tokens == -1
+ * Both quirks change the hypothesis and are reproduced.  The state shares the handle's MT caches with ss_mt_greedy and ss_mt_features,
+ * which write them from row 0: once either has run on a handle whose state is not empty, ss_mt_greedy_incremental returns SS_ERR_STATE
+ * before any launch until ss_mt_incremental_reset (the batched, beam and pool entry points leave the state alone unless they fall back
+ * to ss_mt_greedy, see there).  ss_debug_copy "mt_inc_state" reads the state back.  max_len_b = the caller's max_len for max_new_tokens == -1
  * (min(int(max_len_a * src_len + max_len_b), max_decoder_positions - 1), sequence_generator.py:205-215).  Requires the
  * persistent MT kernel (option persistent_mt = 1).  Synchronises `stream` once per burst.  A prefix token outside [0, tgt_vocab)
  * is SS_ERR_INVALID, refused before anything is launched or the state changes. */
@@ -418,7 +421,11 @@ int ss_set_option(ss_engine* h, const char* name, int value);
 /* synchronous copy of a diagnostic buffer to the host: "persist_ts" = uint64 ns stamps of the last persistent step;
  * "persist_time" / "mt_time" / "pool_resample_time" = double[3] {summed ms, launches, summed algorithmic bytes / executed steps /
  * algorithmic bytes} since the last query;
- * "cluster_steps" = long long, encoder steps taken by the cluster kernel */
+ * "cluster_steps" = long long, encoder steps taken by the cluster kernel;
+ * "mt_inc_state" / "pool_mt_inc_state:<slot>" = the incremental MT state of the handle (ss_mt_greedy_incremental) or of one pool slot
+ * (ss_pool_mt_greedy_incremental): {entries, cross_rows} as int32, then fp32 self-attention K and V, each [mt_layers][entries][mt_dim]
+ * (entry p + kv_off holds position p), then cross-attention K | V [mt_layers][cross_rows][2 * mt_dim].  bytes == 8 copies the two counts
+ * alone; any other size below the whole state is SS_ERR_INVALID.  Synchronises the device. */
 int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes);
 int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev,
                      float* out_dev);

@@ -447,7 +447,7 @@ class StreamSpeechOracle:
             q = (q * hd ** -0.5).view(1, H, hd).transpose(0, 1)         # [H,1,hd]
             kk = k.view(-1, H, hd).transpose(0, 1)                       # [H,n,hd]
             vv = v.view(-1, H, hd).transpose(0, 1)
-            w = F.softmax(torch.bmm(q, kk.transpose(1, 2)), dim=-1, dtype=torch.float32)
+            w = F.softmax(torch.bmm(q, kk.transpose(1, 2)), dim=-1, dtype=q.dtype)  # fp32 in the reference, as in mha()
             a = torch.bmm(w, vv).transpose(0, 1).contiguous().view(1, 1, c.mt_dim)
             return _lin(a, self.sd, prefix + ".out_proj")
 

@@ -174,6 +174,7 @@ struct ss_engine {
   int mt_inc_self_len = 0;           // entries in the self-attention cache (can exceed the hypothesis length: call boundaries
                                      // feed the last prefix token again, speech_to_text.s2tt agent + sequence_generator.py:338-346)
   int mt_inc_cross_rows = 0;         // encoder rows whose cross K / V were appended (never refreshed, transformer_layer.py:492-505)
+  bool mt_inc_overwritten = false;   // ss_mt_greedy / ss_mt_features (mt_begin) wrote over a non-empty incremental state: refused until reset
   int64_t* mt_tok_dev = nullptr;  // [max_pos]
   int64_t* mt_next_pinned = nullptr;
   // vocoder: the unit sequences of the last ss_vocoder_durations_ragged call, cached for ss_vocoder_generate_ragged

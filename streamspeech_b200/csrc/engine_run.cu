@@ -343,6 +343,7 @@ void dec_layer(ss_engine* h, const DecLayerW& L, float* x, int n, int dim, int f
 // keep_rows > 0: rows [0, keep_rows) of every layer survive a reallocation (incremental-state decoding keeps cross K / V across calls)
 int ensure_mt_cross(ss_engine* h, int T, int keep_rows = 0) {
   if (T <= h->mt_cross_cap) return SS_OK;
+  if (keep_rows < h->mt_inc_cross_rows) h->mt_inc_overwritten = true;  // (as mt_begin: the rows of the incremental state are lost)
   const int cap = std::max(T + T / 2, 512);
   const size_t row = (size_t)2 * h->cfg.mt_dim;
   float* fresh = nullptr;
@@ -385,8 +386,10 @@ void mt_project_cross(ss_engine* h, const float* enc, int from, int T, float* ca
 }
 
 // cross-attention K | V of the encoder rows.  Rows the caller declared final (ss_mt_stable_rows) at the previous call were
-// projected then and are not touched again; everything above is (re)computed.
+// projected then and are not touched again; everything above is (re)computed.  The search that follows writes the self-attention
+// cache from entry 0: both are the buffers of the handle's incremental state, which is then no longer the one its calls left.
 void mt_begin(ss_engine* h, const float* enc_dev, int T, cudaStream_t st) {
+  if (h->mt_inc_self_len > 0 || h->mt_inc_cross_rows > 0) h->mt_inc_overwritten = true;
   int from = (h->mt_cross_enc == enc_dev) ? std::min(h->mt_cross_final, T) : 0;
   if (from < 0) from = 0;
   mt_project_cross(h, enc_dev, from, T, h->mt_cross_kv, h->mt_cross_cap, st);
@@ -455,6 +458,9 @@ int mt_incremental_len(ss_engine* h, int slot, int start, int max_new_tokens, in
   const int ml = (max_new_tokens == -1) ? max_len_b : start + max_new_tokens;
   if (ml < 1) return h->fail(SS_ERR_INVALID, "min_len cannot be larger than max_len");
   if (start > ml) return h->fail(SS_ERR_INVALID, "prefix longer than max_len");
+  if (slot < 0 && h->mt_inc_overwritten)
+    return h->fail(SS_ERR_STATE, "ss_mt_greedy or ss_mt_features ran on this handle after the last incremental call and overwrote the incremental "
+                                 "MT state (they share its caches): call ss_mt_incremental_reset before the next ss_mt_greedy_incremental");
   const int off = self_len - start;
   if (off < 0)
     return h->fail(SS_ERR_STATE, slot < 0 ? "incremental MT state is shorter than the prefix (reset missing, or a prefix that this state did not produce)"
@@ -1187,12 +1193,12 @@ int ss_mt_features(ss_engine* h, void* stream, const float* enc_dev, int T, cons
   if (n <= 0 || n > c.max_mt_positions || T <= 0) return h->fail(SS_ERR_INVALID, "bad MT sequence length");
   if (!mt_tokens_in_vocab(h, tokens_host, n)) return h->fail(SS_ERR_INVALID, "ss_mt_features: token outside the vocabulary");
   cudaStream_t st = S(stream);
-  int rc = ensure_mt_cross(h, T);
-  if (rc) return rc;
   int n_valid = n;  // trailing pads (whole_word path, agent:576-591) are masked as keys
   while (n_valid > 0 && tokens_host[n_valid - 1] == c.pad) --n_valid;
   for (int i = 0; i < n_valid; ++i)
     if (tokens_host[i] == c.pad) return h->fail(SS_ERR_INVALID, "pads are only supported as a tail");
+  int rc = ensure_mt_cross(h, T);
+  if (rc) return rc;
   const int dim = c.mt_dim;
   if (!ws_begin(h, ((size_t)n * (dim * 7 + c.mt_ffn) + 4096) * sizeof(float))) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
   DecScratch s = dec_scratch(h, n, dim, c.mt_ffn);
@@ -1367,6 +1373,7 @@ int ss_mt_incremental_reset(ss_engine* h) {
   if (!h) return SS_ERR_INVALID;
   h->mt_inc_self_len = 0;
   h->mt_inc_cross_rows = 0;
+  h->mt_inc_overwritten = false;
   return SS_OK;
 }
 
@@ -1956,6 +1963,49 @@ int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes) 
   if (n == "cluster_steps") {  // long long: encoder steps taken by the cluster kernel so far
     if (bytes < sizeof(long long)) return h->fail(SS_ERR_INVALID, "cluster_steps needs a long long");
     *(long long*)host_dst = h->cl_steps;
+    return SS_OK;
+  }
+  // the incremental MT state of the handle or of one pool slot: {entries, cross_rows} (int32), self K, self V [mt_layers][entries][mt_dim],
+  // cross K | V [mt_layers][cross_rows][2 * mt_dim]; bytes == 8 copies the two counts alone
+  if (n == "mt_inc_state" || n.rfind("pool_mt_inc_state:", 0) == 0) {
+    const ss_config& c = h->cfg;
+    const size_t D = c.mt_dim, NL = c.mt_layers;
+    int entries = h->mt_inc_self_len, rows = h->mt_inc_cross_rows;
+    const float *sk = h->mt_self_k, *sv = h->mt_self_v, *ckv = h->mt_cross_kv;
+    size_t cross_cap = h->mt_cross_cap;
+    if (n[0] == 'p') {
+      ss_engine::StreamPool& P = h->pool;
+      char* end = nullptr;
+      const long slot = std::strtol(n.c_str() + 18, &end, 10);
+      if (!P.n_slots || end == n.c_str() + 18 || *end || slot < 0 || slot >= P.n_slots) return h->fail(SS_ERR_INVALID, "bad pool slot in " + n);
+      entries = P.mt_inc_self_len[slot];
+      rows = P.mt_inc_cross_rows[slot];
+      const size_t self_slot = NL * c.max_mt_positions * D;
+      sk = P.mt_self_kv ? P.mt_self_kv + slot * self_slot : nullptr;
+      sv = P.mt_self_kv ? P.mt_self_kv + (P.n_slots + slot) * self_slot : nullptr;
+      ckv = P.mt_cross ? P.mt_cross + slot * NL * P.Tcap * 2 * D : nullptr;
+      cross_cap = P.Tcap;
+    }
+    int32_t* counts = (int32_t*)host_dst;
+    const size_t need = 2 * sizeof(int32_t) + (2 * NL * entries * D + NL * rows * 2 * D) * sizeof(float);
+    if (bytes == 2 * sizeof(int32_t)) {
+      counts[0] = entries;
+      counts[1] = rows;
+      return SS_OK;
+    }
+    if (bytes < need) return h->fail(SS_ERR_INVALID, n + " needs " + std::to_string(need) + " bytes");
+    counts[0] = entries;
+    counts[1] = rows;
+    float* out = (float*)(counts + 2);
+    cudaDeviceSynchronize();
+    for (size_t l = 0; l < NL && entries > 0; ++l)
+      if (cudaMemcpy(out + l * entries * D, sk + l * c.max_mt_positions * D, entries * D * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
+          cudaMemcpy(out + (NL + l) * entries * D, sv + l * c.max_mt_positions * D, entries * D * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return h->fail(SS_ERR_CUDA, "cudaMemcpy failed");
+    out += 2 * NL * entries * D;
+    for (size_t l = 0; l < NL && rows > 0; ++l)
+      if (cudaMemcpy(out + l * rows * 2 * D, ckv + l * cross_cap * 2 * D, rows * 2 * D * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return h->fail(SS_ERR_CUDA, "cudaMemcpy failed");
     return SS_OK;
   }
   if (n == "mt_time") {  // double[3] = {summed ms, launches, summed steps} of the single-token MT kernel since the last query

@@ -713,6 +713,21 @@ class Engine:
         self._check(self.lib.ss_debug_copy(self._h, b"mt_time", buf, ctypes.sizeof(buf)))
         return float(buf[0]), int(buf[1]), float(buf[2])
 
+    def mt_incremental_state(self, slot: Optional[int] = None) -> Dict[str, object]:
+        """the incremental MT state of the handle (slot None: mt_greedy_incremental's) or of one pool slot (ss_debug_copy "mt_inc_state" /
+        "pool_mt_inc_state:<slot>") as CPU tensors: {"entries", "cross_rows", "self_k", "self_v" [mt_layers, entries, mt_dim],
+        "cross_kv" [mt_layers, cross_rows, 2 * mt_dim]}"""
+        name = b"mt_inc_state" if slot is None else b"pool_mt_inc_state:%d" % int(slot)
+        counts = (ctypes.c_int32 * 2)()
+        self._check(self.lib.ss_debug_copy(self._h, name, counts, ctypes.sizeof(counts)))
+        E, R = int(counts[0]), int(counts[1])
+        L, D = self.cfg.mt_layers, self.cfg.mt_dim
+        buf = torch.empty(2 + 2 * L * E * D + 2 * L * R * D, dtype=torch.float32)
+        self._check(self.lib.ss_debug_copy(self._h, name, buf.data_ptr(), buf.numel() * 4))
+        assert buf[:2].view(torch.int32).tolist() == [E, R]
+        kv = buf[2:2 + 2 * L * E * D].view(2, L, E, D)
+        return {"entries": E, "cross_rows": R, "self_k": kv[0], "self_v": kv[1], "cross_kv": buf[2 + 2 * L * E * D:].view(L, R, 2 * D)}
+
     def cluster_steps(self) -> int:
         """encoder steps taken by the cluster kernel (option persistent_encoder_cluster) since the engine was created"""
         buf = ctypes.c_longlong(0)
