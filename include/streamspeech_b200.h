@@ -466,6 +466,64 @@ int ss_op_ms_depthwise(ss_engine* h, void* stream, const float* x_dev, int64_t s
                        const float* shift_dev, float* y_dev, int ldy, int rows, int C, int k, int n, const int32_t* slot_host, const int32_t* a0_host,
                        const int32_t* nA_host, const int32_t* T_host, const int32_t* conv_chunk_host, const int32_t* row0_host);
 
+/* ---- ASR-BLEU transcriber: fairseq's Wav2VecCtc (wav2vec 2.0 + CTC letter projection), the `en` model of asr_bleu/asr_model_cfgs.json,
+ * as asr_bleu/utils.py:247-288 runs it: model.w2v_encoder(audio, padding_mask)["encoder_out"], then torchaudio's ctc_decoder at
+ * beam 1 without lexicon or LM.  A handle of its own: nothing is shared with an ss_engine.  Same conventions as above (caller-owned
+ * device buffers, work on the caller's stream, negative codes + ss_asr_last_error, all state per handle).
+ * Settings the state dict's shapes do not carry come from the checkpoint's stored cfg (or fairseq's defaults) through ss_asr_config;
+ * everything outside the `en` model's family is refused at ss_asr_create with a message naming the setting. */
+typedef struct ss_asr ss_asr;
+#define SS_ASR_MAX_CONV 8
+typedef struct ss_asr_config {
+  int32_t n_conv;                        /* feature-extractor conv layers (conv_feature_layers), 1 .. SS_ASR_MAX_CONV */
+  int32_t conv_stride[SS_ASR_MAX_CONV];  /* their strides (kernel sizes and widths come from the weights) */
+  int32_t extractor_layer_norm;          /* extractor_mode: 1 = "layer_norm"; 0 = "default" (group norm) is refused */
+  int32_t layer_norm_first;              /* 1 = pre-LN layers; 0 (post-LN) is refused */
+  int32_t pos_conv_depth;                /* 1; deeper positional convs are refused */
+  int32_t conformer;                     /* layer_type: 0 = "transformer"; 1 ("conformer") is refused */
+  int32_t heads;                         /* encoder_attention_heads, 0 = dim / 64; a head dim other than 64 is refused */
+  int32_t normalize;                     /* task.normalize: 1 = layer_norm over each whole waveform (eps 1e-5) before the extractor */
+  int32_t max_frames;                    /* longest utterance in encoder frames (20 ms), 0 = 4096 (81.9 s at 16 kHz) */
+  int32_t time_stages;                   /* 1: CUDA events around each stage (ss_asr_stage_ms); the call then synchronises per group */
+} ss_asr_config;
+/* Encoder frames are counted in launch groups of at most this many padded rows (B_group x longest T of the group); a longer single
+ * utterance forms a group of its own.  The handle's workspace for a full group is about 2 GB at the Large shapes: the extractor's two
+ * ping-pong buffers (conv layer 0 gives ~64 rows of C floats per encoder frame: ~1.07 GB + 0.54 GB at C = 512) and ~45 KB per encoder row. */
+#define SS_ASR_BATCH_ROWS 8192
+int ss_asr_create(ss_asr** out, int device, const ss_asr_config* cfg);
+int ss_asr_destroy(ss_asr* h);
+const char* ss_asr_last_error(const ss_asr* h); /* h == NULL: why this thread's last ss_asr_create was refused */
+/* One fp32 tensor by its fairseq key as stored: "w2v_encoder.w2v_model.*" and "w2v_encoder.proj.*".  Keys the forward pass does not
+ * read (mask_emb, quantizer, ...) are ignored.  pos_conv may come weight-normed (weight_g / weight_v, norm over dims 0 and 1) or folded. */
+int ss_asr_load_tensor(ss_asr* h, const char* key, const float* data_host, int ndim, const int64_t* shape);
+/* Takes every size from the shapes (conv kernels and widths, model dim, FFN, layers, positional-conv kernel and groups, vocabulary),
+ * folds the weight norm, repacks and uploads.  SS_ERR_MISSING names the first missing key; SS_ERR_INVALID a shape the kernels do not take. */
+int ss_asr_finalize(ss_asr* h);
+/* encoder frames of an utterance of n samples: floor((L - k) / s) + 1 per conv layer (0 when some layer gets fewer than k frames);
+ * -1 before ss_asr_finalize */
+int64_t ss_asr_num_frames(const ss_asr* h, int64_t n_samples);
+/* Transcribe B utterances: sample b is audio_dev[offsets_host[b] .. offsets_host[b + 1]) (fp32, 16-bit PCM scaled by 1/32768, at the
+ * model's rate).  Per utterance: emissions = proj(encoder(extractor(audio))) [T_b][V]; arg-max of every row over the raw emissions with
+ * <unk> (index 3) excluded, first index on ties (flashlight's lexicon-free beam-1 step with unk_score = -inf and no LM); then repeats
+ * collapsed and blanks (index 0, "<s>") dropped (torchaudio CTCDecoder._get_tokens).
+ * packed_out_dev: row b at b * packed_stride int64 words = [count (int32 in the first word) | tokens[count]]; packed_stride >= T_b + 1.
+ * argmax_dev (optional) [sum T_b] int64 and emissions_dev (optional) [sum T_b][V] fp32: rows of the utterances in order.
+ * Utterances run in launch groups (SS_ASR_BATCH_ROWS), padded to the group's longest; no GEMM splits K and the attention takes one
+ * kernel for every shape, so an utterance's emissions are bit-identical to a call with that utterance alone.
+ * Errors, before any launch: SS_ERR_STATE before finalize; SS_ERR_INVALID for B <= 0, a null pointer, decreasing offsets, an utterance
+ * too short for one frame or a packed_stride below T_b + 1; SS_ERR_CAPACITY for T_b > max_frames.  Synchronises `stream` once per
+ * launch group (upload of the lengths), and per stage when time_stages is set. */
+int ss_asr_transcribe(ss_asr* h, void* stream, const float* audio_dev, const int64_t* offsets_host, int B, int64_t* packed_out_dev,
+                      int64_t packed_stride, int64_t* argmax_dev, float* emissions_dev);
+/* The activations after one stage of the same forward pass, rows of the utterances in order (test hook): stage 0 = extractor output
+ * [sum T_b][C] (after the last conv block's GELU), 1 = feature LayerNorm + post_extract_proj [.][D], 2 = + positional conv [.][D],
+ * 3 + l = after transformer layer l [.][D], 3 + layers = final LayerNorm [.][D], 4 + layers = emissions [.][V].  Errors as ss_asr_transcribe,
+ * and SS_ERR_INVALID for a stage outside [0, 4 + layers]. */
+int ss_asr_debug_stage(ss_asr* h, void* stream, const float* audio_dev, const int64_t* offsets_host, int B, int stage, float* out_dev);
+/* {extractor, positional conv, transformer layers, final LayerNorm + proj + arg-max + collapse} device ms summed over the calls since
+ * the last query (time_stages = 1; zeros otherwise), and resets them. */
+int ss_asr_stage_ms(ss_asr* h, double* ms_out4);
+
 /* number of kernels this library has launched in this process (bench.py reports the difference over the timed region as
  * gpu_launches; the counter is process-wide, not per handle) */
 int64_t ss_launch_count(const ss_engine* h);

@@ -1,0 +1,175 @@
+"""`python -m streamspeech_b200.asr_bleu`: asr_bleu/compute_asr_bleu.py (and, with --rm-silence, asr_bleu_rm_silence/compute_asr_bleu.py)
+on the engine's transcriber.  Same flags, files and printed score line; the transcriber runs batched on the GPU (asr.ASRTranscriber) and
+BLEU is sacrebleu 2.2.0's corpus_bleu restated (sacrebleu_compat).  Only the `en` model is offered, from local files: nothing is
+downloaded.
+"""
+from __future__ import annotations
+
+import argparse
+import glob
+import os
+import re
+import sys
+from pathlib import Path
+from typing import List, Optional, Sequence
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from streamspeech_b200.asr import AudioRefused  # noqa: E402
+from streamspeech_b200.sacrebleu_compat import corpus_bleu  # noqa: E402
+
+# asr_bleu/asr_model_cfgs.json, en / oct22: the files a user fetches once and passes as --asr-model / --asr-dict
+EN_MODEL_URLS = {"oct22": ("https://dl.fbaipublicfiles.com/fairseq/wav2vec/wav2vec_vox_960h_pl.pt",
+                           "https://dl.fbaipublicfiles.com/fairseq/wav2vec/dict.ltr.txt")}
+
+
+def extract_audio_for_eval(audio_dirpath: str, audio_format: str, sort_numeric: bool = False) -> List[str]:
+    """compute_asr_bleu.py:36-62: for i < the number of *_pred.wav files, {i}_pred.wav or else the one {i}_spk*_pred.wav"""
+    if audio_format != "n_pred.wav":
+        raise NotImplementedError(audio_format)
+    audio_fp_list = glob.glob((Path(audio_dirpath) / "*_pred.wav").as_posix())
+    if sort_numeric:  # the rm_silence variant sorts first (and fails on a name without a numeric prefix)
+        audio_fp_list = sorted(audio_fp_list, key=lambda x: int(os.path.basename(x).split("_")[0]))
+    out = []
+    for i in range(len(audio_fp_list)):
+        fp = (Path(audio_dirpath) / f"{i}_pred.wav").as_posix()
+        if fp not in audio_fp_list:
+            cands = glob.glob((Path(audio_dirpath) / f"{i}_spk*_pred.wav").as_posix())
+            if len(cands) != 1:
+                raise AssertionError(f"{i}_pred.wav does not exist in {audio_dirpath} and {len(cands)} files match {i}_spk*_pred.wav")
+            fp = cands[0]
+        out.append(fp)
+    return out
+
+
+_PANDAS_NA = {"", "#N/A", "#N/A N/A", "#NA", "-1.#IND", "-1.#QNAN", "-NaN", "-nan", "1.#IND", "1.#QNAN", "<NA>", "N/A", "NA", "NULL", "NaN",
+              "None", "n/a", "nan", "null"}  # pd.read_csv's default na_values
+
+
+def _is_number(c: str) -> bool:
+    try:
+        float(c)
+        return True
+    except ValueError:
+        return False
+
+
+def read_tsv_column(path: str, column: str) -> List[str]:
+    """pd.read_csv(path, sep="\\t", quoting=3)[column]: no quote processing, blank lines skipped, the first line is the header"""
+    with open(path, encoding="utf-8") as f:
+        rows = [ln.rstrip("\r\n") for ln in f]
+    rows = [r for r in rows if r.strip() != ""]
+    header = rows[0].split("\t")
+    if column not in header:
+        raise KeyError(column)
+    j = header.index(column)
+    cells = [r.split("\t")[j] for r in rows[1:]]
+    # pandas turns these into NaN, and a column of numbers into numbers; the reference's .strip() then fails on them
+    for i, c in enumerate(cells):
+        if c in _PANDAS_NA:
+            raise ValueError(f"{path}: row {i + 1} of column {column!r} is {c!r}, which pd.read_csv reads as NaN; the reference fails on it")
+    if cells and all(_is_number(c) for c in cells):
+        raise ValueError(f"{path}: column {column!r} holds only numbers, which pd.read_csv reads as numbers; the reference fails on it")
+    return cells
+
+
+def extract_text_for_eval(references_filepath: str, reference_format: str, reference_tsv_column: Optional[str] = None) -> List[str]:
+    """compute_asr_bleu.py:65-78"""
+    if reference_format == "txt":
+        with open(references_filepath, "r") as f:
+            return [ln.strip() for ln in f.readlines()]
+    if reference_format == "tsv":
+        return [s.strip() for s in read_tsv_column(references_filepath, reference_tsv_column)]
+    raise NotImplementedError(reference_format)
+
+
+def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
+    p = argparse.ArgumentParser(description="ASR-BLEU between generated audio and text references, on the engine's GPU transcriber.")
+    p.add_argument("--lang", type=str)
+    p.add_argument("--asr_version", type=str, default="oct22")
+    p.add_argument("--audio_dirpath", type=str)
+    p.add_argument("--reference_path", type=str)
+    p.add_argument("--reference_format", choices=["txt", "tsv"])
+    p.add_argument("--reference_tsv_column", default=None, type=str)
+    p.add_argument("--audio_format", default="n_pred.wav", choices=["n_pred.wav"])
+    p.add_argument("--results_dirpath", default=None, type=str)
+    p.add_argument("--transcripts_path", default=None, type=str, help="write the transcripts here, one per line (the rm_silence variant)")
+    p.add_argument("--rm-silence", action="store_true", help="asr_bleu_rm_silence/: drop runs of >= 10 zero samples; a failed "
+                                                             "transcription raises instead of scoring as an empty string; no pred.txt")
+    p.add_argument("--asr-model", default=None, help="local path of the fairseq checkpoint (or 'synthetic': the seeded test model)")
+    p.add_argument("--asr-dict", default=None, help="local path of dict.ltr.txt")
+    p.add_argument("--asr-setting", action="append", default=[], metavar="KEY=VALUE",
+                   help="override a setting read from the checkpoint's cfg (or the en model's published ones when the cfg cannot be "
+                        "read): conv_feature_layers, extractor_mode, layer_norm_first, pos_conv_depth, layer_type, "
+                        "encoder_attention_heads, normalize, sample_rate")
+    p.add_argument("--device", type=int, default=0)
+    return p.parse_args(argv)
+
+
+def check_model_args(args: argparse.Namespace):
+    if args.lang != "en":
+        raise SystemExit(f"--lang {args.lang}: only the `en` transcriber (fairseq wav2vec 2.0) is offered; the Hugging Face models of other "
+                         "languages and the Hokkien model are not")
+    if args.asr_version not in EN_MODEL_URLS:
+        raise SystemExit(f"--asr_version {args.asr_version}: only {sorted(EN_MODEL_URLS)} exists for en")
+    ckpt_url, dict_url = EN_MODEL_URLS[args.asr_version]
+    for flag, val, url in (("--asr-model", args.asr_model, ckpt_url), ("--asr-dict", args.asr_dict, dict_url)):
+        if val is None and not (flag == "--asr-dict" and args.asr_model == "synthetic"):
+            raise SystemExit(f"{flag} is required: nothing is downloaded; fetch {url} and pass its local path")
+        if val is not None and re.search("^https?://", val):
+            raise SystemExit(f"{flag} {val}: nothing is downloaded; fetch {os.path.basename(val)} and pass its local path")
+
+
+def run_asr_bleu(args: argparse.Namespace, transcriber=None):
+    """-> (transcripts, BLEUScore); writes pred.txt (default variant)"""
+    from streamspeech_b200.asr import ASRTranscriber, parse_settings
+
+    references = extract_text_for_eval(args.reference_path, args.reference_format, args.reference_tsv_column)
+    files = extract_audio_for_eval(args.audio_dirpath, args.audio_format, sort_numeric=args.rm_silence)
+    assert len(files) == len(references)
+    tr = transcriber or ASRTranscriber(args.asr_model, args.asr_dict, args.device, settings=parse_settings(args.asr_setting))
+    waves: List = [None] * len(files)
+    for i, fp in enumerate(files):
+        try:
+            waves[i] = tr.load_audio(fp, rm_silence=args.rm_silence)
+            if tr.num_frames(len(waves[i])) <= 0:
+                raise ValueError(f"{fp}: {len(waves[i])} samples are fewer than one encoder frame needs")
+        except AudioRefused:
+            raise  # a file the reference would transcribe: refused, never scored as ""
+        except Exception:
+            if args.rm_silence:
+                raise
+            waves[i] = None  # compute_asr_bleu.py:141-147: a failed transcription scores as ""
+    ok = [i for i, w in enumerate(waves) if w is not None]
+    texts = tr.transcribe([waves[i] for i in ok])
+    transcripts = [""] * len(files)
+    for i, t in zip(ok, texts):
+        transcripts[i] = t
+    if not args.rm_silence:
+        with open(Path(args.audio_dirpath) / "pred.txt", "w") as f:
+            f.write("\n".join(transcripts))
+    bleu = corpus_bleu(transcripts, [references])
+    print(bleu)
+    return transcripts, bleu
+
+
+def main(argv: Optional[Sequence[str]] = None, transcriber=None):
+    args = parse_args(argv)
+    if transcriber is None:
+        check_model_args(args)
+    transcripts, bleu = run_asr_bleu(args, transcriber)
+    if args.results_dirpath is not None:
+        Path(args.results_dirpath).mkdir(parents=True, exist_ok=True)
+        with open(Path(args.results_dirpath) / f"{args.reference_format}_{args.lang}_bleu.txt", "w") as f:
+            f.write(bleu.format(width=2))
+    if args.transcripts_path is not None:
+        with open(args.transcripts_path, "w") as f:
+            for t in transcripts:
+                f.write(t + "\n")
+    return transcripts, bleu
+
+
+if __name__ == "__main__":
+    main()

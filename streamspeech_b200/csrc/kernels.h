@@ -12,7 +12,7 @@ namespace ss {
 
 extern unsigned long long g_launches;  // kernels launched by this library (process-wide)
 
-enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3 };
+enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3, ACT_GELU = 4 };  // ACT_GELU: exact erf form (gemm_conv, umma2_conv)
 
 // A-operand of a GEMM viewed as a 1-D convolution over a channels-last activation
 // x[B][L_in][C_in]:  A[m][tap*C_in + ci] = pre(x[b][t*stride + tap*dil - pad_left][ci]),

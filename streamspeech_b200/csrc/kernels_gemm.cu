@@ -53,6 +53,7 @@ __device__ __forceinline__ float apply_act(float x, int act) {
     case ACT_RELU: return x > 0.f ? x : 0.f;
     case ACT_SILU: return x / (1.0f + expf(-x));
     case ACT_TANH: return tanhf(x);
+    case ACT_GELU: return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
     default: return x;
   }
 }

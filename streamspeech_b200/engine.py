@@ -36,6 +36,14 @@ class SSConfig(ctypes.Structure):
 
 
 SS_ERR_CAPACITY = -5
+SS_ASR_MAX_CONV = 8
+SS_ASR_BATCH_ROWS = 8192
+
+
+class ASRConfig(ctypes.Structure):
+    _fields_ = [("n_conv", ctypes.c_int32), ("conv_stride", ctypes.c_int32 * SS_ASR_MAX_CONV)] + [
+        (n, ctypes.c_int32) for n in ("extractor_layer_norm", "layer_norm_first", "pos_conv_depth", "conformer", "heads", "normalize",
+                                      "max_frames", "time_stages")]
 
 
 class EngineError(RuntimeError):
@@ -128,11 +136,24 @@ def load_library() -> ctypes.CDLL:
     lib.ss_op_depthwise_bn_silu.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32]
     lib.ss_op_ms_relpos_attention.argtypes = [vp, vp, vp, i32, vp, vp, i64, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     lib.ss_op_ms_depthwise.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.ss_asr_create.argtypes = [ctypes.POINTER(vp), i32, ctypes.POINTER(ASRConfig)]
+    lib.ss_asr_destroy.argtypes = [vp]
+    lib.ss_asr_last_error.argtypes = [vp]
+    lib.ss_asr_last_error.restype = ctypes.c_char_p
+    lib.ss_asr_load_tensor.argtypes = [vp, ctypes.c_char_p, vp, i32, ctypes.POINTER(i64)]
+    lib.ss_asr_finalize.argtypes = [vp]
+    lib.ss_asr_num_frames.argtypes = [vp, i64]
+    lib.ss_asr_num_frames.restype = i64
+    lib.ss_asr_transcribe.argtypes = [vp, vp, vp, vp, i32, vp, i64, vp, vp]
+    lib.ss_asr_debug_stage.argtypes = [vp, vp, vp, vp, i32, i32, vp]
+    lib.ss_asr_stage_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_double)]
     _lib = lib
     return lib
 
 
 EXPORTED_SYMBOLS = [
+    "ss_asr_create", "ss_asr_destroy", "ss_asr_last_error", "ss_asr_load_tensor", "ss_asr_finalize", "ss_asr_num_frames", "ss_asr_transcribe",
+    "ss_asr_debug_stage", "ss_asr_stage_ms",
     "ss_create", "ss_destroy", "ss_last_error", "ss_version", "ss_load_tensor", "ss_finalize", "ss_set_chunk",
     "ss_fbank_num_frames", "ss_fbank", "ss_encoder_out_frames", "ss_encoder_forward", "ss_encoder_stream_reset", "ss_encoder_stream_step", "ss_ctc_greedy", "ss_ctc_greedy_rows", "ss_mt_greedy",
     "ss_mt_features", "ss_mt_stable_rows", "ss_t2u_unit_decode", "ss_unit_position_row", "ss_vocoder_durations", "ss_vocoder_generate", "ss_vocoder_durations_ragged", "ss_vocoder_generate_ragged", "ss_vocoder_hop",
@@ -927,3 +948,98 @@ class Engine:
         self._check(self.lib.ss_op_ms_depthwise(self._h, self._stream(), x.data_ptr(), x.stride(0), x.shape[0], w.data_ptr(), scale.data_ptr(),
                                                 shift.data_ptr(), y.data_ptr(), self._ld(y), y.shape[0], C, k, len(streams),
                                                 *self._ms_args(streams, "conv_chunk")))
+
+
+class ASREngine:
+    """The ASR-BLEU transcriber's handle (ss_asr_*): wav2vec 2.0 CTC emissions, beam-1 arg-max and collapse on one GPU.  `settings`:
+    the ASRConfig fields (n_conv is taken from `strides`)."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], strides: Sequence[int], device: int = 0, **settings):
+        if not torch.cuda.is_available():
+            raise EngineError("streamspeech_b200.ASREngine needs a CUDA device (sm_90a); there is no CPU fallback")
+        self.lib = load_library()
+        self.device = torch.device("cuda", device)
+        self.vocab_size = int(state_dict["w2v_encoder.proj.weight"].shape[0]) if "w2v_encoder.proj.weight" in state_dict else 0
+        c = ASRConfig()
+        c.n_conv = len(strides)
+        for i, s in enumerate(strides[:SS_ASR_MAX_CONV]):
+            c.conv_stride[i] = s
+        defaults = dict(extractor_layer_norm=1, layer_norm_first=1, pos_conv_depth=1, conformer=0, heads=0, normalize=1, max_frames=0,
+                        time_stages=0)
+        defaults.update(settings)
+        for k, v in defaults.items():
+            setattr(c, k, int(v))
+        self._h = ctypes.c_void_p()
+        rc = self.lib.ss_asr_create(ctypes.byref(self._h), device, ctypes.byref(c))
+        if rc != 0:
+            raise EngineError(f"ss_asr_create failed with {rc}: {self.lib.ss_asr_last_error(None).decode()}", rc,
+                              self.lib.ss_asr_last_error(None).decode())
+        try:
+            for k, v in state_dict.items():
+                if v.is_floating_point():
+                    t = v.detach().to(torch.float32).cpu().contiguous()
+                    shape = (ctypes.c_int64 * max(t.dim(), 1))(*t.shape)
+                    self._check(self.lib.ss_asr_load_tensor(self._h, k.encode(), t.data_ptr(), t.dim(), shape))
+            self._check(self.lib.ss_asr_finalize(self._h))
+        except Exception:
+            self.close()
+            raise
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h:
+            self.lib.ss_asr_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, rc: int):
+        if rc != 0:
+            detail = self.lib.ss_asr_last_error(self._h).decode()
+            raise EngineError(f"libstreamspeech_b200 error {rc}: {detail}", rc, detail)
+
+    def num_frames(self, n_samples: int) -> int:
+        return int(self.lib.ss_asr_num_frames(self._h, n_samples))
+
+    def _audio(self, waves: Sequence[torch.Tensor]):
+        offs = [0]
+        for w in waves:
+            offs.append(offs[-1] + int(w.numel()))
+        audio = torch.cat([w.reshape(-1).to(torch.float32) for w in waves]).to(self.device) if offs[-1] else torch.zeros(1, device=self.device)
+        return audio, (ctypes.c_int64 * len(offs))(*offs)
+
+    def transcribe(self, waves: Sequence[torch.Tensor], emissions: bool = False):
+        """-> (token lists, per-frame arg-max list, emissions [sum T][V] or None).  Utterances shorter than one frame raise EngineError."""
+        audio, offs = self._audio(waves)
+        T = [self.num_frames(int(w.numel())) for w in waves]
+        stride = max(T + [0]) + 1
+        packed = torch.zeros(len(waves), stride, dtype=torch.int64, device=self.device)
+        am = torch.empty(max(1, sum(T)), dtype=torch.int64, device=self.device)
+        em = None
+        if emissions:
+            em = torch.empty(max(1, sum(T)), self.vocab_size, dtype=torch.float32, device=self.device)
+        self._check(self.lib.ss_asr_transcribe(self._h, torch.cuda.current_stream(self.device).cuda_stream, audio.data_ptr(), offs, len(waves),
+                                               packed.data_ptr(), stride, am.data_ptr(), None if em is None else em.data_ptr()))
+        host = packed.cpu()
+        toks = []
+        for b in range(len(waves)):
+            n = int(host[b, 0].item() & 0xFFFFFFFF)
+            toks.append(host[b, 1:1 + n].tolist())
+        return toks, am.cpu()[:sum(T)].tolist(), em
+
+    def stage(self, waves: Sequence[torch.Tensor], stage: int, width: int) -> torch.Tensor:
+        """ss_asr_debug_stage: activations after `stage`, rows of the utterances in order"""
+        audio, offs = self._audio(waves)
+        rows = sum(max(0, self.num_frames(int(w.numel()))) for w in waves)
+        out = torch.empty(max(1, rows), width, dtype=torch.float32, device=self.device)
+        self._check(self.lib.ss_asr_debug_stage(self._h, torch.cuda.current_stream(self.device).cuda_stream, audio.data_ptr(), offs, len(waves),
+                                                stage, out.data_ptr()))
+        return out[:rows]
+
+    def stage_ms(self) -> List[float]:
+        buf = (ctypes.c_double * 4)()
+        self._check(self.lib.ss_asr_stage_ms(self._h, buf))
+        return list(buf)

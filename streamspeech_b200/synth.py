@@ -286,3 +286,58 @@ def make_audio(seconds: float, seed: int = 1234, sample_rate: int = 16000) -> to
     x = (x + 2.0 * noise) * env
     x = x / x.abs().max() * 0.3
     return x.float()
+
+
+# ---- the ASR-BLEU transcriber: wav2vec 2.0 Large (LV-60) + CTC, the `en` model of asr_bleu/asr_model_cfgs.json.  The published
+# configuration (conv_feature_layers, 24 pre-LN layers of width 1024, 16 heads, FFN 4096, pos_conv k = 128 in 16 groups); the real
+# checkpoint is not read here.
+W2V_CONV_LAYERS = [(512, 10, 5)] + [(512, 3, 2)] * 4 + [(512, 2, 2)] * 2
+W2V_LETTERS = ["|", "E", "T", "A", "O", "N", "I", "H", "S", "R", "D", "L", "U", "M", "W", "C", "F", "G", "Y", "P", "B", "V", "K", "'", "X",
+               "J", "Q", "Z"]  # dict.ltr.txt's order
+
+
+def make_w2v_ctc_state_dict(seed: int = 7, dim: int = 1024, ffn: int = 4096, layers: int = 24, conv_layers=None, pos_k: int = 128,
+                            pos_groups: int = 16, vocab: int = 32) -> Dict[str, torch.Tensor]:
+    """Seeded fp32 Wav2VecCtc state dict with fairseq's key names ("w2v_encoder.w2v_model.*", "w2v_encoder.proj.*"), pos_conv
+    weight-normed (weight_g / weight_v).  Calibration: weights at std ~ 1/sqrt(fan_in) keep the pre-LN residual stream bounded over 24
+    layers; the final LayerNorm's output then varies little from frame to frame, so the proj is scaled up (std 3 / sqrt(dim)) and the
+    blank gets a small lead (+0.3): a frame's arg-max is blank about half the time (measured 4-62 % on make_audio inputs), not always."""
+    g = torch.Generator().manual_seed(seed)
+    conv_layers = conv_layers or W2V_CONV_LAYERS
+    P = "w2v_encoder.w2v_model."
+    sd: Dict[str, torch.Tensor] = {}
+    cin = 1
+    for i, (c, k, _) in enumerate(conv_layers):
+        sd[f"{P}feature_extractor.conv_layers.{i}.0.weight"] = _normal(g, (c, cin, k), math.sqrt(2.0 / (cin * k)))
+        sd[f"{P}feature_extractor.conv_layers.{i}.0.bias"] = _normal(g, (c,), 0.05)
+        _ln(g, sd, f"{P}feature_extractor.conv_layers.{i}.2.1", c)
+        cin = c
+    _ln(g, sd, P + "layer_norm", cin)
+    sd[P + "post_extract_proj.weight"] = _normal(g, (dim, cin), 1.0 / math.sqrt(cin))
+    sd[P + "post_extract_proj.bias"] = _normal(g, (dim,), 0.02)
+    cg = dim // pos_groups
+    sd[P + "encoder.pos_conv.0.weight_v"] = _normal(g, (dim, cg, pos_k), math.sqrt(4.0 / (pos_k * dim)))
+    sd[P + "encoder.pos_conv.0.weight_g"] = 0.5 + torch.rand((1, 1, pos_k), generator=g)
+    sd[P + "encoder.pos_conv.0.bias"] = _normal(g, (dim,), 0.02)
+    for li in range(layers):
+        pre = f"{P}encoder.layers.{li}."
+        for nm in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            sd[pre + f"self_attn.{nm}.weight"] = _normal(g, (dim, dim), 1.0 / math.sqrt(dim))
+            sd[pre + f"self_attn.{nm}.bias"] = _normal(g, (dim,), 0.02)
+        _ln(g, sd, pre + "self_attn_layer_norm", dim)
+        sd[pre + "fc1.weight"] = _normal(g, (ffn, dim), 1.0 / math.sqrt(dim))
+        sd[pre + "fc1.bias"] = _normal(g, (ffn,), 0.02)
+        sd[pre + "fc2.weight"] = _normal(g, (dim, ffn), 0.5 / math.sqrt(ffn))
+        sd[pre + "fc2.bias"] = _normal(g, (dim,), 0.02)
+        _ln(g, sd, pre + "final_layer_norm", dim)
+    _ln(g, sd, P + "encoder.layer_norm", dim)
+    sd["w2v_encoder.proj.weight"] = _normal(g, (vocab, dim), 3.0 / math.sqrt(dim))
+    bias = _normal(g, (vocab,), 0.1)
+    bias[0] += 0.3
+    sd["w2v_encoder.proj.bias"] = bias
+    return sd
+
+
+def w2v_letter_dict(vocab: int = 32) -> str:
+    """dict.ltr.txt for a vocab of `vocab` entries (the 4 specials are added by the reader)"""
+    return "".join(f"{c} {1000 - i}\n" for i, c in enumerate(W2V_LETTERS[:vocab - 4]))
