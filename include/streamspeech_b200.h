@@ -277,6 +277,39 @@ int ss_t2u_unit_decode_batch_scored(ss_engine* h, void* stream, const float* mt_
 int ss_t2u_unit_decode_ragged(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host,
                               const int32_t* n_pad_tail_host, const float* pos_rows_dev, int mask_eos, int64_t* argmax_dev, int64_t* packed_units_dev);
 
+/* ---- UnitY (researches/translatotron, `fairseq-generate --task speech_to_speech_modified`): the T2U encoder on its own, then the
+ * autoregressive unit decoder searched token by token (examples/speech_to_speech/unity/sequence_generator.py, driven by
+ * sequence_generator_multi_decoder.py:259-268).  A UnitY checkpoint has no CTC heads: ss_finalize then records that, and ss_ctc_greedy,
+ * ss_ctc_greedy_rows, ss_ctc_greedy_pair, ss_ctc_greedy_batch and ss_pool_step return SS_ERR_STATE naming the missing heads.  The unit
+ * search needs "__const__.unit_pos_table" (the sinusoidal table of max_target_positions + pad + 1 rows of unit_dim); with it ss_finalize
+ * refuses a unit decoder that is not 512 wide with 2048-wide FFNs and 8 heads (SS_ERR_INVALID), and a stored
+ * decoder.output_projection.weight that is not the embedding.
+ *
+ * synthesizer_encoder(x, padding_mask) (TransformerEncoderNoEmb) of B samples: mt_feats_dev [B][S_stride][unit_dim] (ss_mt_features_batch's
+ * output), sample b's positions >= S_host[b] are masked keys (prev_output_tokens_mt's pads); causal when the config's uni_encoder is set
+ * (UnitY: bidirectional); no positions are added.  out_dev [B][S_stride][unit_dim] after the final LayerNorm (rows >= S_b computed too).
+ * Samples run in groups of at most max(1, SS_UNIT_BATCH_ROWS / S_stride).  Synchronises `stream` once (upload of the key lengths) when
+ * some S_b < S_stride, not at all otherwise.
+ * Errors: SS_ERR_INVALID for B <= 0, S_stride <= 0 or > max_mt_positions, an S_b outside [1, S_stride] or a null pointer. */
+int ss_t2u_encode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host, float* out_dev);
+/* The unit search at beam 1 (SequenceGenerator.generate_decoder with BeamSearch, beam_size 1, min_len 1, normalize_scores, unk penalty 0,
+ * temperature 1) for B samples: sample b cross-attends to its first S_host[b] rows of t2u_dev [B][S_stride][unit_dim] (ss_t2u_encode_batch's
+ * output), projected once per call into cross K / V of every unit layer.  Step s takes log_softmax over all unit_vocab columns, then pad is
+ * -inf, eos is -inf at step 0 and everything but eos at step max_len; the best token continues the row, eos ends it.  max_len is the
+ * caller's min(int(max_len_a * src_tokens.size(1) + max_len_b), max_decoder_positions - 1): the BATCH's padded source length, so one
+ * max_len for every sample.  Writes sample b's tokens without eos to tokens_out_host[b * max_out ...], their count to n_out_host[b], its
+ * positional scores (the log-probability of every chosen token, eos last) to pos_scores_out_host[b * (max_out + 1) ...] and its score
+ * (their sum over (n_out + 1) ** len_penalty) to scores_out_host[b].  Runs on the batched decoder kernel's beam instantiation at beam 1
+ * (the reference's own search; each row's self-attention cache stays in place, any number of entries), 32 samples per launch group, steps
+ * in bursts of 16 per launch; the host reads one done flag per sample per burst (one synchronisation) and stops once all are set.  Shares
+ * the batched MT searches' device buffers, not the handle's single-stream MT state.
+ * Errors, all before anything is launched: SS_ERR_INVALID for B <= 0, S_stride <= 0, an S_b outside [1, S_stride], max_len < 1, a
+ * non-finite len_penalty or a null pointer; SS_ERR_STATE on a handle without "__const__.unit_pos_table" (a StreamSpeech checkpoint);
+ * SS_ERR_CAPACITY when max_len > max_out, max_len + pad + 2 exceeds the position table's rows, or an S_b > 1024; SS_ERR_CUDA when option
+ * persistent_mt is 0.  A refused cooperative launch is SS_ERR_CUDA (there is no other implementation). */
+int ss_unit_search_batch(ss_engine* h, void* stream, const float* t2u_dev, int B, int S_stride, const int32_t* S_host, int max_len, float len_penalty,
+                         int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host, float* pos_scores_out_host);
+
 /* Positional-embedding row (unit_dim floats, host memory) the CTC unit decoder adds to every upsampled T2U state.  The
  * reference computes positions from x[:, :, 0] viewed as [bsz, seq] (ctc_transformer_unit_decoder.py:176-181, SURVEY.md N1), so
  * every time step of batch element b gets the sinusoidal row pad + 1 + b.  The engine is created with the row of b = 0 (the

@@ -118,6 +118,10 @@ class ModelConfig:
     eos: int = 2
     unk: int = 3
     uni_encoder: bool = True  # --uni-encoder: causal T2U encoder
+    # UnitY (researches/translatotron: unity_conformer_modified): no CTC heads, an autoregressive unit decoder over 4 specials +
+    # 1000 units (no blank) searched token by token, whose sinusoidal positions cover max_target_positions
+    unity: bool = False
+    max_target_positions: int = 1024
     vocoder: VocoderConfig = field(default_factory=VocoderConfig)
 
     @property
@@ -126,8 +130,9 @@ class ModelConfig:
 
     @staticmethod
     def from_state_dict(sd) -> "ModelConfig":
-        """Infer the dimensions from a fairseq StreamSpeech state dict (checkpoint `cfg` is hydra-pickled and
-        not loadable without fairseq; every size is recoverable from tensor shapes)."""
+        """Infer the dimensions from a fairseq StreamSpeech or UnitY state dict (checkpoint `cfg` is hydra-pickled and
+        not loadable without fairseq; every size is recoverable from tensor shapes).  A UnitY unit decoder's
+        max_target_positions is not a shape: it stays 1024 here, use from_checkpoint to read it."""
         c = ModelConfig()
         c.conv_channels, c.feat_dim, c.conv_kernel = (int(x) for x in sd["encoder.subsample.conv_layers.0.weight"].shape)
         c.enc_dim = int(sd["encoder.linear.weight"].shape[0])
@@ -136,8 +141,13 @@ class ModelConfig:
         c.dw_kernel = int(sd["encoder.conformer_layers.0.conv_module.depthwise_conv.weight"].shape[-1])
         n = lambda prefix: 1 + max(int(k[len(prefix):].split(".")[0]) for k in sd if k.startswith(prefix))  # noqa: E731
         c.enc_layers = n("encoder.conformer_layers.")
-        c.src_vocab = int(sd["source_unigram_decoder.proj.weight"].shape[0])
         c.tgt_vocab, c.mt_dim = (int(x) for x in sd["target_unigram_decoder.embed_tokens.weight"].shape)
+        heads = [k in sd for k in ("source_unigram_decoder.proj.weight", "ctc_target_unigram_decoder.proj.weight")]
+        if any(heads) and not all(heads):
+            raise KeyError("a StreamSpeech state dict needs both CTC heads (source_unigram_decoder.proj, ctc_target_unigram_decoder.proj); "
+                           "a UnitY one has neither")
+        c.unity = not any(heads)
+        c.src_vocab = c.tgt_vocab if c.unity else int(sd["source_unigram_decoder.proj.weight"].shape[0])
         c.mt_ffn = int(sd["target_unigram_decoder.layers.0.fc1.weight"].shape[0])
         c.mt_heads = c.mt_dim // 64
         c.mt_layers = n("target_unigram_decoder.layers.")
@@ -146,6 +156,30 @@ class ModelConfig:
         c.unit_ffn = int(sd["decoder.layers.0.fc1.weight"].shape[0])
         c.unit_heads = c.unit_dim // 64
         c.unit_layers = n("decoder.layers.")
+        if c.unity:
+            c.uni_encoder = False  # TransformerEncoderNoEmb: bidirectional
+        return c
+
+    @staticmethod
+    def from_checkpoint(state) -> "ModelConfig":
+        """from_state_dict(state["model"]) plus what only the checkpoint's stored cfg carries: a UnitY unit decoder's
+        max_target_positions (state["cfg"]["model"], or state["args"] in older checkpoints; fairseq's default 1024 when absent).
+        The released UnitY checkpoints were trained with --max-target-positions 1200, which sets the unit search's length limit."""
+        c = ModelConfig.from_state_dict(state["model"])
+        if c.unity:
+            def get(o, k):
+                return None if o is None else (o.get(k) if isinstance(o, dict) else getattr(o, k, None))
+
+            model_cfg = get(get(state, "cfg"), "model") or get(state, "args")
+            c.max_target_positions = int(get(model_cfg, "max_target_positions") or 1024)
+        return c
+
+    @staticmethod
+    def unity_default() -> "ModelConfig":
+        """The released UnitY checkpoints' dimensions (unity.{fr,es,de}-en.pt): StreamSpeech's encoder, MT decoder and T2U encoder,
+        and a 2-layer autoregressive unit decoder over 1004 symbols with 1200 positions"""
+        c = ModelConfig()
+        c.unity, c.uni_encoder, c.unit_vocab, c.max_target_positions = True, False, 1004, 1200
         return c
 
     def tiny(self) -> "ModelConfig":

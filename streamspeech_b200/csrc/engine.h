@@ -123,6 +123,7 @@ struct ss_engine {
   ss::Linear enc_linear;
   std::vector<ss::ConformerLayerW> enc;
   int Tpos = 0;
+  bool has_ctc = true;              // the CTC heads were loaded (StreamSpeech); a UnitY checkpoint has none
   ss::Linear ctc_head[2];
   ss::Linear ctc_pair;              // both heads as one [2V][D] linear (N == 0 when the vocabularies differ)
   unsigned* ctc_ticket = nullptr;   // "last block done" ticket of ctc_argmax_collapse_pair_kernel
@@ -137,6 +138,10 @@ struct ss_engine {
   ss::LNorm unit_ln;
   float* unit_emb = nullptr;
   float* unit_pos_row = nullptr;  // sinusoid row pad+1 (N1 quirk)
+  // UnitY's autoregressive unit decoder (ss_unit_search_batch), loaded when "__const__.unit_pos_table" is
+  float* unit_pos = nullptr;                   // sinusoid table [max_target_positions + pad + 1][unit_dim]
+  int unit_pos_rows = 0;
+  ss::MtLayerP* unit_persist_layers = nullptr;  // [unit_layers] device pointer table for the batched decoder kernel
   float* mel_bank = nullptr;
   float* melT = nullptr;            // mel bank transposed [257][80] (TMA-staged fbank kernels)
   float* window = nullptr;
@@ -202,10 +207,10 @@ struct ss_engine {
   float* mt_part = nullptr;                    // [9][mt_dim] scratch of that kernel (per-head partials + FFN delta)
   int persistent_mt_prefix = 1;                // ... and the forced-prefix pass (M <= 64 rows) as one cooperative kernel
   // batched greedy search (ss_mt_greedy_batch): caches of its own, so that a streaming agent's MT state on the handle survives it
-  float* mtb_self_kv = nullptr;                // K then V: 2 x [mt_layers][MT_BATCH_MAX_ROWS][mtb_tok_ld][mt_dim]
+  float* mtb_self_kv = nullptr;                // K then V: 2 x [max(mt_layers, unit_layers)][MT_BATCH_MAX_ROWS][mtb_tok_ld][mt_dim]
   float* mtb_self_kv2 = nullptr;               // the beam search's second buffer of the same shape (ss_mt_beam_batch)
   int mtb_tok_ld = 0;
-  float* mtb_cross_kv = nullptr;               // [mt_layers][MT_BATCH_MAX_ROWS][mtb_cross_cap][2 * mt_dim]
+  float* mtb_cross_kv = nullptr;               // [max(mt_layers, unit_layers)][MT_BATCH_MAX_ROWS][mtb_cross_cap][2 * mt_dim]
   int mtb_cross_cap = 0;
   int64_t* mtb_tok_pinned = nullptr;           // [MT_BATCH_MAX_ROWS][16] tokens of one burst
   int mt_batch_min_rows = 2;                   // groups with fewer rows decode per sample on the single-token kernel (faster at B = 1)

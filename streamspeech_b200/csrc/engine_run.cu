@@ -13,6 +13,12 @@ namespace {
 
 inline cudaStream_t S(void* s) { return (cudaStream_t)s; }
 
+// entries that project encoder rows through the CTC heads, which a UnitY checkpoint does not have: SS_ERR_STATE before anything is read
+int refuse_without_ctc(ss_engine* h, const char* where) {
+  return h->fail(SS_ERR_STATE, std::string(where) + ": this model has no CTC heads (source_unigram_decoder.proj and "
+                               "ctc_target_unigram_decoder.proj were not loaded: a UnitY checkpoint)");
+}
+
 int check_launch(ss_engine* h, const char* where) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string(where) + ": " + cudaGetErrorString(e));
@@ -378,11 +384,14 @@ void mt_forward(ss_engine* h, int past, int n, int T, const int* self_kv_len_dev
 
 // cross-attention K | V of encoder rows [from, T) of enc into rows [from, T) of a cache whose layers are layer_rows rows apart: one
 // linear per MT layer over the T - from rows (the GEMM routing depends on that M)
-void mt_project_cross(ss_engine* h, const float* enc, int from, int T, float* cache, size_t layer_rows, cudaStream_t st) {
-  const ss_config& c = h->cfg;
+void project_cross(ss_engine* h, const std::vector<DecLayerW>& layers, int in_dim, const float* enc, int from, int T, float* cache, size_t layer_rows,
+                   cudaStream_t st) {
   if (T <= from) return;
-  for (int l = 0; l < c.mt_layers; ++l)
-    linear(h, enc + (size_t)from * c.enc_dim, c.enc_dim, T - from, h->mt[l].ckv, ep_out(cache + (l * layer_rows + from) * 2 * c.mt_dim, 2 * c.mt_dim), st);
+  for (size_t l = 0; l < layers.size(); ++l)
+    linear(h, enc + (size_t)from * in_dim, in_dim, T - from, layers[l].ckv, ep_out(cache + (l * layer_rows + from) * 2 * layers[l].cq.N, 2 * layers[l].cq.N), st);
+}
+void mt_project_cross(ss_engine* h, const float* enc, int from, int T, float* cache, size_t layer_rows, cudaStream_t st) {
+  project_cross(h, h->mt, h->cfg.enc_dim, enc, from, T, cache, layer_rows, st);
 }
 
 // cross-attention K | V of the encoder rows.  Rows the caller declared final (ss_mt_stable_rows) at the previous call were
@@ -579,19 +588,20 @@ int ensure_mt_batch(ss_engine* h, int tok_ld, int Tmax, bool second_self_kv = fa
   const ss_config& c = h->cfg;
   const size_t R = MT_BATCH_MAX_ROWS;
   if (tok_ld > h->mtb_tok_ld || Tmax > h->mtb_cross_cap) cudaDeviceSynchronize();  // earlier launches may still read the old buffers
+  const size_t NL = std::max(c.mt_layers, c.unit_layers);  // (the unit search runs on these buffers too)
   if (tok_ld > h->mtb_tok_ld) {
     if (h->mtb_self_kv) cudaFree(h->mtb_self_kv);
     if (h->mtb_self_kv2) cudaFree(h->mtb_self_kv2);
     h->mtb_self_kv = h->mtb_self_kv2 = nullptr;
     h->mtb_tok_ld = 0;
-    if (cudaMalloc((void**)&h->mtb_self_kv, (size_t)2 * c.mt_layers * R * tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
+    if (cudaMalloc((void**)&h->mtb_self_kv, (size_t)2 * NL * R * tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
       h->mtb_self_kv = nullptr;
       return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt self kv) failed");
     }
     h->mtb_tok_ld = tok_ld;
   }
   if (second_self_kv && !h->mtb_self_kv2 &&
-      cudaMalloc((void**)&h->mtb_self_kv2, (size_t)2 * c.mt_layers * R * h->mtb_tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
+      cudaMalloc((void**)&h->mtb_self_kv2, (size_t)2 * NL * R * h->mtb_tok_ld * c.mt_dim * sizeof(float)) != cudaSuccess) {
     h->mtb_self_kv2 = nullptr;
     return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt self kv, second buffer) failed");
   }
@@ -600,7 +610,7 @@ int ensure_mt_batch(ss_engine* h, int tok_ld, int Tmax, bool second_self_kv = fa
     if (h->mtb_cross_kv) cudaFree(h->mtb_cross_kv);
     h->mtb_cross_kv = nullptr;
     h->mtb_cross_cap = 0;
-    if (cudaMalloc((void**)&h->mtb_cross_kv, (size_t)c.mt_layers * R * cap * 2 * c.mt_dim * sizeof(float)) != cudaSuccess) {
+    if (cudaMalloc((void**)&h->mtb_cross_kv, (size_t)NL * R * cap * 2 * c.mt_dim * sizeof(float)) != cudaSuccess) {
       h->mtb_cross_kv = nullptr;
       return h->fail(SS_ERR_CUDA, "cudaMalloc(batched mt cross kv) failed");
     }
@@ -655,11 +665,26 @@ int mt_batch_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, 
   return mt_batch_bursts(h, st, P, max_len, tokens_out_host + (size_t)g0 * max_out, max_out, n_out_host + g0, "ss_mt_greedy_batch");
 }
 
+// The decoder a beam search runs on the batched decoder kernel: the MT decoder (ss_mt_beam_batch) or UnitY's unit decoder at beam 1
+// (ss_unit_search_batch).  Both are 512 wide with 2048-wide FFNs; cross-attention reads rows of in_dim floats projected by the layers.
+struct SearchDecoder {
+  int n_layers, ffn, vocab, in_dim;
+  const float *emb, *pos, *out_g, *out_b;
+  const MtLayerP* layers_dev;
+  const std::vector<DecLayerW>* layers;
+  const char* where;
+};
+
+SearchDecoder mt_search_decoder(const ss_engine* h) {
+  const ss_config& c = h->cfg;
+  return {c.mt_layers, c.mt_ffn, c.tgt_vocab, c.enc_dim, h->mt_emb, h->mt_pos, h->mt_ln.g, h->mt_ln.b, h->mt_persist_layers, &h->mt, "ss_mt_beam_batch"};
+}
+
 // Beam search of samples g0 .. g0 + Sg - 1 (Sg * beam <= MT_BATCH_MAX_ROWS rows) on mt_decode_batch_kernel's beam instantiation.
 // The steps run in bursts of 16 per launch; after each burst the host reads one done flag per sample and stops once all are set.
 // The search ends with K finalized hypotheses per sample, read once at the end and sorted by score (stable: on equal scores the
 // earlier finalized first).  Returns SS_OK or an error code (reported).
-int mt_beam_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, int Sg, int beam, int T_stride, const int32_t* T_host,
+int mt_beam_group(ss_engine* h, cudaStream_t st, const SearchDecoder& D, const float* enc_dev, int g0, int Sg, int beam, int T_stride, const int32_t* T_host,
                   int max_len, float len_penalty, int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host,
                   float* pos_scores_out_host) {
   const ss_config& c = h->cfg;
@@ -667,29 +692,29 @@ int mt_beam_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, i
   const size_t R = MT_BATCH_MAX_ROWS;
   int Tmax = 0;
   for (int b = 0; b < Sg; ++b) Tmax = std::max(Tmax, (int)T_host[g0 + b]);
-  int rc = ensure_mt_batch(h, max_len + 2, Tmax, true);
+  int rc = ensure_mt_batch(h, max_len + 2, Tmax, K > 1);  // (beam 1 keeps its self-attention cache in place)
   if (rc) return rc;
   const int ld = h->mtb_tok_ld;
   // cross K / V once per sample (its K beams read the same block), as ss_mt_greedy_batch projects it
   for (int b = 0; b < Sg; ++b)
-    mt_project_cross(h, enc_dev + (size_t)(g0 + b) * T_stride * c.enc_dim, 0, T_host[g0 + b], h->mtb_cross_kv + (size_t)b * h->mtb_cross_cap * 2 * dim,
-                     R * h->mtb_cross_cap, st);
-  const size_t floats = (size_t)rows * (dim * 11 + c.mt_ffn + c.tgt_vocab + 2 * ld + 2 * K) + (size_t)nh * (ld + 1);
+    project_cross(h, *D.layers, D.in_dim, enc_dev + (size_t)(g0 + b) * T_stride * D.in_dim, 0, T_host[g0 + b],
+                  h->mtb_cross_kv + (size_t)b * h->mtb_cross_cap * 2 * dim, R * h->mtb_cross_cap, st);
+  const size_t floats = (size_t)rows * (dim * 11 + D.ffn + D.vocab + 2 * ld + 2 * K) + (size_t)nh * (ld + 1);
   const size_t i64s = (size_t)2 * rows * ld + (size_t)nh * ld;
   const size_t ints = (size_t)rows * (4 + 2 * K) + (size_t)Sg * 2 + nh;
   if (!ws_begin(h, floats * sizeof(float) + i64s * sizeof(int64_t) + ints * sizeof(int) + 32 * 256)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
   MtBatchParams P;
-  P.n_layers = c.mt_layers; P.vocab = c.tgt_vocab; P.pad = c.pad; P.eos = c.eos;
+  P.n_layers = D.n_layers; P.vocab = D.vocab; P.pad = c.pad; P.eos = c.eos;
   P.rows = rows; P.tok_ld = ld; P.cross_cap = h->mtb_cross_cap;
-  P.emb = h->mt_emb; P.pos = h->mt_pos; P.out_g = h->mt_ln.g; P.out_b = h->mt_ln.b;
-  P.self_k = h->mtb_self_kv; P.self_v = h->mtb_self_kv + (size_t)c.mt_layers * R * ld * dim; P.cross_kv = h->mtb_cross_kv;
+  P.emb = D.emb; P.pos = D.pos; P.out_g = D.out_g; P.out_b = D.out_b;
+  P.self_k = h->mtb_self_kv; P.self_v = h->mtb_self_kv + (size_t)D.n_layers * R * ld * dim; P.cross_kv = h->mtb_cross_kv;
   P.q = h->ws.f32((size_t)rows * dim); P.part = h->ws.f32((size_t)rows * 8 * dim); P.delta = h->ws.f32((size_t)rows * dim);
-  P.hid = h->ws.f32((size_t)rows * c.mt_ffn); P.logits = h->ws.f32((size_t)rows * c.tgt_vocab);
+  P.hid = h->ws.f32((size_t)rows * D.ffn); P.logits = h->ws.f32((size_t)rows * D.vocab);
   P.tok = (int64_t*)h->ws.raw((size_t)rows * ld * sizeof(int64_t));
   MtBeamParams Bm;
   Bm.beam = K; Bm.max_len = max_len; Bm.len_penalty = len_penalty;
   Bm.tok2 = (int64_t*)h->ws.raw((size_t)rows * ld * sizeof(int64_t));
-  Bm.self_k2 = h->mtb_self_kv2; Bm.self_v2 = h->mtb_self_kv2 + (size_t)c.mt_layers * R * ld * dim;
+  if (K > 1) Bm.self_k2 = h->mtb_self_kv2, Bm.self_v2 = h->mtb_self_kv2 + (size_t)D.n_layers * R * ld * dim;
   Bm.cum = h->ws.f32((size_t)2 * rows * ld); Bm.cand = h->ws.f32((size_t)rows * 2 * K);
   Bm.cand_tok = (int*)h->ws.raw((size_t)rows * 2 * K * sizeof(int)); Bm.parent = (int*)h->ws.raw((size_t)rows * sizeof(int));
   Bm.hyp_tok = (int64_t*)h->ws.raw((size_t)nh * ld * sizeof(int64_t)); Bm.hyp_pos = h->ws.f32((size_t)nh * ld);
@@ -715,12 +740,12 @@ int mt_beam_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, i
   constexpr int kBurst = 16;
   for (int step = 0; step <= max_len; step += kBurst) {  // step max_len forces eos: it still scores and finalizes every beam
     const int cnt = std::min(kBurst, max_len + 1 - step);
-    if (mt_decode_batch(P, h->mt_persist_layers, step, cnt, h->persist_bar, &h->persist_bar_target, st, &Bm) != 0) {
+    if (mt_decode_batch(P, D.layers_dev, step, cnt, h->persist_bar, &h->persist_bar_target, st, &Bm) != 0) {
       cudaGetLastError();
-      return h->fail(SS_ERR_CUDA, "ss_mt_beam_batch: the cooperative launch of the batched MT kernel's beam search was refused");
+      return h->fail(SS_ERR_CUDA, std::string(D.where) + ": the cooperative launch of the batched decoder kernel's beam search was refused");
     }
     cudaMemcpyAsync(done_pinned, Bm.done, Sg * sizeof(int), cudaMemcpyDeviceToHost, st);
-    rc = sync_burst(h, st, nullptr, nullptr, 0, 0, 0, "ss_mt_beam_batch");
+    rc = sync_burst(h, st, nullptr, nullptr, 0, 0, 0, D.where);
     if (rc) return rc;
     if (std::all_of(done_pinned, done_pinned + Sg, [](int d) { return d != 0; })) break;
   }
@@ -732,9 +757,9 @@ int mt_beam_group(ss_engine* h, cudaStream_t st, const float* enc_dev, int g0, i
   cudaMemcpyAsync(score.data(), Bm.hyp_score, nh * sizeof(float), cudaMemcpyDeviceToHost, st);
   cudaMemcpyAsync(len.data(), Bm.hyp_len, nh * sizeof(int), cudaMemcpyDeviceToHost, st);
   cudaMemcpyAsync(nfin.data(), Bm.n_fin, Sg * sizeof(int), cudaMemcpyDeviceToHost, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_mt_beam_batch: ") + cudaGetErrorString(cudaGetLastError()));
+  if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string(D.where) + ": " + cudaGetErrorString(cudaGetLastError()));
   for (int j = 0; j < Sg; ++j) {
-    if (nfin[j] != K) return h->fail(SS_ERR_CUDA, "ss_mt_beam_batch: a sample ended with fewer than beam finalized hypotheses");
+    if (nfin[j] != K) return h->fail(SS_ERR_CUDA, std::string(D.where) + ": a sample ended with fewer than beam finalized hypotheses");
     std::vector<int> order(K);
     for (int i = 0; i < K; ++i) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return score[(size_t)j * K + a] > score[(size_t)j * K + b]; });
@@ -1138,6 +1163,7 @@ int ss_encoder_stream_step(ss_engine* h, void* stream, const float* feats_dev, i
 int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_dev, int rows, int row0, int64_t* argmax_dev,
                        int64_t* tokens_dev, int32_t* index_dev, int32_t* count_dev) {
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (!h->has_ctc) return refuse_without_ctc(h, "ss_ctc_greedy");
   if (head < 0 || head > 1 || rows <= 0 || row0 < 0 || row0 > rows) return h->fail(SS_ERR_INVALID, "bad ctc head / rows");
   const Linear& l = h->ctc_head[head];
   cudaStream_t st = S(stream);
@@ -1156,6 +1182,7 @@ int ss_ctc_greedy_rows(ss_engine* h, void* stream, int head, const float* enc_de
 int ss_ctc_greedy_pair(ss_engine* h, void* stream, const float* enc_dev, int rows, int row0, int64_t* argmax0_dev, int64_t* argmax1_dev,
                        int64_t* packed_out_dev) {
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (!h->has_ctc) return refuse_without_ctc(h, "ss_ctc_greedy_pair");
   if (rows <= 0 || row0 < 0 || row0 > rows) return h->fail(SS_ERR_INVALID, "bad ctc rows");
   cudaStream_t st = S(stream);
   const int V = h->cfg.src_vocab;
@@ -1362,11 +1389,80 @@ int ss_mt_beam_batch(ss_engine* h, void* stream, const float* enc_dev, int B, in
   cudaStream_t st = S(stream);
   const int S_launch = MT_BATCH_MAX_ROWS / beam;  // samples per launch
   for (int g0 = 0; g0 < B; g0 += S_launch) {
-    rc = mt_beam_group(h, st, enc_dev, g0, std::min(S_launch, B - g0), beam, T_stride, T_host, max_len, len_penalty, tokens_out_host, max_out,
-                       n_out_host, scores_out_host, pos_scores_out_host);
+    rc = mt_beam_group(h, st, mt_search_decoder(h), enc_dev, g0, std::min(S_launch, B - g0), beam, T_stride, T_host, max_len, len_penalty,
+                       tokens_out_host, max_out, n_out_host, scores_out_host, pos_scores_out_host);
     if (rc) return rc;
   }
   return check_launch(h, "ss_mt_beam_batch");
+}
+
+int ss_t2u_encode_batch(ss_engine* h, void* stream, const float* mt_feats_dev, int B, int S_stride, const int32_t* S_host, float* out_dev) {
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || S_stride <= 0 || !mt_feats_dev || !S_host || !out_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_t2u_encode_batch");
+  if (S_stride > c.max_mt_positions) return h->fail(SS_ERR_INVALID, "ss_t2u_encode_batch: S_stride > max_mt_positions");
+  bool ragged = false;
+  for (int b = 0; b < B; ++b) {
+    if (S_host[b] < 1 || S_host[b] > S_stride) return h->fail(SS_ERR_INVALID, "ss_t2u_encode_batch: sample length outside [1, S_stride]");
+    ragged |= S_host[b] < S_stride;
+  }
+  const int dim = c.unit_dim;
+  const int G = std::max(1, SS_UNIT_BATCH_ROWS / S_stride);
+  const size_t n_max = (size_t)std::min(G, B) * S_stride;
+  if (!ws_begin(h, n_max * (dim * 8 + c.unit_ffn) * sizeof(float) + (size_t)B * sizeof(int) + 8 * 256)) return h->fail(SS_ERR_CUDA, "workspace allocation failed");
+  int* lens_dev = ragged ? (int*)h->ws.raw((size_t)B * sizeof(int)) : nullptr;
+  DecScratch sc = dec_scratch(h, (int)n_max, dim, c.unit_ffn);
+  float* x = h->ws.f32(n_max * dim);
+  if ((ragged && !lens_dev) || !sc.qkv || !x) return h->fail(SS_ERR_CUDA, "workspace too small");
+  cudaStream_t st = S(stream);
+  if (ragged) {  // the padding mask of prev_output_tokens_mt: keys at or beyond S_b
+    cudaMemcpyAsync(lens_dev, S_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess) return h->fail(SS_ERR_CUDA, std::string("ss_t2u_encode_batch: ") + cudaGetErrorString(cudaGetLastError()));
+  }
+  for (int g0 = 0; g0 < B; g0 += G) {
+    const int Bg = std::min(G, B - g0), n = Bg * S_stride;
+    copy_f32(mt_feats_dev + (size_t)g0 * S_stride * dim, x, (int64_t)n * dim, st);
+    for (int l = 0; l < c.t2u_layers; ++l)
+      dec_layer(h, h->t2u[l], x, n, dim, c.unit_ffn, c.unit_heads, c.uni_encoder != 0, ragged ? lens_dev + g0 : nullptr, nullptr, nullptr, 0, nullptr,
+                0, nullptr, sc, st, 0, nullptr, Bg);
+    layer_norm(x, dim, out_dev + (size_t)g0 * S_stride * dim, dim, h->t2u_ln.g, h->t2u_ln.b, n, dim, st);
+  }
+  return check_launch(h, "ss_t2u_encode_batch");
+}
+
+int ss_unit_search_batch(ss_engine* h, void* stream, const float* t2u_dev, int B, int S_stride, const int32_t* S_host, int max_len, float len_penalty,
+                         int64_t* tokens_out_host, int max_out, int32_t* n_out_host, float* scores_out_host, float* pos_scores_out_host) {
+  if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  const ss_config& c = h->cfg;
+  if (B <= 0 || S_stride <= 0 || !t2u_dev || !S_host || !tokens_out_host || !n_out_host || !scores_out_host || !pos_scores_out_host)
+    return h->fail(SS_ERR_INVALID, "bad arguments to ss_unit_search_batch");
+  if (!h->unit_pos)
+    return h->fail(SS_ERR_STATE, "ss_unit_search_batch: the handle has no autoregressive unit decoder (a StreamSpeech checkpoint; "
+                                 "UnitY loads __const__.unit_pos_table)");
+  if (max_len < 1) return h->fail(SS_ERR_INVALID, "ss_unit_search_batch: min_len cannot be larger than max_len");
+  if (!std::isfinite(len_penalty)) return h->fail(SS_ERR_INVALID, "ss_unit_search_batch: len_penalty is not finite");
+  int Smax = 0;
+  for (int b = 0; b < B; ++b) {
+    if (S_host[b] < 1 || S_host[b] > S_stride) return h->fail(SS_ERR_INVALID, "ss_unit_search_batch: sample length outside [1, S_stride]");
+    Smax = std::max(Smax, (int)S_host[b]);
+  }
+  if (max_len > max_out) return h->fail(SS_ERR_CAPACITY, "ss_unit_search_batch: max_len > max_out");
+  if (max_len + c.pad + 2 > h->unit_pos_rows)
+    return h->fail(SS_ERR_CAPACITY, "ss_unit_search_batch: max_len " + std::to_string(max_len) + " needs " + std::to_string(max_len + c.pad + 2) +
+                                        " rows of the unit position table, which has " + std::to_string(h->unit_pos_rows) + " (max_target_positions + pad + 1)");
+  if (!h->persistent_mt || !mt_decode_persistent_supported(c.unit_dim, c.unit_ffn, c.unit_heads, c.unit_vocab, max_len + 2, Smax))
+    return h->fail(Smax > 1024 ? SS_ERR_CAPACITY : SS_ERR_CUDA,
+                   "ss_unit_search_batch: the unit search runs on the batched decoder kernel, which is off (option persistent_mt) or does not "
+                   "support this shape (T2U states per sample <= 1024)");
+  const SearchDecoder D{c.unit_layers, c.unit_ffn, c.unit_vocab, c.unit_dim, h->unit_emb, h->unit_pos, h->unit_ln.g, h->unit_ln.b,
+                        h->unit_persist_layers, &h->unit, "ss_unit_search_batch"};
+  cudaStream_t st = S(stream);
+  for (int g0 = 0; g0 < B; g0 += MT_BATCH_MAX_ROWS) {
+    const int rc = mt_beam_group(h, st, D, t2u_dev, g0, std::min(MT_BATCH_MAX_ROWS, B - g0), 1, S_stride, S_host, max_len, len_penalty, tokens_out_host,
+                                 max_out, n_out_host, scores_out_host, pos_scores_out_host);
+    if (rc) return rc;
+  }
+  return check_launch(h, "ss_unit_search_batch");
 }
 
 int ss_mt_incremental_reset(ss_engine* h) {
@@ -1436,6 +1532,7 @@ int ss_unit_position_row(ss_engine* h, const float* row_host) {
 
 int ss_ctc_greedy_batch(ss_engine* h, void* stream, const float* enc_dev, int B, int T, int64_t* packed_out_dev) {
   if (!h || !h->finalized) return h ? h->fail(SS_ERR_STATE, "engine not finalized") : SS_ERR_INVALID;
+  if (!h->has_ctc) return refuse_without_ctc(h, "ss_ctc_greedy_batch");
   if (B <= 0 || T <= 0 || !enc_dev || !packed_out_dev) return h->fail(SS_ERR_INVALID, "bad arguments to ss_ctc_greedy_batch");
   const ss_config& c = h->cfg;
   cudaStream_t st = S(stream);

@@ -300,8 +300,10 @@ void finalize_impl(ss_engine* h) {
     if (!h->async_err_pinned && cudaHostAlloc((void**)&h->async_err_pinned, sizeof(unsigned), cudaHostAllocDefault) == cudaSuccess)
       *h->async_err_pinned = 0;
   }
-  // ---- CTC heads
-  if (c.src_vocab == c.tgt_vocab) {
+  // ---- CTC heads (optional: a UnitY checkpoint has neither; a StreamSpeech one needs both)
+  h->has_ctc = h->host.count("source_unigram_decoder.proj.weight") || h->host.count("ctc_target_unigram_decoder.proj.weight");
+  if (!h->has_ctc) {
+  } else if (c.src_vocab == c.tgt_vocab) {
     // one [2V][D] matrix: both heads of a policy() call are ONE GEMM (ss_ctc_greedy_pair); the single heads are views of it
     h->ctc_pair = make_fused(h, {"source_unigram_decoder.proj", "ctc_target_unigram_decoder.proj"}, c.src_vocab, D);
     h->ctc_head[0] = h->ctc_pair;
@@ -360,6 +362,32 @@ void finalize_impl(ss_engine* h) {
     const HostTensor& pr = get(h, "__const__.unit_pos_row");
     expect_shape(pr, "__const__.unit_pos_row", {c.unit_dim});
     h->unit_pos_row = upload(h, pr.data);
+    // the output projection is the embedding (share_decoder_input_output_embed): a stored copy must be that tensor
+    auto op = h->host.find("decoder.output_projection.weight");
+    if (op != h->host.end() && (op->second.shape != e.shape || op->second.data != e.data))
+      throw std::runtime_error("decoder.output_projection.weight differs from decoder.embed_tokens.weight: the unit decoder's output "
+                               "projection must be tied to its embedding");
+  }
+  // ---- UnitY: the autoregressive unit decoder searched on the batched decoder kernel (ss_unit_search_batch)
+  if (h->host.count("__const__.unit_pos_table")) {
+    if (!mt_decode_persistent_supported(c.unit_dim, c.unit_ffn, c.unit_heads, c.unit_vocab, 1, 1))
+      throw std::runtime_error("unit decoder of " + std::to_string(c.unit_dim) + " / " + std::to_string(c.unit_ffn) + " / " +
+                               std::to_string(c.unit_heads) + " (dim / ffn / heads): the autoregressive unit search's kernel takes 512 / 2048 / 8");
+    const HostTensor& pt = get(h, "__const__.unit_pos_table");
+    if (pt.shape.size() != 2 || pt.shape[1] != c.unit_dim || pt.shape[0] < (int64_t)c.pad + 3)
+      throw std::runtime_error("bad __const__.unit_pos_table (needs max_target_positions + pad + 1 rows of unit_dim)");
+    h->unit_pos_rows = (int)pt.shape[0];
+    h->unit_pos = upload(h, pt.data);
+    std::vector<MtLayerP> ul(c.unit_layers);
+    for (int i = 0; i < c.unit_layers; ++i) {
+      const DecLayerW& L = h->unit[i];
+      MtLayerP& q = ul[i];
+      q.self_g = L.self_ln.g; q.self_b = L.self_ln.b; q.wqkv = L.qkv.w; q.bqkv = L.qkv.b; q.wo = L.out.w; q.bo = L.out.b;
+      q.cross_g = L.cross_ln.g; q.cross_b = L.cross_ln.b; q.wcq = L.cq.w; q.bcq = L.cq.b; q.wco = L.cout.w; q.bco = L.cout.b;
+      q.fin_g = L.final_ln.g; q.fin_b = L.final_ln.b; q.w1 = L.fc1.w; q.b1 = L.fc1.b; q.w2 = L.fc2.w; q.b2 = L.fc2.b;
+    }
+    h->unit_persist_layers = dev_alloc<MtLayerP>(h, ul.size());
+    cudaMemcpy(h->unit_persist_layers, ul.data(), ul.size() * sizeof(MtLayerP), cudaMemcpyHostToDevice);
   }
   // ---- vocoder (optional: the ASR / S2TT agents do not load one)
   h->has_vocoder = h->host.count("vocoder.dict.weight") > 0;

@@ -135,7 +135,7 @@ struct MtBatchParams {
 // feeds and writes buffer s & 1 and its selection reorders the rows into buffer (s + 1) & 1.  fin is the host's initial state
 // (1 for every beam but 0 at step 0) and is then kept by the kernel.
 struct MtBeamParams {
-  int beam = 0;                   // K (2 .. MT_BATCH_MAX_ROWS)
+  int beam = 0;                   // K (1 .. MT_BATCH_MAX_ROWS; at 1 the second cache is not used and may be null)
   int max_len = 0;                // eos forced at this step, which ends every sample still searching
   float len_penalty = 1.f;        // finalized score = cumulative score / (step + 1) ** len_penalty
   int64_t* tok2 = nullptr;        // second token buffer, as MtBatchParams::tok ([rows][tok_ld])

@@ -12,7 +12,8 @@
 // MtDecodeParams' self_k / self_v), and the position-p entry of that cache is p + kv_off[r] (the single-token kernel's kv_off).
 // The offline beam search (ss_mt_beam_batch) is a fourth instantiation (MtBeamParams): the same layer phases and logits, then
 // candidates (row i on CTA i) and selection (sample j on CTA j) in place of the arg-max, one more grid barrier per step, and the
-// reorder of the rows' self-attention caches into a second buffer at the start of the next step.
+// reorder of the rows' self-attention caches into a second buffer at the start of the next step.  At beam 1 (UnitY's unit search,
+// ss_unit_search_batch, on the unit decoder's 2 layers) every row is its own parent: the caches stay in place and are not reordered.
 // Every CTA keeps the residual rows of all samples in shared memory (32 x 2 KB); the LayerNorm outputs share a second
 // 64 KB buffer with the FFN hidden rows, which do not fit at once (8 KB each) and are staged 8 rows at a time.
 //
@@ -375,8 +376,10 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
     const int s = step0 + si;
     // beam search: the rows' tokens, scores and self-attention caches alternate between two buffers (step s reads buffer s & 1)
     const bool alt = kMode == kMtbBeam && (s & 1);
+    // beam 1 (the unit search): every row continues itself (parent[r] = r), so its cache stays in one buffer and is not gathered
+    const bool alt_kv = alt && B.beam > 1;
     if constexpr (kMode == kMtbBeam)
-      if (s > 0) beam_gather_kv(P, B, sb, s, alt ? B.self_k2 : P.self_k, alt ? B.self_v2 : P.self_v, alt ? P.self_k : B.self_k2, alt ? P.self_v : B.self_v2);
+      if (s > 0 && B.beam > 1) beam_gather_kv(P, B, sb, s, alt ? B.self_k2 : P.self_k, alt ? B.self_v2 : P.self_v, alt ? P.self_k : B.self_k2, alt ? P.self_v : B.self_v2);
     for (int e = tid; e < sb.nact * DIM; e += MTT) {
       const int r = sb.act[e / DIM], c = e % DIM;
       const int64_t tok = (alt ? B.tok2 : P.tok)[(size_t)r * P.tok_ld + s];
@@ -396,8 +399,8 @@ __global__ void __launch_bounds__(MTT, 1) mt_decode_batch_kernel(MtBatchParams P
         gemv_prefetch<DIM, 6>(P.emb, P.vocab);
         if (si + 1 < nsteps) layer_prefetch(layers[0], in_group, grp_h, grp_j);
       }
-      float* kl = (alt ? B.self_k2 : P.self_k) + (size_t)l * MAXR * P.tok_ld * DIM;
-      float* vl = (alt ? B.self_v2 : P.self_v) + (size_t)l * MAXR * P.tok_ld * DIM;
+      float* kl = (alt_kv ? B.self_k2 : P.self_k) + (size_t)l * MAXR * P.tok_ld * DIM;
+      float* vl = (alt_kv ? B.self_v2 : P.self_v) + (size_t)l * MAXR * P.tok_ld * DIM;
       // (1) x += FFN delta of the previous layer; q | k | v = LN(x) Wqkv^T
       if (l > 0) add_delta_rows(sb, xs, P.delta);
       ln_rows(sb, xs, vb, L.self_g, L.self_b);
@@ -549,7 +552,9 @@ int mt_decode_batch(const MtBatchParams& P, const MtLayerP* layers_dev, int step
   if (rows && (!P.max_len || !P.cross_row || (!P.feats && !inc))) return -1;  // the per-row fields come together
   if (inc && (!rows || !P.kv_off || P.self_ld < 1)) return -1;
   const MtBeamParams B = beam ? *beam_p : MtBeamParams{};
-  if (beam && (rows || B.beam < 1 || B.beam > MAXR || P.rows % B.beam != 0 || 2 * B.beam > P.vocab || B.max_len + 2 > P.tok_ld)) return -1;
+  if (beam && (rows || B.beam < 1 || B.beam > MAXR || P.rows % B.beam != 0 || 2 * B.beam > P.vocab || B.max_len + 2 > P.tok_ld ||
+               (B.beam > 1 && (!B.self_k2 || !B.self_v2))))
+    return -1;
   const void* kernel = beam   ? (const void*)mt_decode_batch_kernel<kMtbBeam>
                        : inc  ? (const void*)mt_decode_batch_kernel<kMtbIncremental>
                        : rows ? (const void*)mt_decode_batch_kernel<kMtbPrefix>

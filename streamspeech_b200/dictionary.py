@@ -55,16 +55,17 @@ class Dictionary:
         return cls([("▁" if i % 3 == 0 else "") + f"w{i}" for i in range(size - 4)])
 
     @classmethod
-    def units(cls, n_units: int) -> "Dictionary":
-        """target dictionary of the S2UT task: "0".."n-1" then <blank>."""
-        return cls([str(i) for i in range(n_units)] + ["<blank>"])
+    def units(cls, n_units: int, blank: bool = True) -> "Dictionary":
+        """target dictionary of the S2UT task: "0".."n-1" then <blank> (speech_to_speech_ctc); UnitY's speech_to_speech task has no
+        blank (fairseq/tasks/speech_to_speech.py: --target-code-size symbols after the specials)."""
+        return cls([str(i) for i in range(n_units)] + (["<blank>"] if blank else []))
 
     @classmethod
     def load_multitask(cls, args, cfg):
         """dict paths from the multitask yaml (configs/<pair>/config_mtl_asr_st_ctcst.yaml) under --data-bin."""
         import yaml
 
-        out = {"tgt": cls.units(cfg.unit_vocab - 5)}
+        out = {"tgt": cls.units(cfg.unit_vocab - 4, blank=False) if cfg.unity else cls.units(cfg.unit_vocab - 5)}
         path = os.path.join(args.data_bin, args.multitask_config_yaml)
         with open(path) as f:
             mt = yaml.safe_load(f)

@@ -129,6 +129,8 @@ def load_library() -> ctypes.CDLL:
     lib.ss_pool_mt_greedy.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32]
     lib.ss_pool_mt_greedy_incremental.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.ss_t2u_unit_decode_ragged.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i32, vp, vp]
+    lib.ss_t2u_encode_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp]
+    lib.ss_unit_search_batch.argtypes = [vp, vp, vp, i32, i32, vp, i32, ctypes.c_float, vp, i32, vp, vp, vp]
     f32 = ctypes.c_float
     lib.ss_op_relpos_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32]
     lib.ss_op_mha_attention.argtypes = [vp, vp, vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, f32, i32, i32, vp, i32]
@@ -161,7 +163,7 @@ EXPORTED_SYMBOLS = [
     "ss_pool_create_rate", "ss_pool_finish", "ss_pool_set_chunk", "ss_mt_greedy_batch", "ss_mt_beam_batch", "ss_ctc_greedy_batch", "ss_mt_features_batch",
     "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
     "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
-    "ss_t2u_unit_decode_batch_scored", "ss_op_argmax_rows",
+    "ss_t2u_unit_decode_batch_scored", "ss_op_argmax_rows", "ss_t2u_encode_batch", "ss_unit_search_batch",
 ]
 
 
@@ -244,6 +246,8 @@ class Engine:
             self._load("__const__.enc_pe", constants.rel_pos_table(max_enc_frames, cfg.enc_dim))
             self._load("__const__.mt_pos_table", constants.sinusoidal_table(max_mt_positions + cfg.pad + 2, cfg.mt_dim, cfg.pad))
             self._load("__const__.unit_pos_row", constants.sinusoidal_table(cfg.pad + 4, cfg.unit_dim, cfg.pad)[cfg.pad + 1])
+            if cfg.unity:  # the autoregressive unit decoder's positions (SinusoidalPositionalEmbedding of max_target_positions)
+                self._load("__const__.unit_pos_table", constants.sinusoidal_table(cfg.max_target_positions + cfg.pad + 1, cfg.unit_dim, cfg.pad))
             if gcmvn is not None:
                 self._load("__const__.gcmvn_mean", torch.as_tensor(gcmvn["mean"], dtype=torch.float32))
                 self._load("__const__.gcmvn_std", torch.as_tensor(gcmvn["std"], dtype=torch.float32))
@@ -564,6 +568,39 @@ class Engine:
         feats = self._f32(B, S, self.cfg.mt_dim)
         self._check(self.lib.ss_mt_features_batch(self._h, self._stream(), enc.data_ptr(), B, T, lens, toks, S, feats.data_ptr()))
         return feats
+
+    def t2u_encode_batch(self, mt_feats: torch.Tensor, lengths: Sequence[int]) -> torch.Tensor:
+        """UnitY's synthesizer_encoder on a padded batch (ss_t2u_encode_batch): mt_feats [B, S, dim], sample b's positions >=
+        lengths[b] are masked keys.  Returns the T2U states [B, S, dim] (device)."""
+        assert mt_feats.is_cuda and mt_feats.is_contiguous() and mt_feats.dim() == 3
+        B, S = int(mt_feats.shape[0]), int(mt_feats.shape[1])
+        if len(lengths) != B:
+            raise EngineError(f"{len(lengths)} lengths for a batch of {B}")
+        out = self._f32(B, S, self.cfg.unit_dim)
+        self._check(self.lib.ss_t2u_encode_batch(self._h, self._stream(), mt_feats.data_ptr(), B, S, _i32_array(lengths), out.data_ptr()))
+        return out
+
+    def unit_search_batch(self, t2u: torch.Tensor, lengths: Sequence[int], max_len: int, len_penalty: float = 1.0) -> List[Dict[str, object]]:
+        """UnitY's unit search at beam 1 (ss_unit_search_batch) over t2u [B, S, dim], sample b cross-attending to its first
+        lengths[b] rows, with one max_len for the batch.  Returns per sample {"tokens": [...] eos last (finalized[b][0]["tokens"]),
+        "score": float, "positional_scores": [...] one per token}."""
+        assert t2u.is_cuda and t2u.is_contiguous() and t2u.dim() == 3
+        B, S = int(t2u.shape[0]), int(t2u.shape[1])
+        if len(lengths) != B:
+            raise EngineError(f"{len(lengths)} lengths for a batch of {B}")
+        cap = max(int(max_len), 1)
+        out = torch.empty(max(B, 1) * cap, dtype=torch.int64)
+        n_out = torch.empty(max(B, 1), dtype=torch.int32)
+        scores = torch.empty(max(B, 1), dtype=torch.float32)
+        pos = torch.empty(max(B, 1) * (cap + 1), dtype=torch.float32)
+        self._check(self.lib.ss_unit_search_batch(self._h, self._stream(), t2u.data_ptr(), B, S, _i32_array(lengths), int(max_len),
+                                                  float(len_penalty), out.data_ptr(), cap, n_out.data_ptr(), scores.data_ptr(), pos.data_ptr()))
+        res = []
+        for b in range(B):
+            n = int(n_out[b])
+            res.append({"tokens": out[b * cap:b * cap + n].tolist() + [self.cfg.eos], "score": float(scores[b]),
+                        "positional_scores": pos[b * (cap + 1):b * (cap + 1) + n + 1].clone()})
+        return res
 
     def t2u_unit_decode_batch(self, mt_feats: torch.Tensor, n_pad_tail: Sequence[int], mask_eos: bool = False):
         """t2u_unit_decode for every sample of a padded batch mt_feats [B, S, mt_dim] (ss_t2u_unit_decode_batch), sample b with

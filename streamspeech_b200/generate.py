@@ -21,6 +21,12 @@ the units.  Each batch is one OfflineS2STGenerator.generate(..., scores=True) ca
 Logger lines are not written.  With `--target-is-code` the reference's dataset creator replaces every target by the empty string
 (speech_to_speech_dataset_modified.py:301-308), so, as there, every `T-` text is empty and BLEU is scored against a lone eos.
 The vocoder is not loaded (fairseq-generate does not load it either); run streamspeech_b200.generate_waveform_from_code on the units.
+
+`--task speech_to_speech_modified` with a UnitY checkpoint (unity.{fr,es,de}-en.pt) is researches/unitY/test_scripts/pred.sh's
+`fairseq-generate --user-dir researches/translatotron ... --beam-mt 10 --beam 1 --max-len-a 1`: each batch is one
+UnitYGenerator.generate call (MT search, T2U encoder, autoregressive unit search with max_len = min(int(max_len_a * F + max_len_b),
+max_target_positions - 1), F the batch's padded fbank length).  stdout then carries only the `D-{id}\t{MT text}` prints
+(sequence_generator_multi_decoder.py:217); the results file is written as above.
 """
 from __future__ import annotations
 
@@ -39,6 +45,7 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if _REPO not in sys.path:
     sys.path.insert(0, _REPO)
 
+TASKS = ("speech_to_speech_ctc", "speech_to_speech_modified")  # StreamSpeech, UnitY
 MAX_SOURCE_POSITIONS = 6000  # fairseq/tasks/speech_to_speech.py: --max-source-positions default
 MAX_TARGET_POSITIONS = 1024  # --max-target-positions default
 ENCODER_SUBSAMPLING = 4      # two stride-2 convolutions: ceil(ceil(F / 2) / 2) encoder frames (ss_encoder_out_frames)
@@ -62,8 +69,8 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     p.add_argument("--beam-mt", type=int, default=1)
     p.add_argument("--beam", type=int, default=5)
     p.add_argument("--nbest", type=int, default=1)
-    p.add_argument("--max-len-a", type=float, default=0, help="accepted and ignored: the CTC unit decoder does not search")
-    p.add_argument("--max-len-b", type=int, default=200, help="accepted and ignored: the CTC unit decoder does not search")
+    p.add_argument("--max-len-a", type=float, default=0, help="UnitY's unit search; ignored by the CTC unit decoder, which does not search")
+    p.add_argument("--max-len-b", type=int, default=200, help="UnitY's unit search; ignored by the CTC unit decoder, which does not search")
     p.add_argument("--max-len-a-mt", type=float, default=0)
     p.add_argument("--max-len-b-mt", type=int, default=200)
     p.add_argument("--lenpen", type=float, default=1.0)
@@ -79,12 +86,16 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     args = p.parse_args(argv)
     if args.cpu:
         p.error("--cpu is not offered: every stage runs on the H100 engine")
-    if args.task != "speech_to_speech_ctc":
-        p.error(f"--task {args.task}: only speech_to_speech_ctc is offered")
+    if args.task not in TASKS:
+        p.error(f"--task {args.task}: only speech_to_speech_ctc (StreamSpeech) and speech_to_speech_modified (UnitY) are offered")
+    unity = args.task == "speech_to_speech_modified"
     if args.beam != 1:
-        p.error(f"--beam {args.beam}: the CTC unit decoder does not search; pass --beam 1 (--beam-mt sets the MT beam)")
+        p.error(f"--beam {args.beam}: " + ("the UnitY unit search runs at beam 1 only" if unity else "the CTC unit decoder does not search")
+                + "; pass --beam 1 (--beam-mt sets the MT beam)")
     if args.nbest != 1:
-        p.error(f"--nbest {args.nbest}: the CTC unit decoder gives one hypothesis; pass --nbest 1")
+        p.error(f"--nbest {args.nbest}: the unit decoder gives one hypothesis here; pass --nbest 1")
+    if unity and not math.isfinite(args.max_len_a):
+        p.error(f"--max-len-a {args.max_len_a}: must be finite")
     if args.max_len_a_mt != 0:
         p.error(f"--max-len-a-mt {args.max_len_a_mt}: only 0 (the reference default) is supported")
     if not 1 <= args.beam_mt <= 32:
@@ -358,8 +369,13 @@ def load_offline_checkpoint(args: argparse.Namespace, capacity: int):
     from streamspeech_b200.config import ModelConfig
     from streamspeech_b200.dictionary import Dictionary
 
+    unity = args.task == "speech_to_speech_modified"
     if str(args.path).startswith("synthetic"):
         seed = int(args.path.split(":")[1]) if ":" in args.path else 0
+        if unity:  # the seeded synthetic UnitY checkpoint at the released dimensions
+            cfg = ModelConfig.unity_default()
+            return cfg, synth.make_unity_state_dict(cfg, seed=seed), {"target_unigram": Dictionary.synthetic(cfg.tgt_vocab),
+                                                                      "tgt": Dictionary.units(cfg.unit_vocab - 4, blank=False)}
         cfg = ModelConfig()
         cfg.uni_encoder = False
         dicts = {k: Dictionary.synthetic(n) for k, n in (("source_unigram", cfg.src_vocab), ("ctc_target_unigram", cfg.tgt_vocab),
@@ -370,10 +386,15 @@ def load_offline_checkpoint(args: argparse.Namespace, capacity: int):
         raise IOError(f"Model file not found: {args.path}")
     state = torch.load(args.path, map_location="cpu", weights_only=False)
     uni, _ = offline_settings(state, capacity)
-    cfg = ModelConfig.from_state_dict(state["model"])
-    cfg.uni_encoder = uni
+    cfg = ModelConfig.from_checkpoint(state)
+    if cfg.unity != unity:
+        raise ValueError(f"--task {args.task} does not match the checkpoint {args.path}: it is a "
+                         f"{'UnitY' if cfg.unity else 'StreamSpeech'} model (pass --task "
+                         f"{'speech_to_speech_modified' if cfg.unity else 'speech_to_speech_ctc'})")
+    if not cfg.unity:
+        cfg.uni_encoder = uni
     if args.multitask_config_yaml is None:
-        raise ValueError("--multitask-config-yaml is required: it names the ASR, ST and MT dictionaries")
+        raise ValueError("--multitask-config-yaml is required: it names the MT dictionary (and StreamSpeech's ASR and ST ones)")
     dicts = Dictionary.load_multitask(argparse.Namespace(data_bin=args.data, multitask_config_yaml=args.multitask_config_yaml), cfg)
     return cfg, state["model"], dicts
 
@@ -437,7 +458,7 @@ def main(argv: Optional[Sequence[str]] = None, stdout=None):
     args = parse_args(argv)
     stdout = stdout or sys.stdout
     from streamspeech_b200.engine import Engine
-    from streamspeech_b200.offline import OfflineS2STGenerator
+    from streamspeech_b200.offline import OfflineS2STGenerator, UnitYGenerator
 
     max_enc_frames = 1024
     config = load_config_yaml(args)
@@ -446,7 +467,14 @@ def main(argv: Optional[Sequence[str]] = None, stdout=None):
     engine = Engine(cfg, sd, None, None, device=args.device_index, max_enc_frames=max_enc_frames)
     out_file = None
     try:
-        gen = OfflineS2STGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, len_penalty=args.lenpen)
+        if cfg.unity:
+            gen = UnitYGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, max_len_a=args.max_len_a,
+                                 max_len_b=args.max_len_b, len_penalty=args.lenpen)
+            prints = (("D", dicts["target_unigram"], "mt_tokens"),)
+        else:
+            gen = OfflineS2STGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, len_penalty=args.lenpen)
+            prints = (("A", dicts["source_unigram"], "asr_tokens"), ("S", dicts["ctc_target_unigram"], "st_tokens"),
+                      ("D", dicts["target_unigram"], "mt_tokens"))
         if args.results_path is not None:
             os.makedirs(args.results_path, exist_ok=True)
             out_file = open(os.path.join(args.results_path, f"generate-{args.gen_subset}.txt"), "w", buffering=1, encoding="utf-8")
@@ -458,8 +486,7 @@ def main(argv: Optional[Sequence[str]] = None, stdout=None):
         for batch in split.batches:
             res = run_batch(gen, split, batch)
             ids = list(batch)  # fairseq's sample["id"]: the dataset index
-            for key, d, tok in (("A", dicts["source_unigram"], "asr_tokens"), ("S", dicts["ctc_target_unigram"], "st_tokens"),
-                                ("D", dicts["target_unigram"], "mt_tokens")):
+            for key, d, tok in prints:
                 for sid, r in zip(ids, res):
                     print(f"{key}-{sid}\t{ctc_text(d, r[tok])}", file=stdout)
             for i, sid, r in zip(batch, ids, res):

@@ -107,6 +107,72 @@ class OfflineS2STGenerator:
         return vocode_whole(self.engine, codes_list, dur_prediction)
 
 
+class UnitYGenerator:
+    """UnitY's `MultiDecoderSequenceGenerator` as `fairseq-generate --task speech_to_speech_modified --beam-mt K --beam 1` runs it
+    (researches/translatotron/sequence_generator_multi_decoder.py:134-268) on the engine, one call per stage for the whole batch:
+
+        batched padded encoder (offline model)                                       ss_encoder_forward(B, lengths)
+        MT search, max_len = max_len_b_mt: K = 1 greedy, K >= 2 beam (finalized[b][0])  ss_mt_greedy_batch / ss_mt_beam_batch
+        prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum             host
+        mt_decoder(features_only) on the padded batch                                 ss_mt_features_batch
+        synthesizer_encoder(x, prev_output_tokens_mt == pad)                          ss_t2u_encode_batch
+        unit search at beam 1, max_len = min(int(max_len_a * F + max_len_b),          ss_unit_search_batch
+          max_target_positions - 1) with F the batch's PADDED fbank length
+
+    There are no CTC prints (UnitY has no CTC heads); the D- text is the MT hypothesis."""
+
+    def __init__(self, engine: Engine, beam_size_mt: int = 1, beam_size: int = 1, max_len_a_mt: float = 0.0, max_len_b_mt: int = 200,
+                 max_len_a: float = 0.0, max_len_b: int = 200, len_penalty: float = 1.0):
+        if not engine.cfg.unity:
+            raise ValueError("UnitYGenerator needs a UnitY checkpoint (OfflineS2STGenerator runs StreamSpeech)")
+        if beam_size != 1:
+            raise NotImplementedError("the H100 UnitY generator implements the unit search at beam_size = 1 only")
+        if int(beam_size_mt) != beam_size_mt or not 1 <= beam_size_mt <= 32:
+            raise ValueError(f"beam_size_mt must be an integer in [1, 32], got {beam_size_mt}")
+        if max_len_a_mt != 0.0:
+            raise NotImplementedError("max_len_a_mt != 0 is not supported (the reference default is 0)")
+        if not math.isfinite(len_penalty) or not math.isfinite(max_len_a):
+            raise ValueError("len_penalty and max_len_a must be finite")
+        self.engine = engine
+        self.cfg = engine.cfg
+        self.beam_size_mt = int(beam_size_mt)
+        self.len_penalty = float(len_penalty)
+        self.max_len_b_mt = int(max_len_b_mt)
+        self.max_len_a, self.max_len_b = float(max_len_a), int(max_len_b)
+        engine.set_chunk(None, None)
+
+    def unit_max_len(self, padded_frames: int) -> int:
+        """generate_decoder's max_len (unity/sequence_generator.py:182-194) for a batch of `padded_frames` fbank frames"""
+        return min(int(self.max_len_a * padded_frames + self.max_len_b), self.cfg.max_target_positions - 1)
+
+    @torch.inference_mode()
+    def generate(self, src_tokens: torch.Tensor, src_lengths: Sequence[int], scores: bool = False) -> List[Dict[str, object]]:
+        """src_tokens [B, F, 80] on the engine's device (zero padded), src_lengths [B].  One dict per sample: mt_tokens (MT
+        hypothesis without eos), units (the reference's finalized[b][0]["tokens"], eos last), unit_score and unit_positional_scores
+        (fp32, one per unit; computed whatever `scores`, which is accepted for OfflineS2STGenerator's signature)."""
+        eng, c = self.engine, self.cfg
+        if src_tokens.dim() != 3 or not src_tokens.is_cuda:
+            raise EngineError("src_tokens must be a [B, F, feat_dim] CUDA tensor")
+        lengths = [int(x) for x in src_lengths]
+        max_len = self.unit_max_len(int(src_tokens.shape[1]))
+        if max_len < 1:
+            raise ValueError("min_len cannot be larger than max_len, please adjust these!")
+        enc = eng.encoder(src_tokens.contiguous(), lengths)
+        out_len = [eng.encoder_out_frames(n) for n in lengths]
+        if self.beam_size_mt == 1:
+            hyps = eng.mt_greedy_batch(enc, out_len, self.max_len_b_mt)
+        else:
+            # (build_generator_dual_decoder passes --lenpen to the unit generator only: the MT generator keeps len_penalty_mt = 1)
+            hyps = [n[0]["tokens"] for n in eng.mt_beam_batch(enc, out_len, self.beam_size_mt, self.max_len_b_mt, 1.0)]
+        S = max(len(h) for h in hyps) + 1
+        feats = eng.mt_features_batch(enc, out_len, [[c.eos] + h + [c.pad] * (S - 1 - len(h)) for h in hyps])
+        t2u_len = [len(h) + 1 for h in hyps]
+        t2u = eng.t2u_encode_batch(feats, t2u_len)
+        units = eng.unit_search_batch(t2u, t2u_len, max_len, self.len_penalty)
+        return [{"mt_tokens": h, "units": u["tokens"], "unit_score": u["score"], "unit_positional_scores": u["positional_scores"]}
+                for h, u in zip(hyps, units)]
+
+
 def vocode_whole(eng, codes_list: Sequence[Sequence[int]], dur_prediction: bool) -> List[torch.Tensor]:
     """Whole-sequence vocoder passes of the code sequences: one durations call, one host read of the cumsums, one generate call."""
     _, cums, _ = eng.vocoder_durations_ragged([[int(u) for u in c] for c in codes_list], dur_prediction)

@@ -195,6 +195,44 @@ def make_model_state_dict(cfg: ModelConfig, seed: int = 0, calibration: Optional
     return {k: v.contiguous().float() if v.is_floating_point() else v for k, v in sd.items()}
 
 
+# UnitY's synthetic unit decoder: its cross-attention branch at full branch gain, so that samples emit different units (the
+# StreamSpeech decoder's is tiny for prefix stability, which an offline search does not need), and eos read from one slow positional
+# feature (period ~1400 steps, rising over the first few hundred) plus the T2U states: with UNITY_EOS_GAIN some samples end within
+# the first tens of units and others run to the forced eos at max_len.
+UNITY_CROSS_GAIN = 1.0
+UNITY_EOS_DIM = 150
+UNITY_EOS_GAIN = 6.0
+# ... and the MT decoder's eos output row (tied with its input row) scaled as oracle.mt_beam_oracle.early_eos_state_dict does, so that
+# MT hypotheses end after 9-16 tokens at different lengths within a batch (the StreamSpeech rows run to max_len_b_mt) and the T2U
+# encoder sees padded positions
+UNITY_MT_EOS_SCALE = -0.15
+
+
+def make_unity_state_dict(cfg: ModelConfig, seed: int = 0, eos_gain: float = UNITY_EOS_GAIN) -> Dict[str, torch.Tensor]:
+    """A seeded UnitY (unity_conformer_modified) state dict at `cfg`'s dimensions (ModelConfig.unity_default(): the released
+    checkpoints'): StreamSpeech's encoder, MT decoder and T2U encoder without the CTC heads, and the autoregressive unit decoder
+    over cfg.unit_vocab symbols (4 specials + units, no blank) with its tied output projection."""
+    assert cfg.unity
+    sd = make_model_state_dict(cfg, seed=seed)
+    for k in [k for k in sd if k.startswith(("source_unigram_decoder.", "ctc_target_unigram_decoder."))]:
+        del sd[k]
+    g = torch.Generator().manual_seed(seed + 7919)
+    U = cfg.unit_dim
+    for i in range(cfg.unit_layers):
+        sd[f"decoder.layers.{i}.encoder_attn.out_proj.weight"] = _xavier(g, U, U, gain=UNITY_CROSS_GAIN)
+    uemb = sd["decoder.embed_tokens.weight"].clone()
+    uemb[cfg.eos] = 0.0
+    uemb[cfg.eos, UNITY_EOS_DIM] = eos_gain
+    uemb[cfg.eos, :READOUT_FREQS] = torch.randn(READOUT_FREQS, generator=g) * U ** -0.5
+    sd["decoder.embed_tokens.weight"] = uemb
+    sd["decoder.output_projection.weight"] = uemb
+    memb = sd["target_unigram_decoder.embed_tokens.weight"].clone()
+    memb[cfg.eos] *= UNITY_MT_EOS_SCALE
+    sd["target_unigram_decoder.embed_tokens.weight"] = memb
+    sd["target_unigram_decoder.output_projection.weight"] = memb
+    return sd
+
+
 def make_vocoder_state_dict(vc: VocoderConfig, seed: int = 1, cal: Calibration = Calibration(), weight_norm: bool = False) -> Dict[str, torch.Tensor]:
     """`torch.load(ckpt)["generator"]` of the CodeHiFiGAN vocoder (agent/tts/vocoder.py:37-45).
 
