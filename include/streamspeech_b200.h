@@ -460,8 +460,51 @@ int ss_set_option(ss_engine* h, const char* name, int value);
  * (entry p + kv_off holds position p), then cross-attention K | V [mt_layers][cross_rows][2 * mt_dim].  bytes == 8 copies the two counts
  * alone; any other size below the whole state is SS_ERR_INVALID.  Synchronises the device. */
 int ss_debug_copy(ss_engine* h, const char* what, void* host_dst, size_t bytes);
-int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev,
-                     float* out_dev);
+/* out rows r * ldy = LayerNorm(x rows r * ldx) * g + b over C columns (eps 1e-5) for r < rows.  Errors: SS_ERR_INVALID, before any
+ * launch, for C outside {32, 64, .., 1024}, ldx or ldy < C, rows < 0 or a null pointer. */
+int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int ldx, int rows, int C, const float* g_dev, const float* b_dev,
+                     float* out_dev, int ldy);
+/* One GEMM of the engine's kernel layer with every field of its launch contract (kernels.h: ConvA, Epilogue), for the parity tests:
+ *   A[m][tap * C_in + ci] = pre_lrelu(x[b][p - x_row0][ci]) with m = b * L_rows + t and p = (t + t_offset) * stride + tap * dil - pad_left,
+ *   zero when p < 0, p >= L_in, p >= lengths[b], p outside [x_row0, x_row0 + x_rows) or (chunk > 0) p at or past the end of the chunk that
+ *   holds (t + t_offset) * stride; x holds x_rows rows (0: L_in) of ldx floats per batch element;
+ *   y = alpha * act(A W^T + bias) (glu: columns are (value, gate) pairs -> value * sigmoid(gate), N / 2 outputs), then
+ *   + res_scale * residual[o] and + out[o] (accumulate), at o = row * ldo + column with row = b * out_L + t * out_row_stride +
+ *   out_row_offset (out_L > 0) or m.  skinny_gemm only: A := LayerNorm(A) (ln_gamma / ln_beta, K = C_in), and split_n > 0 routes output
+ *   column c to out / out2 / out3 by c / split_n (strides ldo / ldo2 / ldo3).
+ * kernel: 0 = the engine's own choice for the shape (its linear routing for a plain B = 1 matrix, its conv routing otherwise, with the
+ * handle's options), 1 = gemm_conv, 2 = skinny_gemm, 3 / 4 = umma2_conv with 2 / 3 bf16 pieces.  splitk: 0 = no split-K scratch (the
+ * call never splits K), 1 = the handle's scratch.  lengths is a device array.  The route_* fields are written: the kernel taken,
+ * gemm_conv's BM x BN tile, the split-K slices (1 = none), skinny's MR / KS / CPT / grid CTAs, umma2's BN / CK / UPT / SB.
+ * Errors, before any launch: SS_ERR_INVALID for a shape or epilogue the chosen kernel cannot take (its *_supported rule, or for
+ * gemm_conv: C_in, ldx not multiples of 4 or x, w not 16-byte aligned), a null pointer, or a kernel outside [0, 4].  enqueue only */
+typedef struct ss_op_gemm_args {
+  const float* x;
+  const int32_t* lengths;
+  int32_t B, L_in, L_rows, C_in, ldx, ksize, stride, dil, pad_left, chunk;
+  float pre_lrelu;
+  int32_t t_offset, x_row0, x_rows, k_tiles_per_split;
+  const float* w;
+  int32_t N;
+  const float* bias;
+  int32_t act, glu;
+  float alpha;
+  const float* residual;
+  float res_scale;
+  int32_t accumulate;
+  float* out;
+  int32_t ldo, out_L, out_row_stride, out_row_offset;
+  const float* ln_gamma;
+  const float* ln_beta;
+  int32_t split_n;
+  float* out2;
+  float* out3;
+  int32_t ldo2, ldo3;
+  int32_t kernel, splitk;
+  int32_t route_kernel, route_bm, route_bn, route_splits, route_mr, route_ks, route_cpt, route_grid, route_u_bn, route_u_ck, route_u_upt,
+      route_u_sb;
+} ss_op_gemm_args;
+int ss_op_gemm(ss_engine* h, void* stream, ss_op_gemm_args* args);
 /* The unit arg-max hook: logits_dev [rows][ld] -> idx_dev [rows] with the first n_masked (<= 3) of pad, unk, eos never selected,
  * through argmax_rows (lprob_dev NULL) or argmax_lprob_rows (lprob_dev [rows]: each winner's log_softmax over all V columns). */
 int ss_op_argmax_rows(ss_engine* h, void* stream, const float* logits_dev, int rows, int V, int ld, int n_masked, int64_t* idx_dev, float* lprob_dev);

@@ -533,13 +533,15 @@ int ss_asr_finalize(ss_asr* h) {
     h->conv_ln[i] = LNorm{upload(h, t->data.data(), cout), upload(h, t2->data.data(), cout), cout};
   }
   const int C = h->C;
+  if (!layer_norm_supported(C)) return h->fail(SS_ERR_INVALID, "ss_asr_finalize: the feature LayerNorm cannot take width " + std::to_string(C));
   if ((rc = need(P + "layer_norm.weight", {C}, &t)) || (rc = need(P + "layer_norm.bias", {C}, &t2))) return rc;
   h->feat_ln = LNorm{upload(h, t->data.data(), C), upload(h, t2->data.data(), C), C};
   const HostTensor* pw = find(h, P + "post_extract_proj.weight");
   if (!pw || pw->shape.size() != 2 || pw->shape[1] != C) return h->fail(SS_ERR_MISSING, "ss_asr_finalize: missing " + P + "post_extract_proj.weight [D][C]");
   const int D = (int)pw->shape[0];
   h->D = D;
-  if (D % 64 || D > 1024) return h->fail(SS_ERR_INVALID, "ss_asr_finalize: model dim " + std::to_string(D) + " must be a multiple of 64 up to 1024");
+  if (D % 64 || D > 1024 || !layer_norm_supported(D))
+    return h->fail(SS_ERR_INVALID, "ss_asr_finalize: model dim " + std::to_string(D) + " must be a multiple of 64 up to 1024");
   h->H = h->cfg.heads > 0 ? h->cfg.heads : D / 64;
   if (D != h->H * 64)
     return h->fail(SS_ERR_INVALID, "ss_asr_finalize: encoder_attention_heads = " + std::to_string(h->H) + " gives head dim " + std::to_string(D / h->H) +

@@ -25,30 +25,49 @@ int check_launch(ss_engine* h, const char* where) {
   return SS_OK;
 }
 
-// conv-as-GEMM dispatch of the vocoder: the wgmma split-bf16 kernel (kernels_umma2.cu; umma_vocoder 12 / 13 = 2 / 3 bf16 pieces per
-// operand) when enabled and the shape fits, the fp32 CUDA-core kernel otherwise.  lane: the split-K region of the launching stream.
-void conv_gemm(ss_engine* h, const ConvA& a, const float* W, int N, const Epilogue& ep, int lane, cudaStream_t st) {
+// The GEMM kernels behind linear() / conv_gemm(), numbered as ss_op_gemm_args.kernel: 1 = gemm_conv, 2 = skinny_gemm, 3 / 4 = umma2_conv
+// with 2 / 3 bf16 pieces per operand.
+enum GemmKernel : int { GK_GEMM_CONV = 1, GK_SKINNY = 2, GK_UMMA2 = 3, GK_UMMA3 = 4 };
+int umma_kernel(int option) { return option - 10 >= 3 ? GK_UMMA3 : GK_UMMA2; }  // option 12 / 13 (umma_vocoder, umma_linear)
+
+// conv-as-GEMM routing of the vocoder: the wgmma split-bf16 kernel (kernels_umma2.cu; umma_vocoder 12 / 13 = 2 / 3 bf16 pieces per
+// operand) when enabled and the shape fits, the fp32 CUDA-core kernel otherwise
+int conv_gemm_kernel(const ss_engine* h, const ConvA& a, int N, const Epilogue& ep) {
   const int rows = a.B * a.L_rows;
   if (h->umma_vocoder >= 12 && rows >= h->umma_min_rows && a.C_in >= h->umma_min_channels && umma2_supported(a, N, ep))
+    return umma_kernel(h->umma_vocoder);
+  return GK_GEMM_CONV;
+}
+
+// lane: the split-K region of the launching stream
+void conv_gemm(ss_engine* h, const ConvA& a, const float* W, int N, const Epilogue& ep, int lane, cudaStream_t st) {
+  if (conv_gemm_kernel(h, a, N, ep) != GK_GEMM_CONV)
     umma2_conv(h->umma2_cache, a, W, N, ep, h->umma_vocoder - 10, &h->splitk[lane], st);
   else
     gemm_conv(a, W, N, ep, &h->splitk[lane], st);
 }
 
-// plain linear: out[M][N] = epilogue(x[M][K] @ W^T).
-// samples > 1: x stacks that many samples of equal row counts.  The tensor-core routing is decided from one sample's rows
-// (M / samples), so that a sample's GEMMs take the same class of kernel (fp32 or wgmma) as in the single-sample call: the batch
-// then reproduces the single-sample rounding instead of adding the split-bf16 error.
+// routing of a plain linear (a: x as B = 1, L_in = L_rows = M, C_in = K, ldx).  samples > 1: x stacks that many samples of equal row
+// counts.  The tensor-core routing is decided from one sample's rows (M / samples), so that a sample's GEMMs take the same class of
+// kernel (fp32 or wgmma) as in the single-sample call: the batch then reproduces the single-sample rounding instead of adding the
+// split-bf16 error.
+int linear_kernel(const ss_engine* h, const ConvA& a, int N, const Epilogue& ep, int samples) {
+  const int M = a.L_rows;
+  if (skinny_gemm_supported(M, N, a.C_in, ep) && (a.ldx & 3) == 0) return GK_SKINNY;
+  if (h->umma_linear >= 12 && M / samples >= h->umma_min_rows && umma2_supported(a, N, ep)) return umma_kernel(h->umma_linear);
+  return GK_GEMM_CONV;
+}
+
+// plain linear: out[M][N] = epilogue(x[M][K] @ W^T)
 void linear(ss_engine* h, const float* x, int ldx, int M, const Linear& l, Epilogue ep, cudaStream_t st, int samples = 1) {
   ConvA a;
   a.x = x; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = l.K; a.ldx = ldx;
   ep.bias = l.b;
-  if (skinny_gemm_supported(M, l.N, l.K, ep) && (ldx & 3) == 0)
-    skinny_gemm(x, ldx, l.w, M, l.N, l.K, ep, st);
-  else if (h->umma_linear >= 12 && M / samples >= h->umma_min_rows && umma2_supported(a, l.N, ep))
-    umma2_conv(h->umma2_cache, a, l.w, l.N, ep, h->umma_linear - 10, &h->splitk[0], st);
-  else
-    gemm_conv(a, l.w, l.N, ep, &h->splitk[0], st);
+  switch (linear_kernel(h, a, l.N, ep, samples)) {
+    case GK_SKINNY: skinny_gemm(x, ldx, l.w, M, l.N, l.K, ep, st); break;
+    case GK_GEMM_CONV: gemm_conv(a, l.w, l.N, ep, &h->splitk[0], st); break;
+    default: umma2_conv(h->umma2_cache, a, l.w, l.N, ep, h->umma_linear - 10, &h->splitk[0], st); break;
+  }
 }
 // out = epilogue(LayerNorm(x) @ W^T).  The LN is fused into the skinny kernel's A load when the shape allows it,
 // otherwise it is a separate launch into `scratch` [M][K].
@@ -2176,6 +2195,8 @@ int ss_op_conv1d(ss_engine* h, void* stream, const float* x_dev, int L, int C_in
   } else if (mode >= 2) {
     return h->fail(SS_ERR_INVALID, "modes 2 / 3 (first-generation tensor-core kernel) were removed: use 12 / 13");
   } else {
+    if (!gemm_conv_supported(a, w_dev, N, ep))
+      return h->fail(SS_ERR_INVALID, "ss_op_conv1d: gemm_conv needs C_in % 4 == 0 and 16-byte aligned x and w");
     gemm_conv(a, w_dev, N, ep, &h->splitk[0], S(stream));
   }
   return check_launch(h, "ss_op_conv1d");
@@ -2187,20 +2208,85 @@ int ss_op_linear(ss_engine* h, void* stream, const float* x_dev, int M, int K, c
   // the plain linear: skinny / fp32 CUDA-core kernels whatever the handle's routing (ss_op_linear_umma is the wgmma hook)
   Epilogue ep = ep_out(out_dev, N, act);
   ep.bias = bias_dev;
-  if (skinny_gemm_supported(M, N, K, ep) && (K & 3) == 0) {
-    skinny_gemm(x_dev, K, w_dev, M, N, K, ep, S(stream));
-  } else {
-    ConvA a;
-    a.x = x_dev; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = K; a.ldx = K;
-    gemm_conv(a, w_dev, N, ep, &h->splitk[0], S(stream));
-  }
+  ConvA a;
+  a.x = x_dev; a.B = 1; a.L_in = M; a.L_rows = M; a.C_in = K; a.ldx = K;
+  // both kernels read x and w as float4: 16-byte alignment and K % 4 == 0
+  if (!gemm_conv_supported(a, w_dev, N, ep)) return h->fail(SS_ERR_INVALID, "ss_op_linear: needs K % 4 == 0 and 16-byte aligned x and w");
+  if (skinny_gemm_supported(M, N, K, ep)) skinny_gemm(x_dev, K, w_dev, M, N, K, ep, S(stream));
+  else gemm_conv(a, w_dev, N, ep, &h->splitk[0], S(stream));
   return check_launch(h, "ss_op_linear");
 }
 
-int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int rows, int C, const float* g_dev, const float* b_dev, float* out_dev) {
+int ss_op_layer_norm(ss_engine* h, void* stream, const float* x_dev, int ldx, int rows, int C, const float* g_dev, const float* b_dev, float* out_dev,
+                     int ldy) {
   if (!h) return SS_ERR_INVALID;
-  layer_norm(x_dev, C, out_dev, C, g_dev, b_dev, rows, C, S(stream));
+  if (!x_dev || !g_dev || !b_dev || !out_dev || rows < 0 || ldx < C || ldy < C)
+    return h->fail(SS_ERR_INVALID, "ss_op_layer_norm: a null pointer, rows < 0 or a row stride below C");
+  if (!layer_norm_supported(C)) return h->fail(SS_ERR_INVALID, "ss_op_layer_norm: C = " + std::to_string(C) + " is not a multiple of 32 in [32, 1024]");
+  layer_norm(x_dev, ldx, out_dev, ldy, g_dev, b_dev, rows, C, S(stream));
   return check_launch(h, "ss_op_layer_norm");
+}
+
+int ss_op_gemm(ss_engine* h, void* stream, ss_op_gemm_args* g) {
+  if (!h) return SS_ERR_INVALID;
+  if (!g) return h->fail(SS_ERR_INVALID, "ss_op_gemm: null arguments");
+  auto refuse = [&](const std::string& why) { return h->fail(SS_ERR_INVALID, "ss_op_gemm: " + why); };
+  ConvA a;
+  a.x = g->x; a.B = g->B; a.L_in = g->L_in; a.L_rows = g->L_rows; a.C_in = g->C_in; a.ldx = g->ldx; a.ksize = g->ksize; a.stride = g->stride;
+  a.dil = g->dil; a.pad_left = g->pad_left; a.chunk = g->chunk; a.pre_lrelu = g->pre_lrelu; a.lengths = g->lengths; a.t_offset = g->t_offset;
+  a.x_row0 = g->x_row0; a.x_rows = g->x_rows; a.k_tiles_per_split = g->k_tiles_per_split;
+  Epilogue ep;
+  ep.bias = g->bias; ep.act = g->act; ep.glu = g->glu; ep.alpha = g->alpha; ep.residual = g->residual; ep.res_scale = g->res_scale;
+  ep.accumulate = g->accumulate; ep.out = g->out; ep.ldo = g->ldo; ep.out_L = g->out_L; ep.out_row_stride = g->out_row_stride;
+  ep.out_row_offset = g->out_row_offset; ep.ln_gamma = g->ln_gamma; ep.ln_beta = g->ln_beta; ep.split_n = g->split_n; ep.out2 = g->out2;
+  ep.out3 = g->out3; ep.ldo2 = g->ldo2; ep.ldo3 = g->ldo3;
+  const int N = g->N, M = a.B * a.L_rows, K = a.ksize * a.C_in;
+  if (!a.x || !g->w || !ep.out) return refuse("null x, w or out");
+  if (a.B < 1 || a.L_in < 1 || a.L_rows < 1 || a.C_in < 1 || a.ldx < a.C_in || a.ksize < 1 || a.stride < 1 || a.dil < 1 || a.pad_left < 0 ||
+      a.chunk < 0 || a.t_offset < 0 || a.x_row0 < 0 || a.x_rows < 0 || a.k_tiles_per_split < 0 || N < 1)
+    return refuse("bad A shape or N");
+  if (ep.act < ACT_NONE || ep.act > ACT_GELU || (ep.glu != 0 && ep.glu != 1) || (ep.accumulate != 0 && ep.accumulate != 1) || ep.out_L < 0 ||
+      ep.ldo < 1 || (ep.ln_gamma == nullptr) != (ep.ln_beta == nullptr) || ep.split_n < 0 ||
+      (ep.split_n > 0 && (!ep.out2 || !ep.out3 || (ep.glu ? N / 2 : N) > 3 * ep.split_n)))
+    return refuse("bad epilogue");
+  if (g->kernel < 0 || g->kernel > GK_UMMA3) return refuse("kernel must be in [0, 4]");
+  if (g->splitk != 0 && g->splitk != 1) return refuse("splitk must be 0 or 1");
+  const bool plain = a.B == 1 && a.ksize == 1 && a.stride == 1 && a.pad_left == 0 && a.chunk == 0 && !a.lengths && a.L_in == a.L_rows &&
+                     a.t_offset == 0 && a.x_row0 == 0 && a.x_rows == 0;
+  int kernel = g->kernel;
+  if (kernel == 0) {
+    kernel = plain ? linear_kernel(h, a, N, ep, 1) : conv_gemm_kernel(h, a, N, ep);
+    // the engine fuses the LayerNorm and the Q|K|V routing only on the skinny kernel (ln_linear, ln_qkv_routed)
+    if ((ep.ln_gamma || ep.split_n) && kernel != GK_SKINNY) return refuse("the fused LayerNorm and split_n routing exist only on skinny_gemm");
+  }
+  float** splitk = g->splitk ? &h->splitk[0] : nullptr;
+  g->route_kernel = kernel;
+  g->route_bm = g->route_bn = g->route_mr = g->route_ks = g->route_cpt = g->route_grid = g->route_u_bn = g->route_u_ck = g->route_u_upt =
+      g->route_u_sb = 0;
+  g->route_splits = 1;
+  const uintptr_t misaligned = (reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(g->w)) & 15;
+  if (kernel == GK_GEMM_CONV) {
+    if (!gemm_conv_supported(a, g->w, N, ep))
+      return refuse("gemm_conv needs C_in and ldx multiples of 4, 16-byte aligned x and w, an even N with glu, and no ln_gamma / split_n");
+    const GemmPlan p = gemm_conv_plan(a, N, ep, splitk != nullptr);
+    g->route_bm = p.BM; g->route_bn = p.BN; g->route_splits = p.splits;
+    gemm_conv(a, g->w, N, ep, splitk, S(stream));
+  } else if (kernel == GK_SKINNY) {
+    if (!plain || !skinny_gemm_supported(M, N, K, ep) || (a.ldx & 3) || misaligned ||
+        (ep.ln_gamma && ((reinterpret_cast<uintptr_t>(ep.ln_gamma) | reinterpret_cast<uintptr_t>(ep.ln_beta)) & 15)))
+      return refuse("skinny_gemm needs a plain matrix with M <= 64, K % 128 == 0, ldx % 4 == 0, 16-byte aligned x, w (and LN vectors), "
+                    "K <= 1024 with LayerNorm, an even N with glu, no out_L and act in [0, 4]");
+    const SkinnyPlan p = skinny_gemm_plan(M, N, K, ep);
+    g->route_mr = p.MR; g->route_ks = p.KS; g->route_cpt = p.CPT; g->route_grid = p.grid;
+    skinny_gemm(a.x, a.ldx, g->w, M, N, K, ep, S(stream));
+  } else {
+    if (!umma2_supported(a, N, ep)) return refuse("shape not supported by the wgmma kernel");
+    const int pieces = kernel == GK_UMMA3 ? 3 : 2;
+    const Umma2Plan p = umma2_plan(a, N, pieces, splitk != nullptr);
+    g->route_splits = p.splits; g->route_u_bn = p.BN; g->route_u_ck = p.CK; g->route_u_upt = p.UPT; g->route_u_sb = p.SB;
+    umma2_conv(h->umma2_cache, a, g->w, N, ep, pieces, splitk, S(stream));
+  }
+  return check_launch(h, "ss_op_gemm");
 }
 
 int ss_op_argmax_rows(ss_engine* h, void* stream, const float* logits_dev, int rows, int V, int ld, int n_masked, int64_t* idx_dev, float* lprob_dev) {

@@ -12,7 +12,7 @@ namespace ss {
 
 extern unsigned long long g_launches;  // kernels launched by this library (process-wide)
 
-enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3, ACT_GELU = 4 };  // ACT_GELU: exact erf form (gemm_conv, umma2_conv)
+enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_TANH = 3, ACT_GELU = 4 };  // ACT_GELU: exact erf form
 
 // A-operand of a GEMM viewed as a 1-D convolution over a channels-last activation
 // x[B][L_in][C_in]:  A[m][tap*C_in + ci] = pre(x[b][t*stride + tap*dil - pad_left][ci]),
@@ -71,6 +71,16 @@ struct Epilogue {
 // C[M,N] = epilogue( A[M,K] * W[N,K]^T ), K = ksize*C_in, W row-major with K contiguous.
 // splitk: the caller's split-K scratch region (nullptr: never split), see splitk_workspace.
 void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, float** splitk, cudaStream_t st);
+// What gemm_conv can take: its A and W loads are float4, so C_in, ldx and K are multiples of 4 and x, W are 16-byte aligned; no
+// skinny-only fusion (ln_gamma, split_n); GLU needs an even N.  Callers with arbitrary shapes (the test hooks) check this first.
+bool gemm_conv_supported(const ConvA& a, const float* W, int N, const Epilogue& ep);
+// gemm_conv's launch: BM x BN tile, implicit-im2col (conv) or plain A, and `splits` slices of `tiles_per_split` k-tiles (splits = 1:
+// one slice of every k-tile).  have_scratch: a split-K region was passed (the launch still takes one slice when it cannot be allocated).
+struct GemmPlan {
+  int BM, BN, splits, tiles_per_split;
+  bool conv;
+};
+GemmPlan gemm_conv_plan(const ConvA& a, int N, const Epilogue& ep, bool have_scratch);
 
 // Split-K scratch: *splitk is a region of splitk_workspace_bytes() that the first GEMM splitting into it allocates and its owner
 // frees; the launches that share a region must be stream-ordered.  Returns the region when `bytes` fit it (nullptr: no region,
@@ -91,6 +101,12 @@ struct Umma2Cache {
 void umma2_cache_clear(Umma2Cache* c);  // frees the packed weights
 void umma2_cache_destroy(Umma2Cache* c);
 bool umma2_supported(const ConvA& a, int N, const Epilogue& ep);
+// umma2_conv's launch: BN-column tiles, CK-channel chunks, NP bf16 pieces, UPT float4 loads per converter thread and chunk (SETS
+// chunk loads in flight), SB weight-ring stages, and the (chunk, tap) units split into `splits` slices of units_per_split units
+struct Umma2Plan {
+  int BN, CK, NP, UPT, SETS, SB, splits, units_per_split;
+};
+Umma2Plan umma2_plan(const ConvA& a, int N, int pieces, bool have_scratch);
 void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, float** splitk, cudaStream_t st);
 // packed copy of W[N][ksize*C_in] in the kernels' tiling (made once per weight matrix and tiling; nullptr when out of memory)
 const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int N, int C_in, int ksize, int BN, int CK, int NP, cudaStream_t st);
@@ -182,9 +198,17 @@ void expand_frames_ragged(const float* emb, const int* cumsum, const VocSeqs& q,
 // Weight-streaming GEMM for M <= 64 rows (plain row-major A): one warp per output column, see kernels_skinny.cu.
 bool skinny_gemm_supported(int M, int N, int K, const Epilogue& ep);
 void skinny_gemm(const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st);
+// skinny_gemm's launch: MR rows per pass, KS K-slices per column group, CPT columns per warp-task, `grid` CTAs (fewer than the tasks
+// need when capped: the CTAs then loop over tasks)
+struct SkinnyPlan {
+  int MR, KS, CPT, grid;
+};
+SkinnyPlan skinny_gemm_plan(int M, int N, int K, const Epilogue& ep);
 
-// y[r] = LayerNorm(x[r]) * gamma + beta, rows of length C (C <= 1024, multiple of 32)
-void layer_norm(const float* x, int ldx, float* y, int ldy, const float* gamma, const float* beta, int rows, int C,
+// y[r] = LayerNorm(x[r]) * gamma + beta, rows of length C.  Takes C % 32 == 0 in [32, 1024] (layer_norm_supported); any other C
+// launches nothing and returns false.
+bool layer_norm_supported(int C);
+bool layer_norm(const float* x, int ldx, float* y, int ldy, const float* gamma, const float* beta, int rows, int C,
                 cudaStream_t st);
 
 // Kaldi fbank + global CMVN for frames [f0, f0+nf) of a 16 kHz signal (already on device, NOT scaled by 2^15).

@@ -286,70 +286,97 @@ void splitk_epilogue(const float* ws, int splits, int M, int N, int L_rows, cons
 namespace {
 
 template <int BM, int BN>
-void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue& ep, bool conv, float** splitk, cudaStream_t st) {
+void launch(const ConvA& a, const float* W, int M, int N, int K, const Epilogue& ep, GemmPlan plan, float** splitk, cudaStream_t st) {
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
-  const long ctas = (long)grid.x * grid.y;
-  const int nk = (K + BK - 1) / BK;
-  int splits = 1;
-  const long sms = std::max(1, current_device_sms());
-  if (a.k_tiles_per_split > 0) {
-    splits = (nk + a.k_tiles_per_split - 1) / a.k_tiles_per_split;
-    if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
-  } else if (ctas < sms && nk >= 8) {
-    splits = (int)std::min<long>((sms + ctas - 1) / ctas, nk / 4);  // >= 4 k-tiles (64 columns) per slice
-    if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
-  }
   float* ws = nullptr;
-  int tiles = nk;
-  if (splits > 1) {
-    ws = splitk_workspace(splitk, (size_t)splits * M * N * sizeof(float));
-    if (!ws) splits = 1;
+  if (plan.splits > 1) {
+    ws = splitk_workspace(splitk, (size_t)plan.splits * M * N * sizeof(float));
+    if (!ws) {
+      plan.splits = 1;
+      plan.tiles_per_split = (K + BK - 1) / BK;
+    }
   }
-  if (splits > 1) {
-    tiles = (nk + splits - 1) / splits;
-    splits = (nk + tiles - 1) / tiles;
-    grid.z = splits;
-  }
-  if (conv)
-    gemm_kernel<BM, BN, true><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws);  // tile GEMMs never launch early (see launch_pdl)
+  grid.z = plan.splits;
+  if (plan.conv)
+    gemm_kernel<BM, BN, true><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, plan.tiles_per_split, ws);  // tile GEMMs never launch early (see launch_pdl)
   else
-    gemm_kernel<BM, BN, false><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, tiles, ws);
-  if (splits > 1) {
+    gemm_kernel<BM, BN, false><<<grid, NT, 0, st>>>(a, W, M, N, K, ep, plan.tiles_per_split, ws);
+  if (plan.splits > 1) {
     ++g_launches;
     int total = M * (ep.glu ? N / 2 : N);
-    launch_pdl(splitk_epilogue_kernel, dim3((total + 255) / 256), dim3(256), 0, st, ws, splits, M, N, a.L_rows, ep);
+    launch_pdl(splitk_epilogue_kernel, dim3((total + 255) / 256), dim3(256), 0, st, ws, plan.splits, M, N, a.L_rows, ep);
   }
 }
 
 }  // namespace
+
+bool gemm_conv_supported(const ConvA& a, const float* W, int N, const Epilogue& ep) {
+  if (!a.x || !W || a.C_in < 1 || a.ldx < a.C_in || (a.C_in & 3) || (a.ldx & 3) || a.ksize < 1 || N < 1) return false;
+  if ((reinterpret_cast<uintptr_t>(a.x) & 15) || (reinterpret_cast<uintptr_t>(W) & 15)) return false;
+  if (ep.ln_gamma || ep.ln_beta || ep.split_n || (ep.glu && (N & 1))) return false;
+  return true;
+}
+
+GemmPlan gemm_conv_plan(const ConvA& a, int N, const Epilogue& ep, bool have_scratch) {
+  const int M = a.B * a.L_rows;
+  const int K = a.ksize * a.C_in;
+  GemmPlan p;
+  p.conv = !(a.ksize == 1 && a.stride == 1 && a.pad_left == 0 && a.chunk == 0 && a.lengths == nullptr && a.L_in == a.L_rows &&
+             a.t_offset == 0 && a.x_row0 == 0 && a.x_rows == 0);
+  // ---- tile
+  auto ctas = [&](int bm, int bn) { return (long)((M + bm - 1) / bm) * ((N + bn - 1) / bn); };
+  const long target = std::max(1, current_device_sms());  // one wave of SMs
+  const int nk = (K + BK - 1) / BK;
+  if (N <= 16 && !ep.glu) {
+    p.BN = 16;
+    p.BM = ctas(128, 16) >= target ? 128 : 32;
+  } else if (N <= 32) {
+    p.BN = 32;
+    p.BM = ctas(64, 32) >= target ? 64 : 32;
+  } else {
+    // Prefer the largest tile that still fills the GPU once split-K (slices of >= 8 k-tiles, at most 8 slices) is counted:
+    // a long K walked by few small CTAs is latency-bound.
+    const long max_splits = std::max(1, std::min(8, nk / 8));
+    if (ctas(128, 64) >= 2 * target) p.BM = 128, p.BN = 64;
+    else if (ctas(64, 64) * max_splits >= target) p.BM = 64, p.BN = 64;
+    else if (ctas(32, 64) * max_splits >= target) p.BM = 32, p.BN = 64;
+    else p.BM = 32, p.BN = 32;
+  }
+  // ---- split-K
+  int splits = 1;
+  const long tile_ctas = ctas(p.BM, p.BN);
+  if (a.k_tiles_per_split > 0) {
+    splits = (nk + a.k_tiles_per_split - 1) / a.k_tiles_per_split;
+    if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
+  } else if (tile_ctas < target && nk >= 8) {
+    splits = (int)std::min<long>((target + tile_ctas - 1) / tile_ctas, nk / 4);  // >= 4 k-tiles (64 columns) per slice
+    if ((size_t)splits * M * N * sizeof(float) > SPLITK_WS_BYTES) splits = 1;
+  }
+  if (!have_scratch) splits = 1;
+  p.tiles_per_split = nk;
+  if (splits > 1) {
+    p.tiles_per_split = (nk + splits - 1) / splits;
+    splits = (nk + p.tiles_per_split - 1) / p.tiles_per_split;
+  }
+  p.splits = splits;
+  return p;
+}
 
 void gemm_conv(const ConvA& a, const float* W, int N, const Epilogue& ep, float** splitk, cudaStream_t st) {
   ++g_launches;
   const int M = a.B * a.L_rows;
   const int K = a.ksize * a.C_in;
   if (M <= 0 || N <= 0) return;
-  const bool conv = !(a.ksize == 1 && a.stride == 1 && a.pad_left == 0 && a.chunk == 0 && a.lengths == nullptr &&
-                      a.L_in == a.L_rows && a.t_offset == 0 && a.x_row0 == 0 && a.x_rows == 0);
-  auto ctas = [&](int bm, int bn) { return (long)((M + bm - 1) / bm) * ((N + bn - 1) / bn); };
-  const long target = std::max(1, current_device_sms());  // one wave of SMs
-  if (N <= 16 && !ep.glu) {
-    if (ctas(128, 16) >= target) launch<128, 16>(a, W, M, N, K, ep, conv, splitk, st);
-    else launch<32, 16>(a, W, M, N, K, ep, conv, splitk, st);
-    return;
+  const GemmPlan p = gemm_conv_plan(a, N, ep, splitk != nullptr);
+  switch (p.BM * 1000 + p.BN) {
+    case 128016: launch<128, 16>(a, W, M, N, K, ep, p, splitk, st); break;
+    case 32016: launch<32, 16>(a, W, M, N, K, ep, p, splitk, st); break;
+    case 64032: launch<64, 32>(a, W, M, N, K, ep, p, splitk, st); break;
+    case 128064: launch<128, 64>(a, W, M, N, K, ep, p, splitk, st); break;
+    case 64064: launch<64, 64>(a, W, M, N, K, ep, p, splitk, st); break;
+    case 32064: launch<32, 64>(a, W, M, N, K, ep, p, splitk, st); break;
+    default: launch<32, 32>(a, W, M, N, K, ep, p, splitk, st); break;
   }
-  if (N <= 32) {
-    if (ctas(64, 32) >= target) launch<64, 32>(a, W, M, N, K, ep, conv, splitk, st);
-    else launch<32, 32>(a, W, M, N, K, ep, conv, splitk, st);
-    return;
-  }
-  // Prefer the largest tile that still fills the GPU once split-K (slices of >= 8 k-tiles, at most 8 slices) is counted:
-  // a long K walked by few small CTAs is latency-bound.
-  const int nk = (K + BK - 1) / BK;
-  const long max_splits = std::max(1, std::min(8, nk / 8));
-  if (ctas(128, 64) >= 2 * target) launch<128, 64>(a, W, M, N, K, ep, conv, splitk, st);
-  else if (ctas(64, 64) * max_splits >= target) launch<64, 64>(a, W, M, N, K, ep, conv, splitk, st);
-  else if (ctas(32, 64) * max_splits >= target) launch<32, 64>(a, W, M, N, K, ep, conv, splitk, st);
-  else launch<32, 32>(a, W, M, N, K, ep, conv, splitk, st);
 }
 
 }  // namespace ss

@@ -296,19 +296,31 @@ __global__ void conv_post_tanh_kernel(const float* __restrict__ x, int L, int C,
 
 }  // namespace
 
-void layer_norm(const float* x, int ldx, float* y, int ldy, const float* gamma, const float* beta, int rows, int C,
-                cudaStream_t st) {
-  ++g_launches;
-  if (rows <= 0) return;
-  const int wpb = 8;
-  dim3 grid((rows + wpb - 1) / wpb);
-  switch (C) {
-    case 128: launch_pdl(layer_norm_kernel<4>, dim3(grid), dim3(wpb * 32), 0, st, x, ldx, y, ldy, gamma, beta, rows); break;
-    case 256: launch_pdl(layer_norm_kernel<8>, dim3(grid), dim3(wpb * 32), 0, st, x, ldx, y, ldy, gamma, beta, rows); break;
-    case 512: launch_pdl(layer_norm_kernel<16>, dim3(grid), dim3(wpb * 32), 0, st, x, ldx, y, ldy, gamma, beta, rows); break;
-    case 1024: launch_pdl(layer_norm_kernel<32>, dim3(grid), dim3(wpb * 32), 0, st, x, ldx, y, ldy, gamma, beta, rows); break;
-    default: break;  // engine validates C at finalize
+namespace {
+
+// layer_norm_kernel<n> for n in [1, N]: C = 32 n
+template <int N>
+bool launch_layer_norm(int n, dim3 grid, dim3 block, cudaStream_t st, const float* x, int ldx, float* y, int ldy, const float* gamma,
+                       const float* beta, int rows) {
+  if (n == N) {
+    launch_pdl(layer_norm_kernel<N>, grid, block, 0, st, x, ldx, y, ldy, gamma, beta, rows);
+    return true;
   }
+  if constexpr (N > 1) return launch_layer_norm<N - 1>(n, grid, block, st, x, ldx, y, ldy, gamma, beta, rows);
+  return false;
+}
+
+}  // namespace
+
+bool layer_norm_supported(int C) { return C >= 32 && C <= 1024 && C % 32 == 0; }
+
+bool layer_norm(const float* x, int ldx, float* y, int ldy, const float* gamma, const float* beta, int rows, int C,
+                cudaStream_t st) {
+  if (!layer_norm_supported(C)) return false;
+  ++g_launches;
+  if (rows <= 0) return true;
+  const int wpb = 8;
+  return launch_layer_norm<32>(C / 32, dim3((rows + wpb - 1) / wpb), dim3(wpb * 32), st, x, ldx, y, ldy, gamma, beta, rows);
 }
 
 void depthwise_bn_silu(const float* x, int ldx, const float* w, const float* scale, const float* shift, float* y, int ldy,

@@ -25,7 +25,8 @@ __device__ __forceinline__ float sk_act(float x, int act) {
     case ACT_RELU: return x > 0.f ? x : 0.f;
     case ACT_SILU: return x / (1.0f + expf(-x));
     case ACT_TANH: return tanhf(x);
-    default: return x;
+    case ACT_GELU: return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
+    default: return x;  // ACT_NONE (skinny_gemm_supported refuses any other value)
   }
 }
 
@@ -204,25 +205,25 @@ __global__ void __launch_bounds__(SK_WARPS * 32) skinny_gemm_kernel(const float*
 }
 
 template <int MR, int KS, int CPT, bool GLU>
-void launch_skinny(const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st) {
-  const int ntasks = N / CPT;
-  const int per_cta = SK_WARPS / KS;
-  int grid = (ntasks + per_cta - 1) / per_cta;
-  // with a fused LayerNorm every CTA recomputes the row statistics: keep the grid at two CTAs per SM and loop over tasks
-  const int sms = std::max(1, current_device_sms());
-  const int cap = ep.ln_gamma ? sms * 2 : sms * 8;
-  if (grid > cap) grid = cap;
+void launch_skinny(const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, int grid, cudaStream_t st) {
   launch_pdl_always(skinny_gemm_kernel<MR, KS, CPT, GLU>, dim3(grid), dim3(SK_WARPS * 32), 0, st, A, lda, W, M, N, K, ep);
 }
 
 template <int MR, int CPT, bool GLU>
-void dispatch_ks(int ks, const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st) {
-  switch (ks) {
-    case 1: launch_skinny<MR, 1, CPT, GLU>(A, lda, W, M, N, K, ep, st); break;
-    case 2: launch_skinny<MR, 2, CPT, GLU>(A, lda, W, M, N, K, ep, st); break;
-    case 4: launch_skinny<MR, 4, CPT, GLU>(A, lda, W, M, N, K, ep, st); break;
-    default: launch_skinny<MR, 8, CPT, GLU>(A, lda, W, M, N, K, ep, st); break;
+void dispatch_ks(const SkinnyPlan& p, const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st) {
+  switch (p.KS) {
+    case 1: launch_skinny<MR, 1, CPT, GLU>(A, lda, W, M, N, K, ep, p.grid, st); break;
+    case 2: launch_skinny<MR, 2, CPT, GLU>(A, lda, W, M, N, K, ep, p.grid, st); break;
+    case 4: launch_skinny<MR, 4, CPT, GLU>(A, lda, W, M, N, K, ep, p.grid, st); break;
+    default: launch_skinny<MR, 8, CPT, GLU>(A, lda, W, M, N, K, ep, p.grid, st); break;
   }
+}
+
+template <int MR>
+void dispatch_cpt(const SkinnyPlan& p, const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st) {
+  if (ep.glu) dispatch_ks<MR, 2, true>(p, A, lda, W, M, N, K, ep, st);
+  else if (p.CPT == 4) dispatch_ks<MR, 4, false>(p, A, lda, W, M, N, K, ep, st);
+  else dispatch_ks<MR, 1, false>(p, A, lda, W, M, N, K, ep, st);
 }
 
 }  // namespace
@@ -231,30 +232,34 @@ bool skinny_gemm_supported(int M, int N, int K, const Epilogue& ep) {
   if (M < 1 || M > 64 || (K & 127) != 0 || ep.out_L > 0) return false;
   if (ep.ln_gamma && K > 1024) return false;
   if (ep.glu && (N & 1)) return false;
+  if (ep.act < ACT_NONE || ep.act > ACT_GELU) return false;  // the activations sk_act implements
   return true;
+}
+
+SkinnyPlan skinny_gemm_plan(int M, int N, int K, const Epilogue& ep) {
+  SkinnyPlan p;
+  p.MR = M == 1 ? 1 : M <= 8 ? 8 : 16;
+  // columns per warp-task: 4 independent W rows in flight per lane and one A load shared by 4 columns
+  p.CPT = ep.glu ? 2 : ((N & 3) == 0 && (ep.split_n == 0 || (ep.split_n & 3) == 0) ? 4 : 1);
+  const int ntasks = N / p.CPT;
+  // K-slices per column group: enough warp-tasks to cover the SMs, every slice a multiple of 128 columns
+  p.KS = 1;
+  while (p.KS < 8 && (long)ntasks * p.KS < 1184 && K % (p.KS * 2 * 128) == 0) p.KS *= 2;
+  const int per_cta = SK_WARPS / p.KS;
+  p.grid = (ntasks + per_cta - 1) / per_cta;
+  // with a fused LayerNorm every CTA recomputes the row statistics: keep the grid at two CTAs per SM and loop over tasks
+  const int sms = std::max(1, current_device_sms());
+  const int cap = ep.ln_gamma ? sms * 2 : sms * 8;
+  if (p.grid > cap) p.grid = cap;
+  return p;
 }
 
 void skinny_gemm(const float* A, int lda, const float* W, int M, int N, int K, const Epilogue& ep, cudaStream_t st) {
   ++g_launches;
-  // columns per warp-task: 4 independent W rows in flight per lane and one A load shared by 4 columns
-  const int cpt = ep.glu ? 2 : ((N & 3) == 0 && (ep.split_n == 0 || (ep.split_n & 3) == 0) ? 4 : 1);
-  const int ntasks = N / cpt;
-  // K-slices per column group: enough warp-tasks to cover the SMs, every slice a multiple of 128 columns
-  int ks = 1;
-  while (ks < 8 && (long)ntasks * ks < 1184 && K % (ks * 2 * 128) == 0) ks *= 2;
-  if (M == 1) {
-    if (ep.glu) dispatch_ks<1, 2, true>(ks, A, lda, W, M, N, K, ep, st);
-    else if (cpt == 4) dispatch_ks<1, 4, false>(ks, A, lda, W, M, N, K, ep, st);
-    else dispatch_ks<1, 1, false>(ks, A, lda, W, M, N, K, ep, st);
-  } else if (M <= 8) {
-    if (ep.glu) dispatch_ks<8, 2, true>(ks, A, lda, W, M, N, K, ep, st);
-    else if (cpt == 4) dispatch_ks<8, 4, false>(ks, A, lda, W, M, N, K, ep, st);
-    else dispatch_ks<8, 1, false>(ks, A, lda, W, M, N, K, ep, st);
-  } else {
-    if (ep.glu) dispatch_ks<16, 2, true>(ks, A, lda, W, M, N, K, ep, st);
-    else if (cpt == 4) dispatch_ks<16, 4, false>(ks, A, lda, W, M, N, K, ep, st);
-    else dispatch_ks<16, 1, false>(ks, A, lda, W, M, N, K, ep, st);
-  }
+  const SkinnyPlan p = skinny_gemm_plan(M, N, K, ep);
+  if (p.MR == 1) dispatch_cpt<1>(p, A, lda, W, M, N, K, ep, st);
+  else if (p.MR == 8) dispatch_cpt<8>(p, A, lda, W, M, N, K, ep, st);
+  else dispatch_cpt<16>(p, A, lda, W, M, N, K, ep, st);
 }
 
 }  // namespace ss

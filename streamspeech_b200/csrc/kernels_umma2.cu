@@ -444,9 +444,8 @@ void u2_launch_v(const U2Params& p, dim3 grid, size_t smem, cudaStream_t st) {
 }
 
 template <int BN, int NP>
-void u2_launch(const U2Params& p, dim3 grid, size_t smem, cudaStream_t st) {
-  const int n_a = p.rs * (p.CK / 4);  // float4 units per staged chunk
-  if (n_a <= 4 * U2_CONVERTERS) u2_launch_v<BN, NP, 4, 3>(p, grid, smem, st);
+void u2_launch(const U2Params& p, int upt, dim3 grid, size_t smem, cudaStream_t st) {
+  if (upt == 4) u2_launch_v<BN, NP, 4, 3>(p, grid, smem, st);
   else u2_launch_v<BN, NP, U2_MAX_UNITS, 2>(p, grid, smem, st);
 }
 
@@ -502,15 +501,45 @@ const unsigned char* umma2_packed_weights(Umma2Cache* cache, const float* W, int
   return wp;
 }
 
+Umma2Plan umma2_plan(const ConvA& a, int N, int pieces, bool have_scratch) {
+  Umma2Plan q;
+  const int M = a.L_rows;
+  q.NP = pieces >= 3 ? 3 : 2;
+  q.BN = u2_bn(N);
+  q.CK = (a.C_in % 32 == 0) ? 32 : 16;
+  const int k = a.ksize;
+  const int rs = U2_BM + (k - 1) * a.dil;  // staged rows per chunk
+  const int rs_pad = ((rs + 7) & ~7) + 4;
+  const int n_a = rs * (q.CK / 4);  // float4 units per staged chunk
+  q.UPT = n_a <= 4 * U2_CONVERTERS ? 4 : U2_MAX_UNITS;
+  q.SETS = q.UPT == 4 ? 3 : 2;
+  const size_t a_bytes = (size_t)2 * q.NP * (q.CK >> 3) * rs_pad * 16;
+  const size_t b_unit = (size_t)q.NP * q.BN * q.CK * 2;
+  q.SB = (((a_bytes + 127) & ~(size_t)127) + 4 * b_unit <= 110 * 1024) ? 4 : 3;
+  // ---- split over (chunk, tap) units when the tile grid cannot fill the GPU
+  const int units_total = (a.C_in / q.CK) * k;
+  const int m_tiles = (M + U2_BM - 1) / U2_BM;
+  const long base = (long)m_tiles * ((N + q.BN - 1) / q.BN);
+  int splits = 1;
+  if (base < U2_SPLIT_BELOW && units_total >= 2 * U2_MIN_UNITS) {
+    const long sms = std::max(1, current_device_sms());
+    splits = (int)std::min<long>((sms + base - 1) / base, units_total / U2_MIN_UNITS);
+    while (splits > 1 && (size_t)splits * M * N * sizeof(float) > (32u << 20)) --splits;
+  }
+  if (!have_scratch) splits = 1;
+  q.units_per_split = (units_total + splits - 1) / splits;
+  q.splits = (units_total + q.units_per_split - 1) / q.units_per_split;
+  return q;
+}
+
 void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const Epilogue& ep, int pieces, float** splitk, cudaStream_t st) {
   const int M = a.L_rows;
   if (M <= 0) {
     ++g_launches;
     return;
   }
-  const int NP = pieces >= 3 ? 3 : 2;
-  const int BN = u2_bn(N);
-  const int CK = (a.C_in % 32 == 0) ? 32 : 16;
+  const Umma2Plan q = umma2_plan(a, N, pieces, splitk != nullptr);
+  const int NP = q.NP, BN = q.BN, CK = q.CK;
   const int k = a.ksize;
   // ---- packed weights (once per weight matrix and tiling)
   const unsigned char* wp = umma2_packed_weights(cache, W, N, a.C_in, k, BN, CK, NP, st);
@@ -519,7 +548,6 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
     return;
   }
   ++g_launches;
-  const int n_chunks = a.C_in / CK;
   const int n_tiles = (N + BN - 1) / BN;
   U2Params p;
   p.a = a;
@@ -532,18 +560,9 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   p.dil = a.dil;
   p.rs = U2_BM + (k - 1) * a.dil;
   p.rs_pad = ((p.rs + 7) & ~7) + 4;  // planes 64 bytes out of phase: halves the bank conflicts of the 8-byte piece stores
-  p.units_total = n_chunks * k;
-  // ---- split over (chunk, tap) units when the tile grid cannot fill the GPU
+  p.units_total = (a.C_in / CK) * k;
   const int m_tiles = (M + U2_BM - 1) / U2_BM;
-  const long base = (long)m_tiles * n_tiles;
-  int splits = 1;
-  if (base < U2_SPLIT_BELOW && p.units_total >= 2 * U2_MIN_UNITS) {
-    const long sms = std::max(1, current_device_sms());
-    splits = (int)std::min<long>((sms + base - 1) / base, p.units_total / U2_MIN_UNITS);
-    while (splits > 1 && (size_t)splits * M * N * sizeof(float) > (32u << 20)) --splits;
-  }
-  int ups = (p.units_total + splits - 1) / splits;
-  splits = (p.units_total + ups - 1) / ups;
+  int splits = q.splits, ups = q.units_per_split;
   float* ws = nullptr;
   if (splits > 1) {
     ws = splitk_workspace(splitk, (size_t)splits * M * N * sizeof(float));
@@ -555,24 +574,24 @@ void umma2_conv(Umma2Cache* cache, const ConvA& a, const float* W, int N, const 
   p.units_per_split = ups;
   p.ws = ws;
   p.dbg = cache->dbg;
+  p.SB = q.SB;
   const size_t a_bytes = (size_t)2 * NP * (CK >> 3) * p.rs_pad * 16;
   const size_t b_unit = (size_t)NP * BN * CK * 2;
-  p.SB = (((a_bytes + 127) & ~(size_t)127) + 4 * b_unit <= 110 * 1024) ? 4 : 3;
   const size_t smem = std::max<size_t>(((a_bytes + 127) & ~(size_t)127) + p.SB * b_unit, (size_t)U2_BM * (BN + 8) * sizeof(float)) + 256;  // >= the epilogue's output tile
   dim3 grid(n_tiles, m_tiles, splits);
   if (NP == 3) {
     switch (BN) {
-      case 128: u2_launch<128, 3>(p, grid, smem, st); break;
-      case 64: u2_launch<64, 3>(p, grid, smem, st); break;
-      case 32: u2_launch<32, 3>(p, grid, smem, st); break;
-      default: u2_launch<16, 3>(p, grid, smem, st); break;
+      case 128: u2_launch<128, 3>(p, q.UPT, grid, smem, st); break;
+      case 64: u2_launch<64, 3>(p, q.UPT, grid, smem, st); break;
+      case 32: u2_launch<32, 3>(p, q.UPT, grid, smem, st); break;
+      default: u2_launch<16, 3>(p, q.UPT, grid, smem, st); break;
     }
   } else {
     switch (BN) {
-      case 128: u2_launch<128, 2>(p, grid, smem, st); break;
-      case 64: u2_launch<64, 2>(p, grid, smem, st); break;
-      case 32: u2_launch<32, 2>(p, grid, smem, st); break;
-      default: u2_launch<16, 2>(p, grid, smem, st); break;
+      case 128: u2_launch<128, 2>(p, q.UPT, grid, smem, st); break;
+      case 64: u2_launch<64, 2>(p, q.UPT, grid, smem, st); break;
+      case 32: u2_launch<32, 2>(p, q.UPT, grid, smem, st); break;
+      default: u2_launch<16, 2>(p, q.UPT, grid, smem, st); break;
     }
   }
   if (splits > 1) splitk_epilogue(ws, splits, M, N, a.L_rows, ep, st);

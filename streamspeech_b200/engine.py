@@ -46,6 +46,26 @@ class ASRConfig(ctypes.Structure):
                                       "max_frames", "time_stages")]
 
 
+_P, _I, _F = ctypes.c_void_p, ctypes.c_int32, ctypes.c_float
+
+
+class GemmArgs(ctypes.Structure):
+    """ctypes mirror of `struct ss_op_gemm_args` (the ss_op_gemm parity hook)"""
+    _fields_ = (
+        [("x", _P), ("lengths", _P)]
+        + [(n, _I) for n in ("B", "L_in", "L_rows", "C_in", "ldx", "ksize", "stride", "dil", "pad_left", "chunk")]
+        + [("pre_lrelu", _F)]
+        + [(n, _I) for n in ("t_offset", "x_row0", "x_rows", "k_tiles_per_split")]
+        + [("w", _P), ("N", _I), ("bias", _P), ("act", _I), ("glu", _I), ("alpha", _F), ("residual", _P), ("res_scale", _F),
+           ("accumulate", _I), ("out", _P)]
+        + [(n, _I) for n in ("ldo", "out_L", "out_row_stride", "out_row_offset")]
+        + [("ln_gamma", _P), ("ln_beta", _P), ("split_n", _I), ("out2", _P), ("out3", _P), ("ldo2", _I), ("ldo3", _I),
+           ("kernel", _I), ("splitk", _I)]
+        + [(n, _I) for n in ("route_kernel", "route_bm", "route_bn", "route_splits", "route_mr", "route_ks", "route_cpt", "route_grid",
+                             "route_u_bn", "route_u_ck", "route_u_upt", "route_u_sb")]
+    )
+
+
 class EngineError(RuntimeError):
     """code: the ss_status of a failed library call (None for errors raised on the host side); detail: the library's message"""
 
@@ -109,7 +129,8 @@ def load_library() -> ctypes.CDLL:
     lib.ss_op_linear_umma.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, i32, vp]
     lib.ss_op_conv1d.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, ctypes.c_float, i32, vp]
     lib.ss_set_option.argtypes = [vp, ctypes.c_char_p, i32]
-    lib.ss_op_layer_norm.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
+    lib.ss_op_layer_norm.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, i32]
+    lib.ss_op_gemm.argtypes = [vp, vp, ctypes.POINTER(GemmArgs)]
     lib.ss_op_argmax_rows.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp, vp]
     lib.ss_debug_copy.argtypes = [vp, ctypes.c_char_p, vp, ctypes.c_size_t]
     lib.ss_launch_count.argtypes = [vp]
@@ -164,6 +185,7 @@ EXPORTED_SYMBOLS = [
     "ss_t2u_unit_decode_batch", "ss_pool_mt_greedy", "ss_pool_mt_greedy_incremental", "ss_t2u_unit_decode_ragged", "ss_op_relpos_attention", "ss_op_mha_attention",
     "ss_op_grouped_causal_attention", "ss_op_depthwise_bn_silu", "ss_op_ms_relpos_attention", "ss_op_ms_depthwise",
     "ss_t2u_unit_decode_batch_scored", "ss_op_argmax_rows", "ss_t2u_encode_batch", "ss_unit_search_batch",
+    "ss_op_gemm",
 ]
 
 
@@ -906,10 +928,21 @@ class Engine:
     def set_option(self, name: str, value: int):
         self._check(self.lib.ss_set_option(self._h, name.encode(), int(value)))
 
-    def op_layer_norm(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-        out = torch.empty_like(x)
-        self._check(self.lib.ss_op_layer_norm(self._h, self._stream(), x.data_ptr(), x.shape[0], x.shape[1], g.data_ptr(), b.data_ptr(), out.data_ptr()))
+    def op_layer_norm(self, x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """LayerNorm over the C = g.numel() columns of the rows of x [rows, >= C] (row stride x.stride(0)) into out [rows, >= C] (default: a
+        new [rows, C] tensor)"""
+        C = g.numel()
+        if out is None:
+            out = self._f32(x.shape[0], C)
+        self._check(self.lib.ss_op_layer_norm(self._h, self._stream(), x.data_ptr(), self._ld(x), x.shape[0], C, g.data_ptr(), b.data_ptr(),
+                                              out.data_ptr(), self._ld(out)))
         return out
+
+    def op_gemm(self, args: GemmArgs) -> GemmArgs:
+        """ss_op_gemm: one GEMM with every field of the kernel layer's contract (pointers are device addresses); the route_* fields of
+        `args` are filled in"""
+        self._check(self.lib.ss_op_gemm(self._h, self._stream(), ctypes.byref(args)))
+        return args
 
     def op_argmax_rows(self, logits: torch.Tensor, n_masked: int, scored: bool):
         """ss_op_argmax_rows on a 2-D fp32 device tensor: (indices, log-probabilities or None)"""

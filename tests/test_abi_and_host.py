@@ -49,6 +49,29 @@ def test_ss_config_struct_layout_matches_header():
     assert names == [n for n, _ in SSConfig._fields_], (names, [n for n, _ in SSConfig._fields_])
 
 
+def test_ss_op_gemm_args_struct_layout_matches_header():
+    """ctypes mirror of `struct ss_op_gemm_args`: same field order, names and C types as the header, so every offset agrees."""
+    import ctypes
+
+    from streamspeech_b200.engine import GemmArgs
+
+    header = open(os.path.join(ROOT, "include", "streamspeech_b200.h")).read()
+    body = header[header.index("typedef struct ss_op_gemm_args {") + len("typedef struct ss_op_gemm_args {"):header.index("} ss_op_gemm_args;")]
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    ctype = {"float*": ctypes.c_void_p, "int32_t*": ctypes.c_void_p, "int32_t": ctypes.c_int32, "float": ctypes.c_float}
+    fields = []
+    for decl in body.split(";"):
+        decl = " ".join(decl.split())
+        if not decl:
+            continue
+        m = re.fullmatch(r"(?:const )?(float|int32_t)(\*?) ?(.*)", decl)
+        assert m, decl
+        for name in m.group(3).split(","):
+            fields.append((name.strip(), ctype[m.group(1) + m.group(2)]))
+    assert [(n, t) for n, t in GemmArgs._fields_] == fields, ([n for n, _ in GemmArgs._fields_], [n for n, _ in fields])
+    assert "ss_op_gemm" in re.findall(r"\b(ss_[a-z0-9_]+)\s*\(", header)
+
+
 def test_constants_match_oracle_tables():
     from oracle import streamspeech_oracle as so
     from streamspeech_b200 import constants

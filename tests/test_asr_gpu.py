@@ -1,6 +1,9 @@
 """GPU: the ASR-BLEU transcriber (ss_asr_*) on the seeded Large-shape wav2vec 2.0 CTC checkpoint against the float64 oracle
 (oracle/asr_oracle.py, run on the same device): every stage, conv-stride edges, a long input, ragged batches over several launch groups,
-batch-of-one identity, letters against the fp64 arg-max, and refusals."""
+batch-of-one identity, letters against the fp64 arg-max, and refusals; the fixture's two small configurations (extractor width 64) against
+fairseq's modules and the oracle, and wav2vec 2.0 Base's width (D = 768)."""
+import os
+
 import pytest
 import torch
 
@@ -164,3 +167,71 @@ def test_refusals_return_errors():
     del missing["w2v_encoder.proj.bias"]
     with pytest.raises(EngineError, match="w2v_encoder.proj.bias"):
         ASREngine(missing, STRIDES, 0)
+
+
+def small_stage_index(name: str, layers: int) -> int:
+    if name.startswith("layer"):
+        return 3 + int(name[5:])
+    return {"extractor": 0, "proj": 1, "pos": 2, "final_ln": 3 + layers, "emissions": 4 + layers}[name]
+
+
+def small_bar(name: str) -> float:
+    return BARS[name] if name in BARS else BARS["layer11"]  # layers past the first take the deep-layer bar
+
+
+@pytest.mark.parametrize("name", ["a", "b"])
+def test_fixture_configurations(name):
+    """Both configurations of tests/golden/asr_w2v.npz (extractor width 64, D = 128, conv_bias on / off, even / odd positional kernel):
+    every stage against fairseq's own modules (the fixture) and against the float64 oracle.  Width 64 is outside the LayerNorm widths
+    the encoder uses, so this also pins the feature LayerNorm at that width."""
+    import numpy as np
+
+    from oracle.gen_golden_asr import CONV, LAYERS, LENGTHS, config_state_dict
+    from streamspeech_b200.engine import ASREngine
+
+    golden = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "asr_w2v.npz"))
+    sd = config_state_dict(name)
+    strides = [s for (_, _, s) in CONV]
+    layers = LAYERS
+    eng = ASREngine(sd, strides, 0)
+    sd64 = {k: v.to("cuda", torch.float64) for k, v in sd.items()}
+    worst = {}
+    try:
+        for j, n in enumerate(LENGTHS):
+            wav = torch.from_numpy(golden[f"{name}_{j}_wav"])
+            r = ao.forward(sd64, wav, strides, normalize=True, dtype=torch.float64, device="cuda")
+            for st in ["extractor", "proj", "pos"] + [f"layer{i}" for i in range(layers)] + ["final_ln", "emissions"]:
+                fx = torch.from_numpy(golden[f"{name}_{j}_{st}"]).to("cuda", torch.float64)
+                got = eng.stage([wav], small_stage_index(st, layers), fx.shape[1]).double()
+                assert got.shape == fx.shape == r[st].shape, st
+                for against, ref_ in (("fairseq", fx), ("fp64", r[st])):
+                    rel = float((got - ref_).abs().max() / ref_.abs().max())
+                    worst[(st, against)] = max(worst.get((st, against), 0.0), rel)
+                    assert rel < small_bar(st), (name, j, st, against, rel)
+    finally:
+        eng.close()
+    print(f"ASR fixture config {name} max rel err:", {f"{k[0]}/{k[1]}": f"{v:.1e}" for k, v in worst.items()})
+
+
+def test_base_width_against_fp64():
+    """wav2vec 2.0 Base's model width (D = 768, 12 heads; 3 layers, extractor width 512) against the float64 oracle at every stage"""
+    from streamspeech_b200.engine import ASREngine
+
+    layers = 3
+    sd = synth.make_w2v_ctc_state_dict(seed=21, dim=768, ffn=3072, layers=layers, pos_k=128, pos_groups=16)
+    eng = ASREngine(sd, STRIDES, 0)
+    sd64 = {k: v.to("cuda", torch.float64) for k, v in sd.items()}
+    worst = {}
+    try:
+        for seconds, seed in ((1.0, 31), (2.3, 32)):
+            wav = synth.make_audio(seconds, seed=seed)
+            r = ref(sd64, wav)
+            for st in ["extractor", "proj", "pos"] + [f"layer{i}" for i in range(layers)] + ["final_ln", "emissions"]:
+                got = eng.stage([wav], small_stage_index(st, layers), r[st].shape[1]).double()
+                assert got.shape == r[st].shape, st
+                rel = float((got - r[st]).abs().max() / r[st].abs().max())
+                worst[st] = max(worst.get(st, 0.0), rel)
+                assert rel < small_bar(st), (st, rel)
+    finally:
+        eng.close()
+    print("ASR D = 768 max rel err:", {k: f"{v:.1e}" for k, v in worst.items()})

@@ -55,3 +55,22 @@ def test_get_tokens_equals_torchaudio(golden):
     for i in range(len(golden["gt_in_off"]) - 1):
         path = golden["gt_in"][golden["gt_in_off"][i]:golden["gt_in_off"][i + 1]].tolist()
         assert ao.get_tokens(path) == golden["gt_out"][golden["gt_out_off"][i]:golden["gt_out_off"][i + 1]].tolist(), i
+
+
+def test_fixture_configurations_need_no_reference_tree():
+    """oracle/gen_golden_asr.config_state_dict, which the GPU tests import, opens nothing under the reference tree"""
+    import subprocess
+    import sys
+
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    code = ("import sys, os\n"
+            "ref = os.environ['STREAMSPEECH_REFERENCE']\n"
+            "opened = []\n"
+            "sys.addaudithook(lambda ev, a: opened.append(str(a[0])) if ev == 'open' and str(a[0]).startswith(ref) else None)\n"
+            "from oracle.gen_golden_asr import config_state_dict\n"
+            "sds = [config_state_dict(n) for n in ('a', 'b')]\n"
+            "assert all(len(sd) > 10 for sd in sds)\n"
+            "assert not opened, opened\n")
+    env = dict(os.environ, STREAMSPEECH_REFERENCE=os.path.join(root, "no-such-reference-tree"), PYTHONPATH=root)
+    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-2000:]
