@@ -9,7 +9,8 @@ through one agent.  Here every stream of a `StreamPool` plays its own instance: 
 segment and pops every agent (one batched flush), and an instance that has read its whole source frees its stream for the next
 index of the list.  Each stream follows SimulEval's reset rule on its own: its agent is reset once before the first instance and
 whenever an instance's prediction finishes, and never between instances otherwise.  With `--streams 1` (the default) the single
-agent runs the list in order, without the pool.
+agent runs the list in order, without the pool.  The wait-k agents (UnitY checkpoints) have no pooled form and run `--streams 1`
+only.
 
 What SimulEval writes is written the same way, so `simuleval --score-only --output DIR` scores the run: `instances.log` (one
 `summarize()` dict per line, in index order), `config.yaml`, and for speech output `wavs/{index}_pred.wav`.  The instance classes
@@ -41,6 +42,9 @@ AGENTS = {
     "speech_to_speech.streamspeech.agent.py": ("speech", "StreamSpeechS2STAgent", "PooledS2STAgent"),
     "speech_to_text.s2tt.streamspeech.agent.py": ("text", "StreamSpeechS2TTAgent", "PooledS2TTAgent"),
     "speech_to_text.asr.streamspeech.agent.py": ("text", "StreamSpeechASRAgent", "PooledASRAgent"),
+    # the wait-k-stride-n baselines on UnitY checkpoints (streamspeech_b200/waitk.py): one stream, no pooled class
+    "speech_to_speech.wait-k-stride-n.agent.py": ("speech", "WaitkS2STAgent", None),
+    "speech_to_text.wait-k-stride-n.agent.py": ("text", "WaitkS2TTAgent", None),
 }
 
 
@@ -304,6 +308,14 @@ def agent_kind(agent_path: str):
     return AGENTS[name]
 
 
+def single_agent_class(name: str):
+    """the single-stream agent class of that name: streamspeech_b200.agent's, or the wait-k agents of streamspeech_b200.waitk"""
+    from streamspeech_b200 import agent as _agents
+    from streamspeech_b200 import waitk as _waitk
+
+    return getattr(_agents, name) if hasattr(_agents, name) else getattr(_waitk, name)
+
+
 def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     pre = argparse.ArgumentParser(add_help=False)
     pre.add_argument("--agent")
@@ -313,9 +325,7 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     _add_evaluator_args(parser)
     if known.agent is not None:
         target_type, single_name, _ = agent_kind(known.agent)
-        from streamspeech_b200 import agent as _agents
-
-        getattr(_agents, single_name).add_args(parser)
+        single_agent_class(single_name).add_args(parser)
         if target_type == "text":  # the text agents share the S2ST agent's flags; the reference's text agents take no vocoder
             for action in parser._actions:
                 if action.dest in ("vocoder", "vocoder_cfg"):
@@ -326,6 +336,8 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
                      "is undefined; the non-computation-aware latency metrics are scored from instances.log")
     if args.streams < 1:
         parser.error("--streams must be at least 1")
+    if args.streams > 1 and agent_kind(args.agent)[2] is None:
+        parser.error(f"--streams {args.streams}: the wait-k agent {os.path.basename(args.agent)} runs one stream (pass --streams 1)")
     return args
 
 
@@ -420,11 +432,10 @@ def check_source(path: str, sample_rate: int) -> AudioInfo:
 def build_agents(args: argparse.Namespace, max_seconds: int = 60):
     """(agents, pool, target type): `args.streams` pooled agents on one StreamPool of the engine the single agent loads, or the
     single agent alone for one stream (the pool step is slower for one stream: it does not use the single-stream encoder kernels)"""
-    from streamspeech_b200 import agent as _agents
     from streamspeech_b200 import scheduler
 
     target_type, single_name, pooled_name = agent_kind(args.agent)
-    single = getattr(_agents, single_name)(args)
+    single = single_agent_class(single_name)(args)
     if args.streams == 1:
         return [single], None, target_type
     ctc_heads = 1 if pooled_name == "PooledASRAgent" else 2
