@@ -73,8 +73,9 @@ class UnitYOracle:
     def unit_search(self, t2u: torch.Tensor, lengths: Sequence[int], max_len: int, len_penalty: float = 1.0,
                     min_len: int = 1) -> List[Dict[str, object]]:
         """t2u [B, S, D] (t2u_encode's output), lengths[b] = the sample's keys.  One dict per sample: tokens (eos last),
-        positional_scores, score, margins = the gap between the best and the second-best finite candidate at each step (how far
-        the search is from changing that decision) and margin = their minimum."""
+        positional_scores, score, margins = the gap between the best candidate and the best finite one of a lower score at each step
+        (how far the search is from changing that decision; exactly equal scores go to the lower index), margin = their minimum and
+        ties = the steps whose best score was held by more than one token."""
         c, dt = self.cfg, self.dtype
         assert min_len <= max_len
         B, S, D = t2u.shape
@@ -89,7 +90,7 @@ class UnitYOracle:
         selfk = [torch.zeros(B, 0, D, dtype=dt) for _ in range(c.unit_layers)]
         selfv = [torch.zeros(B, 0, D, dtype=dt) for _ in range(c.unit_layers)]
         tok = torch.full((B,), c.eos, dtype=torch.long)
-        out = [{"tokens": [], "cum": [], "score": None, "margin": math.inf, "margins": []} for _ in range(B)]
+        out = [{"tokens": [], "cum": [], "score": None, "margin": math.inf, "margins": [], "ties": 0} for _ in range(B)]
         live = list(range(B))
         cum = torch.zeros(B, dtype=dt)
         for step in range(max_len + 1):
@@ -120,9 +121,13 @@ class UnitYOracle:
             keep = []
             for i, b in enumerate(live):
                 row = sc[i].to(torch.float64)
-                top = torch.topk(row, 2)
-                best = int(torch.nonzero(sc[i] == sc[i].max())[0])  # lowest index among exact ties
-                gap = float(top.values[0] - top.values[1]) if math.isfinite(float(top.values[1])) else math.inf
+                mx = row.max()
+                tied = torch.nonzero(sc[i] == sc[i].max()).view(-1)
+                best = int(tied[0])  # lowest index among exact ties
+                out[b]["ties"] += len(tied) > 1
+                below = row[row < mx]  # the gap to the best distinct score (exact ties are decided by the index, not arithmetic)
+                second = float(below.max()) if below.numel() else -math.inf
+                gap = float(mx) - second if math.isfinite(second) else math.inf
                 out[b]["margins"].append(gap)
                 out[b]["margin"] = min(out[b]["margin"], gap)
                 out[b]["tokens"].append(best)

@@ -66,6 +66,25 @@ def test_oracle_reproduces_reference_nbest(gold, early):
         assert any(min(n) < max(n) < int(g["early_max_len_b_mt"]) + 1 for n in lengths), lengths
 
 
+def test_oracle_trace_of_finalization_events():
+    """mt_beam's trace on the early-eos checkpoint (float64): three hypotheses at step 1, the fourth slot filled at step 8 with
+    more eos in the first K than slots left, eos at ranks K .. 2K - 1; tracing leaves the result unchanged"""
+    from oracle.mt_beam_oracle import early_eos_state_dict, mt_beam
+
+    cfg = offline_cfg()
+    sd = early_eos_state_dict(synth.make_model_state_dict(cfg, 0), cfg.eos, -0.2)
+    o = oracle64(sd)
+    enc = torch.randn(19, 1, cfg.enc_dim, generator=torch.Generator().manual_seed(2))
+    r = mt_beam(o, enc, 4, 40, trace=True)
+    tr = r["trace"]
+    assert [s["n_fin"] for s in tr] == [0, 3, 3, 3, 3, 3, 3, 3, 4]
+    assert tr[1]["new_fin"] == 3 and tr[8]["new_fin"] == 1 and tr[8]["capped"] > 0
+    assert sum(s["eos_out"] for s in tr) > 0 and sum(s["ties"] for s in tr) == 0 and r["fin_ties"] == 0
+    assert len(r["margins"]) == len(r["tops"]) == len(tr) and r["margin"] == min(r["margins"]) > 0
+    plain = mt_beam(o, enc, 4, 40)
+    assert plain["hyps"] == r["hyps"] and "trace" not in plain
+
+
 def test_generator_argument_checks():
     from streamspeech_b200.offline import OfflineS2STGenerator
 
