@@ -82,6 +82,44 @@ class VocoderConfig:
             return VocoderConfig.from_json_dict(json.load(f))
 
 
+UNITY_VARIANTS = ("unity", "uni_unity", "chunk_unity")
+# the registered arch names of the UnitY family (researches/translatotron, researches/uni_unity, researches/chunk_unity and fairseq's own)
+UNITY_ARCHS = {
+    "unity_conformer_modified": "unity",
+    "unity_conformer": "unity",
+    "uni_unity_conformer": "uni_unity",
+    "uni_unity_conformer_waitk": "uni_unity",
+    "chunk_unity_conformer": "chunk_unity",
+}
+# stored settings the engine's Conformer encoder assumes (every recipe of the family trains with them), and their values
+UNITY_FIXED_SETTINGS = (("pos_enc_type", "rel_pos"), ("attn_type", "espnet"), ("conv_version", "s2t_transformer"))
+
+
+def unity_variant_of(get):
+    """(unity_variant, uni_encoder, chunk_size) of a UnitY-family checkpoint from its stored model cfg (`get(key)`, None when
+    absent).  A checkpoint without an arch is UnitY, as are unity_conformer_modified ones: both take the bidirectional encoder and T2U
+    encoder whatever else is stored (their models read neither --uni-encoder nor --chunk-size).  Raises ValueError, naming the
+    setting, for any arch or stored setting the engine does not reproduce."""
+    arch = get("arch")
+    if arch is not None and arch not in UNITY_ARCHS:
+        raise ValueError(f"arch {arch!r}: not a UnitY-family model the engine runs (one of {', '.join(sorted(UNITY_ARCHS))})")
+    for key, want in UNITY_FIXED_SETTINGS:
+        have = get(key)
+        if have is not None and have != want:
+            raise ValueError(f"{key} {have!r}: the engine's encoder implements {key} {want!r} only")
+    variant = UNITY_ARCHS.get(arch, "unity")
+    if variant == "unity":
+        return variant, False, 0
+    uni = bool(get("uni_encoder") or False)
+    if variant == "uni_unity":
+        return variant, uni, 0
+    chunk = get("chunk_size")
+    if chunk is None or not 0 < int(chunk) < 999 or int(chunk) % 2:
+        raise ValueError(f"chunk_size {chunk!r}: a chunk_unity_conformer checkpoint runs on the engine with an even --chunk-size "
+                         "between 2 and 998 (its attention and convolution chunk)")
+    return variant, uni, int(chunk)
+
+
 @dataclass
 class ModelConfig:
     # front-end
@@ -122,11 +160,26 @@ class ModelConfig:
     # 1000 units (no blank) searched token by token, whose sinusoidal positions cover max_target_positions
     unity: bool = False
     max_target_positions: int = 1024
+    # which UnitY-family model (unity only; see UNITY_ARCHS): "unity" (bidirectional encoder), "uni_unity" (the Conformer with a
+    # future mask on self-attention when uni_encoder is set, symmetric convolutions) or "chunk_unity" (StreamSpeech's chunk encoder at
+    # the training --chunk-size, attention mask and convolutions alike).  uni_encoder makes the T2U encoder causal in both variants.
+    unity_variant: str = "unity"
+    chunk_size: int = 0  # chunk_unity: the training --chunk-size (encoder frames)
     vocoder: VocoderConfig = field(default_factory=VocoderConfig)
 
     @property
     def unit_blank(self) -> int:
         return self.unit_vocab - 1
+
+    def encoder_chunk(self):
+        """(attention chunk, conv chunk) of Engine.set_chunk for a UnitY-family model's whole-prefix encoder: (None, None) is the
+        bidirectional encoder, (1, 0) a future mask with symmetric convolutions, (c, c) the chunk encoder of chunk size c"""
+        assert self.unity
+        if self.unity_variant == "uni_unity" and self.uni_encoder:
+            return 1, 0
+        if self.unity_variant == "chunk_unity":
+            return self.chunk_size, self.chunk_size
+        return None, None
 
     @staticmethod
     def from_state_dict(sd) -> "ModelConfig":
@@ -172,14 +225,23 @@ class ModelConfig:
 
             model_cfg = get(get(state, "cfg"), "model") or get(state, "args")
             c.max_target_positions = int(get(model_cfg, "max_target_positions") or 1024)
+            c.unity_variant, c.uni_encoder, c.chunk_size = unity_variant_of(lambda k: get(model_cfg, k))
         return c
 
     @staticmethod
-    def unity_default() -> "ModelConfig":
+    def unity_default(variant: str = "unity") -> "ModelConfig":
         """The released UnitY checkpoints' dimensions (unity.{fr,es,de}-en.pt): StreamSpeech's encoder, MT decoder and T2U encoder,
-        and a 2-layer autoregressive unit decoder over 1004 symbols with 1200 positions"""
+        and a 2-layer autoregressive unit decoder over 1004 symbols with 1200 positions.  `variant` "uni_unity" / "chunk_unity" is the
+        same model with the training recipes' --uni-encoder (and --chunk-size 8) of researches/{uni,chunk}_unity/train_scripts."""
+        if variant not in UNITY_VARIANTS:
+            raise ValueError(f"unknown UnitY variant {variant!r}; one of {', '.join(UNITY_VARIANTS)}")
         c = ModelConfig()
         c.unity, c.uni_encoder, c.unit_vocab, c.max_target_positions = True, False, 1004, 1200
+        c.unity_variant = variant
+        if variant != "unity":
+            c.uni_encoder = True
+        if variant == "chunk_unity":
+            c.chunk_size = 8
         return c
 
     def tiny(self) -> "ModelConfig":

@@ -26,7 +26,10 @@ The vocoder is not loaded (fairseq-generate does not load it either); run stream
 `fairseq-generate --user-dir researches/translatotron ... --beam-mt 10 --beam 1 --max-len-a 1`: each batch is one
 UnitYGenerator.generate call (MT search, T2U encoder, autoregressive unit search with max_len = min(int(max_len_a * F + max_len_b),
 max_target_positions - 1), F the batch's padded fbank length).  stdout then carries only the `D-{id}\t{MT text}` prints
-(sequence_generator_multi_decoder.py:217); the results file is written as above.
+(sequence_generator_multi_decoder.py:217); the results file is written as above.  A Uni-UnitY checkpoint (arch uni_unity_conformer
+or uni_unity_conformer_waitk) is researches/uni_unity/test_scripts/pred.sh (`--user-dir researches/uni_unity`): the same batching
+and files, its encoder with a future mask and its T2U encoder causal, and the MT prints of fairseq's own generator, which that task
+builds: `{MT text} (None-{id})`.  Chunk-UnitY is a simultaneous model and is refused here (offline_settings).
 """
 from __future__ import annotations
 
@@ -57,7 +60,7 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     p = argparse.ArgumentParser(prog="python -m streamspeech_b200.generate", description=__doc__,
                                 formatter_class=argparse.RawDescriptionHelpFormatter)
     p.add_argument("data", help="directory of the split manifests ({gen_subset}.tsv) and the configs")
-    p.add_argument("--user-dir", default=None, help="accepted and ignored: the task is built in")
+    p.add_argument("--user-dir", default=None, help="the task is built in; with --path synthetic it names the UnitY-family model")
     p.add_argument("--config-yaml", default="config.yaml")
     p.add_argument("--multitask-config-yaml", default=None)
     p.add_argument("--task", default="speech_to_speech_ctc")
@@ -361,6 +364,15 @@ def offline_settings(state: dict, capacity: int) -> Tuple[bool, Optional[int]]:
     return uni, None
 
 
+def mt_print_line(cfg, sample_id: int, text: str) -> str:
+    """the MT hypothesis line the UnitY generators print to stdout: researches/translatotron's MultiDecoderSequenceGenerator (UnitY)
+    prints "D-{id}\\t{text}"; fairseq's own (examples/speech_to_speech/unity), which researches/uni_unity's task builds, prints
+    "{text} (None-{id})"."""
+    if cfg.unity_variant == "uni_unity":
+        return "{} (None-{})".format(text, sample_id)
+    return "D-{}\t{}".format(sample_id, text)
+
+
 def load_offline_checkpoint(args: argparse.Namespace, capacity: int):
     """(cfg, model state dict, dictionaries) of --path; `synthetic[:seed]` is the seeded synthetic offline checkpoint"""
     import torch
@@ -372,10 +384,12 @@ def load_offline_checkpoint(args: argparse.Namespace, capacity: int):
     unity = args.task == "speech_to_speech_modified"
     if str(args.path).startswith("synthetic"):
         seed = int(args.path.split(":")[1]) if ":" in args.path else 0
-        if unity:  # the seeded synthetic UnitY checkpoint at the released dimensions
-            cfg = ModelConfig.unity_default()
-            return cfg, synth.make_unity_state_dict(cfg, seed=seed), {"target_unigram": Dictionary.synthetic(cfg.tgt_vocab),
-                                                                      "tgt": Dictionary.units(cfg.unit_vocab - 4, blank=False)}
+        if unity:  # the seeded synthetic UnitY checkpoint at the released dimensions; --user-dir researches/uni_unity: Uni-UnitY's
+            state = synth.make_unity_checkpoint(synth.synthetic_unity_variant(args.user_dir), seed=seed)
+            offline_settings(state, capacity)
+            cfg = ModelConfig.from_checkpoint(state)
+            return cfg, state["model"], {"target_unigram": Dictionary.synthetic(cfg.tgt_vocab),
+                                         "tgt": Dictionary.units(cfg.unit_vocab - 4, blank=False)}
         cfg = ModelConfig()
         cfg.uni_encoder = False
         dicts = {k: Dictionary.synthetic(n) for k, n in (("source_unigram", cfg.src_vocab), ("ctc_target_unigram", cfg.tgt_vocab),
@@ -488,7 +502,8 @@ def main(argv: Optional[Sequence[str]] = None, stdout=None):
             ids = list(batch)  # fairseq's sample["id"]: the dataset index
             for key, d, tok in prints:
                 for sid, r in zip(ids, res):
-                    print(f"{key}-{sid}\t{ctc_text(d, r[tok])}", file=stdout)
+                    text = ctc_text(d, r[tok])
+                    print(mt_print_line(cfg, sid, text) if cfg.unity else f"{key}-{sid}\t{text}", file=stdout)
             for i, sid, r in zip(batch, ids, res):
                 target_tokens = encode_line(tgt, split.target(i))
                 target_str = unit_string(tgt, target_tokens, escape_unk=True)

@@ -111,7 +111,7 @@ class UnitYGenerator:
     """UnitY's `MultiDecoderSequenceGenerator` as `fairseq-generate --task speech_to_speech_modified --beam-mt K --beam 1` runs it
     (researches/translatotron/sequence_generator_multi_decoder.py:134-268) on the engine, one call per stage for the whole batch:
 
-        batched padded encoder (offline model)                                       ss_encoder_forward(B, lengths)
+        batched padded encoder (UnitY: offline model; Uni-UnitY: future mask)         ss_encoder_forward(B, lengths)
         MT search, max_len = max_len_b_mt: K = 1 greedy, K >= 2 beam (finalized[b][0])  ss_mt_greedy_batch / ss_mt_beam_batch
         prev_output_tokens_mt = [eos, hyp..., pad...] to the batch maximum             host
         mt_decoder(features_only) on the padded batch                                 ss_mt_features_batch
@@ -119,7 +119,9 @@ class UnitYGenerator:
         unit search at beam 1, max_len = min(int(max_len_a * F + max_len_b),          ss_unit_search_batch
           max_target_positions - 1) with F the batch's PADDED fbank length
 
-    There are no CTC prints (UnitY has no CTC heads); the D- text is the MT hypothesis."""
+    There are no CTC prints (UnitY has no CTC heads); the D- text is the MT hypothesis.  A Uni-UnitY checkpoint
+    (researches/uni_unity) runs the same stages with its encoder's future mask and a causal T2U encoder (cfg.uni_encoder), under
+    fairseq's own MultiDecoderSequenceGenerator, which prints the MT text as "{text} (None-{id})" (generate.mt_print_line)."""
 
     def __init__(self, engine: Engine, beam_size_mt: int = 1, beam_size: int = 1, max_len_a_mt: float = 0.0, max_len_b_mt: int = 200,
                  max_len_a: float = 0.0, max_len_b: int = 200, len_penalty: float = 1.0):
@@ -139,7 +141,9 @@ class UnitYGenerator:
         self.len_penalty = float(len_penalty)
         self.max_len_b_mt = int(max_len_b_mt)
         self.max_len_a, self.max_len_b = float(max_len_a), int(max_len_b)
-        engine.set_chunk(None, None)
+        if self.cfg.unity_variant == "chunk_unity":
+            raise NotImplementedError("Chunk-UnitY is a simultaneous model: it runs in the wait-k agents, not the offline generator")
+        engine.set_chunk(*self.cfg.encoder_chunk())  # UnitY: the offline model; Uni-UnitY: a future mask, symmetric convolutions
 
     def unit_max_len(self, padded_frames: int) -> int:
         """generate_decoder's max_len (unity/sequence_generator.py:182-194) for a batch of `padded_frames` fbank frames"""

@@ -233,6 +233,31 @@ def make_unity_state_dict(cfg: ModelConfig, seed: int = 0, eos_gain: float = UNI
     return sd
 
 
+# the stored model cfg of each UnitY-family recipe (researches/unitY, uni_unity and chunk_unity train_scripts): what
+# ModelConfig.from_checkpoint reads back
+UNITY_RECIPES = {
+    "unity": {"arch": "unity_conformer_modified"},
+    "uni_unity": {"arch": "uni_unity_conformer", "uni_encoder": True},
+    "chunk_unity": {"arch": "chunk_unity_conformer", "uni_encoder": True, "chunk_size": 8},
+}
+
+
+def synthetic_unity_variant(user_dir: Optional[str]) -> str:
+    """the UnitY-family model a `synthetic[:seed]` model path stands for: the one the --user-dir's research directory registers
+    (researches/uni_unity, researches/chunk_unity), else UnitY"""
+    name = os.path.basename(os.path.normpath(user_dir)) if user_dir else ""
+    return name if name in ("uni_unity", "chunk_unity") else "unity"
+
+
+def make_unity_checkpoint(variant: str = "unity", seed: int = 0) -> Dict[str, object]:
+    """A seeded `torch.load(ckpt)` of a UnitY-family checkpoint: {"model": make_unity_state_dict (the same keys for every variant),
+    "cfg": {"model": the recipe's stored settings}} at ModelConfig.unity_default(variant)'s dimensions"""
+    cfg = ModelConfig.unity_default(variant)
+    model_cfg = dict(UNITY_RECIPES[variant], max_target_positions=cfg.max_target_positions, pos_enc_type="rel_pos", attn_type="espnet",
+                     conv_version="s2t_transformer")
+    return {"model": make_unity_state_dict(cfg, seed=seed), "cfg": {"model": model_cfg}}
+
+
 def make_vocoder_state_dict(vc: VocoderConfig, seed: int = 1, cal: Calibration = Calibration(), weight_norm: bool = False) -> Dict[str, torch.Tensor]:
     """`torch.load(ckpt)["generator"]` of the CodeHiFiGAN vocoder (agent/tts/vocoder.py:37-45).
 

@@ -1,4 +1,4 @@
-"""The reference's wait-k-stride-n baselines on UnitY checkpoints, backed by the H100 engine: same classes, flags and policy() behaviour as
+"""The reference's wait-k-stride-n baselines on UnitY, Uni-UnitY and Chunk-UnitY checkpoints, backed by the H100 engine: same classes, flags and policy() behaviour as
 
   agent/speech_to_speech.wait-k-stride-n.agent.py   (WaitkS2STAgent, :101-581)
   agent/speech_to_text.wait-k-stride-n.agent.py     (EnglishSpeechCounter, :100-477; WaitkS2TTAgent here)
@@ -8,10 +8,15 @@ search emit one subword per `stride_n` segments, and the unit search `unit_per_s
 `lagging_k2`.  Every policy() call that passes the gate runs, like the reference (whose generators keep no incremental state):
 
   fbank + gcmvn of the whole source                       ss_fbank (frames cached: each depends only on its own samples)
-  forward_encoder on the whole prefix (bidirectional)     ss_encoder_forward, B = 1, every row recomputed
-  MT search with the previous hypothesis as prefix        ss_mt_greedy (cross K / V of every encoder row re-projected)
+  forward_encoder on the whole prefix                     UnitY (bidirectional) and Uni-UnitY (future mask, symmetric convs):
+                                                            ss_encoder_forward, B = 1, every row recomputed;
+                                                          Chunk-UnitY (chunk mask and chunk-causal convs at the training
+                                                            --chunk-size): ss_encoder_stream_step, the rows of the open chunk
+                                                            group only (earlier rows are final)
+  MT search with the previous hypothesis as prefix        ss_mt_greedy (cross K / V of every encoder row re-projected; Chunk-UnitY:
+                                                            of the rows that are not final, ss_mt_stable_rows)
   S2ST: MT decoder features of [eos, tokens...]           the rows of the same ss_mt_greedy pass (causal decoder)
-  S2ST: synthesizer_encoder                               ss_t2u_encode_batch, B = 1
+  S2ST: synthesizer_encoder                               ss_t2u_encode_batch, B = 1 (causal with --uni-encoder: Uni-UnitY, Chunk-UnitY)
   S2ST: unit search from BOS (tgt_units_indices is        ss_unit_search_batch, B = 1, max_len = the absolute unit count
         never assigned in the reference)                    or min(F + 200, max_decoder_positions - 1) once the source ended
   S2ST: vocoder on all units, the new units' samples      the S2ST agent's receptive-field tail window (_vocode)
@@ -41,13 +46,15 @@ DEFAULT_EOS = 2
 
 
 def load_unity_checkpoint(args):
-    """(cfg, model state dict, gcmvn, dictionaries) of --model-path: `synthetic[:seed]` is the seeded synthetic UnitY checkpoint
-    (synth.make_unity_state_dict at ModelConfig.unity_default()); anything else is a fairseq `.pt`, which must hold a UnitY model."""
+    """(cfg, model state dict, gcmvn, dictionaries) of --model-path: `synthetic[:seed]` is the seeded synthetic checkpoint of the
+    UnitY-family model --user-dir names (synth.make_unity_checkpoint: researches/uni_unity, researches/chunk_unity, else UnitY);
+    anything else is a fairseq `.pt`, which must hold a UnitY, Uni-UnitY or Chunk-UnitY model (ModelConfig.from_checkpoint)."""
     if str(args.model_path).startswith("synthetic"):
         seed = int(args.model_path.split(":")[1]) if ":" in args.model_path else 0
-        cfg = ModelConfig.unity_default()
+        state = synth.make_unity_checkpoint(synth.synthetic_unity_variant(getattr(args, "user_dir", None)), seed=seed)
+        cfg = ModelConfig.from_checkpoint(state)
         dicts = {"target_unigram": Dictionary.synthetic(cfg.tgt_vocab), "tgt": Dictionary.units(cfg.unit_vocab - 4, blank=False)}
-        return cfg, synth.make_unity_state_dict(cfg, seed=seed), synth.make_gcmvn(cfg), dicts
+        return cfg, state["model"], synth.make_gcmvn(cfg), dicts
     if not os.path.exists(args.model_path):
         raise IOError("Model file not found: {}".format(args.model_path))
     state = torch.load(args.model_path, map_location="cpu", weights_only=False)
@@ -92,8 +99,14 @@ class _WaitkMixin(_EngineAgentMixin):
         # the MT search of an ended source runs to at most max_decoder_positions - 1 tokens and needs two more positions
         self.engine = Engine(cfg, sd, vsd, gcmvn, device=getattr(args, "device_index", 0), max_enc_frames=getattr(args, "max_enc_frames", 1024),
                              max_mt_positions=max(getattr(args, "max_mt_positions", 1024), cfg.max_target_positions + 1))
-        self.engine.set_chunk(None, None)  # UnitY's encoder is the offline (bidirectional) one
+        # UnitY: the offline (bidirectional) encoder; Uni-UnitY: a future mask with symmetric convolutions, whose rows still change as
+        # the source grows (re-encoded whole on every call, as the reference does); Chunk-UnitY: the chunk encoder, whose rows of
+        # complete chunk groups are final (encoded incrementally, their MT cross K / V projected once)
+        self.engine.set_chunk(*cfg.encoder_chunk())
+        self.incremental = cfg.unity_variant == "chunk_unity"
         self.torch_device = self.engine.device
+        if self.incremental:
+            self.enc_buf = torch.zeros(getattr(args, "max_enc_frames", 1024), cfg.enc_dim, dtype=torch.float32, device=self.torch_device)
         self.sample_rate = args.sample_rate
         self.audio = _DeviceAudio(self.torch_device, engine=self.engine, sample_rate=args.sample_rate)
         self.feat_cache = torch.zeros(6000, cfg.feat_dim, dtype=torch.float32, device=self.torch_device)
@@ -139,8 +152,14 @@ class _WaitkMixin(_EngineAgentMixin):
         F = int(feature.size(0))
         if F == 0 and not self.states.source_finished:
             return None
-        enc = self.engine.encoder(feature.unsqueeze(0))[0]  # the whole prefix; no stable-rows hint: every row changes
-        tokens, feats = self.engine.mt_greedy(enc, self.tgt_subwords_indices, new_subword_tokens, max_len_b=self._full_max_len(F))
+        if self.incremental:  # only the rows of the open chunk group are computed; rows below t_final are final
+            T, t_final = self.engine.encoder_stream_step(feature, self.enc_buf)
+            enc, stable = self.enc_buf[:T], t_final
+        else:
+            enc, stable = self.engine.encoder(feature.unsqueeze(0))[0], 0  # the whole prefix; no stable-rows hint: every row changes
+        self._enc_final = stable
+        tokens, feats = self.engine.mt_greedy(enc, self.tgt_subwords_indices, new_subword_tokens, max_len_b=self._full_max_len(F),
+                                              stable_rows=stable)
         self.trace["mt_tokens"] = list(tokens)
         self.tgt_subwords_indices = list(tokens)
         return tokens, feats, F

@@ -39,6 +39,8 @@ def main():
     ap.add_argument("--seconds", type=float, default=6.0)
     ap.add_argument("--beam-mt", type=int, default=10)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--variant", choices=("unity", "uni_unity"), default="unity",
+                    help="the synthetic checkpoint: UnitY, or Uni-UnitY (future-masked encoder, causal T2U encoder)")
     a = ap.parse_args()
     from streamspeech_b200 import generate as G
     from streamspeech_b200 import synth
@@ -47,7 +49,7 @@ def main():
     from streamspeech_b200.offline import UnitYGenerator
 
     torch.set_grad_enabled(False)
-    cfg = ModelConfig.unity_default()
+    cfg = ModelConfig.unity_default(a.variant)
     eng = Engine(cfg, synth.make_unity_state_dict(cfg, 0), None, None, device=0)
     gen = UnitYGenerator(eng, beam_size_mt=a.beam_mt, max_len_a=1.0, max_len_b=200)
     rng = np.random.default_rng(0)
@@ -55,7 +57,7 @@ def main():
     x = torch.from_numpy(rng.standard_normal((a.samples, F, 80)).astype(np.float32)).cuda()
     lens = [F - int(v) for v in rng.integers(0, F // 4, a.samples)]
     lens[0] = F
-    res = {"card": card(), "samples": a.samples, "fbank_frames": F, "beam_mt": a.beam_mt}
+    res = {"card": card(), "variant": a.variant, "samples": a.samples, "fbank_frames": F, "beam_mt": a.beam_mt}
     gen.generate(x, lens)  # warm-up of every shape
     stages = {k: [] for k in ("encoder", "mt_search", "mt_features", "t2u_encoder", "unit_search")}
     for _ in range(a.reps):
@@ -112,7 +114,7 @@ def main():
                 p = os.path.join(data, f"u{i}.npy")
                 np.save(p, rng.standard_normal((n, 80)).astype(np.float32))
                 f.write(f"u{i}\t{p}\t{n}\t\t0\n")
-        argv = [data, "--task", "speech_to_speech_modified", "--target-is-code", "--target-code-size", "1000", "--path", "synthetic",
+        argv = [data, "--user-dir", f"researches/{a.variant}", "--task", "speech_to_speech_modified", "--target-is-code", "--target-code-size", "1000", "--path", "synthetic",
                 "--gen-subset", "test", "--beam-mt", str(a.beam_mt), "--beam", "1", "--max-len-a", "1", "--max-tokens", "10000",
                 "--required-batch-size-multiple", "1", "--results-path", os.path.join(d, "out")]
         with open(os.devnull, "w") as null:

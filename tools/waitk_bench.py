@@ -27,7 +27,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-STAGES = {"encoder": "encoder", "mt_greedy": "mt_search", "t2u_encode_batch": "mt_features_t2u", "unit_search_batch": "unit_search",
+STAGES = {"encoder": "encoder", "encoder_stream_step": "encoder", "mt_greedy": "mt_search", "t2u_encode_batch": "mt_features_t2u", "unit_search_batch": "unit_search",
           "vocoder_durations": "vocoder", "vocoder_generate": "vocoder"}
 
 
@@ -56,6 +56,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--utterances", type=int, default=4)
     ap.add_argument("--seconds", type=float, default=10.0)
+    ap.add_argument("--variant", choices=("unity", "uni_unity", "chunk_unity"), default="unity",
+                    help="the synthetic UnitY-family checkpoint (Uni-UnitY re-encodes the prefix, Chunk-UnitY encodes incrementally)")
     a = ap.parse_args()
     from streamspeech_b200 import synth
     from streamspeech_b200.simuleval_compat import SpeechSegment
@@ -65,8 +67,8 @@ def main():
         raise SystemExit("waitk_bench needs a CUDA device")
     p = argparse.ArgumentParser()
     add_waitk_args(p)
-    agent = WaitkS2STAgent(p.parse_args(["--model-path", "synthetic", "--data-bin", ".", "--vocoder", "synthetic", "--vocoder-cfg", "none",
-                                         "--dur-prediction"]))
+    agent = WaitkS2STAgent(p.parse_args(["--model-path", "synthetic", "--user-dir", f"researches/{a.variant}", "--data-bin", ".",
+                                         "--vocoder", "synthetic", "--vocoder-cfg", "none", "--dur-prediction"]))
     eng = agent.engine
     wavs = [synth.make_audio(a.seconds, seed=900 + i).tolist() for i in range(a.utterances)]
     step = 16 * 320
@@ -116,7 +118,7 @@ def main():
         stream(w, on_call)
     full = [c for c in calls if "syncs" in c]  # calls that passed the gate
     stages = sorted({s for c in full for s in STAGES.values() if s in c})
-    res = {"card": card(), "utterances": a.utterances, "seconds": a.seconds, "segment_ms": 320,
+    res = {"card": card(), "variant": a.variant, "utterances": a.utterances, "seconds": a.seconds, "segment_ms": 320,
            "audio_s_per_s": round(a.utterances * a.seconds / wall, 3), "policy_calls": len(calls), "calls_past_gate": len(full),
            "stage_ms_per_call": {s: round(float(np.mean([c.get(s, 0.0) for c in full])), 3) for s in stages},
            "stage_ms_max": {s: round(float(np.max([c.get(s, 0.0) for c in full])), 3) for s in stages},
