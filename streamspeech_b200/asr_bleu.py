@@ -155,6 +155,35 @@ def run_asr_bleu(args: argparse.Namespace, transcriber=None):
     return transcripts, bleu
 
 
+class SimulEvalASRFailed(Exception):
+    """where the compute_asr_bleu.py run that SimulEval makes fails on the run's files: a missing wav, a file too short to transcribe"""
+
+
+def transcribe_simuleval(audio_dirpath: str, reference_path: str, make_transcriber) -> List[str]:
+    """The run of fairseq's examples/speech_to_speech/asr_bleu/compute_asr_bleu.py that SimulEval's ASR_BLEU scorer makes
+    (`--reference_path instances.log --reference_format txt`): the *_pred.wav files in numeric order, one per line of the reference
+    file, each transcribed as written (no silence removal) in one batched pass -> the lower-cased transcripts, transcript i of
+    {i}_pred.wav.  Where the script fails on the files, this raises SimulEvalASRFailed naming the cause: a wav {i}_pred.wav missing for
+    some i below the number of lines, or a file too short for one encoder frame.  Anything else (an unreadable file, a transcriber
+    error) propagates as it is.  make_transcriber() builds the transcriber, once the files are known to be there.  The script's own
+    BLEU against the log's lines is not computed: SimulEval ignores it."""
+    references = extract_text_for_eval(reference_path, "txt")
+    try:
+        files = extract_audio_for_eval(audio_dirpath, "n_pred.wav", sort_numeric=True)
+    except AssertionError as e:
+        raise SimulEvalASRFailed(str(e)) from e
+    if len(files) != len(references):
+        missing = [f"{i}_pred.wav" for i in range(len(references)) if not (Path(audio_dirpath) / f"{i}_pred.wav").exists()]
+        raise SimulEvalASRFailed(f"{len(files)} *_pred.wav files in {audio_dirpath} for {len(references)} lines of {reference_path}; "
+                                 f"missing: {', '.join(missing) or 'none'}")
+    tr = make_transcriber()
+    waves = [tr.load_audio(fp) for fp in files]
+    for fp, w in zip(files, waves):
+        if tr.num_frames(len(w)) <= 0:
+            raise SimulEvalASRFailed(f"{fp}: {len(w)} samples are fewer than one encoder frame needs")
+    return tr.transcribe(waves)
+
+
 def main(argv: Optional[Sequence[str]] = None, transcriber=None):
     args = parse_args(argv)
     if transcriber is None:

@@ -12,10 +12,16 @@ whenever an instance's prediction finishes, and never between instances otherwis
 agent runs the list in order, without the pool.  The wait-k agents (UnitY checkpoints) have no pooled form and run `--streams 1`
 only.
 
-What SimulEval writes is written the same way, so `simuleval --score-only --output DIR` scores the run: `instances.log` (one
-`summarize()` dict per line, in index order), `config.yaml`, and for speech output `wavs/{index}_pred.wav`.  The instance classes
-below restate SimulEval's (evaluator/instance.py); `simuleval` itself is not imported (its package import needs optional
-dependencies).  `--computation-aware` is refused: the pooled streams share each flush, so one stream's compute time is undefined.
+What SimulEval writes is written the same way: `instances.log` (one `summarize()` dict per line, in index order), `config.yaml`,
+and for speech output `wavs/{index}_pred.wav`.  The instance classes below restate SimulEval's (evaluator/instance.py); `simuleval`
+itself is not imported (its package import needs optional dependencies).  `--computation-aware` is refused: the pooled streams
+share each flush, so one stream's compute time is undefined.
+
+Scoring (streamspeech_b200/simuleval_scoring.py): with `--quality-metrics` or `--latency-metrics` the run is scored as SimulEval
+scores it (the other flag then takes SimulEval's defaults), writing `scores.tsv` and `metrics.tsv` and printing the results table;
+`ASR_BLEU` transcribes `wavs/` on the GPU transcriber (`--asr-model`, `--asr-dict`) after the agents' engine is closed.  A run with
+neither flag is not scored (SimulEval would score it with its defaults).  `--score-only --output DIR` scores a finished run from its
+`instances.log`, as `simuleval --score-only` does.
 """
 from __future__ import annotations
 
@@ -35,6 +41,7 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if _REPO not in sys.path:
     sys.path.insert(0, _REPO)
 
+from streamspeech_b200 import simuleval_scoring as scoring  # noqa: E402
 from streamspeech_b200.simuleval_compat import EmptySegment, SpeechSegment  # noqa: E402
 
 # --agent file name -> (target type, single agent class name, pooled agent class name)
@@ -252,9 +259,11 @@ class SpeechToSpeechInstance(SpeechInstance):
         self.delays.append(self.step_to_delay(self.step))
 
     def waveform(self):
-        """(the written samples: each prediction at its delay, silence where it waits for the source; prediction_offset)"""
+        """(the written samples: each prediction at its delay, silence where it waits for the source; prediction_offset).  Sets
+        intervals ([start, duration] per prediction) and silences (the length of each wait), as SimulEval's summarize() does."""
         samples: List[float] = []
         self.intervals = []
+        self.silences: List[float] = []
         if not self.prediction_list:
             return samples, self.source_length
         start = prev_end = prediction_offset = self.delays[0]
@@ -262,6 +271,7 @@ class SpeechToSpeechInstance(SpeechInstance):
             start = max(prev_end, delay)
             if start > prev_end:
                 samples += [0.0] * int(self.target_sample_rate * (start - prev_end) / 1000)
+                self.silences.append(start - prev_end)
             samples += self.prediction_list[i]
             prev_end = start + self.durations[i]
             self.intervals.append([start, self.durations[i]])
@@ -282,8 +292,7 @@ class SpeechToSpeechInstance(SpeechInstance):
 # ------------------------------------------------------------------------------------------------------------------------ arguments
 
 def _add_evaluator_args(parser: argparse.ArgumentParser):
-    """SimulEval's flags (options.py, dataloader.py) that a run of a speech source list needs, and those its scripts pass for
-    scoring, which this run accepts and leaves to `simuleval --score-only`"""
+    """SimulEval's flags (options.py, dataloader.py) that a run of a speech source list needs, and its scoring flags"""
     parser.add_argument("--agent", required=True, help="one of the agent files under streamspeech_b200/agents/ (matched by file name)")
     parser.add_argument("--source", required=True, help="list of source WAV files, one per line")
     parser.add_argument("--target", required=True, help="list of references, one per line")
@@ -295,10 +304,27 @@ def _add_evaluator_args(parser: argparse.ArgumentParser):
     parser.add_argument("--streams", type=int, default=1,
                         help="instances in flight; above 1 they share one stream pool, 1 runs the single agent")
     parser.add_argument("--computation-aware", action="store_true", default=False, help="refused (see --help of this module)")
-    for flag in ("--quality-metrics", "--latency-metrics"):
-        parser.add_argument(flag, nargs="+", default=None, help="accepted and ignored: score with `simuleval --score-only`")
-    parser.add_argument("--target-speech-lang", type=str, default="en", help="accepted and ignored (ASR-BLEU scoring)")
+    _add_scoring_args(parser)
     parser.add_argument("--device", type=str, default="gpu", help="accepted and ignored: the engine runs on --device-index")
+
+
+def _add_scoring_args(parser: argparse.ArgumentParser):
+    """SimulEval's scoring flags, and the ASR_BLEU transcriber's (those of the asr_bleu front door)"""
+    parser.add_argument("--quality-metrics", nargs="+", default=None,
+                        help=f"any of {list(scoring.QUALITY_METRICS)}; given alone, the latency metrics default to SimulEval's "
+                             f"{scoring.DEFAULT_LATENCY}; neither flag: the run is not scored")
+    parser.add_argument("--latency-metrics", nargs="+", default=None,
+                        help=f"any of {list(scoring.LATENCY_METRICS)}; given alone, the quality metrics default to "
+                             f"{scoring.DEFAULT_QUALITY}")
+    parser.add_argument("--sacrebleu-tokenizer", type=str, default="13a", help="only 13a is offered")
+    parser.add_argument("--no-use-ref-len", action="store_true", default=False,
+                        help="latency metrics take the prediction's length, not the reference's, as the target length")
+    parser.add_argument("--target-speech-lang", type=str, default="en", help="the language of the target speech (ASR_BLEU); only en")
+    parser.add_argument("--asr-model", default=None, help="ASR_BLEU: local path of the fairseq wav2vec 2.0 CTC checkpoint (or "
+                                                          "'synthetic': the seeded test model)")
+    parser.add_argument("--asr-dict", default=None, help="ASR_BLEU: local path of dict.ltr.txt")
+    parser.add_argument("--asr-setting", action="append", default=[], metavar="KEY=VALUE",
+                        help="ASR_BLEU: override a transcriber setting read from the checkpoint (see python -m streamspeech_b200.asr_bleu)")
 
 
 def agent_kind(agent_path: str):
@@ -368,6 +394,10 @@ class Evaluation:
             self.infos[i] = check_source(self.sources[i], args.sample_rate)
         self.source_seconds = sum(info.frames / info.samplerate for info in self.infos.values())
         self.max_in_flight = 0
+        # index -> what the scorers read from the finished instance (not its samples), in index order whatever order the streams
+        # finish in; None: the run is not scored
+        self.kept: Optional[Dict[int, scoring.ScoredInstance]] = None
+        self.scores: Optional[Dict[str, object]] = None
 
     def _instance(self, index: int):
         samples, info = read_wav(self.sources[index])
@@ -388,6 +418,7 @@ class Evaluation:
         queue = iter(self.indices)
         active: Dict[int, object] = {}  # stream -> its instance
         done: Dict[int, str] = {}        # index -> its log line, until every smaller index has been written
+        done_kept: Dict[int, scoring.ScoredInstance] = {}  # the same, for what the scorers read
         next_to_write = self.indices.start
         for a in self.agents:
             a.reset()
@@ -412,11 +443,17 @@ class Evaluation:
                     if inst.finish_prediction:  # evaluator.py:224-229
                         self.agents[j].reset()
                     if inst.source_finished_reading:
-                        done[inst.index] = json.dumps(inst.summarize())
+                        summary = inst.summarize()
+                        done[inst.index] = json.dumps(summary)
+                        if self.kept is not None:
+                            done_kept[inst.index] = scoring.live_instance(summary, self.args.eval_latency_unit,
+                                                                          getattr(inst, "silences", None))
                         del active[j]
                         admit(j)
                 while next_to_write in done:
                     log.write(done.pop(next_to_write) + "\n")
+                    if self.kept is not None:  # in index order, as SimulEval scores and as the log lists them
+                        self.kept[next_to_write] = done_kept.pop(next_to_write)
                     next_to_write += 1
         finally:
             log.close()
@@ -450,20 +487,98 @@ def build_agents(args: argparse.Namespace, max_seconds: int = 60):
     return agents, pool, target_type
 
 
+def parse_score_only_args(argv: Sequence[str]) -> argparse.Namespace:
+    """`--score-only --output DIR` and the scoring flags; --agent, --source and --target are not required (and are ignored)"""
+    parser = argparse.ArgumentParser(prog="python -m streamspeech_b200.evaluate --score-only",
+                                     description="score the run in --output from its instances.log, as `simuleval --score-only` does")
+    parser.add_argument("--score-only", action="store_true", required=True)
+    parser.add_argument("--output", required=True, help="the output directory of a run")
+    for flag in ("--agent", "--source", "--target"):
+        parser.add_argument(flag, default=None, help="accepted and ignored")
+    parser.add_argument("--eval-latency-unit", type=str, default="word", choices=["word", "char"],
+                        help="accepted and ignored: SimulEval's LogInstance counts reference words whatever the unit")
+    parser.add_argument("--computation-aware", action="store_true", default=False, help="refused")
+    parser.add_argument("--device-index", type=int, default=0, help="CUDA device of the ASR_BLEU transcriber")
+    _add_scoring_args(parser)
+    parser.add_argument("--device", type=str, default="gpu", help="accepted and ignored")
+    args = parser.parse_args(argv)
+    if args.computation_aware:
+        parser.error("--computation-aware is not offered: the computation-aware metrics are not scored")
+    return args
+
+
+def _transcriber_factory(args: argparse.Namespace):
+    def make():
+        from streamspeech_b200.asr import ASRTranscriber, parse_settings
+
+        return ASRTranscriber(args.asr_model, args.asr_dict, getattr(args, "device_index", 0), settings=parse_settings(args.asr_setting))
+
+    return make
+
+
+def _check_scoring(args: argparse.Namespace, metrics, speech_output: Optional[bool], score_only: bool, n_instances: Optional[int]):
+    quality, latency = metrics
+    scoring.check_request(quality, latency, tokenizer=args.sacrebleu_tokenizer, target_speech_lang=args.target_speech_lang,
+                          speech_output=speech_output, score_only=score_only, asr_model=args.asr_model, n_instances=n_instances)
+    if args.asr_model is not None and "ASR_BLEU" in quality:
+        from streamspeech_b200.asr import parse_settings
+
+        try:
+            parse_settings(args.asr_setting)
+        except ValueError as e:
+            raise SystemExit(str(e)) from None
+
+
+def score_run(args: argparse.Namespace, instances: Dict[int, "scoring.ScoredInstance"], metrics) -> Dict[str, object]:
+    """score the instances, write scores.tsv and metrics.tsv into --output and print the results table"""
+    quality, latency = metrics
+    scores = scoring.score(instances, quality, latency, use_ref_len=not args.no_use_ref_len, make_transcriber=_transcriber_factory(args))
+    scoring.dump(Path(args.output), instances, scores)
+    return scores
+
+
+def score_only(argv: Sequence[str]) -> Dict[str, object]:
+    args = parse_score_only_args(argv)
+    metrics = scoring.metric_lists(args.quality_metrics, args.latency_metrics) or (scoring.DEFAULT_QUALITY, scoring.DEFAULT_LATENCY)
+    _check_scoring(args, metrics, None, True, None)
+    instances = scoring.read_log(Path(args.output))
+    _check_scoring(args, metrics, None, True, len(instances))
+    if "ASR_BLEU" in metrics[0] and instances and not str(next(iter(instances.values())).prediction).endswith("_pred.wav"):
+        raise SystemExit("--quality-metrics ASR_BLEU needs speech output; the run in --output wrote text")
+    return score_run(args, instances, metrics)
+
+
 def main(argv: Optional[Sequence[str]] = None):
+    argv = list(sys.argv[1:] if argv is None else argv)
+    if "--score-only" in argv:
+        return score_only(argv)
     args = parse_args(argv)
     target_type = agent_kind(args.agent)[0]
+    metrics = scoring.metric_lists(args.quality_metrics, args.latency_metrics)
+    if metrics is not None:  # refused before the model is loaded, so a long run does not fail at its end
+        _check_scoring(args, metrics, target_type == "speech", False, None)
     ev = Evaluation(args, [], target_type)  # sources checked before the model is loaded
+    if metrics is not None:
+        _check_scoring(args, metrics, target_type == "speech", False, len(ev.indices))
+        ev.kept = {}
     longest = max((info.frames / info.samplerate for info in ev.infos.values()), default=1.0)
     agents, pool, _ = build_agents(args, max_seconds=math.ceil(longest) + 1)
     ev.agents = agents
     t0 = time.perf_counter()
     ev.run()
     seconds = time.perf_counter() - t0
-    print(json.dumps({"instances": len(ev.indices), "streams": args.streams, "source_seconds": round(ev.source_seconds, 3),
-                      "wall_seconds": round(seconds, 3), "audio_s_per_s": round(ev.source_seconds / max(seconds, 1e-9), 2),
-                      "output": str(ev.output)}))
-    (pool.engine if pool is not None else agents[0].engine).close()
+    line = {"instances": len(ev.indices), "streams": args.streams, "source_seconds": round(ev.source_seconds, 3),
+            "wall_seconds": round(seconds, 3), "audio_s_per_s": round(ev.source_seconds / max(seconds, 1e-9), 2),
+            "output": str(ev.output)}
+    if metrics is None:
+        print(json.dumps(line))
+    engine = pool.engine if pool is not None else agents[0].engine
+    engine.close()
+    if metrics is not None:  # after the engine is closed: the transcriber never shares the device with it
+        t1 = time.perf_counter()
+        ev.scores = score_run(args, ev.kept, metrics)
+        line["scoring_seconds"] = round(time.perf_counter() - t1, 3)
+        print(json.dumps(line))
     return ev
 
 
