@@ -1,7 +1,8 @@
 """`python -m streamspeech_b200.asr_bleu`: asr_bleu/compute_asr_bleu.py (and, with --rm-silence, asr_bleu_rm_silence/compute_asr_bleu.py)
 on the engine's transcriber.  Same flags, files and printed score line; the transcriber runs batched on the GPU (asr.ASRTranscriber) and
 BLEU is sacrebleu 2.2.0's corpus_bleu restated (sacrebleu_compat).  Only the `en` model is offered, from local files: nothing is
-downloaded.
+downloaded.  `--devices LIST` transcribes groups of files on one worker process per entry (streamspeech_b200/workers.py) and writes the
+same files and score line.
 """
 from __future__ import annotations
 
@@ -10,13 +11,16 @@ import glob
 import os
 import re
 import sys
+from contextlib import closing
+from functools import partial
 from pathlib import Path
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+from streamspeech_b200 import workers  # noqa: E402
 from streamspeech_b200.asr import AudioRefused  # noqa: E402
 from streamspeech_b200.sacrebleu_compat import corpus_bleu  # noqa: E402
 
@@ -85,7 +89,7 @@ def extract_text_for_eval(references_filepath: str, reference_format: str, refer
     raise NotImplementedError(reference_format)
 
 
-def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
+def _parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(description="ASR-BLEU between generated audio and text references, on the engine's GPU transcriber.")
     p.add_argument("--lang", type=str)
     p.add_argument("--asr_version", type=str, default="oct22")
@@ -105,7 +109,12 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
                         "read): conv_feature_layers, extractor_mode, layer_norm_first, pos_conv_depth, layer_type, "
                         "encoder_attention_heads, normalize, sample_rate")
     p.add_argument("--device", type=int, default=0)
-    return p.parse_args(argv)
+    workers.add_devices_arg(p)
+    return p
+
+
+def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
+    return workers.parse_with_devices(_parser(), argv, "--device")
 
 
 def check_model_args(args: argparse.Namespace):
@@ -122,6 +131,98 @@ def check_model_args(args: argparse.Namespace):
             raise SystemExit(f"{flag} {val}: nothing is downloaded; fetch {os.path.basename(val)} and pass its local path")
 
 
+# ------------------------------------------------------------------------------------------------------------------- transcription
+
+def asr_bleu_wave(tr, fp: str, rm_silence: bool):
+    """compute_asr_bleu.py's reading of one file: its waveform, or None where the script's transcription fails and scores as ""
+    (compute_asr_bleu.py:141-147).  A file the reference would transcribe but this transcriber refuses raises AudioRefused; with
+    rm_silence every failure raises."""
+    try:
+        w = tr.load_audio(fp, rm_silence=rm_silence)
+        if tr.num_frames(len(w)) <= 0:
+            raise ValueError(f"{fp}: {len(w)} samples are fewer than one encoder frame needs")
+        return w
+    except AudioRefused:
+        raise  # never scored as ""
+    except Exception:
+        if rm_silence:
+            raise
+        return None
+
+
+def simuleval_wave(tr, fp: str):
+    """the waveform of one file as SimulEval's compute_asr_bleu.py run reads it; too short for one encoder frame: SimulEvalASRFailed"""
+    w = tr.load_audio(fp)
+    if tr.num_frames(len(w)) <= 0:
+        raise SimulEvalASRFailed(f"{fp}: {len(w)} samples are fewer than one encoder frame needs")
+    return w
+
+
+def transcribe_group(tr, files: Sequence[str], read) -> List[object]:
+    """Per file its transcript, or the exception read(tr, file) raised (then nothing is transcribed).  read returns the waveform, or
+    None for a file that transcribes as ""; the readable files are transcribed in one batched call."""
+    waves: List[object] = []
+    for fp in files:
+        try:
+            waves.append(read(tr, fp))
+        except Exception as e:  # noqa: BLE001 (raised by transcribe_files in file order)
+            waves.append(e)
+    if any(isinstance(w, Exception) for w in waves):
+        return waves
+    ok = [i for i, w in enumerate(waves) if w is not None]
+    out: List[object] = [""] * len(files)
+    for i, t in zip(ok, tr.transcribe([waves[i] for i in ok])):
+        out[i] = t
+    return out
+
+
+class DeviceTranscribers:
+    """The transcription of `--devices`: one ASRTranscriber per entry of devices, each in its own worker process, over groups of
+    files pulled from a shared queue (streamspeech_b200/workers.py); transcripts come back in file order.  A transcript does not
+    depend on the batch it ran in (the transcriber's batch-of-one identity), so it equals the single-device one.  An error that is not
+    scored (a refused or unreadable file) raises in its worker and stops every worker (workers.WorkerFailed names the device and the
+    error); SimulEval's failure (a file too short for one frame) comes back and is raised in file order, to be scored as 0."""
+
+    def __init__(self, devices: Sequence[int], model_path: str, dict_path: Optional[str], settings: Dict[str, object]):
+        self.devices, self.model_path, self.dict_path, self.settings = list(devices), model_path, dict_path, settings
+
+    def transcribe_files(self, files: Sequence[str], read) -> List[object]:
+        size = max(1, min(64, -(-len(files) // (4 * len(self.devices)))))  # about four groups per worker, for balance
+        groups = [(k, list(files[i:i + size])) for k, i in enumerate(range(0, len(files), size))]
+        out: List[object] = []
+        with closing(workers.run(self.devices, _transcribe_job, (self.model_path, self.dict_path, self.settings, read), groups)) as results:
+            for _, outcomes in results:
+                out += outcomes
+        return out
+
+
+def _transcribe_job(device: int, payload, next_item, emit):
+    from streamspeech_b200.asr import ASRTranscriber
+
+    model_path, dict_path, settings, read = payload
+    tr = ASRTranscriber(model_path, dict_path, device, settings=settings)
+    try:
+        for key, files in iter(next_item, None):
+            outcomes = transcribe_group(tr, files, read)
+            for o in outcomes:  # an error the run cannot score stops every worker now (SimulEval's failure is scored, as 0)
+                if isinstance(o, Exception) and not isinstance(o, SimulEvalASRFailed):
+                    raise o
+            emit(key, outcomes)
+    finally:
+        tr.engine.close()
+
+
+def transcribe_files(tr, files: Sequence[str], read) -> List[str]:
+    """the transcripts of files on tr (an ASRTranscriber, or DeviceTranscribers); read(tr, file) as in transcribe_group.  Where a
+    read raised, the first such error in file order is raised, a SimulEvalASRFailed only when no other error was: as a single pass
+    that reads every file before it checks any length raises."""
+    outcomes = tr.transcribe_files(files, read) if isinstance(tr, DeviceTranscribers) else transcribe_group(tr, files, read)
+    errors = [o for o in outcomes if isinstance(o, Exception)]
+    for e in [e for e in errors if not isinstance(e, SimulEvalASRFailed)] + errors:
+        raise e
+    return outcomes
+
+
 def run_asr_bleu(args: argparse.Namespace, transcriber=None):
     """-> (transcripts, BLEUScore); writes pred.txt (default variant)"""
     from streamspeech_b200.asr import ASRTranscriber, parse_settings
@@ -129,24 +230,13 @@ def run_asr_bleu(args: argparse.Namespace, transcriber=None):
     references = extract_text_for_eval(args.reference_path, args.reference_format, args.reference_tsv_column)
     files = extract_audio_for_eval(args.audio_dirpath, args.audio_format, sort_numeric=args.rm_silence)
     assert len(files) == len(references)
-    tr = transcriber or ASRTranscriber(args.asr_model, args.asr_dict, args.device, settings=parse_settings(args.asr_setting))
-    waves: List = [None] * len(files)
-    for i, fp in enumerate(files):
-        try:
-            waves[i] = tr.load_audio(fp, rm_silence=args.rm_silence)
-            if tr.num_frames(len(waves[i])) <= 0:
-                raise ValueError(f"{fp}: {len(waves[i])} samples are fewer than one encoder frame needs")
-        except AudioRefused:
-            raise  # a file the reference would transcribe: refused, never scored as ""
-        except Exception:
-            if args.rm_silence:
-                raise
-            waves[i] = None  # compute_asr_bleu.py:141-147: a failed transcription scores as ""
-    ok = [i for i, w in enumerate(waves) if w is not None]
-    texts = tr.transcribe([waves[i] for i in ok])
-    transcripts = [""] * len(files)
-    for i, t in zip(ok, texts):
-        transcripts[i] = t
+    if transcriber is not None:
+        tr = transcriber
+    elif args.devices is not None:
+        tr = DeviceTranscribers(args.devices, args.asr_model, args.asr_dict, parse_settings(args.asr_setting))
+    else:
+        tr = ASRTranscriber(args.asr_model, args.asr_dict, args.device, settings=parse_settings(args.asr_setting))
+    transcripts = transcribe_files(tr, files, partial(asr_bleu_wave, rm_silence=args.rm_silence))
     if not args.rm_silence:
         with open(Path(args.audio_dirpath) / "pred.txt", "w") as f:
             f.write("\n".join(transcripts))
@@ -176,12 +266,7 @@ def transcribe_simuleval(audio_dirpath: str, reference_path: str, make_transcrib
         missing = [f"{i}_pred.wav" for i in range(len(references)) if not (Path(audio_dirpath) / f"{i}_pred.wav").exists()]
         raise SimulEvalASRFailed(f"{len(files)} *_pred.wav files in {audio_dirpath} for {len(references)} lines of {reference_path}; "
                                  f"missing: {', '.join(missing) or 'none'}")
-    tr = make_transcriber()
-    waves = [tr.load_audio(fp) for fp in files]
-    for fp, w in zip(files, waves):
-        if tr.num_frames(len(w)) <= 0:
-            raise SimulEvalASRFailed(f"{fp}: {len(w)} samples are fewer than one encoder frame needs")
-    return tr.transcribe(waves)
+    return transcribe_files(make_transcriber(), files, simuleval_wave)
 
 
 def main(argv: Optional[Sequence[str]] = None, transcriber=None):

@@ -22,6 +22,10 @@ scores it (the other flag then takes SimulEval's defaults), writing `scores.tsv`
 `ASR_BLEU` transcribes `wavs/` on the GPU transcriber (`--asr-model`, `--asr-dict`) after the agents' engine is closed.  A run with
 neither flag is not scored (SimulEval would score it with its defaults).  `--score-only --output DIR` scores a finished run from its
 `instances.log`, as `simuleval --score-only` does.
+
+`--devices LIST` (streamspeech_b200/workers.py) runs the list on one worker process per entry, each with `--streams` agents on its own
+engine on that device; the workers write the waveforms, and this process writes `config.yaml` and `instances.log` in index order and
+scores the run (ASR_BLEU transcribed on the same devices).  Every file is the one the single-process run writes.
 """
 from __future__ import annotations
 
@@ -42,6 +46,7 @@ if _REPO not in sys.path:
     sys.path.insert(0, _REPO)
 
 from streamspeech_b200 import simuleval_scoring as scoring  # noqa: E402
+from streamspeech_b200 import workers  # noqa: E402
 from streamspeech_b200.simuleval_compat import EmptySegment, SpeechSegment  # noqa: E402
 
 # --agent file name -> (target type, single agent class name, pooled agent class name)
@@ -304,6 +309,7 @@ def _add_evaluator_args(parser: argparse.ArgumentParser):
     parser.add_argument("--streams", type=int, default=1,
                         help="instances in flight; above 1 they share one stream pool, 1 runs the single agent")
     parser.add_argument("--computation-aware", action="store_true", default=False, help="refused (see --help of this module)")
+    workers.add_devices_arg(parser)
     _add_scoring_args(parser)
     parser.add_argument("--device", type=str, default="gpu", help="accepted and ignored: the engine runs on --device-index")
 
@@ -356,7 +362,7 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
             for action in parser._actions:
                 if action.dest in ("vocoder", "vocoder_cfg"):
                     action.required = False
-    args = parser.parse_args(argv)
+    args = workers.parse_with_devices(parser, argv, "--device-index")
     if args.computation_aware:
         parser.error("--computation-aware is not offered: pooled streams share every batched step, so a per-stream compute time "
                      "is undefined; the non-computation-aware latency metrics are scored from instances.log")
@@ -406,57 +412,108 @@ class Evaluation:
             return SpeechToSpeechInstance(index, samples.tolist(), wav_path=(self.output / "wavs" / f"{index}_pred.wav").absolute(), **common)
         return SpeechToTextInstance(index, samples.tolist(), **common)
 
-    def run(self):
-        from streamspeech_b200.scheduler import pushpop_many
-
+    def _open_output(self):
         self.output.mkdir(parents=True, exist_ok=True)
         if self.target_type == "speech":
             (self.output / "wavs").mkdir(exist_ok=True)
         with open(self.output / "config.yaml", "w") as f:  # evaluator.py:86-93, target_type written as the source type as there
             f.write("source_type: speech\ntarget_type: speech\n")
-        log = open(self.output / "instances.log", "w")
-        queue = iter(self.indices)
+        return open(self.output / "instances.log", "w")
+
+    def _write(self, log, index: int, line: str, kept: Optional["scoring.ScoredInstance"]):
+        log.write(line + "\n")
+        if self.kept is not None:  # in index order, as SimulEval scores and as the log lists them
+            self.kept[index] = kept
+
+    def play(self, next_index: Callable[[], Optional[int]], finished: Callable[[int, str, Optional["scoring.ScoredInstance"]], None]):
+        """Play the instances next_index() returns (None: no more) on the agents, and call finished(index, log line, what the
+        scorers read or None) for each as it finishes, in the order the streams finish them"""
+        from streamspeech_b200.scheduler import pushpop_many
+
         active: Dict[int, object] = {}  # stream -> its instance
-        done: Dict[int, str] = {}        # index -> its log line, until every smaller index has been written
-        done_kept: Dict[int, scoring.ScoredInstance] = {}  # the same, for what the scorers read
-        next_to_write = self.indices.start
         for a in self.agents:
             a.reset()
 
         def admit(stream):
-            i = next(queue, None)
+            i = next_index()
             if i is not None:
                 active[stream] = self._instance(i)
 
         for j in range(len(self.agents)):
             admit(j)
         seg_ms = self.args.source_segment_size
+        while active:
+            self.max_in_flight = max(self.max_in_flight, len(active))
+            streams = sorted(active)
+            segments = [active[j].send_source(seg_ms) for j in streams]
+            outputs = pushpop_many([self.agents[j] for j in streams], segments)
+            for j, out in zip(streams, outputs):
+                inst = active[j]
+                inst.receive_prediction(out)
+                if inst.finish_prediction:  # evaluator.py:224-229
+                    self.agents[j].reset()
+                if inst.source_finished_reading:
+                    summary = inst.summarize()
+                    kept = None
+                    if self.kept is not None:
+                        kept = scoring.live_instance(summary, self.args.eval_latency_unit, getattr(inst, "silences", None))
+                    finished(inst.index, json.dumps(summary), kept)
+                    del active[j]
+                    admit(j)
+
+    def run(self):
+        log = self._open_output()
+        queue = iter(self.indices)
+        done: Dict[int, tuple] = {}  # index -> (its log line, what the scorers read), until every smaller index has been written
+        next_to_write = [self.indices.start]
+
+        def finished(index, line, kept):
+            done[index] = (line, kept)
+            while next_to_write[0] in done:
+                self._write(log, next_to_write[0], *done.pop(next_to_write[0]))
+                next_to_write[0] += 1
+
         try:
-            while active:
-                self.max_in_flight = max(self.max_in_flight, len(active))
-                streams = sorted(active)
-                segments = [active[j].send_source(seg_ms) for j in streams]
-                outputs = pushpop_many([self.agents[j] for j in streams], segments)
-                for j, out in zip(streams, outputs):
-                    inst = active[j]
-                    inst.receive_prediction(out)
-                    if inst.finish_prediction:  # evaluator.py:224-229
-                        self.agents[j].reset()
-                    if inst.source_finished_reading:
-                        summary = inst.summarize()
-                        done[inst.index] = json.dumps(summary)
-                        if self.kept is not None:
-                            done_kept[inst.index] = scoring.live_instance(summary, self.args.eval_latency_unit,
-                                                                          getattr(inst, "silences", None))
-                        del active[j]
-                        admit(j)
-                while next_to_write in done:
-                    log.write(done.pop(next_to_write) + "\n")
-                    if self.kept is not None:  # in index order, as SimulEval scores and as the log lists them
-                        self.kept[next_to_write] = done_kept.pop(next_to_write)
-                    next_to_write += 1
+            self.play(lambda: next(queue, None), finished)
         finally:
             log.close()
+
+    def run_devices(self, devices: Sequence[int], max_seconds: int):
+        """run() with the instances spread over one worker process per entry of devices, each with --streams agents of its own on
+        its own engine; the workers write the waveforms, the log is written here in index order"""
+        from contextlib import closing
+
+        from streamspeech_b200 import workers
+
+        log = self._open_output()
+        try:
+            with closing(workers.run(devices, _evaluate_job, (self.args, self.target_type, self.kept is not None, max_seconds),
+                                     [(i, None) for i in self.indices])) as results:
+                for index, (line, kept) in results:
+                    self._write(log, index, line, kept)
+        finally:
+            log.close()
+
+
+def _evaluate_job(device: int, payload, next_item, emit):
+    """one --devices worker: the agents of build_agents on `device`, playing the indices of the shared queue"""
+    import copy
+
+    args, target_type, scored, max_seconds = payload
+    args = copy.copy(args)
+    args.device_index = device
+    agents, pool, _ = build_agents(args, max_seconds=max_seconds)
+    ev = Evaluation(args, agents, target_type)
+    ev.kept = {} if scored else None
+
+    def next_index():
+        item = next_item()
+        return None if item is None else item[0]
+
+    try:
+        ev.play(next_index, lambda index, line, kept: emit(index, (line, kept)))
+    finally:
+        (pool.engine if pool is not None else agents[0].engine).close()
 
 
 def check_source(path: str, sample_rate: int) -> AudioInfo:
@@ -499,9 +556,10 @@ def parse_score_only_args(argv: Sequence[str]) -> argparse.Namespace:
                         help="accepted and ignored: SimulEval's LogInstance counts reference words whatever the unit")
     parser.add_argument("--computation-aware", action="store_true", default=False, help="refused")
     parser.add_argument("--device-index", type=int, default=0, help="CUDA device of the ASR_BLEU transcriber")
+    workers.add_devices_arg(parser)
     _add_scoring_args(parser)
     parser.add_argument("--device", type=str, default="gpu", help="accepted and ignored")
-    args = parser.parse_args(argv)
+    args = workers.parse_with_devices(parser, argv, "--device-index")
     if args.computation_aware:
         parser.error("--computation-aware is not offered: the computation-aware metrics are not scored")
     return args
@@ -511,6 +569,10 @@ def _transcriber_factory(args: argparse.Namespace):
     def make():
         from streamspeech_b200.asr import ASRTranscriber, parse_settings
 
+        if getattr(args, "devices", None) is not None:
+            from streamspeech_b200.asr_bleu import DeviceTranscribers
+
+            return DeviceTranscribers(args.devices, args.asr_model, args.asr_dict, parse_settings(args.asr_setting))
         return ASRTranscriber(args.asr_model, args.asr_dict, getattr(args, "device_index", 0), settings=parse_settings(args.asr_setting))
 
     return make
@@ -562,18 +624,25 @@ def main(argv: Optional[Sequence[str]] = None):
         _check_scoring(args, metrics, target_type == "speech", False, len(ev.indices))
         ev.kept = {}
     longest = max((info.frames / info.samplerate for info in ev.infos.values()), default=1.0)
-    agents, pool, _ = build_agents(args, max_seconds=math.ceil(longest) + 1)
-    ev.agents = agents
-    t0 = time.perf_counter()
-    ev.run()
+    if args.devices is not None:  # the workers build the agents, each on its own device
+        t0 = time.perf_counter()
+        ev.run_devices(args.devices, max_seconds=math.ceil(longest) + 1)
+    else:
+        agents, pool, _ = build_agents(args, max_seconds=math.ceil(longest) + 1)
+        ev.agents = agents
+        t0 = time.perf_counter()
+        ev.run()
     seconds = time.perf_counter() - t0
-    line = {"instances": len(ev.indices), "streams": args.streams, "source_seconds": round(ev.source_seconds, 3),
-            "wall_seconds": round(seconds, 3), "audio_s_per_s": round(ev.source_seconds / max(seconds, 1e-9), 2),
-            "output": str(ev.output)}
+    line = {"instances": len(ev.indices), "streams": args.streams}
+    if args.devices is not None:  # streams is per worker; wall_seconds includes the workers' start-up and engine builds
+        line["devices"] = ",".join(map(str, args.devices))
+    line.update(source_seconds=round(ev.source_seconds, 3), wall_seconds=round(seconds, 3),
+                audio_s_per_s=round(ev.source_seconds / max(seconds, 1e-9), 2), output=str(ev.output))
     if metrics is None:
         print(json.dumps(line))
-    engine = pool.engine if pool is not None else agents[0].engine
-    engine.close()
+    if args.devices is None:
+        engine = pool.engine if pool is not None else agents[0].engine
+        engine.close()
     if metrics is not None:  # after the engine is closed: the transcriber never shares the device with it
         t1 = time.perf_counter()
         ev.scores = score_run(args, ev.kept, metrics)

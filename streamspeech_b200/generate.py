@@ -48,6 +48,8 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if _REPO not in sys.path:
     sys.path.insert(0, _REPO)
 
+from streamspeech_b200 import workers  # noqa: E402
+
 TASKS = ("speech_to_speech_ctc", "speech_to_speech_modified")  # StreamSpeech, UnitY
 MAX_SOURCE_POSITIONS = 6000  # fairseq/tasks/speech_to_speech.py: --max-source-positions default
 MAX_TARGET_POSITIONS = 1024  # --max-target-positions default
@@ -85,8 +87,9 @@ def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
     p.add_argument("--skip-invalid-size-inputs-valid-test", action="store_true")
     p.add_argument("--results-path", default=None, help="directory of generate-{gen_subset}.txt (default: the file goes to stdout)")
     p.add_argument("--device-index", type=int, default=0)
+    workers.add_devices_arg(p)
     p.add_argument("--cpu", action="store_true", help="refused: the engine runs on the GPU")
-    args = p.parse_args(argv)
+    args = workers.parse_with_devices(p, argv, "--device-index")
     if args.cpu:
         p.error("--cpu is not offered: every stage runs on the H100 engine")
     if args.task not in TASKS:
@@ -468,27 +471,61 @@ def run_batch(gen, split: Split, batch: Sequence[int]):
     return gen.generate(x.to(gen.engine.device), [f.shape[0] for f in feats], scores=True)
 
 
+# (key, dictionary, result field) of the stdout prints per batch: StreamSpeech's A- / S- / D- CTC and MT texts, UnitY's MT text
+STREAMSPEECH_PRINTS = (("A", "source_unigram", "asr_tokens"), ("S", "ctc_target_unigram", "st_tokens"), ("D", "target_unigram", "mt_tokens"))
+UNITY_PRINTS = (("D", "target_unigram", "mt_tokens"),)
+
+
+def make_generator(args: argparse.Namespace, cfg, engine):
+    from streamspeech_b200.offline import OfflineS2STGenerator, UnitYGenerator
+
+    if cfg.unity:
+        return UnitYGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, max_len_a=args.max_len_a,
+                              max_len_b=args.max_len_b, len_penalty=args.lenpen)
+    return OfflineS2STGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, len_penalty=args.lenpen)
+
+
+def batch_outputs(res, prints) -> List[Dict[str, object]]:
+    """what the print loop reads from a batch's results, on the host: the printed tokens, units, unit score and positional scores"""
+    return [{**{tok: [int(t) for t in r[tok]] for _, _, tok in prints}, "units": [int(t) for t in r["units"]],
+             "unit_score": r["unit_score"], "unit_positional_scores": r["unit_positional_scores"].numpy()} for r in res]
+
+
+def _generate_job(device: int, payload, next_item, emit):
+    """one --devices worker: its own engine and generator on `device`, running whole batches of the split"""
+    from streamspeech_b200.engine import Engine
+
+    args, split, max_enc_frames = payload
+    cfg, sd, _ = load_offline_checkpoint(args, max_enc_frames)
+    engine = Engine(cfg, sd, None, None, device=device, max_enc_frames=max_enc_frames)
+    try:
+        gen = make_generator(args, cfg, engine)
+        prints = UNITY_PRINTS if cfg.unity else STREAMSPEECH_PRINTS
+        for key, batch in iter(next_item, None):
+            emit(key, batch_outputs(run_batch(gen, split, batch), prints))
+    finally:
+        engine.close()
+
+
 def main(argv: Optional[Sequence[str]] = None, stdout=None):
     args = parse_args(argv)
     stdout = stdout or sys.stdout
     from streamspeech_b200.engine import Engine
-    from streamspeech_b200.offline import OfflineS2STGenerator, UnitYGenerator
 
     max_enc_frames = 1024
     config = load_config_yaml(args)
     split = Split(args, config, max_enc_frames)  # the split is checked before the model is loaded
     cfg, sd, dicts = load_offline_checkpoint(args, max_enc_frames)
-    engine = Engine(cfg, sd, None, None, device=args.device_index, max_enc_frames=max_enc_frames)
-    out_file = None
+    prints = UNITY_PRINTS if cfg.unity else STREAMSPEECH_PRINTS
+    engine = results = out_file = None
     try:
-        if cfg.unity:
-            gen = UnitYGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, max_len_a=args.max_len_a,
-                                 max_len_b=args.max_len_b, len_penalty=args.lenpen)
-            prints = (("D", dicts["target_unigram"], "mt_tokens"),)
-        else:
-            gen = OfflineS2STGenerator(engine, beam_size_mt=args.beam_mt, max_len_b_mt=args.max_len_b_mt, len_penalty=args.lenpen)
-            prints = (("A", dicts["source_unigram"], "asr_tokens"), ("S", dicts["ctc_target_unigram"], "st_tokens"),
-                      ("D", dicts["target_unigram"], "mt_tokens"))
+        if args.devices is None:
+            engine = Engine(cfg, sd, None, None, device=args.device_index, max_enc_frames=max_enc_frames)
+            gen = make_generator(args, cfg, engine)
+            results = ((k, batch_outputs(run_batch(gen, split, batch), prints)) for k, batch in enumerate(split.batches))
+        else:  # whole batches to the workers, each with its own engine, and their results back in batch order
+            del sd  # every worker loads the checkpoint itself; this process keeps only cfg and the dictionaries
+            results = workers.run(args.devices, _generate_job, (args, split, max_enc_frames), list(enumerate(split.batches)))
         if args.results_path is not None:
             os.makedirs(args.results_path, exist_ok=True)
             out_file = open(os.path.join(args.results_path, f"generate-{args.gen_subset}.txt"), "w", buffering=1, encoding="utf-8")
@@ -497,28 +534,32 @@ def main(argv: Optional[Sequence[str]] = None, stdout=None):
         scorer = BleuScorer(tgt.pad(), tgt.eos(), tgt.unk())
         t0 = time.perf_counter()
         seconds = 0.0
-        for batch in split.batches:
-            res = run_batch(gen, split, batch)
+        for k, res in results:
+            batch = split.batches[k]
             ids = list(batch)  # fairseq's sample["id"]: the dataset index
-            for key, d, tok in prints:
+            for key, dname, tok in prints:
                 for sid, r in zip(ids, res):
-                    text = ctc_text(d, r[tok])
+                    text = ctc_text(dicts[dname], r[tok])
                     print(mt_print_line(cfg, sid, text) if cfg.unity else f"{key}-{sid}\t{text}", file=stdout)
             for i, sid, r in zip(batch, ids, res):
                 target_tokens = encode_line(tgt, split.target(i))
                 target_str = unit_string(tgt, target_tokens, escape_unk=True)
-                for line in hypothesis_lines(sid, target_str, unit_string(tgt, r["units"]), r["unit_score"], r["unit_positional_scores"].numpy()):
+                for line in hypothesis_lines(sid, target_str, unit_string(tgt, r["units"]), r["unit_score"], r["unit_positional_scores"]):
                     print(line, file=out)
                 scorer.add(target_tokens, r["units"])
             seconds += sum(split.src_n_frames[i] for i in batch) / 100.0
         print("Generate {} with beam={}: {}".format(args.gen_subset, args.beam, scorer.result_string()), file=out)
         wall = time.perf_counter() - t0
+        on = "" if args.devices is None else f" on devices {','.join(map(str, args.devices))}"
         print(f"| {len(split.rows)} samples in {len(split.batches)} batches, {seconds:.1f} s of source in {wall:.2f} s "
-              f"({seconds / max(wall, 1e-9):.1f} audio-s/s)", file=sys.stderr)
+              f"({seconds / max(wall, 1e-9):.1f} audio-s/s){on}", file=sys.stderr)
     finally:
+        if results is not None:
+            results.close()  # stops the workers of --devices
         if out_file is not None:
             out_file.close()
-        engine.close()
+        if engine is not None:
+            engine.close()
     return split
 
 
