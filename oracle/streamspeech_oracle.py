@@ -147,7 +147,7 @@ def rel_positional_encoding(T: int, d_model: int) -> torch.Tensor:
 
 def rel_shift(x: torch.Tensor) -> torch.Tensor:
     """RelPositionMultiHeadedAttention.rel_shift (uni_unity/modules/espnet_multihead_attention.py:133-152)."""
-    zero_pad = torch.zeros((*x.size()[:3], 1), dtype=x.dtype)
+    zero_pad = torch.zeros((*x.size()[:3], 1), dtype=x.dtype, device=x.device)
     xp = torch.cat([zero_pad, x], dim=-1)
     xp = xp.view(*x.size()[:2], x.size(3) + 1, x.size(2))
     return xp[:, :, 1:].view_as(x)[:, :, :, : x.size(-1) // 2 + 1]
@@ -240,16 +240,19 @@ def depthwise_bn_silu_core(y, w, bn_mean, bn_var, bn_weight, bn_bias, conv_chunk
 # --------------------------------------------------------------------------------------
 class StreamSpeechOracle:
     def __init__(self, cfg, model_sd: Dict[str, torch.Tensor], vocoder_sd: Optional[Dict[str, torch.Tensor]] = None,
-                 gcmvn=None, chunk_size: Optional[int] = 8, conv_chunk_size: Optional[int] = None, dtype: torch.dtype = torch.float32):
+                 gcmvn=None, chunk_size: Optional[int] = 8, conv_chunk_size: Optional[int] = None, dtype: torch.dtype = torch.float32,
+                 device="cpu"):
         """dtype: the arithmetic of every block (float64 makes a high-precision reference of the fp32 model).  Weights are taken as
         fp32 and then converted, and the position tables are computed in fp32 and then converted, so a float64 oracle sees exactly
-        the numbers the fp32 model (and the engine) see; inputs are converted on entry."""
+        the numbers the fp32 model (and the engine) see; inputs are converted on entry.  device: where the weights live and every
+        block runs (inputs are moved there; float64 on a GPU keeps long sequences affordable)."""
         self.cfg = cfg
         self.dtype = dtype
-        self.sd = {k: (v.float().to(dtype) if v.is_floating_point() else v) for k, v in model_sd.items()}
+        self.device = torch.device(device)
+        self.sd = {k: (v.float().to(self.device, dtype) if v.is_floating_point() else v.to(self.device)) for k, v in model_sd.items()}
         self.vsd = None
         if vocoder_sd is not None:
-            self.vsd = {k: v.to(dtype) for k, v in _remove_weight_norm({k: v.float() for k, v in vocoder_sd.items()}).items()}
+            self.vsd = {k: v.to(self.device, dtype) for k, v in _remove_weight_norm({k: v.float() for k, v in vocoder_sd.items()}).items()}
         self.gcmvn = gcmvn
         self.set_chunk(chunk_size, conv_chunk_size)
 
@@ -262,7 +265,7 @@ class StreamSpeechOracle:
 
     # ---- E1 Conv1dSubsampler (chunk_unity/modules/convolution.py:75-89)
     def subsample(self, feats: torch.Tensor, lengths: torch.Tensor):
-        x = feats.to(self.dtype).transpose(1, 2).contiguous()  # B x C x T
+        x = feats.to(self.device, self.dtype).transpose(1, 2).contiguous()  # B x C x T
         for i in range(2):
             w = self.sd[f"encoder.subsample.conv_layers.{i}.weight"]
             b = self.sd[f"encoder.subsample.conv_layers.{i}.bias"]
@@ -325,11 +328,12 @@ class StreamSpeechOracle:
         """feats [B,F,80], lengths [B] -> dict like the fairseq encoder_out."""
         x, out_len = self.subsample(feats, lengths)
         T, B, C = x.shape
-        pad_mask = torch.arange(T).unsqueeze(0) >= out_len.unsqueeze(1)  # lengths_to_padding_mask
+        pad_mask = torch.arange(T).unsqueeze(0) >= out_len.cpu().unsqueeze(1)  # lengths_to_padding_mask
+        pad_mask = pad_mask.to(self.device)
         x = math.sqrt(C) * x
-        pos = rel_positional_encoding(T, C).to(self.dtype).unsqueeze(1)  # [2T-1,1,C]
+        pos = rel_positional_encoding(T, C).to(self.device, self.dtype).unsqueeze(1)  # [2T-1,1,C]
         x = _lin(x, self.sd, "encoder.linear")
-        mask = chunk_mask(T, self.chunk_size) if self.chunk_size is not None else None
+        mask = chunk_mask(T, self.chunk_size).to(self.device) if self.chunk_size is not None else None
         layers = []
         for i in range(self.cfg.enc_layers):
             x = self.conformer_layer(x, i, pos, mask, pad_mask)
@@ -340,7 +344,7 @@ class StreamSpeechOracle:
 
     # ---- C1 CTCDecoder.generate (agent/ctc_decoder.py:40-111)
     def ctc_logits(self, name: str, enc_out: torch.Tensor) -> torch.Tensor:
-        return _lin(enc_out.to(self.dtype), self.sd, f"{name}_decoder.proj").transpose(0, 1)  # B x T x V
+        return _lin(enc_out.to(self.device, self.dtype), self.sd, f"{name}_decoder.proj").transpose(0, 1)  # B x T x V
 
     def ctc_greedy(self, name: str, enc_out: torch.Tensor):
         lprobs = F.log_softmax(self.ctc_logits(name, enc_out), dim=-1)
@@ -373,13 +377,16 @@ class StreamSpeechOracle:
         c = self.cfg
         B, L = prev_tokens.shape
         pfx = "target_unigram_decoder"
-        enc_out = enc_out.to(self.dtype)
-        table = sinusoidal_table(max(1024, c.pad + 1 + L + 1), c.mt_dim, c.pad).to(self.dtype)
+        prev_tokens = prev_tokens.to(self.device)
+        enc_out = enc_out.to(self.device, self.dtype)
+        if enc_pad is not None:
+            enc_pad = enc_pad.to(self.device)
+        table = sinusoidal_table(max(1024, c.pad + 1 + L + 1), c.mt_dim, c.pad).to(self.device, self.dtype)
         pos = table.index_select(0, make_positions(prev_tokens, c.pad).view(-1)).view(B, L, -1)
         x = math.sqrt(c.mt_dim) * F.embedding(prev_tokens, self.sd[pfx + ".embed_tokens.weight"]) + pos
         x = x.transpose(0, 1)
         self_pad = prev_tokens.eq(c.pad) if prev_tokens.eq(c.pad).any() else None
-        causal = torch.triu(torch.ones(L, L, dtype=torch.bool), 1)
+        causal = torch.triu(torch.ones(L, L, dtype=torch.bool, device=self.device), 1)
         for i in range(c.mt_layers):
             x = self._decoder_layer(x, enc_out, f"{pfx}.layers.{i}", c.mt_heads, causal, self_pad, enc_pad)
         x = _ln(x, self.sd, pfx + ".layer_norm")
@@ -391,8 +398,9 @@ class StreamSpeechOracle:
     # ---- M1 greedy specialisation (beam=1) of SequenceGenerator.generate_decoder
     #      (agent/sequence_generator.py:165-582, fairseq/sequence_generator.py:630-739, search.py:110-146)
     def mt_greedy(self, enc_out: torch.Tensor, prefix: Optional[List[int]], max_new_tokens: int,
-                  max_len_b: int = 100, max_decoder_positions: int = 1024, min_len: int = 1) -> List[int]:
-        """Returns the finalized hypothesis tokens INCLUDING the trailing eos (as `finalize_hypos` does)."""
+                  max_len_b: int = 100, max_decoder_positions: int = 1024, min_len: int = 1, margins: Optional[List[float]] = None) -> List[int]:
+        """Returns the finalized hypothesis tokens INCLUDING the trailing eos (as `finalize_hypos` does).  margins: a list that gets
+        each searched step's gap between its two best candidates (how far the search is from another decision at that step)."""
         c = self.cfg
         prefix = list(prefix) if prefix is not None else []
         start = len(prefix)
@@ -415,7 +423,10 @@ class StreamSpeechOracle:
                 lprobs[c.eos] = NEG_INF
             if step > 0:
                 lprobs = lprobs + score  # BeamSearch.step adds the cumulative score
-            best = int(torch.topk(lprobs, 2)[1][0])
+            top = torch.topk(lprobs, 2)
+            best = int(top[1][0])
+            if margins is not None:
+                margins.append(float(top[0][0] - top[0][1]))
             score = float(lprobs[best])
             if best == c.eos:
                 return tokens[1:] + [c.eos]
@@ -436,8 +447,8 @@ class StreamSpeechOracle:
         prev_key length and concatenates (transformer_layer.py:492-505, static_kv otherwise).  Returns logits [vocab]."""
         c = self.cfg
         pfx = "target_unigram_decoder"
-        enc_out = enc_out.to(self.dtype)
-        table = sinusoidal_table(max(1024, c.pad + 1 + step + 2), c.mt_dim, c.pad).to(self.dtype)
+        enc_out = enc_out.to(self.device, self.dtype)
+        table = sinusoidal_table(max(1024, c.pad + 1 + step + 2), c.mt_dim, c.pad).to(self.device, self.dtype)
         p = c.pad if token == c.pad else c.pad + 1 + step
         x = math.sqrt(c.mt_dim) * self.sd[pfx + ".embed_tokens.weight"][token] + table[p]
         x = x.view(1, 1, -1)
@@ -507,9 +518,11 @@ class StreamSpeechOracle:
     def t2u_encoder(self, x: torch.Tensor, pad_mask: Optional[torch.Tensor]) -> torch.Tensor:
         """x [S,B,512] -> [S,B,512]."""
         c = self.cfg
-        x = x.to(self.dtype)
+        x = x.to(self.device, self.dtype)
+        if pad_mask is not None:
+            pad_mask = pad_mask.to(self.device)
         S = x.size(0)
-        causal = torch.triu(torch.ones(S, S, dtype=torch.bool), 1) if c.uni_encoder else None
+        causal = torch.triu(torch.ones(S, S, dtype=torch.bool, device=self.device), 1) if c.uni_encoder else None
         for i in range(c.t2u_layers):
             p = f"synthesizer_encoder.layers.{i}"
             res = x
@@ -575,7 +588,7 @@ class StreamSpeechOracle:
     def vocoder(self, codes: List[int], dur_prediction: bool = True):
         """CodeHiFiGANVocoderWithDur.forward (agent/tts/vocoder.py:48-60): returns (wav [N*hop], dur [1,U])."""
         v = self.vsd
-        code = torch.tensor([c for c in codes if c >= 0], dtype=torch.long).view(1, -1)
+        code = torch.tensor([c for c in codes if c >= 0], dtype=torch.long, device=self.device).view(1, -1)
         x = F.embedding(code, v["dict.weight"]).transpose(1, 2)  # 1 x 128 x U
         dur = None
         if dur_prediction:

@@ -35,14 +35,15 @@ def unity_max_len(max_len_a: float, max_len_b: int, padded_src_len: int, max_dec
 
 
 class UnitYOracle:
-    def __init__(self, cfg, model_sd: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32):
+    def __init__(self, cfg, model_sd: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32, device="cpu"):
         assert cfg.unity and not cfg.uni_encoder
         self.cfg = cfg
         self.dtype = dtype
-        self.o = StreamSpeechOracle(cfg, model_sd, None, None, chunk_size=None, dtype=dtype)
+        self.o = StreamSpeechOracle(cfg, model_sd, None, None, chunk_size=None, dtype=dtype, device=device)
+        self.device = self.o.device
         self.sd = self.o.sd
         # computed in fp32, then converted (what the engine loads as __const__.unit_pos_table)
-        self.pos = sinusoidal_table(cfg.max_target_positions + cfg.pad + 1, cfg.unit_dim, cfg.pad).to(dtype)
+        self.pos = sinusoidal_table(cfg.max_target_positions + cfg.pad + 1, cfg.unit_dim, cfg.pad).to(self.device, dtype)
 
     def t2u_encode(self, feats: torch.Tensor, lengths: Sequence[int]) -> torch.Tensor:
         """feats [B, S, D] (MT decoder features of [eos, hyp..., pad...]), lengths[b] = non-pad positions -> [B, S, D]"""
@@ -79,20 +80,21 @@ class UnitYOracle:
         c, dt = self.cfg, self.dtype
         assert min_len <= max_len
         B, S, D = t2u.shape
-        t2u = t2u.to(dt)
+        dev = self.device
+        t2u = t2u.to(dev, dt)
         scale = 64 ** -0.5
-        kpad = torch.arange(S).view(1, S) >= torch.tensor([int(n) for n in lengths]).view(B, 1)
+        kpad = (torch.arange(S).view(1, S) >= torch.tensor([int(n) for n in lengths]).view(B, 1)).to(dev)
         cross = []
         for l in range(c.unit_layers):
             p = f"decoder.layers.{l}.encoder_attn"
             cross.append((self._lin(t2u, p + ".k_proj"), self._lin(t2u, p + ".v_proj")))
         E = self.sd["decoder.embed_tokens.weight"]
-        selfk = [torch.zeros(B, 0, D, dtype=dt) for _ in range(c.unit_layers)]
-        selfv = [torch.zeros(B, 0, D, dtype=dt) for _ in range(c.unit_layers)]
-        tok = torch.full((B,), c.eos, dtype=torch.long)
+        selfk = [torch.zeros(B, 0, D, dtype=dt, device=dev) for _ in range(c.unit_layers)]
+        selfv = [torch.zeros(B, 0, D, dtype=dt, device=dev) for _ in range(c.unit_layers)]
+        tok = torch.full((B,), c.eos, dtype=torch.long, device=dev)
         out = [{"tokens": [], "cum": [], "score": None, "margin": math.inf, "margins": [], "ties": 0} for _ in range(B)]
         live = list(range(B))
-        cum = torch.zeros(B, dtype=dt)
+        cum = torch.zeros(B, dtype=dt, device=dev)
         for step in range(max_len + 1):
             x = math.sqrt(D) * E[tok] + self.pos[c.pad + 1 + step]
             for l in range(c.unit_layers):
@@ -143,7 +145,7 @@ class UnitYOracle:
                     cum[i] = sc[i, best]
             if not keep:
                 break
-            idx = torch.tensor(keep)
+            idx = torch.tensor(keep, device=dev)
             live = [live[i] for i in keep]
             tok, cum, kpad = nxt[idx], cum[idx], kpad[idx]
             selfk = [k[idx] for k in selfk]

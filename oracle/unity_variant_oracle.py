@@ -43,8 +43,8 @@ def _unity_base(cfg):
 
 
 class VariantUnitYOracle(UnitYOracle):
-    def __init__(self, cfg, model_sd, dtype: torch.dtype = torch.float32):
-        super().__init__(_unity_base(cfg), model_sd, dtype)
+    def __init__(self, cfg, model_sd, dtype: torch.dtype = torch.float32, device="cpu"):
+        super().__init__(_unity_base(cfg), model_sd, dtype, device)
         self.cfg = cfg
         configure(self.o, cfg)
 

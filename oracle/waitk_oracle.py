@@ -77,7 +77,10 @@ class _OracleWaitk:
             return None
         eo = self.o.encoder(feature.unsqueeze(0), torch.tensor([F]))["encoder_out"][0]
         max_len_b = min(F + 200, self.max_decoder_positions - 1)
-        hyp = self.o.mt_greedy(eo, self.tgt_subwords_indices, new_sub, max_len_b=max_len_b, max_decoder_positions=self.max_decoder_positions)
+        margins = []
+        hyp = self.o.mt_greedy(eo, self.tgt_subwords_indices, new_sub, max_len_b=max_len_b, max_decoder_positions=self.max_decoder_positions,
+                               margins=margins)
+        trace["mt_margin"] = min(margins)
         self.tgt_subwords_indices = hyp[:-1]
         trace["mt_tokens"] = list(hyp[:-1])
         return hyp, eo, F
